@@ -1,5 +1,4 @@
-"""In-tree build of the native pieces (no JIT cache: the .so files travel with the repo
-snapshot to the GPU box).  `python -m ai00_server_b200.build` or `__graft_entry__.build()`."""
+"""In-tree build of the native pieces for sm_90a (H100); no JIT cache, the .so files sit next to the sources.  `python -m ai00_server_b200.build` or `__graft_entry__.build()`."""
 from __future__ import annotations
 
 import os
@@ -15,7 +14,7 @@ SYNTH = os.path.join(HERE, "_synthfill.so")
 ORACLE_C = os.path.join(ROOT, "oracle", "liboracle_ref.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-shared",
 ]
 

@@ -1,4 +1,4 @@
-// Device-side helpers shared by all kernels (sm_100a only).
+// Device-side helpers shared by all kernels (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -31,12 +31,12 @@ struct MetaView {
 
 // ---------------------------------------------------------------------------------------
 // "A16" activation layout: the f16 operand of every projection, stored so that (a) the slice a GEMM stage needs -- one
-// 128-wide k block of ALL tokens of the step -- is ONE contiguous run (one bulk TMA copy) and (b) that run IS the UMMA
-// canonical K-major / no-swizzle operand of `th` token rows, which ONE tcgen05.mma with N = th consumes:
+// 128-wide k block of ALL tokens of the step -- is ONE contiguous run (one bulk TMA copy) and (b) that run IS the wgmma
+// canonical K-major / no-swizzle B operand of `th` token rows, which ONE wgmma with N = th consumes:
 //   [k block (128 k)][k8 chunk 16][th token rows][8 halves]      (8 rows x 16 B = one 128-byte core matrix)
 // th = 16 x (token tiles of the step) = 16 / 32 / 64 / 128; a step's producers and consumers agree on it (the engine passes
-// it to every launch).  Measured (profiles/r02_findings.md §8): a tcgen05.mma with N = 16 costs ~80 cycles whatever N is, so
-// eight N = 16 MMAs per k step (128-token steps) made the projections MMA-bound; one N = 128 MMA does not.
+// it to every launch).  One wide MMA per k step instead of one N = 16 MMA per token tile keeps the MMA issue count of a
+// stage independent of the step's token count.
 // Split operands (precision 1): th = 32, rows 0-15 hold the hi halves of the 16 tokens, rows 16-31 the lo halves.
 // Every buffer reserves 128 token rows per k block and K padded to whole k blocks (padding k is multiplied by zero weights).
 // ---------------------------------------------------------------------------------------
@@ -226,72 +226,69 @@ __device__ __forceinline__ void mma_16816(float (&c)[4], uint32_t a0, uint32_t a
 }
 
 // ---------------------------------------------------------------------------------------
-// tcgen05 (5th-gen tensor core) wrappers: TMEM allocation, single-thread MMA issue, commit to an
-// mbarrier, TMEM -> register loads.  SASS: UTCHMMA / UTCBAR / LDTM.
+// wgmma (Hopper warpgroup MMA): the four warps of a warpgroup issue one m64nNk16 MMA together, both operands read
+// from shared memory through matrix descriptors, the f32 accumulator in registers.  SASS: HGMMA.
+// Accumulator fragment of m64nN: thread t of the warpgroup holds d[i], i < N/2, at row 16 (t / 32) + (t % 32) / 4 +
+// 8 ((i % 4) / 2) and column 8 (i / 4) + 2 (t % 4) + (i % 2).
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// whole warp; writes the TMEM base address to shared memory at `smem_dst`
-__device__ __forceinline__ void tc_alloc(uint32_t smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tc_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// shared-memory matrix descriptor, K-major, no swizzle: core matrix = 8 rows x 16 bytes (128 B
-// contiguous); lbo = byte distance between the two 16-byte k chunks of one k16 step, sbo = byte
-// distance between 8-row groups.  Bits [46,48) = 1: Blackwell descriptor version.
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// shared-memory matrix descriptor, K-major, no swizzle: core matrix = 8 rows x 16 bytes (128 B contiguous);
+// lbo = byte distance between the two 16-byte k chunks of one k16 step, sbo = byte distance between 8-row groups.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-           ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 46);
+           ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32);
 }
-// instruction descriptor, kind::f16: f16 x f16 -> f32, both operands K-major
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// same, A operand (M = 128 rows x K = 16) read from tensor memory: lane m = row m, 8 columns of two f16 each (k even in the low half)
-__device__ __forceinline__ void tc_mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// 16 registers per thread -> 32 lanes x 16 consecutive 32-bit columns (lane i of the warp = TMEM lane base+i); SASS: STTM
-__device__ __forceinline__ void tc_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-        "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns -> 16 registers per thread (lane i of the warp = TMEM lane base+i)
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+// orders the warpgroup's register accesses (accumulator zeroing, epilogue reads) before the MMAs that follow
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// wait until at most N committed MMA groups of this warp are still running
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x N] += A[64 x 16] * B[N x 16]^T, f16 operands (both K-major) -> f32, D in registers
+template <int N>
+struct Wgmma;
+template <>
+struct Wgmma<16> {
+    static __device__ __forceinline__ void mma(float (&d)[8], uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(a), "l"(b));
+    }
+};
+template <>
+struct Wgmma<32> {
+    static __device__ __forceinline__ void mma(float (&d)[16], uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(a), "l"(b));
+    }
+};
+template <>
+struct Wgmma<64> {
+    static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(a), "l"(b));
+    }
+};
+template <>
+struct Wgmma<128> {
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(a), "l"(b));
+    }
+};
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc) {
+    Wgmma<N>::mma(d, a_desc, b_desc);
 }
 
 // Programmatic dependent launch: everything before griddepcontrol.wait may overlap the tail of the preceding kernel in the

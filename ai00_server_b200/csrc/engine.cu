@@ -415,7 +415,7 @@ struct Group {
 struct b200rwkv_engine {
     std::unique_ptr<Group> group;             // set on rank 0 of an in-process tensor-parallel engine
     b200rwkv_info info;
-    int dev = 0, rank = 0, world = 1, num_sms = 148;
+    int dev = 0, rank = 0, world = 1, num_sms = 132;
     int S = 0, chunk = 0, maxT = A16_MAX_ROWS, precision = 0;      // steps of up to 128 tokens
     int L = 0, C = 0, F = 0, V = 0, H = 0, N = 64, Cl = 0, Hl = 0, Fl = 0, Vl = 0;
     bool use_graph = true, use_pdl = true;
@@ -508,7 +508,6 @@ struct b200rwkv_engine {
     A16Buf a16_alloc(int K, int nmat = 1);
     GemmLaunch make_launch(std::vector<SegDesc>& segs, int force_grid = 0, int qtype = QT_NONE);
     int quant_layers = 0, quant_type = QT_NONE;     // the first `quant_layers` layers hold Int8 / NF4 projection matrices
-    bool q_ts = true;                               // expanded weights go to tensor memory (qgemm.cuh); false = reference variant
     int pick_split(int K, int tiles) const;
     void finalize_tp();
     template <typename P, typename... X>
@@ -642,7 +641,7 @@ void b200rwkv_engine::blend_loras(const StTensor& t) {
         DevTmp da(a->nbytes), db(b->nbytes);
         CK(cudaMemcpy(da.p, a->data, a->nbytes, cudaMemcpyHostToDevice));
         CK(cudaMemcpy(db.p, b->data, b->nbytes, cudaMemcpyHostToDevice));
-        lora_blend_kernel<<<148 * 8, 256>>>(d_tmp, (const __half*)db.p, (const __half*)da.p, out, in, r, lo.alpha);
+        lora_blend_kernel<<<num_sms * 8, 256>>>(d_tmp, (const __half*)db.p, (const __half*)da.p, out, in, r, lo.alpha);
         CK(cudaGetLastError());
         CK(cudaDeviceSynchronize());
     }
@@ -725,7 +724,7 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
         }
         if (qtype != QT_NONE) {
             const size_t nwarp = (size_t)sg.tiles * sg.KB * GEMM_BN;
-            const int grid = (int)std::min<size_t>((nwarp + 7) / 8, 148 * 32);
+            const int grid = (int)std::min<size_t>((nwarp + 7) / 8, (size_t)num_sms * 32);
             uint8_t* dstq = W + (size_t)sg.blk_begin * blk_bytes;
             if (qtype == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, sg.KB, dstq);
             else quantize_weight_kernel<QT_NF4><<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, sg.KB, dstq);
@@ -734,7 +733,7 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
             continue;
         }
         const size_t nchunk = (size_t)sg.tiles * sg.KB * (GEMM_WBYTES / 16);
-        const int grid = (int)std::min<size_t>((nchunk + 255) / 256, 148 * 16);
+        const int grid = (int)std::min<size_t>((nchunk + 255) / 256, (size_t)num_sms * 16);
         repack_weight_kernel<<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, d.K, sg.tiles, sg.KB,
                                             reinterpret_cast<uint4*>(W + (size_t)sg.blk_begin * GEMM_WBYTES));
         CK(cudaGetLastError());
@@ -744,17 +743,15 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
     g.grid = std::min(g.grid, blk);
     if (force_grid > 0) g.grid = std::min(force_grid, blk);
     else {
-        // Whole tiles per CTA whenever that keeps >= 3/4 of the SMs streaming: no cross-CTA fix-up in the tail, and
-        // (measured, profiles/r01_findings.md §7) grids of <= 16 CTAs per GPC finish together while 144-148 CTAs skew
-        // by 25 % because the 18/20-SM GPCs share the same GPC bandwidth as the 16-SM ones.
+        // Whole tiles per CTA whenever that keeps >= 3/4 of the SMs streaming: no cross-CTA fix-up in the tail, and a grid
+        // that leaves some SMs idle need not finish later than a full one, whose CTAs skew across GPCs of unequal SM counts.
         if (tile <= num_sms && tile * 4 >= num_sms * 3) g.grid = tile;
         else if (tile > num_sms)
             for (int cand = num_sms; cand * 4 >= num_sms * 3; --cand)
                 if (tile % cand == 0) { g.grid = cand; break; }
     }
     // Steps of 64 / 128 tokens: a partial accumulator tile is 32 / 64 KB per contributor, and the last arriver of a cut tile
-    // spends tens of microseconds summing them (measured: 3B K+R at 128 tokens, last MMA at 9-15 us, slowest CTA exits at
-    // 82 us; profiles/r02_steptrace_prefill128_3b.log).  Those steps run whole tiles per CTA, even if that leaves SMs idle.
+    // spends tens of microseconds summing them.  Those steps run whole tiles per CTA, even if that leaves SMs idle.
     g.grid_wide = g.grid;
     if (force_grid <= 0) {
         if (tile <= num_sms) g.grid_wide = tile;
@@ -816,11 +813,8 @@ void b200rwkv_engine::launch_gemm(const GemmLaunch& g, int MT, cudaStream_t s, P
     if (g.qtype != QT_NONE) {
         REQUIRE(!split, B200RWKV_ERR_UNSUPPORTED, "internal: quantised projections run with f16 activations");
         const int grid = MT >= 4 ? g.grid_wide : g.grid;
-#define QLAUNCH(MT_, QT_) launch_k(qgemm_kernel<MT_, QT_, true>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<MT_, QT_, true>::SMEM_BYTES, g.p, KC_GEMM, s, prof)
-        if (!q_ts && MT == 1) {      // reference variant (expanded weights through shared memory), decode shape only
-            if (g.qtype == QT_INT8) launch_k(qgemm_kernel<1, QT_INT8, false>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<1, QT_INT8, false>::SMEM_BYTES, g.p, KC_GEMM, s, prof);
-            else launch_k(qgemm_kernel<1, QT_NF4, false>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<1, QT_NF4, false>::SMEM_BYTES, g.p, KC_GEMM, s, prof);
-        } else if (g.qtype == QT_INT8) {
+#define QLAUNCH(MT_, QT_) launch_k(qgemm_kernel<MT_, QT_>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<MT_, QT_>::SMEM_BYTES, g.p, KC_GEMM, s, prof)
+        if (g.qtype == QT_INT8) {
             switch (MT) { case 1: QLAUNCH(1, QT_INT8); break; case 2: QLAUNCH(2, QT_INT8); break; case 4: QLAUNCH(4, QT_INT8); break; default: QLAUNCH(8, QT_INT8); break; }
         } else {
             switch (MT) { case 1: QLAUNCH(1, QT_NF4); break; case 2: QLAUNCH(2, QT_NF4); break; case 4: QLAUNCH(4, QT_NF4); break; default: QLAUNCH(8, QT_NF4); break; }
@@ -880,12 +874,9 @@ void b200rwkv_engine::build(const StFile& st) {
         REQUIRE(quant_type == QT_INT8 || quant_type == QT_NF4, B200RWKV_ERR_UNSUPPORTED, "quant_type must be Int8 or NF4 (SF4 is not implemented)");
         REQUIRE(world == 1, B200RWKV_ERR_UNSUPPORTED, "quantised layers are single-GPU in this version");
         REQUIRE(precision == 0, B200RWKV_ERR_UNSUPPORTED, "quantised layers run with precision 0 (f16 operands)");
-#define QATTR(MT_, QT_) CK(cudaFuncSetAttribute(qgemm_kernel<MT_, QT_, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, QGemmCfg<MT_, QT_, true>::SMEM_BYTES))
+#define QATTR(MT_, QT_) CK(cudaFuncSetAttribute(qgemm_kernel<MT_, QT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, QGemmCfg<MT_, QT_>::SMEM_BYTES))
         QATTR(1, QT_INT8); QATTR(2, QT_INT8); QATTR(4, QT_INT8); QATTR(8, QT_INT8);
         QATTR(1, QT_NF4); QATTR(2, QT_NF4); QATTR(4, QT_NF4); QATTR(8, QT_NF4);
-        CK(cudaFuncSetAttribute(qgemm_kernel<1, QT_INT8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, QGemmCfg<1, QT_INT8, false>::SMEM_BYTES));
-        CK(cudaFuncSetAttribute(qgemm_kernel<1, QT_NF4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, QGemmCfg<1, QT_NF4, false>::SMEM_BYTES));
-        if (const char* v = dbg_env("B200RWKV_QTS")) q_ts = atoi(v) != 0;
 #undef QATTR
     }
     {   // prefill steps of up to 128 tokens: per-token decay rows of a slot live in dynamic shared memory
@@ -1773,7 +1764,7 @@ void b200rwkv_engine::state_xform(int slot, bool import, float* snap) {
     }
     x.L = L; x.C = C; x.Hl = Hl; x.h0 = rank * Hl; x.transpose = (info.version != 7);
     const size_t total = (size_t)L * (N + 2) * C;
-    const int grid = (int)std::min<size_t>((total + 255) / 256, 148 * 32);
+    const int grid = (int)std::min<size_t>((total + 255) / 256, (size_t)num_sms * 32);
     if (import) state_xform_kernel<true><<<grid, 256, 0, stream>>>(x);
     else state_xform_kernel<false><<<grid, 256, 0, stream>>>(x);
     CK(cudaGetLastError());
@@ -1916,8 +1907,8 @@ static int32_t create_rank(const uint8_t* st, size_t len, int32_t device, int32_
     }
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
-    REQUIRE(prop.major == 10, B200RWKV_ERR_UNSUPPORTED,
-            "this library is built for sm_100a (B200) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
+    REQUIRE(prop.major == 9 && prop.minor == 0, B200RWKV_ERR_UNSUPPORTED,
+            "this library is built for sm_90a (H100) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
     StFile f(st, len);
     std::vector<std::unique_ptr<StFile>> lora_files;
     std::unique_ptr<b200rwkv_engine> e(new b200rwkv_engine());
@@ -2356,6 +2347,10 @@ static int32_t rank_bench_decode(b200rwkv_engine* e, int32_t nslot, const int32_
     }
     CK(cudaEventRecord(eb, e->stream));
     CK(cudaStreamSynchronize(e->stream));
+    if (e->d_keep && e->rank == 0) {          // every step kept each slot's logits row (enqueue_keep): sample_topk may read it
+        std::lock_guard<std::mutex> lk2(e->keep_mu);
+        for (int i = 0; i < nslot; ++i) e->keep_valid[slot[i]] = 1;
+    }
     CK(cudaEventElapsedTime(ms_out, ea, eb));
     for (int i = 0; i < (int)marks.size(); ++i) {
         CK(cudaEventElapsedTime(step_ms_out + i, i == 0 ? ea : marks[i - 1], marks[i]));
@@ -2497,7 +2492,9 @@ int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int3
     DevTmp src((size_t)N * K * 2), dst(total);
     CK(cudaMemcpy(src.p, w_f16, (size_t)N * K * 2, cudaMemcpyHostToDevice));
     const size_t nwarp = (size_t)tiles * KB * GEMM_BN;
-    const int grid = (int)std::min<size_t>((nwarp + 7) / 8, 148 * 32);
+    int nsm = 0;
+    CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
+    const int grid = (int)std::min<size_t>((nwarp + 7) / 8, (size_t)nsm * 32);
     if (quant_type == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256>>>((const __half*)src.p, K, 0, 0, N, tiles, KB, (uint8_t*)dst.p);
     else quantize_weight_kernel<QT_NF4><<<grid, 256>>>((const __half*)src.p, K, 0, 0, N, tiles, KB, (uint8_t*)dst.p);
     CK(cudaGetLastError());
@@ -2761,7 +2758,7 @@ int32_t b200rwkv_debug_gemm_time(b200rwkv_engine* e, int32_t which, int32_t reps
 #ifdef B200RWKV_DEBUG
 // Streaming micro-benchmark (see streamtest.cuh).  kind 0: vector loads; kind 1: bulk-TMA ring.
 int32_t b200rwkv_debug_stream(int32_t device, int32_t kind, double gbytes, int32_t stage_bytes, int32_t nstage, int32_t use_hint,
-                              int32_t consumer, int32_t split, int32_t producers, int32_t reps, float* ms_out) {
+                              int32_t split, int32_t producers, int32_t reps, float* ms_out) {
     int32_t extra = 0;
     if (stage_bytes % 16384 != 0 && stage_bytes > 16384) { extra = stage_bytes % 16384; }
     API_BEGIN((b200rwkv_engine*)nullptr)
@@ -2783,7 +2780,7 @@ int32_t b200rwkv_debug_stream(int32_t device, int32_t kind, double gbytes, int32
     CK(cudaEventCreate(&b));
     StreamParams sp;
     sp.src = buf; sp.bytes_per_cta = per_cta; sp.stage_bytes = stage_bytes; sp.nstage = nstage; sp.use_hint = use_hint;
-    sp.consumer = consumer; sp.split = split; sp.producers = producers; sp.extra = extra;
+    sp.split = split; sp.producers = producers; sp.extra = extra;
     const size_t smem = (size_t)nstage * stage_bytes + 2 * nstage * 8 + 64;
     if (kind == 1) CK(cudaFuncSetAttribute(stream_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     for (int r = 0; r < reps + 1; ++r) {
@@ -2812,7 +2809,9 @@ int32_t b200rwkv_debug_prefetch(int32_t device, double mbytes, int32_t consumers
     const int stage = 32768, nstage = 5;
     size_t per_cta = (size_t)(mbytes * 1e6 / consumers) / stage * stage;
     const size_t total = per_cta * consumers;
-    const size_t flush_bytes = (size_t)148 * stage * 64;       // ~310 MB through the same ring kernel
+    int nsm = 0;
+    CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
+    const size_t flush_bytes = (size_t)nsm * stage * 64;       // 2 MB per SM through the same ring kernel, several times the L2
     uint8_t *buf = nullptr, *fl = nullptr;
     CK(cudaMalloc(&buf, total + 1024));
     CK(cudaMalloc(&fl, flush_bytes + 1024));
@@ -2829,7 +2828,7 @@ int32_t b200rwkv_debug_prefetch(int32_t device, double mbytes, int32_t consumers
     CK(cudaEventCreate(&a)); CK(cudaEventCreate(&b)); CK(cudaEventCreate(&c));
     double s0 = 0, s1 = 0;
     for (int r = 0; r < reps + 1; ++r) {
-        stream_ring_kernel<<<148, 128, smem>>>(fp);
+        stream_ring_kernel<<<nsm, 128, smem>>>(fp);
         CK(cudaEventRecord(a));
         prefetch_probe_kernel<<<pf_grid, 128>>>(buf, per_cta, consumers, skip, nblk, mode, (unsigned long long)(idle_us * 1e3));
         CK(cudaEventRecord(b));
@@ -2849,24 +2848,6 @@ int32_t b200rwkv_debug_prefetch(int32_t device, double mbytes, int32_t consumers
     API_END
 }
 
-// tcgen05.mma rate of one instruction shape (streamtest.cuh): cycles[0] = issue loop, cycles[1] = until retired, for n MMAs.
-int32_t b200rwkv_debug_mma_rate(int32_t device, int32_t M, int32_t N, int32_t a_in_tmem, int32_t n, int64_t* cycles) {
-    API_BEGIN((b200rwkv_engine*)nullptr)
-    REQUIRE((M == 64 || M == 128) && N >= 16 && N <= 256 && N % 16 == 0 && n >= 1 && cycles, B200RWKV_ERR_INVALID, "bad argument");
-    CK(cudaSetDevice(device));
-    const size_t smem = 32768 + 65536 + 64;
-    CK(cudaFuncSetAttribute(mma_rate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    DevTmp out(16);
-    for (int r = 0; r < 2; ++r) {          // first launch warms the instruction cache
-        mma_rate_kernel<<<1, 128, smem>>>(M, N, a_in_tmem, n, (long long*)out.p);
-        CK(cudaGetLastError());
-        CK(cudaDeviceSynchronize());
-    }
-    long long h[2];
-    CK(cudaMemcpy(h, out.p, 16, cudaMemcpyDeviceToHost));
-    cycles[0] = h[0]; cycles[1] = h[1];
-    API_END
-}
 #endif   // B200RWKV_DEBUG
 
 // ---- exported SPMD entries: one rank, or all ranks of an in-process tensor-parallel engine at once ----

@@ -6,20 +6,18 @@
 //
 // HBM-bound by construction (T <= 64 rows per pass, each weight byte is used once per step), so
 // the design is about keeping ~200 KB of weight bytes in flight per SM and never stalling the
-// stream.  At batch 16 the math is 16 FLOP per weight byte = ~100 TFLOP/s at HBM rate: measured
-// on B200 the legacy mma.sync path tops out near 140 TFLOP/s (HMMA.16816 issues once per 32
-// cycles per sub-partition; profiles/r01_gemm_mma_sync.md), so the tensor work is on tcgen05:
-//   * swap-AB: the WEIGHT tile is the 128-row M operand, the token tile is the N=16 operand, the
-//     f32 accumulator (128 lanes x 16 columns) lives in TMEM; one elected thread issues
-//     tcgen05.mma.cta_group::1.kind::f16, eight k16 steps per 32 KB stage;
+// stream.  The tensor work is on Hopper's warpgroup MMA (wgmma):
+//   * swap-AB: the WEIGHT tile (128 rows = two m64 MMAs) is the M operand, the token tile is the N = 16 MT operand,
+//     both read from shared memory through descriptors; the f32 accumulator lives in the registers of the consumer
+//     warpgroup, eight k16 steps per 32 KB stage;
 //   * weights are re-tiled ONCE at load into 32 KB stage blocks (128 output rows x 128 k) already
-//     in the UMMA canonical K-major / no-swizzle shared-memory layout, so a pipeline stage is ONE
+//     in the canonical K-major / no-swizzle shared-memory layout, so a pipeline stage is ONE
 //     contiguous 1-D bulk TMA copy (cp.async.bulk -> UBLKCP) that the tensor core reads in place;
 //     activations use the matching A16 layout (common.cuh): one bulk copy of MT x 4 KB per stage (the
-//     issue rate of bulk copies, ~0.3 us each per thread, is what sizes the stage);
-//   * warp roles: one TMA producer lane drives a 4-6 stage mbarrier ring; one MMA lane consumes
-//     it (tcgen05.commit releases each slot when its MMAs retire); four epilogue warps drain the
-//     double-buffered TMEM accumulator with tcgen05.ld while the next tile's MMAs run;
+//     issue rate of bulk copies is what sizes the stage);
+//   * warp roles: one TMA producer lane drives a 3-6 stage mbarrier ring; the consumer warpgroup (4 warps) issues the
+//     MMAs of a stage, keeps one stage of MMAs in flight and releases each slot when its MMAs retire, then runs the
+//     epilogue of the tile from its registers while the producer keeps the ring full;
 //   * work is split stream-K style: the launch's stage blocks (all segments, all tiles) form one
 //     linear sequence cut into equal contiguous ranges, so every SM streams the same number of
 //     bytes whatever the matrix shapes;
@@ -35,18 +33,19 @@
 
 namespace b200 {
 
-constexpr int GEMM_BN = 128;                 // output rows (weight rows) per tile = UMMA M
-constexpr int GEMM_BK = 128;                 // k per stage block (8 x UMMA K=16)
+constexpr int GEMM_BN = 128;                 // output rows (weight rows) per tile = two wgmma M = 64
+constexpr int GEMM_BK = 128;                 // k per stage block (8 x wgmma K = 16)
 constexpr int GEMM_WBYTES = GEMM_BN * GEMM_BK * 2;   // 32 KB
 constexpr int GEMM_ABYTES = 16 * GEMM_BK * 2;        // 4 KB per 16-token tile
 constexpr int GEMM_K8 = GEMM_BK / 8;                 // 16-byte k chunks per stage
-constexpr int GEMM_EPI_WARPS = 4;            // one per TMEM lane quarter
+constexpr int GEMM_EPI_WARPS = 4;            // the consumer warpgroup: MMA issue and epilogue, thread t = output row t of a tile
 constexpr int GEMM_EPI_THREADS = GEMM_EPI_WARPS * 32;
-constexpr int GEMM_THREADS = (GEMM_EPI_WARPS + 2) * 32;   // + MMA warp + TMA producer warp
+constexpr int GEMM_THREADS = (GEMM_EPI_WARPS + 1) * 32;   // + TMA producer warp
 constexpr int GEMM_MAX_SEG = 8;
 constexpr int GEMM_STAGE_PITCH = 24;         // halves per row of the A16 epilogue staging buffer (16 tokens + padding, 48 B)
-constexpr int GEMM_SMEM_BUDGET = 221184;     // 216 KB for stages
-// canonical K-major no-swizzle strides of the two operands in shared memory
+constexpr int GEMM_SMEM_BUDGET = 221184;     // 216 KB for stages (227 KB per block, less the static transpose buffer)
+constexpr int GEMM_XPOSE_FLOATS = GEMM_BN * 16;   // accumulator -> row transpose of one 16-token tile (8 KB), shared with the A16 staging
+// canonical K-major no-swizzle strides of the two operands in shared memory (wgmma descriptors)
 constexpr uint32_t GEMM_W_LBO = 16 * 128;    // weight stage [k8 chunk 16][row group 16][8 rows][16 B]
 constexpr uint32_t GEMM_W_SBO = 128;
 constexpr uint32_t GEMM_A_LBO = 2 * 128;     // token operand [k8 chunk 16][16 MT rows][16 B]: MT x this (set in the MMA role)
@@ -87,7 +86,7 @@ struct GemmParams {
     float* ws;              // [total_tiles][max_contrib][128][MT*16] partial tiles
     unsigned* counters;     // [total_tiles], zero between launches
     const int* nrows;       // device: valid token rows
-    uint32_t w_lbo, w_sbo, a_lbo, a_sbo;   // UMMA descriptor strides (bytes)
+    uint32_t w_lbo, w_sbo, a_lbo, a_sbo;   // wgmma descriptor strides (bytes)
     unsigned long long* trace;             // profiling aid: 8 globaltimer stamps of CTA 0 (null in production)
     // L2 prefetch of the NEXT projection launch of the step (set per launch by the engine): when this CTA's producer
     // has requested its last block it asks L2 for the first `prefetch_blocks` blocks the same CTA index will stream in
@@ -108,9 +107,8 @@ struct GemmCfg {
     static constexpr int BUDGET = RING == 1 ? (GEMM_SMEM_BUDGET / 2) : GEMM_SMEM_BUDGET;
     static constexpr int NFIT = (BUDGET / STAGE_BYTES) > 12 ? 12 : (BUDGET / STAGE_BYTES);
     static constexpr int NSTAGE = (RING == 2 && NFIT > 2) ? NFIT - 1 : NFIT;
-    static constexpr int BAR_BYTES = (2 * NSTAGE + 4) * 8 + 16;
+    static constexpr int BAR_BYTES = 2 * NSTAGE * 8 + 16;
     static constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + BAR_BYTES + 64;
-    static constexpr int TMEM_COLS = (2 * 16 * MT) < 32 ? 32 : (2 * 16 * MT);   // double-buffered accumulator
 };
 
 __device__ __forceinline__ int gemm_find_seg(const GemmParams& p, int b) {
@@ -159,296 +157,322 @@ struct SegWalk {
 };
 
 // ---------------------------------------------------------------------------------------
-// MMA role (one thread): consume ring stages, accumulate each tile segment in TMEM.
+// Consumer warpgroup: MMAs of a tile segment into register accumulators, then the tile's epilogue.
 // ---------------------------------------------------------------------------------------
-template <int MT, int NSTAGE, int STAGE_BYTES>
-__device__ __forceinline__ void gemm_mma_role(const GemmParams& p, const int b0, const int b1, const uint32_t smem_base,
-                                              const uint32_t full_bar, const uint32_t empty_bar, const uint32_t tfull_bar,
-                                              const uint32_t tempty_bar, const uint32_t tmem_base, RingPos& rp, unsigned& segcount) {
-    constexpr uint32_t IDESC = umma_idesc_f16(GEMM_BN, 16 * MT);
+// element (row r, token column c < 16) of the transpose buffer; the 16-byte column groups are rotated by r / 2 so that
+// eight consecutive rows reading the same group hit eight different bank quads
+__device__ __forceinline__ int gemm_xpose_index(const int r, const int c) {
+    return r * 16 + ((((c >> 2) ^ (r >> 1)) & 3) << 2) + (c & 3);
+}
+template <int N>
+__device__ __forceinline__ void wgmma_fence_operand(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// fragment layout (common.cuh, wgmma) -> thread t holds output row t: v[mt][j] = token 16 mt + j
+template <int MT>
+__device__ __forceinline__ void gemm_acc_to_rows(float (&acc)[2][8 * MT], float (&v)[MT][16], float* s_x) {
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) {
+        named_bar_sync(3, GEMM_EPI_THREADS);                  // the previous readers of the buffer are done
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {                     // fragment pairs 8 mt + 2 e: n8 block e / 2, row half e % 2
+                const int i = 8 * mt + 2 * e;
+                const int r = 64 * h + 16 * warp + (lane >> 2) + 8 * (e & 1);
+                const int c = 8 * (e >> 1) + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(s_x + gemm_xpose_index(r, c)) = make_float2(acc[h][i], acc[h][i + 1]);
+            }
+        named_bar_sync(3, GEMM_EPI_THREADS);
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+            const float4 q = *reinterpret_cast<const float4*>(s_x + gemm_xpose_index(tid, 4 * g));
+            v[mt][4 * g] = q.x; v[mt][4 * g + 1] = q.y; v[mt][4 * g + 2] = q.z; v[mt][4 * g + 3] = q.w;
+        }
+    }
+    named_bar_sync(3, GEMM_EPI_THREADS);                      // the buffer is the epilogue's A16 staging next
+}
+
+// Epilogue of one tile segment (128 threads, thread t owns output row t of the tile, v = its 16 MT token values):
+// deterministic cross-CTA reduction of split tiles, fused epilogue.
+// SPLIT (precision 1, MT = 2): the two token tiles are the hi and lo halves of the SAME 16 tokens
+// (common.cuh split_h): the accumulator tiles are added before the epilogue and A16 outputs are written as hi / lo again.
+template <int MT, bool SPLIT = false>
+__device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const SegWalk& w, const int cta, const int G, float (&v)[MT][16],
+                                                   const int nrows, volatile int* s_last_p, __half* s_stage) {
+    const int tid = threadIdx.x;
+    const unsigned TB = (unsigned)p.total_blocks;
+    const GemmSeg& sg = p.seg[w.seg];
+    constexpr int ROWF = 16 * MT;
+    const unsigned tb0 = (unsigned)(sg.blk_begin + w.tile_local * sg.KB);
+    const int c_first = (int)(((unsigned long long)(tb0 + 1) * (unsigned)G - 1) / TB);
+    const int c_last = (int)(((unsigned long long)(tb0 + sg.KB) * (unsigned)G - 1) / TB);
+    const int ncontrib = c_last - c_first + 1;
+    const int gtile = sg.tile_begin + w.tile_local;
+    bool do_epilogue = true;
+    if (ncontrib > 1) {
+        float* wsl = p.ws + ((size_t)gtile * p.max_contrib + (cta - c_first)) * (GEMM_BN * ROWF) + (size_t)tid * ROWF;
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+            for (int j = 0; j < 16; j += 4)
+                *reinterpret_cast<float4*>(wsl + mt * 16 + j) = make_float4(v[mt][j], v[mt][j + 1], v[mt][j + 2], v[mt][j + 3]);
+        // publish: the barrier orders every thread's partial stores before thread 0's gpu-scope
+        // fence (fences are cumulative), then one counter bump per CTA
+        named_bar_sync(3, GEMM_EPI_THREADS);
+        if (tid == 0) {
+            const unsigned old = atom_add_acq_rel_gpu(p.counters + gtile, 1u);   // release ours, acquire the others'
+            *s_last_p = (old == (unsigned)(ncontrib - 1));
+            if (*s_last_p) p.counters[gtile] = 0;  // ready for the next launch
+        }
+        named_bar_sync(3, GEMM_EPI_THREADS);
+        do_epilogue = (*s_last_p != 0);
+        if (do_epilogue) {
+            const float* ws0 = p.ws + (size_t)gtile * p.max_contrib * (GEMM_BN * ROWF) + (size_t)tid * ROWF;
+#pragma unroll
+            for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+                for (int j = 0; j < 16; ++j) v[mt][j] = 0.f;
+            // fixed slot order -> deterministic; four contributors' loads in flight at a time
+            constexpr int UB = (MT >= 4) ? 1 : (MT == 2 ? 2 : 4);
+            for (int s0 = 0; s0 < ncontrib; s0 += UB) {
+                float4 pv[UB][MT][4];
+#pragma unroll
+                for (int u = 0; u < UB; ++u) {
+                    const float* w_ = ws0 + (size_t)(s0 + u) * (GEMM_BN * ROWF);
+#pragma unroll
+                    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+                        for (int j = 0; j < 4; ++j)
+                            pv[u][mt][j] = (s0 + u < ncontrib) ? __ldcg(reinterpret_cast<const float4*>(w_ + mt * 16 + 4 * j))
+                                                               : make_float4(0.f, 0.f, 0.f, 0.f);
+                }
+#pragma unroll
+                for (int u = 0; u < UB; ++u)
+#pragma unroll
+                    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {
+                            v[mt][4 * j] += pv[u][mt][j].x; v[mt][4 * j + 1] += pv[u][mt][j].y;
+                            v[mt][4 * j + 2] += pv[u][mt][j].z; v[mt][4 * j + 3] += pv[u][mt][j].w;
+                        }
+            }
+        }
+    }
+    if (do_epilogue) {
+        // The segment descriptor lives in kernel-parameter space (stand-alone kernel) or global
+        // memory (whole-step kernel): hoist every field the loop needs into registers once.
+        const int n = w.tile_local * GEMM_BN + tid;
+        const int segN = sg.N, out_mode = sg.out_mode, act = sg.act, ldo = sg.ldo, grp = sg.grp, grp_stride = sg.grp_stride;
+        const int ld_aux = sg.ld_aux;
+        void* const outp = sg.out;
+        const float* const biasp = sg.bias;
+        const float* const aux0 = sg.aux0;
+        const float* const aux1 = sg.aux1;
+        const float* const aux2 = sg.aux2;
+        if (SPLIT) {
+            static_assert(!SPLIT || MT == 2, "split operands use two token tiles");
+#pragma unroll
+            for (int j = 0; j < 16; ++j) v[0][j] += v[MT - 1][j];
+        }
+        constexpr int MTE = SPLIT ? 1 : MT;        // token tiles the epilogue writes
+        const bool row_ok = n < segN;
+        const float bias = (row_ok && biasp) ? biasp[n] : 0.f;
+        const int mmax = min(nrows, MTE * 16);
+        if (out_mode == OUT_F32) {
+            if (row_ok) {
+                float* o = reinterpret_cast<float*>(outp) + n;
+                if (MTE == 1) {         // decode shape: straight from registers, all 16 stores in flight
+#pragma unroll
+                    for (int m = 0; m < 16; ++m)
+                        if (m < mmax) o[(size_t)m * ldo] = apply_act(v[0][m] + bias, act);
+                } else {
+                    // Multi-tile steps: unrolled over tiles and tokens with compile-time register indices (a dynamically
+                    // indexed copy of the accumulator would live in local memory, and next to a 200 KB ring there is no
+                    // L1 to hold it); the activation is a compile-time parameter of the unrolled body, otherwise the
+                    // run-time switch is replicated 16 MT times and the epilogue outgrows the instruction cache.
+                    auto body = [&](auto act_c) {
+                        constexpr int ACT_C = decltype(act_c)::value;
+#pragma unroll
+                        for (int mt = 0; mt < MTE; ++mt)
+#pragma unroll
+                            for (int j = 0; j < 16; ++j) {
+                                const int m = mt * 16 + j;
+                                if (m < mmax) o[(size_t)m * ldo] = apply_act(v[mt][j] + bias, ACT_C);
+                            }
+                    };
+                    switch (act) {
+                        case ACT_TANH: body(std::integral_constant<int, ACT_TANH>{}); break;
+                        case ACT_SIGMOID: body(std::integral_constant<int, ACT_SIGMOID>{}); break;
+                        case ACT_SILU: body(std::integral_constant<int, ACT_SILU>{}); break;
+                        case ACT_RELU2: body(std::integral_constant<int, ACT_RELU2>{}); break;
+                        case ACT_EXPNEGEXP: body(std::integral_constant<int, ACT_EXPNEGEXP>{}); break;
+                        case ACT_V7DECAY: body(std::integral_constant<int, ACT_V7DECAY>{}); break;
+                        default: body(std::integral_constant<int, ACT_NONE>{}); break;
+                    }
+                }
+            }
+        } else {
+            // A16 outputs (operand of a following projection).  Thread t holds output row n = one k index of that operand
+            // for 16 tokens; the layout wants, per token, 8 consecutive k in one 16-byte chunk.  Written straight from the
+            // registers that is one 2-byte store per token and row, four 32-byte sectors per warp instruction -- measured
+            // 33 us per 128-token tile (r02_findings.md §8).  So the tile is transposed through 6 KB of shared memory:
+            // every thread stages its 16 tokens, then writes two (token, chunk) pairs as 16-byte stores, 16 lanes = 256
+            // contiguous bytes.  All 128 epilogue threads take part (rows past the segment stage zeros).
+            const bool lerp = (out_mode == OUT_LERP_A16);
+            const float mu = (lerp && row_ok) ? aux2[n] : 0.f;
+            __half* const base0 = reinterpret_cast<__half*>(outp);
+            const int row0 = w.tile_local * GEMM_BN;         // first output row of this tile within the segment
+            auto stage_and_store = [&](const int mt, const __half (&h)[16], const int rowoff) {
+                uint4 p0, p1;
+                p0.x = (uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16);
+                p0.y = (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16);
+                p0.z = (uint32_t)__half_as_ushort(h[4]) | ((uint32_t)__half_as_ushort(h[5]) << 16);
+                p0.w = (uint32_t)__half_as_ushort(h[6]) | ((uint32_t)__half_as_ushort(h[7]) << 16);
+                p1.x = (uint32_t)__half_as_ushort(h[8]) | ((uint32_t)__half_as_ushort(h[9]) << 16);
+                p1.y = (uint32_t)__half_as_ushort(h[10]) | ((uint32_t)__half_as_ushort(h[11]) << 16);
+                p1.z = (uint32_t)__half_as_ushort(h[12]) | ((uint32_t)__half_as_ushort(h[13]) << 16);
+                p1.w = (uint32_t)__half_as_ushort(h[14]) | ((uint32_t)__half_as_ushort(h[15]) << 16);
+                *reinterpret_cast<uint4*>(s_stage + tid * GEMM_STAGE_PITCH) = p0;
+                *reinterpret_cast<uint4*>(s_stage + tid * GEMM_STAGE_PITCH + 8) = p1;
+                named_bar_sync(3, GEMM_EPI_THREADS);
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int q = tid + GEMM_EPI_THREADS * i;
+                    const int c = q >> 4, m = q & 15;               // chunk of 8 rows, token of the tile
+                    const int nc = row0 + c * 8;                    // first output row of the chunk (N % 8 == 0: whole chunks)
+                    if (nc < segN && mt * 16 + m < mmax) {
+                        const __half* src = s_stage + (c * 8) * GEMM_STAGE_PITCH + m;
+                        uint4 o;
+                        o.x = (uint32_t)__half_as_ushort(src[0]) | ((uint32_t)__half_as_ushort(src[GEMM_STAGE_PITCH]) << 16);
+                        o.y = (uint32_t)__half_as_ushort(src[2 * GEMM_STAGE_PITCH]) | ((uint32_t)__half_as_ushort(src[3 * GEMM_STAGE_PITCH]) << 16);
+                        o.z = (uint32_t)__half_as_ushort(src[4 * GEMM_STAGE_PITCH]) | ((uint32_t)__half_as_ushort(src[5 * GEMM_STAGE_PITCH]) << 16);
+                        o.w = (uint32_t)__half_as_ushort(src[6 * GEMM_STAGE_PITCH]) | ((uint32_t)__half_as_ushort(src[7 * GEMM_STAGE_PITCH]) << 16);
+                        __half* base = base0;
+                        int nn = nc;
+                        if (grp > 0) {
+                            const int gi = nc / grp;
+                            base += (size_t)gi * grp_stride;
+                            nn = nc - gi * grp;
+                        }
+                        *reinterpret_cast<uint4*>(base + a16_index(mt * 16 + m + rowoff, nn, ldo)) = o;
+                    }
+                }
+                named_bar_sync(3, GEMM_EPI_THREADS);            // the staging buffer is rewritten by the next tile
+            };
+            auto body = [&](auto act_c) {
+                constexpr int ACT_C = decltype(act_c)::value;
+#pragma unroll
+                for (int mt = 0; mt < MTE; ++mt) {
+                    if (mt * 16 < mmax) {                           // uniform over the CTA
+                        float x0[16], x1[16];                       // the lerp operands of the tile's 16 tokens, requested together
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) {
+                            const int m = mt * 16 + j;
+                            const bool ok = lerp && row_ok && m < mmax;
+                            const size_t a_ = (size_t)m * ld_aux + n;
+                            x0[j] = ok ? aux0[a_] : 0.f;
+                            x1[j] = ok ? aux1[a_] : 0.f;
+                        }
+                        __half hi[16], lo[16];
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) {
+                            float y = apply_act(v[mt][j] + bias, ACT_C);
+                            if (lerp) y = x0[j] + x1[j] * (mu + y);
+                            if (!row_ok) y = 0.f;
+                            if (SPLIT) split_h(y, hi[j], lo[j]);
+                            else hi[j] = f2h_sat(y);
+                        }
+                        stage_and_store(mt, hi, 0);
+                        if (SPLIT) stage_and_store(mt, lo, 16);
+                    }
+                }
+            };
+            switch (act) {
+                case ACT_TANH: body(std::integral_constant<int, ACT_TANH>{}); break;
+                case ACT_SIGMOID: body(std::integral_constant<int, ACT_SIGMOID>{}); break;
+                case ACT_SILU: body(std::integral_constant<int, ACT_SILU>{}); break;
+                case ACT_RELU2: body(std::integral_constant<int, ACT_RELU2>{}); break;
+                case ACT_EXPNEGEXP: body(std::integral_constant<int, ACT_EXPNEGEXP>{}); break;
+                case ACT_V7DECAY: body(std::integral_constant<int, ACT_V7DECAY>{}); break;
+                default: body(std::integral_constant<int, ACT_NONE>{}); break;
+            }
+        }
+    }
+}
+
+template <int MT, int NSTAGE, int STAGE_BYTES, bool SPLIT>
+__device__ __forceinline__ void gemm_consumer_role(const GemmParams& p, const int cta, const int G, const int b0, const int b1,
+                                                   const uint32_t smem_base, const uint32_t full_bar, const uint32_t empty_bar,
+                                                   const int nrows, volatile int* s_last_p, float* s_x, unsigned long long* tr) {
+    const int lane = threadIdx.x & 31;
     const uint32_t w_lbo = p.w_lbo, w_sbo = p.w_sbo, a_sbo = p.a_sbo;
     constexpr uint32_t a_lbo = 16 * MT * 16;          // bytes between the k8 chunks of the token operand: 16 MT rows x 16 B
+    RingPos rp{0, 0u};
     SegWalk w;
     w.init(p, b0, b1);
     while (!w.done()) {
         const int nblk = w.nblk();
-        const unsigned acc = segcount & 1u, use = segcount >> 1;
-        if (use > 0) mbar_wait(tempty_bar + acc * 8, (use - 1) & 1u, 11);     // epilogue drained this buffer
-        tc_fence_after();
-        const uint32_t d0 = tmem_base + acc * (16 * MT);
+        float acc[2][8 * MT];                          // weight rows 0-63 and 64-127 of the tile
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < 8 * MT; ++i) acc[h][i] = 0.f;
+        int prev = -1;
         for (int i = 0; i < nblk; ++i) {
             mbar_wait(full_bar + rp.stage * 8, rp.phase, 12);
-            tc_fence_after();
+            if (tr && threadIdx.x == 0 && i == 0 && rp.stage == 0 && rp.phase == 0) tr[3] = globaltimer_ns();
             const uint32_t st = smem_base + rp.stage * STAGE_BYTES;
-            // one MMA per k16 step over all 16 x MT token rows of the stage (N = 16 MT): the token operand of a stage is one
-            // canonical tile [k8 chunk][16 MT rows][16 B] (common.cuh), chunk stride = 16 MT x 16 bytes
+            wgmma_fence_operand(acc[0]);
+            wgmma_fence_operand(acc[1]);
+            wgmma_fence();
+            // one MMA per k16 step and weight half over all 16 x MT token rows of the stage (N = 16 MT): the token operand
+            // of a stage is one canonical tile [k8 chunk][16 MT rows][16 B] (common.cuh), chunk stride = 16 MT x 16 bytes
 #pragma unroll
             for (int k16 = 0; k16 < GEMM_BK / 16; ++k16) {
-                const uint64_t adesc = umma_desc(st + k16 * 2 * w_lbo, w_lbo, w_sbo);
-                const uint64_t bdesc = umma_desc(st + GEMM_WBYTES + k16 * 2 * a_lbo, a_lbo, a_sbo);
-                tc_mma_f16(d0, adesc, bdesc, IDESC, (i > 0 || k16 > 0) ? 1u : 0u);
+                const uint64_t bdesc = gmma_desc(st + GEMM_WBYTES + k16 * 2 * a_lbo, a_lbo, a_sbo);
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    wgmma_f16<16 * MT>(acc[h], gmma_desc(st + h * 8 * w_sbo + k16 * 2 * w_lbo, w_lbo, w_sbo), bdesc);
             }
-            tc_commit(empty_bar + rp.stage * 8);          // slot is free once these MMAs have read it
+            wgmma_commit();
+            wgmma_wait<1>();                           // the previous stage's MMAs have retired: its slot may be refilled
+            if (prev >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty_bar + prev * 8);
+            }
+            prev = rp.stage;
             rp.advance<NSTAGE>(1);
         }
-        tc_commit(tfull_bar + acc * 8);                   // accumulator complete -> epilogue
-        ++segcount;
-        w.next();
-    }
-}
-
-// ---------------------------------------------------------------------------------------
-// Epilogue role (4 warps = 128 threads, thread t owns output row t of the tile): drain TMEM,
-// deterministic cross-CTA reduction of split tiles, fused epilogue.
-// ---------------------------------------------------------------------------------------
-// SPLIT (precision 1, MT = 2): the two token tiles are the hi and lo halves of the SAME 16 tokens
-// (common.cuh split_h): the accumulator tiles are added before the epilogue and A16 outputs are written as hi / lo again.
-template <int MT, bool SPLIT = false>
-__device__ __forceinline__ void gemm_epilogue_role(const GemmParams& p, const int cta, const int G, const int b0, const int b1,
-                                                   const uint32_t tfull_bar, const uint32_t tempty_bar, const uint32_t tmem_base,
-                                                   unsigned& segcount, const int nrows, volatile int* s_last_p, __half* s_stage,
-                                                   unsigned long long* tr = nullptr) {
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const unsigned TB = (unsigned)p.total_blocks;
-    auto stamp = [&](int i) {
-        if (tr && tid == 0) {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-            tr[i] = t;
-        }
-    };
-    SegWalk w;
-    w.init(p, b0, b1);
-    while (!w.done()) {
-        const GemmSeg& sg = p.seg[w.seg];
-        const unsigned acc = segcount & 1u, use = segcount >> 1;
-        constexpr int ROWF = 16 * MT;
-        mbar_wait(tfull_bar + acc * 8, use & 1u, 13);
-        stamp(8);
-        tc_fence_after();
-        float v[MT][16];
-#pragma unroll
-        for (int mt = 0; mt < MT; ++mt) tc_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + acc * (16 * MT) + mt * 16, v[mt]);
-        tc_fence_before();
+        wgmma_wait<0>();
+        wgmma_fence_operand(acc[0]);
+        wgmma_fence_operand(acc[1]);
         __syncwarp();
-        if (lane == 0) mbar_arrive(tempty_bar + acc * 8);     // TMEM buffer may be overwritten
-        ++segcount;
-        stamp(9);
-
-        const unsigned tb0 = (unsigned)(sg.blk_begin + w.tile_local * sg.KB);
-        const int c_first = (int)(((unsigned long long)(tb0 + 1) * (unsigned)G - 1) / TB);
-        const int c_last = (int)(((unsigned long long)(tb0 + sg.KB) * (unsigned)G - 1) / TB);
-        const int ncontrib = c_last - c_first + 1;
-        const int gtile = sg.tile_begin + w.tile_local;
-        bool do_epilogue = true;
-        if (ncontrib > 1) {
-            float* wsl = p.ws + ((size_t)gtile * p.max_contrib + (cta - c_first)) * (GEMM_BN * ROWF) + (size_t)tid * ROWF;
-#pragma unroll
-            for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-                for (int j = 0; j < 16; j += 4)
-                    *reinterpret_cast<float4*>(wsl + mt * 16 + j) = make_float4(v[mt][j], v[mt][j + 1], v[mt][j + 2], v[mt][j + 3]);
-            // publish: the barrier orders every thread's partial stores before thread 0's gpu-scope
-            // fence (fences are cumulative), then one counter bump per CTA
-            named_bar_sync(3, GEMM_EPI_THREADS);
-            if (tid == 0) {
-                const unsigned old = atom_add_acq_rel_gpu(p.counters + gtile, 1u);   // release ours, acquire the others'
-                *s_last_p = (old == (unsigned)(ncontrib - 1));
-                if (*s_last_p) p.counters[gtile] = 0;  // ready for the next launch
-            }
-            named_bar_sync(3, GEMM_EPI_THREADS);
-            do_epilogue = (*s_last_p != 0);
-            if (do_epilogue) {
-                const float* ws0 = p.ws + (size_t)gtile * p.max_contrib * (GEMM_BN * ROWF) + (size_t)tid * ROWF;
-#pragma unroll
-                for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) v[mt][j] = 0.f;
-                // fixed slot order -> deterministic; four contributors' loads in flight at a time
-                constexpr int UB = (MT >= 4) ? 1 : (MT == 2 ? 2 : 4);
-                for (int s0 = 0; s0 < ncontrib; s0 += UB) {
-                    float4 pv[UB][MT][4];
-#pragma unroll
-                    for (int u = 0; u < UB; ++u) {
-                        const float* w_ = ws0 + (size_t)(s0 + u) * (GEMM_BN * ROWF);
-#pragma unroll
-                        for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-                            for (int j = 0; j < 4; ++j)
-                                pv[u][mt][j] = (s0 + u < ncontrib) ? __ldcg(reinterpret_cast<const float4*>(w_ + mt * 16 + 4 * j))
-                                                                   : make_float4(0.f, 0.f, 0.f, 0.f);
-                    }
-#pragma unroll
-                    for (int u = 0; u < UB; ++u)
-#pragma unroll
-                        for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                v[mt][4 * j] += pv[u][mt][j].x; v[mt][4 * j + 1] += pv[u][mt][j].y;
-                                v[mt][4 * j + 2] += pv[u][mt][j].z; v[mt][4 * j + 3] += pv[u][mt][j].w;
-                            }
-                }
-            }
-        }
-        if (do_epilogue) {
-            // The segment descriptor lives in kernel-parameter space (stand-alone kernel) or global
-            // memory (whole-step kernel): hoist every field the loop needs into registers once.
-            const int n = w.tile_local * GEMM_BN + tid;
-            const int segN = sg.N, out_mode = sg.out_mode, act = sg.act, ldo = sg.ldo, grp = sg.grp, grp_stride = sg.grp_stride;
-            const int ld_aux = sg.ld_aux;
-            void* const outp = sg.out;
-            const float* const biasp = sg.bias;
-            const float* const aux0 = sg.aux0;
-            const float* const aux1 = sg.aux1;
-            const float* const aux2 = sg.aux2;
-            if (SPLIT) {
-                static_assert(!SPLIT || MT == 2, "split operands use two token tiles");
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[0][j] += v[MT - 1][j];
-            }
-            constexpr int MTE = SPLIT ? 1 : MT;        // token tiles the epilogue writes
-            const bool row_ok = n < segN;
-            const float bias = (row_ok && biasp) ? biasp[n] : 0.f;
-            const int mmax = min(nrows, MTE * 16);
-            if (out_mode == OUT_F32) {
-                if (row_ok) {
-                    float* o = reinterpret_cast<float*>(outp) + n;
-                    if (MTE == 1) {         // decode shape: straight from registers, all 16 stores in flight
-#pragma unroll
-                        for (int m = 0; m < 16; ++m)
-                            if (m < mmax) o[(size_t)m * ldo] = apply_act(v[0][m] + bias, act);
-                    } else {
-                        // Multi-tile steps: unrolled over tiles and tokens with compile-time register indices (a dynamically
-                        // indexed copy of the accumulator would live in local memory, and next to a 200 KB ring there is no
-                        // L1 to hold it); the activation is a compile-time parameter of the unrolled body, otherwise the
-                        // run-time switch is replicated 16 MT times and the epilogue outgrows the instruction cache.
-                        auto body = [&](auto act_c) {
-                            constexpr int ACT_C = decltype(act_c)::value;
-#pragma unroll
-                            for (int mt = 0; mt < MTE; ++mt)
-#pragma unroll
-                                for (int j = 0; j < 16; ++j) {
-                                    const int m = mt * 16 + j;
-                                    if (m < mmax) o[(size_t)m * ldo] = apply_act(v[mt][j] + bias, ACT_C);
-                                }
-                        };
-                        switch (act) {
-                            case ACT_TANH: body(std::integral_constant<int, ACT_TANH>{}); break;
-                            case ACT_SIGMOID: body(std::integral_constant<int, ACT_SIGMOID>{}); break;
-                            case ACT_SILU: body(std::integral_constant<int, ACT_SILU>{}); break;
-                            case ACT_RELU2: body(std::integral_constant<int, ACT_RELU2>{}); break;
-                            case ACT_EXPNEGEXP: body(std::integral_constant<int, ACT_EXPNEGEXP>{}); break;
-                            case ACT_V7DECAY: body(std::integral_constant<int, ACT_V7DECAY>{}); break;
-                            default: body(std::integral_constant<int, ACT_NONE>{}); break;
-                        }
-                    }
-                }
-            } else {
-                // A16 outputs (operand of a following projection).  Thread t holds output row n = one k index of that operand
-                // for 16 tokens; the layout wants, per token, 8 consecutive k in one 16-byte chunk.  Written straight from the
-                // registers that is one 2-byte store per token and row, four 32-byte sectors per warp instruction -- measured
-                // 33 us per 128-token tile (r02_findings.md §8).  So the tile is transposed through 6 KB of shared memory:
-                // every thread stages its 16 tokens, then writes two (token, chunk) pairs as 16-byte stores, 16 lanes = 256
-                // contiguous bytes.  All 128 epilogue threads take part (rows past the segment stage zeros).
-                const bool lerp = (out_mode == OUT_LERP_A16);
-                const float mu = (lerp && row_ok) ? aux2[n] : 0.f;
-                __half* const base0 = reinterpret_cast<__half*>(outp);
-                const int row0 = w.tile_local * GEMM_BN;         // first output row of this tile within the segment
-                auto stage_and_store = [&](const int mt, const __half (&h)[16], const int rowoff) {
-                    uint4 p0, p1;
-                    p0.x = (uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16);
-                    p0.y = (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16);
-                    p0.z = (uint32_t)__half_as_ushort(h[4]) | ((uint32_t)__half_as_ushort(h[5]) << 16);
-                    p0.w = (uint32_t)__half_as_ushort(h[6]) | ((uint32_t)__half_as_ushort(h[7]) << 16);
-                    p1.x = (uint32_t)__half_as_ushort(h[8]) | ((uint32_t)__half_as_ushort(h[9]) << 16);
-                    p1.y = (uint32_t)__half_as_ushort(h[10]) | ((uint32_t)__half_as_ushort(h[11]) << 16);
-                    p1.z = (uint32_t)__half_as_ushort(h[12]) | ((uint32_t)__half_as_ushort(h[13]) << 16);
-                    p1.w = (uint32_t)__half_as_ushort(h[14]) | ((uint32_t)__half_as_ushort(h[15]) << 16);
-                    *reinterpret_cast<uint4*>(s_stage + tid * GEMM_STAGE_PITCH) = p0;
-                    *reinterpret_cast<uint4*>(s_stage + tid * GEMM_STAGE_PITCH + 8) = p1;
-                    named_bar_sync(3, GEMM_EPI_THREADS);
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        const int q = tid + GEMM_EPI_THREADS * i;
-                        const int c = q >> 4, m = q & 15;               // chunk of 8 rows, token of the tile
-                        const int nc = row0 + c * 8;                    // first output row of the chunk (N % 8 == 0: whole chunks)
-                        if (nc < segN && mt * 16 + m < mmax) {
-                            const __half* src = s_stage + (c * 8) * GEMM_STAGE_PITCH + m;
-                            uint4 o;
-                            o.x = (uint32_t)__half_as_ushort(src[0]) | ((uint32_t)__half_as_ushort(src[GEMM_STAGE_PITCH]) << 16);
-                            o.y = (uint32_t)__half_as_ushort(src[2 * GEMM_STAGE_PITCH]) | ((uint32_t)__half_as_ushort(src[3 * GEMM_STAGE_PITCH]) << 16);
-                            o.z = (uint32_t)__half_as_ushort(src[4 * GEMM_STAGE_PITCH]) | ((uint32_t)__half_as_ushort(src[5 * GEMM_STAGE_PITCH]) << 16);
-                            o.w = (uint32_t)__half_as_ushort(src[6 * GEMM_STAGE_PITCH]) | ((uint32_t)__half_as_ushort(src[7 * GEMM_STAGE_PITCH]) << 16);
-                            __half* base = base0;
-                            int nn = nc;
-                            if (grp > 0) {
-                                const int gi = nc / grp;
-                                base += (size_t)gi * grp_stride;
-                                nn = nc - gi * grp;
-                            }
-                            *reinterpret_cast<uint4*>(base + a16_index(mt * 16 + m + rowoff, nn, ldo)) = o;
-                        }
-                    }
-                    named_bar_sync(3, GEMM_EPI_THREADS);            // the staging buffer is rewritten by the next tile
-                };
-                auto body = [&](auto act_c) {
-                    constexpr int ACT_C = decltype(act_c)::value;
-#pragma unroll
-                    for (int mt = 0; mt < MTE; ++mt) {
-                        if (mt * 16 < mmax) {                           // uniform over the CTA
-                            float x0[16], x1[16];                       // the lerp operands of the tile's 16 tokens, requested together
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) {
-                                const int m = mt * 16 + j;
-                                const bool ok = lerp && row_ok && m < mmax;
-                                const size_t a_ = (size_t)m * ld_aux + n;
-                                x0[j] = ok ? aux0[a_] : 0.f;
-                                x1[j] = ok ? aux1[a_] : 0.f;
-                            }
-                            __half hi[16], lo[16];
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) {
-                                float y = apply_act(v[mt][j] + bias, ACT_C);
-                                if (lerp) y = x0[j] + x1[j] * (mu + y);
-                                if (!row_ok) y = 0.f;
-                                if (SPLIT) split_h(y, hi[j], lo[j]);
-                                else hi[j] = f2h_sat(y);
-                            }
-                            stage_and_store(mt, hi, 0);
-                            if (SPLIT) stage_and_store(mt, lo, 16);
-                        }
-                    }
-                };
-                switch (act) {
-                    case ACT_TANH: body(std::integral_constant<int, ACT_TANH>{}); break;
-                    case ACT_SIGMOID: body(std::integral_constant<int, ACT_SIGMOID>{}); break;
-                    case ACT_SILU: body(std::integral_constant<int, ACT_SILU>{}); break;
-                    case ACT_RELU2: body(std::integral_constant<int, ACT_RELU2>{}); break;
-                    case ACT_EXPNEGEXP: body(std::integral_constant<int, ACT_EXPNEGEXP>{}); break;
-                    case ACT_V7DECAY: body(std::integral_constant<int, ACT_V7DECAY>{}); break;
-                    default: body(std::integral_constant<int, ACT_NONE>{}); break;
-                }
-            }
-        }
+        if (lane == 0) mbar_arrive(empty_bar + prev * 8);
+        float v[MT][16];
+        gemm_acc_to_rows<MT>(acc, v, s_x);
+        gemm_epilogue_tile<MT, SPLIT>(p, w, cta, G, v, nrows, s_last_p, reinterpret_cast<__half*>(s_x));
         w.next();
     }
+    if (tr && threadIdx.x == 0) tr[4] = globaltimer_ns();
 }
 
 // ---------------------------------------------------------------------------------------
-// stand-alone kernel: warps 0-3 epilogue, warp 4 MMA issuer (+ TMEM allocation), warp 5 TMA producer
+// stand-alone kernel: warps 0-3 consumer warpgroup (MMA + epilogue), warp 4 TMA producer
 // ---------------------------------------------------------------------------------------
 template <int MT, int RING = 0, bool SPLIT = false>
 __global__ void __launch_bounds__(GEMM_THREADS, RING == 1 ? 2 : 1) gemm_kernel(const __grid_constant__ GemmParams p) {
     using Cfg = GemmCfg<MT, RING>;
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ int s_last;
-    __shared__ __align__(16) __half s_stage[GEMM_EPI_THREADS * GEMM_STAGE_PITCH];     // A16 epilogue transpose (6 KB)
+    __shared__ __align__(16) float s_x[GEMM_XPOSE_FLOATS];     // accumulator transpose, then A16 epilogue staging
+    static_assert(GEMM_EPI_THREADS * GEMM_STAGE_PITCH * 2 <= GEMM_XPOSE_FLOATS * 4, "A16 staging fits the transpose buffer");
     const uint32_t smem_base = smem_u32(smem);
     const uint32_t full_bar = smem_base + Cfg::NSTAGE * Cfg::STAGE_BYTES;
     const uint32_t empty_bar = full_bar + Cfg::NSTAGE * 8;
-    const uint32_t tfull_bar = empty_bar + Cfg::NSTAGE * 8;
-    const uint32_t tempty_bar = tfull_bar + 2 * 8;
-    const uint32_t tmem_slot = tempty_bar + 2 * 8;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const long long TB = p.total_blocks;
@@ -468,23 +492,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, RING == 1 ? 2 : 1) gemm_kernel(c
         stamp(0);
         for (int s = 0; s < Cfg::NSTAGE; ++s) {
             mbar_init(full_bar + s * 8, 1);
-            mbar_init(empty_bar + s * 8, 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(tfull_bar + s * 8, 1);
-            mbar_init(tempty_bar + s * 8, GEMM_EPI_WARPS);
+            mbar_init(empty_bar + s * 8, GEMM_EPI_WARPS);
         }
         mbar_fence_init();
     }
-    if (warp == GEMM_EPI_WARPS) tc_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem + (tmem_slot - smem_base));
     if (tid == 0) stamp(1);
     pdl_launch_dependents();     // let the next kernel's CTAs queue up and prefetch their weights
 
-    if (warp == GEMM_EPI_WARPS + 1) {
+    if (warp == GEMM_EPI_WARPS) {
         // ===================== producer: one lane streams stage blocks =====================
         if (lane == 0) {
             const uint64_t pol_w = l2_policy_evict_first();
@@ -532,39 +548,27 @@ __global__ void __launch_bounds__(GEMM_THREADS, RING == 1 ? 2 : 1) gemm_kernel(c
                 for (int i = 0; i < np; ++i) bulk_prefetch_l2(p.next_W + (size_t)(n0 + i) * GEMM_WBYTES, GEMM_WBYTES);
             }
         }
-    } else if (warp == GEMM_EPI_WARPS) {
-        // ===================== MMA issuer: one lane =====================
-        if (lane == 0) {
-            RingPos rp{0, 0u};
-            unsigned segcount = 0;
-            if (tr) { mbar_wait(full_bar, 0); stamp(3); }
-            gemm_mma_role<MT, Cfg::NSTAGE, Cfg::STAGE_BYTES>(p, b0, b1, smem_base, full_bar, empty_bar, tfull_bar, tempty_bar,
-                                                             tmem_base, rp, segcount);
-            stamp(4);
-            if (p.trace) {       // every CTA: SM id and the time its last MMA was issued (skew across the grid)
-                unsigned smid;
-                asm volatile("mov.u32 %0, %smid;" : "=r"(smid));
-                p.trace[8 + 3 * cta] = smid;
-                p.trace[8 + 3 * cta + 1] = globaltimer_ns();
-            }
-        }
     } else {
-        // ===================== epilogue: 4 warps =====================
+        // ===================== consumer warpgroup: MMA + epilogue =====================
         pdl_wait();
         if (tid == 0) stamp(5);
-        unsigned segcount = 0;
-        gemm_epilogue_role<MT, SPLIT>(p, cta, G, b0, b1, tfull_bar, tempty_bar, tmem_base, segcount, *p.nrows, &s_last, s_stage, tr);
+        gemm_consumer_role<MT, Cfg::NSTAGE, Cfg::STAGE_BYTES, SPLIT>(p, cta, G, b0, b1, smem_base, full_bar, empty_bar, *p.nrows, &s_last,
+                                                                     s_x, tr);
         if (tid == 0) stamp(6);
+        if (tid == 0 && p.trace) {       // every CTA: SM id and the time its MMAs were done (skew across the grid)
+            unsigned smid;
+            asm volatile("mov.u32 %0, %smid;" : "=r"(smid));
+            p.trace[8 + 3 * cta] = smid;
+            p.trace[8 + 3 * cta + 1] = globaltimer_ns();
+        }
     }
-    tc_fence_before();
     __syncthreads();
     if (tid == 0) stamp(7);
     if (tid == 0 && p.trace) p.trace[8 + 3 * cta + 2] = globaltimer_ns();
-    if (warp == GEMM_EPI_WARPS) tc_dealloc(tmem_base, Cfg::TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------------------
-// One-time weight re-tiling:  W[N, K] row-major f16  ->  stage blocks in the UMMA canonical
+// One-time weight re-tiling:  W[N, K] row-major f16  ->  stage blocks in the canonical
 // K-major / no-swizzle layout:  block(tile, kb) = [k8 chunk 16][row group 16][row 8][8 halves], zero padded.
 // Supports a row-parallel / column-parallel shard: source sub-matrix rows [n0, n0+N), cols [k0, k0+K)
 // of a matrix with row stride ld.

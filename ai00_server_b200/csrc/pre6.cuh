@@ -3,9 +3,8 @@
 // Replaces, on the path `Runtime::infer` (reference run.rs:1143; SURVEY.md §2.2 K1-K3, App. A), web-rwkv's
 // `layer_norm` + `token_shift` (+ for RWKV-6 the two LoRA matmuls of the data-dependent token shift) dispatches.
 //
-// Why: measured on B200 (profiles/r01_findings.md §3) the per-op chain spends 10 us in the one-CTA-per-token LN launch and
-// 15.5 + 19 us in the two 2.6 MB LoRA GEMM launches of every RWKV-6 layer -- 45 us in which HBM idles, against 66 us of
-// weight streaming per layer.  Nothing here is bandwidth: it is a chain of L2 round trips, so the shape is chosen for
+// Why: as separate launches, the one-CTA-per-token LN launch and the two 2.6 MB LoRA GEMM launches of every RWKV-6 layer
+// are time in which HBM idles, comparable to the layer's weight streaming.  Nothing here is bandwidth: it is a chain of L2 round trips, so the shape is chosen for
 // the shortest chain:
 //   phase 1  cluster g = token g, CTA rank s = channel slice s (C/8 channels, one float4 per thread): residual update, LN
 //            statistics through distributed shared memory (two cluster syncs), token shift, static mixes.
@@ -16,8 +15,8 @@
 //   -- grid barrier --
 //   phase 3  CTA b = channels [32 b, 32 b + 32) x 5 mixes: W2 fragments (also preloaded), y = xx + sx * (mu + W2 tanh),
 //            written as the A16 operands of the R/K/V/G/decay projections.
-// The tensor cores are used through legacy mma.sync on purpose: each CTA issues a few dozen MMAs, and tcgen05 would add
-// TMEM allocation plus shared-memory operand staging to a chain that is pure latency.
+// The tensor cores are used through legacy mma.sync on purpose: each CTA issues a few dozen MMAs, and wgmma would add
+// warpgroup-wide issue plus shared-memory operand staging to a chain that is pure latency.
 // The kernel keeps < 16 KB of shared memory so the next projection's CTAs (200 KB ring, launched early through PDL) can
 // sit on the same SMs and fill their rings while these phases run.
 #pragma once

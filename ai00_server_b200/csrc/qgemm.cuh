@@ -6,19 +6,14 @@
 // consecutive input elements with (min, max) in f16 and round(255 (w - min) / (max - min)) per element; NF4 = blocks of 64
 // with absmax in f16 and the index of the nearest NormalFloat4 level per element.
 //
-// The projection stays the HBM-bound stream of gemm.cuh -- same stream-K split, same TMEM accumulator, same epilogue role --
-// but a stage block is 16.5 KB (Int8) or 8.5 KB (NF4) of HBM traffic instead of 32 KB.  tcgen05.mma has no operand format for
-// affine u8 or table-coded 4-bit weights, so four more warps sit between the TMA ring and the MMA issuer: thread r owns
-// weight row r of the stage, reads its codes (16-byte LDS) and expands them to f16 with two-wide arithmetic.  Where the
-// expanded rows go decides the speed (measured, profiles/r02_quant_probe.log):
-//   TS = false: into one of two 32 KB shared-memory buffers in the UMMA canonical layout, `fence.proxy.async`, mbarrier arrive.
-//       The proxy fence alone stalls the warp ~600 cycles per block and the tensor core re-reads the 32 KB from shared
-//       memory: ~1.0 us per block, no faster than streaming f16.  Kept as the reference variant.
-//   TS = true (production): straight from registers into TENSOR MEMORY with tcgen05.st -- thread r = TMEM lane r, a 128-wide k
-//       block = 64 columns of two f16 -- and the MMA takes its A operand from TMEM (`tcgen05.mma [d], [a_tmem], b_desc`): no
-//       shared-memory round trip, no proxy fence (tcgen05.wait::st + tcgen05.fence), three 64-column A buffers beside the
-//       accumulator.
-// tcgen05.commit hands a buffer back.  Raw blocks are pre-tiled at load so that every shared-memory access of the expansion is a
+// The projection stays the HBM-bound stream of gemm.cuh -- same stream-K split, same consumer warpgroup and epilogue --
+// but a stage block is 16.5 KB (Int8) or 8.5 KB (NF4) of HBM traffic instead of 32 KB.  wgmma has no operand format for
+// affine u8 or table-coded 4-bit weights, so four expansion warps sit between the TMA ring and the consumer warpgroup:
+// thread r owns weight row r of the stage, reads its codes (16-byte LDS), expands them to f16 with two-wide arithmetic and
+// writes the row into one of two 32 KB shared-memory buffers in the canonical K-major layout of gemm.cuh; after
+// `fence.proxy.async` (generic-proxy stores -> visible to the tensor core's async-proxy reads) an mbarrier arrival hands the
+// buffer to the consumer, whose MMAs read it exactly like an f16 weight stage, and the consumer hands it back once those
+// MMAs have retired.  Raw blocks are pre-tiled at load so that every shared-memory access of the expansion is a
 // conflict-free 16-byte access:
 //   Int8 block (128 rows x 128 k): [k16 chunk 8][row 128][16 codes] | [row 128]{f16 scale, f16 min}
 //   NF4  block (128 rows x 128 k): [k32 group 4][row 128][16 B = 32 codes, element i of a u32 in bits 4i..4i+3] | [row 128]{f16 absmax k<64, f16 absmax k>=64}
@@ -35,12 +30,10 @@ enum QuantType : int { QT_NONE = 0, QT_INT8 = 1, QT_NF4 = 2 };
 constexpr int Q_PARAM_BYTES = GEMM_BN * 4;                                  // 4 bytes of block parameters per weight row
 constexpr int Q_INT8_BYTES = GEMM_BN * GEMM_BK + Q_PARAM_BYTES;             // 16 896
 constexpr int Q_NF4_BYTES = GEMM_BN * GEMM_BK / 2 + Q_PARAM_BYTES;          //  8 704
-constexpr int Q_DQ_BUFS = 2;                                                // TS = false: expanded f16 weight buffers in shared memory (32 KB each)
-constexpr int Q_TS_BUFS = 3;                                                // TS = true: expanded weight buffers in tensor memory (64 columns each)
-constexpr int Q_TS_COLS = GEMM_BK / 2;                                      // 32-bit columns per buffer
+constexpr int Q_DQ_BUFS = 2;                                                // expanded f16 weight buffers in shared memory (32 KB each)
 constexpr int Q_DQ_WARPS = 4;
 constexpr int Q_DQ_THREADS = Q_DQ_WARPS * 32;                               // = GEMM_BN: one thread per weight row
-constexpr int QGEMM_THREADS = GEMM_THREADS + Q_DQ_THREADS;                  // 4 epilogue + MMA + producer + 4 expansion warps
+constexpr int QGEMM_THREADS = GEMM_THREADS + Q_DQ_THREADS;                  // consumer warpgroup + producer + 4 expansion warps
 constexpr int Q_LUT_BYTES = 256 * 32 * 4;                                   // NF4: [code byte 256][lane 32] half2
 
 __host__ __device__ constexpr int q_block_bytes(int qt) { return qt == QT_INT8 ? Q_INT8_BYTES : (qt == QT_NF4 ? Q_NF4_BYTES : GEMM_WBYTES); }
@@ -50,22 +43,18 @@ __constant__ float c_nf4_levels[16] = {
     -0.09105003625154495f, 0.0f, 0.07958029955625534f, 0.16093020141124725f, 0.24611230194568634f, 0.33791524171829224f,
     0.44070982933044434f, 0.5626170039176941f, 0.7229568362236023f, 1.0f};
 
-template <int MT, int QT, bool TS = true>
+template <int MT, int QT>
 struct QGemmCfg {
     static constexpr int RAW_W = QT == QT_INT8 ? Q_INT8_BYTES : Q_NF4_BYTES;
     static constexpr int STAGE_BYTES = RAW_W + MT * GEMM_ABYTES;
     static constexpr int LUT = QT == QT_NF4 ? Q_LUT_BYTES : 0;
-    static constexpr int NBUF = TS ? Q_TS_BUFS : Q_DQ_BUFS;
-    static constexpr int DQ_BYTES = TS ? 0 : Q_DQ_BUFS * GEMM_WBYTES;
+    static constexpr int NBUF = Q_DQ_BUFS;
+    static constexpr int DQ_BYTES = Q_DQ_BUFS * GEMM_WBYTES;
     static constexpr int FIXED = DQ_BYTES + LUT;
     static constexpr int NFIT = (GEMM_SMEM_BUDGET - FIXED) / STAGE_BYTES;
     static constexpr int NSTAGE = NFIT > 12 ? 12 : NFIT;
-    static constexpr int BAR_BYTES = (2 * NSTAGE + 4 + 2 * NBUF) * 8 + 16;
+    static constexpr int BAR_BYTES = (2 * NSTAGE + 2 * NBUF) * 8 + 16;
     static constexpr int SMEM_BYTES = FIXED + NSTAGE * STAGE_BYTES + BAR_BYTES + 64;
-    static constexpr int ACC_COLS = 2 * 16 * MT;                              // double-buffered accumulator
-    static constexpr int NEED_COLS = ACC_COLS + (TS ? Q_TS_BUFS * Q_TS_COLS : 0);
-    static constexpr int TMEM_COLS = NEED_COLS <= 32 ? 32 : (NEED_COLS <= 64 ? 64 : (NEED_COLS <= 128 ? 128 : (NEED_COLS <= 256 ? 256 : 512)));
-    static_assert(NEED_COLS <= 512, "tensor memory has 512 columns");
     static_assert(NSTAGE >= 2, "ring needs two stages");
     static_assert(RAW_W % 128 == 0 && STAGE_BYTES % 128 == 0, "stage blocks stay 128-byte aligned");
 };
@@ -94,7 +83,7 @@ __device__ __forceinline__ uint32_t int8_pair(const uint32_t w, const uint32_t s
 }
 
 // ---------------------------------------------------------------------------------------
-// expansion role: 128 threads, thread r = weight row r of every stage block
+// expansion role: 128 threads, thread r = weight row r of every stage block, into the canonical layout of gemm.cuh
 // ---------------------------------------------------------------------------------------
 template <int QT>
 __device__ __forceinline__ void q_expand_block(const uint32_t raw, const uint32_t dq, const uint32_t lut, const int r, const int lane) {
@@ -136,74 +125,25 @@ __device__ __forceinline__ void q_expand_block(const uint32_t raw, const uint32_
     }
 }
 
-// TS variant: the same rows, 32 k at a time, from registers into 16 columns of the thread's tensor-memory lane
-template <int QT>
-__device__ __forceinline__ void q_expand_block_ts(const uint32_t raw, const uint32_t a_taddr, const uint32_t lut, const int r, const int lane) {
-    if (QT == QT_INT8) {
-        const uint32_t sm = lds32(raw + GEMM_BN * GEMM_BK + r * 4);            // lo = scale, hi = min
-        const __half2 s2 = u32_as_h2(prmt(sm, 0u, 0x1010u));
-        const __half2 m2 = u32_as_h2(prmt(sm, 0u, 0x3232u));
-        uint4 q[8];
-#pragma unroll
-        for (int c = 0; c < 8; ++c) q[c] = lds128(raw + (uint32_t)(c * GEMM_BN + r) * 16);
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {                                          // k = 32g .. 32g+31 = k16 chunks 2g, 2g+1
-            uint32_t o[16];
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const uint4 v = q[2 * g + h];
-                o[8 * h + 0] = int8_pair(v.x, 0x4140u, s2, m2); o[8 * h + 1] = int8_pair(v.x, 0x4342u, s2, m2);
-                o[8 * h + 2] = int8_pair(v.y, 0x4140u, s2, m2); o[8 * h + 3] = int8_pair(v.y, 0x4342u, s2, m2);
-                o[8 * h + 4] = int8_pair(v.z, 0x4140u, s2, m2); o[8 * h + 5] = int8_pair(v.z, 0x4342u, s2, m2);
-                o[8 * h + 6] = int8_pair(v.w, 0x4140u, s2, m2); o[8 * h + 7] = int8_pair(v.w, 0x4342u, s2, m2);
-            }
-            tc_st16(a_taddr + 16 * g, o);
-        }
-    } else {
-        const uint32_t am = lds32(raw + GEMM_BN * GEMM_BK / 2 + r * 4);        // lo = absmax of k < 64, hi = of k >= 64
-        const uint32_t lut_lane = lut + lane * 4;
-        uint4 q[4];
-#pragma unroll
-        for (int g = 0; g < 4; ++g) q[g] = lds128(raw + (uint32_t)(g * GEMM_BN + r) * 16);
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-            const __half2 a2 = u32_as_h2(prmt(am, 0u, g < 2 ? 0x1010u : 0x3232u));
-            const uint32_t w[4] = {q[g].x, q[g].y, q[g].z, q[g].w};
-            uint32_t o[16];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                o[4 * j + 0] = h2_as_u32(__hmul2(u32_as_h2(lds32(lut_lane + ((w[j] & 0xffu) << 7))), a2));
-                o[4 * j + 1] = h2_as_u32(__hmul2(u32_as_h2(lds32(lut_lane + (((w[j] >> 8) & 0xffu) << 7))), a2));
-                o[4 * j + 2] = h2_as_u32(__hmul2(u32_as_h2(lds32(lut_lane + (((w[j] >> 16) & 0xffu) << 7))), a2));
-                o[4 * j + 3] = h2_as_u32(__hmul2(u32_as_h2(lds32(lut_lane + ((w[j] >> 24) << 7))), a2));
-            }
-            tc_st16(a_taddr + 16 * g, o);
-        }
-    }
-}
-
 // ---------------------------------------------------------------------------------------
-// kernel: warps 0-3 epilogue (gemm.cuh), warp 4 MMA issuer, warp 5 TMA producer, warps 6-9 expansion
+// kernel: warps 0-3 consumer warpgroup (MMA + gemm.cuh epilogue), warp 4 TMA producer, warps 5-8 expansion
 // ---------------------------------------------------------------------------------------
-template <int MT, int QT, bool TS = true>
+template <int MT, int QT>
 __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_constant__ GemmParams p) {
-    using Cfg = QGemmCfg<MT, QT, TS>;
+    using Cfg = QGemmCfg<MT, QT>;
     constexpr int NBUF = Cfg::NBUF;
     constexpr int NSTAGE = Cfg::NSTAGE, STAGE_BYTES = Cfg::STAGE_BYTES, RAW_W = Cfg::RAW_W;
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ int s_last;
-    __shared__ __align__(16) __half s_stage[GEMM_EPI_THREADS * GEMM_STAGE_PITCH];
+    __shared__ __align__(16) float s_x[GEMM_XPOSE_FLOATS];
     const uint32_t smem_base = smem_u32(smem);
     const uint32_t dq_base = smem_base;
     const uint32_t lut_base = dq_base + Cfg::DQ_BYTES;
     const uint32_t ring_base = lut_base + Cfg::LUT;
     const uint32_t full_bar = ring_base + NSTAGE * STAGE_BYTES;
     const uint32_t empty_bar = full_bar + NSTAGE * 8;
-    const uint32_t tfull_bar = empty_bar + NSTAGE * 8;
-    const uint32_t tempty_bar = tfull_bar + 2 * 8;
-    const uint32_t dfull_bar = tempty_bar + 2 * 8;
+    const uint32_t dfull_bar = empty_bar + NSTAGE * 8;
     const uint32_t dfree_bar = dfull_bar + NBUF * 8;
-    const uint32_t tmem_slot = dfree_bar + NBUF * 8;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const long long TB = p.total_blocks;
@@ -211,44 +151,44 @@ __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_co
     const int b0 = (int)((long long)cta * TB / G);
     const int b1 = (int)((long long)(cta + 1) * TB / G);
     unsigned long long* const tr = (p.trace && cta == 0) ? p.trace : nullptr;
-    // hand-off variants (bit 0) and timing diagnostics (bits 1-3: results are wrong with those set; debug builds only)
+    // hand-off variant (bit 0: one arrival per expansion warp, set in production).  The timing diagnostics (bits 1-3: skip the
+    // expansion, the MMAs, the proxy fence; results are wrong with those set) exist in the debug build only, so that the
+    // product kernel's MMA issue is unconditional.
     const int qv = p.qvar;
-    const bool q_elect = qv & 1, q_noexpand = qv & 2, q_nomma = qv & 4, q_nofence = qv & 8;
+    const bool q_elect = qv & 1;
+#ifdef B200RWKV_DEBUG
+    const bool q_noexpand = qv & 2, q_nomma = qv & 4, q_nofence = qv & 8;
+#else
+    constexpr bool q_noexpand = false, q_nomma = false, q_nofence = false;
+#endif
     constexpr int QTR = 460;          // CTA 0's cycle accounts live behind the per-CTA stamps of the trace row
+    constexpr int EXP_WARP0 = GEMM_THREADS / 32;
 
     if (tid == 0) {
         if (tr) tr[0] = globaltimer_ns();
         for (int s = 0; s < NSTAGE; ++s) {
             mbar_init(full_bar + s * 8, 1);
-            mbar_init(empty_bar + s * 8, 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(tfull_bar + s * 8, 1);
-            mbar_init(tempty_bar + s * 8, GEMM_EPI_WARPS);
+            mbar_init(empty_bar + s * 8, GEMM_EPI_WARPS);
         }
         for (int s = 0; s < NBUF; ++s) {
-            mbar_init(dfull_bar + s * 8, (q_elect && !TS) ? Q_DQ_WARPS : Q_DQ_THREADS);
-            mbar_init(dfree_bar + s * 8, 1);
+            mbar_init(dfull_bar + s * 8, q_elect ? Q_DQ_WARPS : Q_DQ_THREADS);
+            mbar_init(dfree_bar + s * 8, GEMM_EPI_WARPS);
         }
         mbar_fence_init();
     }
-    if (warp == GEMM_EPI_WARPS) tc_alloc(tmem_slot, Cfg::TMEM_COLS);
-    if (QT == QT_NF4 && warp >= GEMM_EPI_WARPS + 2) {
+    if (QT == QT_NF4 && warp >= EXP_WARP0) {
         // level-pair table, one copy per lane: entry (byte, lane) = {level[byte & 15], level[byte >> 4]}
-        const int t = tid - (GEMM_EPI_WARPS + 2) * 32;
+        const int t = tid - GEMM_THREADS;
         for (int i = t; i < 256 * 32; i += Q_DQ_THREADS) {
             const int byte = i >> 5;
             const __half2 e = __halves2half2(__float2half_rn(c_nf4_levels[byte & 15]), __float2half_rn(c_nf4_levels[byte >> 4]));
             *reinterpret_cast<__half2*>(smem + (lut_base - smem_base) + (size_t)i * 4) = e;
         }
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem + (tmem_slot - smem_base));
     pdl_launch_dependents();
 
-    if (warp == GEMM_EPI_WARPS + 1) {
+    if (warp == GEMM_EPI_WARPS) {
         // ===================== producer =====================
         if (lane == 0) {
             const uint64_t pol_w = l2_policy_evict_first();
@@ -290,67 +230,11 @@ __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_co
             }
             if (tr) { tr[QTR + 10] = (unsigned long long)c_wait; tr[QTR + 11] = (unsigned long long)(clock64() - c_begin); }
         }
-    } else if (warp == GEMM_EPI_WARPS) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            constexpr uint32_t IDESC = umma_idesc_f16(GEMM_BN, 16 * MT);
-            constexpr uint32_t a_lbo = 16 * MT * 16;
-            RingPos rp{0, 0u};
-            unsigned segcount = 0;
-            int it = 0;
-            long long c_full = 0, c_dfull = 0, c_tempty = 0;
-            const long long c_begin = clock64();
-            SegWalk w;
-            w.init(p, b0, b1);
-            while (!w.done()) {
-                const int nblk = w.nblk();
-                const unsigned acc = segcount & 1u, use = segcount >> 1;
-                long long c0 = tr ? clock64() : 0;
-                if (use > 0) mbar_wait(tempty_bar + acc * 8, (use - 1) & 1u, 11);
-                if (tr) c_tempty += clock64() - c0;
-                tc_fence_after();
-                const uint32_t d0 = tmem_base + acc * (16 * MT);
-                for (int i = 0; i < nblk; ++i, ++it) {
-                    const int d = it % NBUF;
-                    c0 = tr ? clock64() : 0;
-                    mbar_wait(full_bar + rp.stage * 8, rp.phase, 12);                     // token operand landed
-                    const long long c1 = tr ? clock64() : 0;
-                    mbar_wait(dfull_bar + d * 8, (unsigned)(it / NBUF) & 1u, 15);         // weights expanded
-                    if (tr) { c_full += c1 - c0; c_dfull += clock64() - c1; }
-                    tc_fence_after();
-                    const uint32_t wst = dq_base + d * GEMM_WBYTES;
-                    const uint32_t ast = ring_base + rp.stage * STAGE_BYTES + RAW_W;
-#pragma unroll
-                    for (int k16 = 0; k16 < GEMM_BK / 16; ++k16) {
-                        const uint64_t bdesc = umma_desc(ast + k16 * 2 * a_lbo, a_lbo, GEMM_A_SBO);
-                        if (TS) {
-                            // weights: rows = TMEM lanes, this k16 step = 8 columns of buffer d (behind the accumulator columns)
-                            if (!q_nomma) tc_mma_f16_ts(d0, tmem_base + Cfg::ACC_COLS + d * Q_TS_COLS + k16 * 8, bdesc, IDESC, (i > 0 || k16 > 0) ? 1u : 0u);
-                        } else {
-                            const uint64_t adesc = umma_desc(wst + k16 * 2 * GEMM_W_LBO, GEMM_W_LBO, GEMM_W_SBO);
-                            if (!q_nomma) tc_mma_f16(d0, adesc, bdesc, IDESC, (i > 0 || k16 > 0) ? 1u : 0u);
-                        }
-                    }
-                    tc_commit(empty_bar + rp.stage * 8);
-                    tc_commit(dfree_bar + d * 8);
-                    rp.advance<NSTAGE>(1);
-                }
-                tc_commit(tfull_bar + acc * 8);
-                ++segcount;
-                w.next();
-            }
-            if (tr) {
-                tr[QTR + 5] = (unsigned long long)c_full; tr[QTR + 6] = (unsigned long long)c_dfull;
-                tr[QTR + 7] = (unsigned long long)c_tempty; tr[QTR + 8] = (unsigned long long)(clock64() - c_begin);
-            }
-        }
-    } else if (warp >= GEMM_EPI_WARPS + 2) {
+    } else if (warp >= EXP_WARP0) {
         // ===================== expansion: 4 warps =====================
-        // TS: a warp reaches the tensor-memory lanes of its own quadrant (warp index mod 4) only -> its rows are that quadrant's
-        const int r = TS ? ((warp & 3) * 32 + lane) : (tid - (GEMM_EPI_WARPS + 2) * 32);
-        const uint32_t a_lane_base = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + Cfg::ACC_COLS;
+        const int r = tid - GEMM_THREADS;
         RingPos rp{0, 0u};
-        const bool acct = tr && warp == GEMM_EPI_WARPS + 2 && lane == 0;
+        const bool acct = tr && warp == EXP_WARP0 && lane == 0;
         long long c_full = 0, c_dfree = 0, c_expand = 0, c_hand = 0;
         for (int b = b0, it = 0; b < b1; ++b, ++it) {
             const int d = it % NBUF;
@@ -360,25 +244,14 @@ __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_co
             const long long c1 = acct ? clock64() : 0;
             if (u > 0) mbar_wait(dfree_bar + d * 8, (unsigned)(u - 1) & 1u, 17);          // the MMAs that read this buffer retired
             const long long c2 = acct ? clock64() : 0;
-            if (TS) {
-                tc_fence_after();                    // the retired MMAs' reads of this buffer are ordered before the stores below
-                if (!q_noexpand) q_expand_block_ts<QT>(ring_base + rp.stage * STAGE_BYTES, a_lane_base + d * Q_TS_COLS, lut_base, r, lane);
-            } else {
-                if (!q_noexpand) q_expand_block<QT>(ring_base + rp.stage * STAGE_BYTES, dq_base + d * GEMM_WBYTES, lut_base, r, lane);
-            }
+            if (!q_noexpand) q_expand_block<QT>(ring_base + rp.stage * STAGE_BYTES, dq_base + d * GEMM_WBYTES, lut_base, r, lane);
             const long long c3 = acct ? clock64() : 0;
-            if (TS) {
-                tc_wait_st();                        // the stores have landed in tensor memory
-                tc_fence_before();
-                mbar_arrive(dfull_bar + d * 8);
+            if (!q_nofence) fence_proxy_async();     // generic-proxy stores -> visible to the tensor core's async-proxy reads
+            if (q_elect) {
+                __syncwarp();                        // the other lanes' (fenced) stores happen before lane 0's release
+                if (lane == 0) mbar_arrive(dfull_bar + d * 8);
             } else {
-                if (!q_nofence) fence_proxy_async(); // generic-proxy stores -> visible to the tensor core's async-proxy reads
-                if (q_elect) {
-                    __syncwarp();                    // the other lanes' (fenced) stores happen before lane 0's release
-                    if (lane == 0) mbar_arrive(dfull_bar + d * 8);
-                } else {
-                    mbar_arrive(dfull_bar + d * 8);
-                }
+                mbar_arrive(dfull_bar + d * 8);
             }
             if (acct) { const long long c4 = clock64(); c_full += c1 - c0; c_dfree += c2 - c1; c_expand += c3 - c2; c_hand += c4 - c3; }
             rp.advance<NSTAGE>(1);
@@ -388,16 +261,72 @@ __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_co
             tr[QTR + 3] = (unsigned long long)c_hand; tr[QTR + 4] = (unsigned long long)(b1 - b0);
         }
     } else {
-        // ===================== epilogue: 4 warps =====================
+        // ===================== consumer warpgroup: MMA + epilogue =====================
         pdl_wait();
-        unsigned segcount = 0;
-        gemm_epilogue_role<MT, false>(p, cta, G, b0, b1, tfull_bar, tempty_bar, tmem_base, segcount, *p.nrows, &s_last, s_stage, nullptr);
+        constexpr uint32_t a_lbo = 16 * MT * 16;
+        RingPos rp{0, 0u};
+        int it = 0;
+        long long c_full = 0, c_dfull = 0;
+        const long long c_begin = clock64();
+        SegWalk w;
+        w.init(p, b0, b1);
+        while (!w.done()) {
+            const int nblk = w.nblk();
+            float acc[2][8 * MT];
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int i = 0; i < 8 * MT; ++i) acc[h][i] = 0.f;
+            int prev_stage = -1, prev_d = -1;
+            for (int i = 0; i < nblk; ++i, ++it) {
+                const int d = it % NBUF;
+                const long long c0 = tr ? clock64() : 0;
+                mbar_wait(full_bar + rp.stage * 8, rp.phase, 12);                     // token operand landed
+                const long long c1 = tr ? clock64() : 0;
+                mbar_wait(dfull_bar + d * 8, (unsigned)(it / NBUF) & 1u, 15);         // weights expanded
+                if (tr) { c_full += c1 - c0; c_dfull += clock64() - c1; }
+                const uint32_t wst = dq_base + d * GEMM_WBYTES;
+                const uint32_t ast = ring_base + rp.stage * STAGE_BYTES + RAW_W;
+                wgmma_fence_operand(acc[0]);
+                wgmma_fence_operand(acc[1]);
+                wgmma_fence();
+                if (!q_nomma) {
+#pragma unroll
+                    for (int k16 = 0; k16 < GEMM_BK / 16; ++k16) {
+                        const uint64_t bdesc = gmma_desc(ast + k16 * 2 * a_lbo, a_lbo, GEMM_A_SBO);
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            wgmma_f16<16 * MT>(acc[h], gmma_desc(wst + h * 8 * GEMM_W_SBO + k16 * 2 * GEMM_W_LBO, GEMM_W_LBO, GEMM_W_SBO), bdesc);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                     // the previous block's MMAs retired: its ring slot and buffer go back
+                if (prev_stage >= 0) {
+                    __syncwarp();
+                    if (lane == 0) { mbar_arrive(empty_bar + prev_stage * 8); mbar_arrive(dfree_bar + prev_d * 8); }
+                }
+                prev_stage = rp.stage;
+                prev_d = d;
+                rp.advance<NSTAGE>(1);
+            }
+            wgmma_wait<0>();
+            wgmma_fence_operand(acc[0]);
+            wgmma_fence_operand(acc[1]);
+            __syncwarp();
+            if (lane == 0) { mbar_arrive(empty_bar + prev_stage * 8); mbar_arrive(dfree_bar + prev_d * 8); }
+            float v[MT][16];
+            gemm_acc_to_rows<MT>(acc, v, s_x);
+            gemm_epilogue_tile<MT, false>(p, w, cta, G, v, *p.nrows, &s_last, reinterpret_cast<__half*>(s_x));
+            w.next();
+        }
+        if (tr && tid == 0) {
+            tr[QTR + 5] = (unsigned long long)c_full; tr[QTR + 6] = (unsigned long long)c_dfull;
+            tr[QTR + 7] = 0; tr[QTR + 8] = (unsigned long long)(clock64() - c_begin);
+        }
     }
-    tc_fence_before();
     __syncthreads();
     if (tid == 0 && tr) tr[7] = globaltimer_ns();
     if (tid == 0 && p.trace) p.trace[8 + 3 * cta + 2] = globaltimer_ns();
-    if (warp == GEMM_EPI_WARPS) tc_dealloc(tmem_base, Cfg::TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------------------

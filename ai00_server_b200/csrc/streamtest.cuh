@@ -1,6 +1,6 @@
-// Streaming micro-benchmarks (debug entry point b200rwkv_debug_stream): how fast can one B200 pull
+// Streaming micro-benchmarks (debug entry point b200rwkv_debug_stream): how fast can one GPU pull
 // a large buffer from HBM through (a) plain vector loads, (b) the 1-D bulk-TMA stage ring used by
-// the projection GEMM with a trivial consumer, (c) the same ring drained by tcgen05.mma.
+// the projection GEMM with a trivial consumer.
 // Not on the product path; used to size the ring and to separate producer limits from consumer limits.
 #pragma once
 #include "gemm.cuh"
@@ -27,7 +27,6 @@ struct StreamParams {
     int stage_bytes;     // multiple of 1024
     int nstage;
     int use_hint;        // 0 none, 1 evict_first
-    int consumer;        // 0 trivial (wait + arrive), 1 tcgen05.mma over the stage, 2 = 1 with commit only every stage
     int split;           // bulk copies per stage (1, 2, 4)
     int producers;       // producer warps issuing in round robin (1..3)
     int extra;           // bytes of the stage sent as a separate small copy (the GEMM's activation slice)
@@ -40,17 +39,12 @@ __global__ void __launch_bounds__(128, 1) stream_ring_kernel(const __grid_consta
     const int NS = p.nstage, SB = p.stage_bytes;
     const uint32_t full_bar = smem_base + NS * SB;
     const uint32_t empty_bar = full_bar + NS * 8;
-    const uint32_t tmem_slot = empty_bar + NS * 8;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (tid == 0) {
         for (int s = 0; s < NS; ++s) { mbar_init(full_bar + s * 8, 1); mbar_init(empty_bar + s * 8, 1); }
         mbar_fence_init();
     }
-    if (warp == 1) tc_alloc(tmem_slot, 32);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem + (tmem_slot - smem_base));
     const size_t nst = p.bytes_per_cta / SB;
     const uint8_t* src = p.src + (size_t)blockIdx.x * p.bytes_per_cta;
     // producers: lane 0 of warps 0, 2, 3 (round robin over stages); consumer: lane 0 of warp 1
@@ -75,31 +69,15 @@ __global__ void __launch_bounds__(128, 1) stream_ring_kernel(const __grid_consta
             while (stage >= NS) { stage -= NS; par ^= 1u; }
         }
     } else if (warp == 1 && lane == 0) {
-        constexpr uint32_t IDESC = umma_idesc_f16(128, 16);
         int stage = 0;
         uint32_t par = 0;
         for (size_t it = 0; it < nst; ++it) {
             mbar_wait(full_bar + stage * 8, par);
-            if (p.consumer == 0) {
-                mbar_arrive(empty_bar + stage * 8);
-            } else {
-                tc_fence_after();
-                const uint32_t st = smem_base + stage * SB;
-                for (int blk = 0; blk < SB / 16384; ++blk)
-                    for (int k16 = 0; k16 < 4; ++k16) {
-                        const uint64_t a_ = umma_desc(st + blk * 16384 + k16 * 2 * 2048, 2048, 128);
-                        const uint64_t b_ = umma_desc(st + k16 * 2 * GEMM_A_LBO, GEMM_A_LBO, GEMM_A_SBO);   // garbage operand, same smem
-                        tc_mma_f16(tmem_base, a_, b_, IDESC, 1u);
-                    }
-                tc_commit(empty_bar + stage * 8);
-            }
-            if (it + 1 == nst && p.consumer != 0) mbar_wait(empty_bar + stage * 8, par);   // all MMAs retired
+            mbar_arrive(empty_bar + stage * 8);
             if (++stage == NS) { stage = 0; par ^= 1u; }
         }
     }
-    tc_fence_before();
     __syncthreads();
-    if (warp == 1) tc_dealloc(tmem_base, 32);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -127,58 +105,6 @@ __global__ void __launch_bounds__(128) prefetch_probe_kernel(const uint8_t* src,
         }
     }
     while (globaltimer_ns() - t0 < idle_ns) { }
-}
-
-// ---------------------------------------------------------------------------------------
-// tcgen05.mma issue / execution rate for one instruction shape (debug entry point b200rwkv_debug_mma_rate): one CTA, one
-// lane issues `n` kind::f16 MMAs back to back (A from shared memory or from tensor memory, eight distinct k16 slices of a
-// zeroed operand tile in rotation, like the projection's main loop), commits, waits.  Answers what a [M x 16] x [16 x N]
-// instruction costs when nothing else is in the way -- the projection GEMMs are bound by this, not by HBM, once the weight
-// bytes per block shrink (r02_findings.md §11).
-// ---------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) mma_rate_kernel(int M, int N, int a_in_tmem, int n, long long* cycles_out) {
-    extern __shared__ __align__(1024) uint8_t smem[];       // A tile: 128 rows x 128 k (32 KB) | B tile: 256 rows x 128 k (64 KB) | barrier
-    const uint32_t smem_base = smem_u32(smem);
-    const uint32_t a_base = smem_base, b_base = smem_base + 32768, bar = smem_base + 32768 + 65536, slot = bar + 8;
-    const int tid = threadIdx.x, warp = tid >> 5;
-    for (int i = tid; i < (32768 + 65536) / 16; i += 128) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-    if (tid == 0) { mbar_init(bar, 1); mbar_fence_init(); }
-    if (warp == 0) tc_alloc(slot, 512);
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem + (slot - smem_base));
-    if (a_in_tmem) {          // defined contents in the A columns (256 .. 319)
-        uint32_t z[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) z[i] = 0;
-        for (int c = 0; c < 64; c += 16) tc_st16(tmem_base + ((uint32_t)(warp * 32) << 16) + 256 + c, z);
-        tc_wait_st();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (tid == 0) {
-        const uint32_t idesc = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-        const uint32_t a_lbo = 16 * 128, b_lbo = (uint32_t)N * 16;          // bytes between the two k8 chunks of a k16 step
-        const long long c0 = clock64();
-        for (int i = 0; i < n; ++i) {
-            const int k16 = i & 7;
-            const uint64_t bdesc = umma_desc(b_base + k16 * 2 * b_lbo, b_lbo, 128);
-            if (a_in_tmem) tc_mma_f16_ts(tmem_base, tmem_base + 256 + k16 * 8, bdesc, idesc, i > 0 ? 1u : 0u);
-            else tc_mma_f16(tmem_base, umma_desc(a_base + k16 * 2 * a_lbo, a_lbo, 128), bdesc, idesc, i > 0 ? 1u : 0u);
-        }
-        const long long c1 = clock64();
-        tc_commit(bar);
-        mbar_wait(bar, 0);
-        const long long c2 = clock64();
-        cycles_out[0] = c1 - c0;      // issue loop
-        cycles_out[1] = c2 - c0;      // until the last MMA has retired
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tc_dealloc(tmem_base, 512);
 }
 
 }  // namespace b200

@@ -115,7 +115,7 @@ def tensor_spec(s: Shape) -> list[tuple[str, tuple[int, ...], float, float]]:
             add(a + "g1", (s.Dg, C), -1.0 * _sq(C), 1.0 * _sq(C))
             # gate LoRA / output gains sized so that the synthetic model is as well conditioned as the RWKV-6 presets: with
             # gain 2 / 0.5 here the random RWKV-7 stack is chaotic (two f32 implementations that differ only in summation
-            # order are 3e-3 apart after one token at 32 layers, f16 vs f32 operands 0.3: profiles/r02_findings.md), which
+            # order are 3e-3 apart after one token at 32 layers, f16 vs f32 operands 0.3), which
             # says nothing about an engine; trained RWKV-7 checkpoints initialise both near zero.
             add(a + "g2", (C, s.Dg), -1.0 * _sq(s.Dg), 1.0 * _sq(s.Dg))
             add(a + "k_k", (1, 1, C), 0.5, 1.2)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — decode tokens/s of the RWKV hot path on B200 (BASELINE.json metric).
+"""bench.py — decode tokens/s of the RWKV hot path on H100 (BASELINE.json metric).
 
 A "step" is one decode step of the whole model for every slot of the batch (one token per
 slot): the per-layer WKV recurrence + token shift + GroupNorm, all projections and the head.
@@ -16,6 +16,12 @@ there are no checkpoints offline).
   cpu_baseline / --impl reference
             the C/OpenMP oracle (oracle/rwkv_ref.c) on the host cores, same weights/tokens
             (the reference's own web-rwkv+lavapipe path cannot be built here: no Rust, no Vulkan)
+
+  --dump-outputs DIR
+            after the timed steps, writes what the timed path computed in its last step as DIR/<name>.npy:
+            decode: every slot's last logits row (logits.npy, [B, V]), a fixed, seeded sample of every slot's
+            recurrent state, and the GPU sampler's top-128 of each row; prefill: a fixed, seeded sample of every
+            sequence's final state (the embedding).  The same arguments give the same inputs on every run.
 """
 from __future__ import annotations
 
@@ -50,11 +56,11 @@ def read_peaks():
             return json.load(open(p)), "measured"
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback"        # H100 SXM data sheet (700 W), dense
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -155,6 +161,42 @@ def cpu_arm(weights, batch: int, steps: int, warmup: int, toks_bt: np.ndarray, b
     return batch * done / dt, dt / done * 1e3, rc.num_threads(), done
 
 
+DUMP_STATE_SAMPLE = 65536          # decode: state elements per slot written by --dump-outputs (fixed seeded positions)
+DUMP_PREFILL_SAMPLE = 16384        # prefill: the same per sequence (256 sequences x 16384 x 4 B = 16 MB)
+
+
+def state_sample_index(numel: int, n: int) -> np.ndarray:
+    """Fixed, seeded positions into a flattened state: the same on every run and every build."""
+    return np.sort(np.random.default_rng(0).choice(numel, size=min(n, numel), replace=False))
+
+
+def dump_outputs(out_dir: str, model, slots) -> None:
+    """--dump-outputs (decode): what the timed decode path computed in its last step, as a caller receives it -- every
+    slot's last logits row over the whole vocabulary (logits.npy, [B, V]) and every slot's recurrent state, of which a fixed
+    seeded sample is kept (state_sample.npy; the full states of a 7B batch are ~550 MB).  Both are read through a device
+    snapshot of the slot (State::read + snapshot_back, the cache item {state, output}).  topk_ids / topk_probs: the GPU
+    sampler's front half over the same rows (top 128, no penalties)."""
+    os.makedirs(out_dir, exist_ok=True)
+    logits, states, idx = [], [], None
+    for s_ in slots:
+        snap = model.state.read(s_)
+        try:
+            st_, lg = model.state.snapshot_back(snap, with_logits=True)
+        finally:
+            snap.free()
+        st_ = np.asarray(st_, np.float32).reshape(-1)
+        if idx is None:
+            idx = state_sample_index(st_.size, DUMP_STATE_SAMPLE)
+        logits.append(np.asarray(lg, np.float32))
+        states.append(st_[idx])
+    np.save(os.path.join(out_dir, "logits.npy"), np.stack(logits, 0))
+    np.save(os.path.join(out_dir, "state_sample.npy"), np.stack(states, 0))
+    np.save(os.path.join(out_dir, "state_sample_index.npy"), idx.astype(np.float64))
+    ids, probs = model.sample_topk(slots, top_k=128)
+    np.save(os.path.join(out_dir, "topk_ids.npy"), ids.astype(np.float64))
+    np.save(os.path.join(out_dir, "topk_probs.npy"), probs.astype(np.float32))
+
+
 def prefill_main(args):
     """cfg 5 (BASELINE.json configs[4]): `seqs` prompts of `seq_len` tokens through the embeddings route's path -- prefill with
     no logits, then State::back of every slot (run.rs:984-989 returns the backed state as the embedding).  A "step" is one
@@ -165,7 +207,7 @@ def prefill_main(args):
     preset = args.preset if args.preset != "v6-7b" or "--preset" in sys.argv else "v6-3b"
     shape = synth.PRESETS[preset]
     B, Tn = args.seqs, args.seq_len
-    steps, warm = max(1, min(args.steps, 4)), max(3, args.warmup if args.warmup < 8 else 3)
+    steps, warm = args.steps, args.warmup
     metric = f"prefill tokens/s {MODEL_NAMES.get(preset, preset)} fp16 {B}x{Tn}-token inputs (embeddings route)"
     st = synth.make_st(shape, 0)
     PASS = 128                                              # tokens per weight pass (the engine's largest step)
@@ -204,6 +246,12 @@ def prefill_main(args):
     ntok = B * Tn
     dt, de = float(np.mean(t_dev)), float(np.mean(t_e2e))
     checksum = [float(state_buf.astype(np.float64).sum()), float(np.abs(state_buf).astype(np.float64).sum())]
+    if args.dump_outputs:          # the last pass's embeddings (every sequence's backed state), a fixed seeded sample of each
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        flat = state_buf.reshape(B, -1)
+        idx = state_sample_index(flat.shape[1], DUMP_PREFILL_SAMPLE)
+        np.save(os.path.join(args.dump_outputs, "state_sample.npy"), np.ascontiguousarray(flat[:, idx]))
+        np.save(os.path.join(args.dump_outputs, "state_sample_index.npy"), idx.astype(np.float64))
     # parity spot check + CPU baseline (outside the timed region): the first sequences' first tokens against the C oracle
     w = O.parse_st(st)
     from oracle import ref_c
@@ -265,9 +313,9 @@ def prefill_main(args):
                          "frac": n_pass * pass_bytes / dt / 1e9 / peaks["hbm_gbs"], "traffic": None,
                          "peak_source": f"MEASURED_PEAKS.json ({peak_src})", "passes": n_pass, "bytes_per_pass": int(pass_bytes),
                          "tensor_tflops_achieved": flops / dt / 1e12, "tensor_tflops_peak_sustained": peaks.get("bf16_tflops_sustained"),
-                         "note": f"the route turns tensor-bound at >= 280 FLOP/B = ~300 tokens per weight pass; at {PASS} tokens per pass "
-                                 "(shared memory: 32 KB weights + 32 KB tokens per stage, TMEM: 256 of 512 columns) it is still bound by "
-                                 "streaming the weights, which is what `achieved` measures"},
+                         "note": f"the route turns tensor-bound at ~295 FLOP/B (989 TFLOP/s over 3.35 TB/s) = ~300 tokens per weight "
+                                 f"pass; at {PASS} tokens per pass (shared memory: 32 KB weights + 32 KB tokens per stage) it is still "
+                                 "bound by streaming the weights, which is what `achieved` measures"},
             "cpu_baseline": {"value": nb * nt / cdt, "unit": "tokens/s", "cores": rc.num_threads(), "kind": "port",
                              "sample": f"first {nt} tokens of the first {nb} sequences, C/OpenMP oracle (token by token)"},
             "pass_breakdown": breakdown,
@@ -284,7 +332,7 @@ def main():
     global PRESET, BATCH
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=128)
+    ap.add_argument("--steps", type=int, default=None, help="timed steps (default: 128 decode steps, 4 prefill passes)")
     ap.add_argument("--warmup", type=int, default=8)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--cpu-steps", type=int, default=int(os.environ.get("B200RWKV_BENCH_CPU_STEPS", "6")))
@@ -298,8 +346,16 @@ def main():
     ap.add_argument("--quant-layers", type=int, default=-1, help="the reference's `quant`: first N layers (default: all)")
     ap.add_argument("--seqs", type=int, default=256)
     ap.add_argument("--seq-len", type=int, default=512)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (GPU arm, one GPU)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
+    if args.steps is None:
+        args.steps = 4 if args.mode == "prefill" else 128
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and (args.impl != "b200" or args.gpus != 1):
+        ap.error("--dump-outputs: single-GPU GPU arm only")
     PRESET, BATCH = args.preset, args.batch
     METRIC = metric_name(PRESET, BATCH)
     if args.quant != "none":
@@ -310,6 +366,8 @@ def main():
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
+    if args.dump_outputs and world != 1:
+        ap.error("--dump-outputs: single-GPU GPU arm only")
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
 
     from ai00_server_b200 import synth
@@ -318,7 +376,7 @@ def main():
     config = {"workload": f"{PRESET} decode, batch {BATCH} slots x 1 token/step, {PROMPT}-token synthetic prompt per slot",
               "preset": PRESET, "batch": BATCH, "prompt_tokens": PROMPT, "parallelism": f"tp{world}",
               "activations": "f32-exact (split f16 hi+lo operands)" if args.exact else "f16 operands",
-              "l2": "inputs larger than L2 (14.7 GB of weights streamed per step vs 126 MB L2), no flush"}
+              "l2": "inputs larger than L2 (14.7 GB of weights streamed per step vs 50 MB L2), no flush"}
 
     # ------------------------------------------------------------------ reference arm (CPU)
     if args.impl == "reference":
@@ -339,7 +397,7 @@ def main():
         print(json.dumps(line))
         return
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     import torch                                  # plumbing only: device selection + distributed barrier
     from ai00_server_b200 import runtime
     if world > 1:
@@ -389,6 +447,8 @@ def main():
         ms = float(t.item())
     ms_per_step = ms / args.steps
     value = BATCH * args.steps / (ms * 1e-3)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, model, slots)
 
     # ---- e2e: host tokens in, host logits out, every step, through Runtime.infer ----
     out = np.empty((BATCH, shape.V), np.float32)       # rank 0 receives the gathered full-vocabulary logits
@@ -477,17 +537,10 @@ def main():
         mats = ([(C_, C_)] * (5 if shape.version != 7 else 4)) + [(F_, C_), (C_, F_)] + ([(C_, C_)] if shape.version != 7 else [])
         per = (lambda n, k: n * k + n * k // 128 * 4) if args.quant == "int8" else (lambda n, k: n * k // 2 + n * k // 64 * 2)
         alg_bytes += qlayers * sum(per(n, k) - 2 * n * k for n, k in mats)
-    traffic = None       # DRAM bytes of the same launches from the committed ncu capture (N = 1 capture of this workload)
-    tpath = os.path.join(ROOT, "profiles", "r01_gemm_traffic.json")
-    if world == 1 and PRESET == "v6-7b" and BATCH == 16 and args.quant == "none" and os.path.exists(tpath):
-        tj = json.load(open(tpath))
-        traffic = tj["layers"] * sum(x["dram_bytes"] for x in tj["per_layer_gemm_launches"]) + tj["head"]["algorithmic_weight_bytes"]
     windows_sum_us = sum(v[0] for v in cls.values())
-    roofline = {"bound": "hbm", "kernel": "gemm_kernel (tcgen05 projection GEMM: every launch of one step, per GPU)",
+    roofline = {"bound": "hbm", "kernel": "gemm_kernel (wgmma projection GEMM: every launch of one step, per GPU)",
                 "achieved": gemm_gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": gemm_gbs / peaks["hbm_gbs"],
-                "peak_source": f"MEASURED_PEAKS.json ({peak_src})", "traffic": traffic,
-                "traffic_note": "per step, summed over the same projection launches as `achieved`: ncu dram read+write bytes of one "
-                                "captured layer x 32 + the head's algorithmic bytes (profiles/r01_gemm_traffic.json)",
+                "peak_source": f"MEASURED_PEAKS.json ({peak_src})",
                 "how": "in situ: algorithmic weight bytes of the step's projection launches / sum of their windows [griddepcontrol.wait "
                        "released, last CTA exit] inside a graph-replayed step (globaltimer stamps, mean of 5 replays)",
                 "algorithmic_bytes_per_step_gemm": int(gemm_bytes), "gemm_us_per_step": gemm_us, "gemm_launches_per_step": int(gemm_n),
@@ -515,8 +568,8 @@ def main():
         m2.infer_raw(slots, [PROMPT] * BATCH, toks[:, :PROMPT].reshape(-1).tolist(), [2] * BATCH)
         ms2, _ = m2.bench_decode(slots, dec, args.warmup, args.steps)
         exact_rec = {"ms_per_step": ms2 / args.steps, "value": BATCH * args.steps / (ms2 * 1e-3), "unit": "tokens/s",
-                     "what": "b200rwkv_create(precision = 1): split f16 hi+lo operands, no activation rounded; logits within 1.6e-4 of the "
-                             "f32 oracle at the 7B shape (tests/test_gpu_zfullsize.py, profiles/r02_parity_fullsize.jsonl)"}
+                     "what": "b200rwkv_create(precision = 1): split f16 hi+lo operands, no activation rounded; logits checked against "
+                             "the f32 oracle at the 7B shape by tests/test_gpu_zfullsize.py"}
         m2.close()
 
     # ---- cpu baseline (rank 0, N=1 only) ----

@@ -1,4 +1,4 @@
-/* b200rwkv.h — C ABI of the B200-native RWKV inference engine.
+/* b200rwkv.h — C ABI of the H100-native RWKV inference engine.
  *
  * This is the drop-in boundary underneath crates/ai00-core: every entry point replaces one
  * use of the `web-rwkv` crate at a call site of the reference (paths relative to the
@@ -15,7 +15,7 @@
  *   - threading mirrors the reference: ONE task calls infer/state ops
  *     (crates/ai00-core/src/run.rs:1232) and ONE task calls softmax (run.rs:1237); the engine
  *     serialises each group with an internal mutex.
- *   - there is no CPU fallback: creation fails if no sm_100 device is present.
+ *   - there is no CPU fallback: creation fails if no sm_90 (H100) device is present.
  */
 #ifndef B200RWKV_H
 #define B200RWKV_H
@@ -273,13 +273,9 @@ int32_t b200rwkv_debug_gemm_time(b200rwkv_engine*, int32_t which, int32_t reps, 
  * micro-benchmarks (csrc/streamtest.cuh).  The debug build also honours the B200RWKV_* bring-up environment switches;
  * the product library ignores the environment. */
 int32_t b200rwkv_debug_stream(int32_t device, int32_t kind, double gbytes, int32_t stage_bytes, int32_t nstage,
-                              int32_t use_hint, int32_t consumer, int32_t split, int32_t producers, int32_t reps,
-                              float* ms_out);
+                              int32_t use_hint, int32_t split, int32_t producers, int32_t reps, float* ms_out);
 int32_t b200rwkv_debug_prefetch(int32_t device, double mbytes, int32_t consumers, int32_t pf_grid, int32_t skip, int32_t nblk,
                                 int32_t mode, double idle_us, int32_t reps, float* ms_out);
-/* SM cycles for n back-to-back tcgen05.mma kind::f16 of shape [M x 16] x [16 x N] on one SM, A operand from shared memory or
- * tensor memory: cycles[0] = the issue loop, cycles[1] = until the last one has retired. */
-int32_t b200rwkv_debug_mma_rate(int32_t device, int32_t M, int32_t N, int32_t a_in_tmem, int32_t n, int64_t* cycles);
 #endif
 
 const char* b200rwkv_last_error(b200rwkv_engine*);

@@ -4,7 +4,7 @@ TEST INFRASTRUCTURE (CPU only).  On a synthetic model of the given preset this c
   (a) the C/OpenMP oracle under the f16-operand contract vs the same code under the pure-f32 contract, and
   (b) the C oracle vs the NumPy oracle, both under the f16-operand contract (they differ only in f32 summation order).
 (b) is the noise floor of ANY parity check at that depth: a rounding flip of one f16 operand is 1e-3 of that element and
-32 layers of LayerNorm + projections amplify it.  Recorded output: profiles/r01_noise_floor.txt.
+32 layers of LayerNorm + projections amplify it.
 
     python -m oracle.noise_floor v6-3b [steps]
 """

@@ -1,4 +1,4 @@
-"""One engine object over N GPUs of the box (b200rwkv_create_ex, worker thread per rank): decode throughput of the bench
+"""One engine object over N GPUs of the machine (b200rwkv_create_ex, worker thread per rank): decode throughput of the bench
 workload and the in-situ windows of rank 0's step.  usage: gpu_inproc_tp.py N [preset] [batch]"""
 import os, sys, time
 import numpy as np

@@ -1,8 +1,7 @@
 """Where a quantised projection launch spends its time (debug build): per-role cycle accounts of CTA 0 (qgemm.cuh) and the launch
-windows, for the hand-off variants / diagnostic switches of B200RWKV_QVAR.
-B200RWKV_QTS=1: expanded weights go to tensor memory (production); 0: through shared memory + fence.proxy.async (reference variant;
-there bit 0: one arrive per expansion warp instead of one per thread, bit 3: skip the proxy fence).  bit 1: skip the expansion; bit 2: skip
-the MMAs (bits 1-3 give wrong results: timing only)."""
+windows, for the hand-off variants / diagnostic switches of B200RWKV_QVAR: bit 0: one arrive per expansion warp instead of one
+per thread (production); bit 1: skip the expansion; bit 2: skip the MMAs; bit 3: skip the proxy fence (bits 1-3 give wrong
+results: timing only)."""
 import ctypes as C, dataclasses, os, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -15,9 +14,8 @@ st = synth.make_st(shape, 0)
 rng = np.random.default_rng(0)
 ROW, QTR = 512, 460
 for qt in ("int8", "nf4"):
-    for ts, qv in ((1, 0), (1, 2), (1, 4), (1, 6), (0, 1)):
+    for qv in (1, 0, 3, 5, 9, 7):
         os.environ["B200RWKV_QVAR"] = str(qv)
-        os.environ["B200RWKV_QTS"] = str(ts)
         m = runtime.Model(st, max_batch=B, token_chunk_size=64, quant=shape.L, quant_type=qt)
         slots = list(range(B))
         for i in range(4):
@@ -34,11 +32,11 @@ for qt in ("int8", "nf4"):
             a = agg.setdefault(int(types[i]) - 1000000, [])
             q = full[i, QTR:QTR + 12]
             a.append([(full[i, 7] - full[i, 2]) / 1e3] + q.tolist())
-        print(f"{qt} {'tensor-memory' if ts else 'shared-memory'} hand-off qvar={qv} step {step_us:.1f} us")
+        print(f"{qt} qvar={qv} step {step_us:.1f} us")
         for mb, rows in sorted(agg.items()):
             r = np.asarray(rows, np.float64).mean(0)
             nb = r[5]
             print(f"  gemm {mb:4d} MiB x{len(rows)}: window {r[0]:6.2f} us, {nb:.0f} blocks/CTA = {r[0] / nb:5.3f} us/block | expand warps (cycles/block): "
-                  f"wait full {r[1]/nb:6.0f} wait dfree {r[2]/nb:6.0f} expand {r[3]/nb:6.0f} fence+arrive {r[4]/nb:6.0f} | mma lane: wait full {r[6]/nb:6.0f} "
-                  f"wait dfull {r[7]/nb:6.0f} wait tmem {r[8]/nb:6.0f} total {r[9]/nb:6.0f} | producer: wait empty {r[11]/nb:6.0f} total {r[12]/nb:6.0f}")
+                  f"wait full {r[1]/nb:6.0f} wait dfree {r[2]/nb:6.0f} expand {r[3]/nb:6.0f} fence+arrive {r[4]/nb:6.0f} | consumer: wait full {r[6]/nb:6.0f} "
+                  f"wait dfull {r[7]/nb:6.0f} total {r[9]/nb:6.0f} | producer: wait empty {r[11]/nb:6.0f} total {r[12]/nb:6.0f}")
         m.close()

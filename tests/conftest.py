@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run on the GPU box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (select with -m gpu)")
 
 
 def _has_gpu() -> bool:

@@ -1,4 +1,4 @@
-"""`bench.py --impl reference` (the CPU arm the driver runs next to the B200 arm) prints one contract-shaped JSON line.
+"""`bench.py --impl reference` (the CPU arm beside the GPU arm) prints one contract-shaped JSON line.
 Runs the C/OpenMP oracle on a CI-sized preset; nothing here touches a GPU."""
 import json
 import os
