@@ -43,6 +43,17 @@ class Options(C.Structure):
 QUANT_NONE, QUANT_INT8, QUANT_NF4 = 0, 1, 2
 
 
+class GemmSeg(C.Structure):
+    """b200rwkv_gemm_seg (include/b200rwkv.h)."""
+    _fields_ = [("N", C.c_int32), ("K", C.c_int32), ("w", C.c_void_p), ("x", C.c_void_p), ("bias", C.c_void_p),
+                ("act", C.c_int32), ("out_mode", C.c_int32), ("grp", C.c_int32),
+                ("lerp_xx", C.c_void_p), ("lerp_sx", C.c_void_p), ("lerp_mu", C.c_void_p), ("ldo", C.c_int32), ("out", C.c_void_p)]
+
+
+ACT_NONE, ACT_TANH, ACT_SIGMOID, ACT_SILU, ACT_RELU2, ACT_EXPNEGEXP, ACT_V7DECAY = range(7)
+OUT_F32, OUT_A16, OUT_LERP_A16 = 0, 1, 2
+
+
 class B200Error(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"b200rwkv error {code}: {msg}")
@@ -82,6 +93,7 @@ SYMBOLS = [
     ("b200rwkv_profile_insitu", C.c_int32, [_P, C.c_int32, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, C.POINTER(C.c_double)]),
     ("b200rwkv_op_quantize", C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P]),
     ("b200rwkv_op_wkv", C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32] + [_P] * 14),
+    ("b200rwkv_op_gemm", C.c_int32, [C.c_int32] * 7 + [C.POINTER(GemmSeg), C.POINTER(C.c_int32 * 4)]),
     ("b200rwkv_launch_count", C.c_int32, [_P, C.POINTER(C.c_int64)]),
     ("b200rwkv_keep_hidden", C.c_int32, [_P, C.c_int32]),
     ("b200rwkv_last_hidden", C.c_int32, [_P, _P, C.c_size_t]),
@@ -171,3 +183,33 @@ def op_wkv(version: int, r, k, v, w, state, u=None, a=None, k_k=None, k_a=None, 
     check(lib().b200rwkv_op_wkv(device, version, T, H, p(r), p(k), p(v), p(w), p(u), p(a), p(k_k), p(k_a), p(r_k), p(g), p(lnx_w),
                                 p(lnx_b), p(st), p(out)))
     return out, st
+
+
+def gemm_rows(T: int, precision: int = 0) -> int:
+    """Token rows of b200rwkv_op_gemm's outputs: 16 x the token tiles of the kernel the engine runs for T tokens."""
+    if precision == 1:
+        return 32
+    return 16 if T <= 16 else 32 if T <= 32 else 64 if T <= 64 else 128
+
+
+def op_gemm(T: int, segs: list[dict], precision: int = 0, quant_type: int = QUANT_NONE, grid: int = 0, launches: int = 1,
+            device: int = 0):
+    """One projection launch (b200rwkv_op_gemm).  Each segment is a dict: w [N, K] f16, x [launches, T, K] f32, optional bias
+    [N], act, out_mode, grp, xx / sx [launches, T, N] and mu [N] (ddlerp), and out [launches, gemm_rows(T), ldo] (float32 for
+    OUT_F32, uint16 f16 bits otherwise), whose contents are uploaded first and overwritten in place where the kernel writes.
+    Returns the plan: (grid, stage blocks, tiles, most contributing CTAs of one tile)."""
+    f32 = lambda a: None if a is None else np.ascontiguousarray(a, np.float32)
+    keep, arr = [], (GemmSeg * len(segs))()
+    for i, d in enumerate(segs):
+        w = np.ascontiguousarray(d["w"], np.float16)
+        x, bias, xx, sx, mu = (f32(d.get(k)) for k in ("x", "bias", "xx", "sx", "mu"))
+        out = d["out"]
+        assert out.flags.c_contiguous and out.dtype == (np.float32 if d.get("out_mode", OUT_F32) == OUT_F32 else np.uint16)
+        assert x.shape == (launches, T, w.shape[1]) and out.shape[:2] == (launches, gemm_rows(T, precision))
+        keep += [w, x, bias, xx, sx, mu]
+        p = lambda a: None if a is None else ptr(a)
+        arr[i] = GemmSeg(w.shape[0], w.shape[1], p(w), p(x), p(bias), d.get("act", ACT_NONE), d.get("out_mode", OUT_F32),
+                         d.get("grp", 0), p(xx), p(sx), p(mu), out.shape[2], ptr(out))
+    plan = (C.c_int32 * 4)()
+    check(lib().b200rwkv_op_gemm(device, T, precision, quant_type, grid, launches, len(segs), arr, C.byref(plan)))
+    return tuple(plan)

@@ -847,6 +847,21 @@ int b200rwkv_engine::pick_split(int K, int tiles) const {
     return best;
 }
 
+// dynamic shared memory limits of every projection kernel launch_gemm can pick (the quantised ones only for Int8 / NF4 plans)
+static void gemm_smem_limits(int qtype) {
+    CK(cudaFuncSetAttribute(gemm_kernel<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<1, 2>::SMEM_BYTES));
+    CK(cudaFuncSetAttribute(gemm_kernel<2, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<2, 2>::SMEM_BYTES));
+    CK(cudaFuncSetAttribute(gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<2>::SMEM_BYTES));
+    CK(cudaFuncSetAttribute(gemm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<4>::SMEM_BYTES));
+    CK(cudaFuncSetAttribute(gemm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<8>::SMEM_BYTES));
+    if (qtype == QT_INT8 || qtype == QT_NF4) {
+#define QATTR(MT_, QT_) CK(cudaFuncSetAttribute(qgemm_kernel<MT_, QT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, QGemmCfg<MT_, QT_>::SMEM_BYTES))
+        QATTR(1, QT_INT8); QATTR(2, QT_INT8); QATTR(4, QT_INT8); QATTR(8, QT_INT8);
+        QATTR(1, QT_NF4); QATTR(2, QT_NF4); QATTR(4, QT_NF4); QATTR(8, QT_NF4);
+#undef QATTR
+    }
+}
+
 // -----------------------------------------------------------------------------------------
 // model build
 // -----------------------------------------------------------------------------------------
@@ -865,20 +880,12 @@ void b200rwkv_engine::build(const StFile& st) {
 
     CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&sm_stream, cudaStreamNonBlocking));
-    CK(cudaFuncSetAttribute(gemm_kernel<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<1, 2>::SMEM_BYTES));
-    CK(cudaFuncSetAttribute(gemm_kernel<2, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<2, 2>::SMEM_BYTES));
-    CK(cudaFuncSetAttribute(gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<2>::SMEM_BYTES));
-    CK(cudaFuncSetAttribute(gemm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<4>::SMEM_BYTES));
-    CK(cudaFuncSetAttribute(gemm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<8>::SMEM_BYTES));
     if (quant_layers > 0 && quant_type != QT_NONE) {
         REQUIRE(quant_type == QT_INT8 || quant_type == QT_NF4, B200RWKV_ERR_UNSUPPORTED, "quant_type must be Int8 or NF4 (SF4 is not implemented)");
         REQUIRE(world == 1, B200RWKV_ERR_UNSUPPORTED, "quantised layers are single-GPU in this version");
         REQUIRE(precision == 0, B200RWKV_ERR_UNSUPPORTED, "quantised layers run with precision 0 (f16 operands)");
-#define QATTR(MT_, QT_) CK(cudaFuncSetAttribute(qgemm_kernel<MT_, QT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, QGemmCfg<MT_, QT_>::SMEM_BYTES))
-        QATTR(1, QT_INT8); QATTR(2, QT_INT8); QATTR(4, QT_INT8); QATTR(8, QT_INT8);
-        QATTR(1, QT_NF4); QATTR(2, QT_NF4); QATTR(4, QT_NF4); QATTR(8, QT_NF4);
-#undef QATTR
     }
+    gemm_smem_limits(quant_layers > 0 ? quant_type : (int)QT_NONE);
     {   // prefill steps of up to 128 tokens: per-token decay rows of a slot live in dynamic shared memory
         const int wkv_smem_max = 96 * 1024;
         CK(cudaFuncSetAttribute(wkv_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
@@ -2594,6 +2601,169 @@ int32_t b200rwkv_op_wkv(int32_t device, int32_t version, int32_t T, int32_t H, c
     for (int t = 0; t < T; ++t)
         for (int c = 0; c < Cc; ++c) out[(size_t)t * Cc + c] = __half2float(ho[a16_index(t, c, 64)]);
     CK(cudaMemcpy(state, p.state, (size_t)H * 64 * 64 * 4, cudaMemcpyDeviceToHost));
+    API_END
+}
+
+// Operator-level entry for the parity tests: ONE projection plan built by the engine's own planner (make_launch: grid choice,
+// stream-K cuts, workspace slots, repacking or quantisation) over caller-supplied matrices, launched by launch_gemm (kernel
+// per token-tile count, ring size, split operands, programmatic dependent launch) `launches` times back to back, as the
+// engine reuses a plan step after step.  A temporary engine object carries just what those two need.
+int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t quant_type, int32_t grid, int32_t launches,
+                         int32_t nseg, const b200rwkv_gemm_seg* seg, int32_t* plan_out) {
+    API_BEGIN((b200rwkv_engine*)nullptr)
+    REQUIRE(seg && nseg >= 1 && nseg <= GEMM_MAX_SEG, B200RWKV_ERR_INVALID, "nseg must be 1..8");
+    REQUIRE(T >= 1 && T <= A16_MAX_ROWS, B200RWKV_ERR_INVALID, "T must be 1..128");
+    REQUIRE(precision == 0 || precision == 1, B200RWKV_ERR_INVALID, "precision must be 0 or 1");
+    REQUIRE(grid >= 0 && launches >= 1 && launches <= 16, B200RWKV_ERR_INVALID, "grid must be >= 0 and launches 1..16");
+    REQUIRE(quant_type == QT_NONE || quant_type == QT_INT8 || quant_type == QT_NF4, B200RWKV_ERR_UNSUPPORTED, "quant_type must be 0, 1 or 2");
+    REQUIRE(precision == 0 || (T <= 16 && quant_type == QT_NONE), B200RWKV_ERR_UNSUPPORTED,
+            "precision 1 runs decode-shaped steps (T <= 16) over f16 weights");
+    for (int i = 0; i < nseg; ++i) {
+        const b200rwkv_gemm_seg& s = seg[i];
+        const std::string tag = "segment " + std::to_string(i) + ": ";
+        REQUIRE(s.N >= 1 && s.K >= 1 && (int64_t)s.N * s.K <= ((int64_t)1 << 31) && s.w && s.x && s.out, B200RWKV_ERR_INVALID,
+                tag + "bad N / K or a null matrix");
+        REQUIRE(s.act >= ACT_NONE && s.act <= ACT_V7DECAY && s.out_mode >= OUT_F32 && s.out_mode <= OUT_LERP_A16 && s.grp >= 0,
+                B200RWKV_ERR_INVALID, tag + "bad act / out_mode / grp");
+        REQUIRE(s.ldo >= s.N && s.ldo <= (1 << 24), B200RWKV_ERR_INVALID, tag + "ldo must be >= N");
+        REQUIRE(s.out_mode != OUT_LERP_A16 || (s.lerp_xx && s.lerp_sx && s.lerp_mu), B200RWKV_ERR_INVALID, tag + "ddlerp needs xx, sx and mu");
+        REQUIRE(s.out_mode == OUT_F32 || (s.N % 8 == 0 && s.grp % 8 == 0), B200RWKV_ERR_UNSUPPORTED,
+                tag + "f16 outputs are written in chunks of 8 columns: N and grp must be multiples of 8");
+        REQUIRE(quant_type == QT_NONE || s.K % GEMM_BK == 0, B200RWKV_ERR_UNSUPPORTED, tag + "quantised matrices need K % 128 == 0");
+    }
+    const bool split = precision == 1;
+    const int MT = split ? 2 : mt_bucket(T);       // token tiles of the kernel: split operands are the hi and lo tiles of 16 tokens
+    const int th = 16 * MT;                        // token rows of every operand / output in the A16 layout, rows of `out`
+    const int mt_launch = split ? 1 : MT;          // what the engine's step passes to launch_gemm
+    CK(cudaSetDevice(device));
+    std::unique_ptr<b200rwkv_engine> e(new b200rwkv_engine());
+    e->dev = device;
+    CK(cudaDeviceGetAttribute(&e->num_sms, cudaDevAttrMultiProcessorCount, device));
+    e->maxT = th;                                  // sizes the stream-K workspace (make_launch)
+    CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
+    gemm_smem_limits(quant_type);
+    e->d_meta = (int*)e->dalloc(64);               // meta[0] = T: the valid token rows of every launch
+    CK(cudaMemcpy(e->d_meta, &T, 4, cudaMemcpyHostToDevice));
+
+    auto up = [&](const void* h, size_t bytes) {
+        void* d = e->dalloc(bytes, false);
+        CK(cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice));
+        return d;
+    };
+    // f16 destination in the A16 layout: `grp` columns per matrix (one matrix of ldo columns without groups)
+    struct Dst { int grp = 0, nmat = 1; size_t stride = 0; };
+    std::vector<Dst> dst(nseg);
+    std::vector<StTensor> wt(nseg);
+    std::vector<SegDesc> sv(nseg);
+    size_t wmax = 0;
+    for (int i = 0; i < nseg; ++i) {
+        const b200rwkv_gemm_seg& s = seg[i];
+        wt[i].name = "op_gemm." + std::to_string(i);
+        wt[i].dtype = "F16";
+        wt[i].shape = {s.N, s.K};
+        wt[i].data = reinterpret_cast<const uint8_t*>(s.w);
+        wt[i].nbytes = (size_t)s.N * s.K * 2;
+        wmax = std::max(wmax, wt[i].nbytes);
+        SegDesc& d = sv[i];
+        d.t = &wt[i]; d.N = s.N; d.K = s.K;
+        d.proto.out_mode = s.out_mode; d.proto.act = s.act; d.proto.grp = s.out_mode == OUT_F32 ? 0 : s.grp;
+        d.proto.bias = s.bias ? (const float*)up(s.bias, (size_t)s.N * 4) : nullptr;
+        if (s.out_mode == OUT_LERP_A16) { d.proto.aux2 = (const float*)up(s.lerp_mu, (size_t)s.N * 4); d.proto.ld_aux = s.N; }
+        if (s.out_mode != OUT_F32) {
+            Dst& o = dst[i];
+            o.grp = s.grp;
+            const int cols = o.grp > 0 ? o.grp : s.ldo;
+            o.nmat = o.grp > 0 ? cdiv(s.ldo, o.grp) : 1;
+            o.stride = (size_t)cdiv(cols, GEMM_BK) * A16_KB_HALVES;
+            d.proto.grp_stride = (int)o.stride;
+            d.proto.ldo = th;
+        } else {
+            d.proto.ldo = s.ldo;
+        }
+    }
+    CK(cudaMalloc(&e->d_tmp, wmax));               // make_launch uploads each matrix through the engine's staging buffer
+    e->d_tmp_bytes = wmax;
+    GemmLaunch g = e->make_launch(sv, grid, quant_type);
+    e->gemm_ws = (float*)e->dalloc(e->gemm_ws_floats * 4, false);
+    g.p.ws = e->gemm_ws;
+
+    // the plan as launch_gemm will run it, and the cut of every tile by the kernel's own formula
+    const int G = mt_launch >= 4 ? g.grid_wide : g.grid;
+    const unsigned TB = (unsigned)g.p.total_blocks;
+    int maxc = 0;
+    for (int i = 0; i < nseg; ++i) {
+        const GemmSeg& sg = g.p.seg[i];
+        for (int t = 0; t < sg.tiles; ++t) {
+            const unsigned tb0 = (unsigned)(sg.blk_begin + t * sg.KB);
+            const int c_first = (int)(((unsigned long long)(tb0 + 1) * (unsigned)G - 1) / TB);
+            const int c_last = (int)(((unsigned long long)(tb0 + sg.KB) * (unsigned)G - 1) / TB);
+            maxc = std::max(maxc, c_last - c_first + 1);
+        }
+    }
+    REQUIRE(maxc <= g.p.max_contrib, B200RWKV_ERR_INVALID, "internal: a tile has more contributors than workspace slots");
+    if (plan_out) { plan_out[0] = G; plan_out[1] = g.p.total_blocks; plan_out[2] = g.total_tiles; plan_out[3] = maxc; }
+
+    // operands and outputs of every launch; the caller's output contents go up first
+    std::vector<GemmLaunch> runs(launches, g);
+    std::vector<std::vector<uint16_t>> h16(nseg);         // f16 bits of an A16 destination
+    DevTmp xs((size_t)T * std::max_element(seg, seg + nseg, [](const b200rwkv_gemm_seg& a, const b200rwkv_gemm_seg& b) { return a.K < b.K; })->K * 4);
+    for (int l = 0; l < launches; ++l) {
+        for (int i = 0; i < nseg; ++i) {
+            const b200rwkv_gemm_seg& s = seg[i];
+            GemmSeg& sg = runs[l].p.seg[i];
+            __half* a = (__half*)e->dalloc((size_t)sg.KB * A16_KB_HALVES * 2, true);
+            CK(cudaMemcpy(xs.p, s.x + (size_t)l * T * s.K, (size_t)T * s.K * 4, cudaMemcpyHostToDevice));
+            a16_from_f32_kernel<<<(int)std::min<size_t>(((size_t)T * s.K + 255) / 256, (size_t)e->num_sms * 8), 256>>>((const float*)xs.p, T, s.K, th, split, a);
+            CK(cudaGetLastError());
+            CK(cudaDeviceSynchronize());           // xs is refilled by the next upload
+            sg.A = a;
+            const size_t cells = (size_t)th * s.ldo;
+            if (s.out_mode == OUT_F32) {
+                sg.out = up((const float*)s.out + l * cells, cells * 4);
+                continue;
+            }
+            const Dst& o = dst[i];
+            const uint16_t* src = (const uint16_t*)s.out + l * cells;
+            std::vector<uint16_t>& h = h16[i];
+            h.assign(o.stride * o.nmat, 0);
+            for (int m = 0; m < th; ++m)
+                for (int n = 0; n < s.ldo; ++n) {
+                    const int gi = o.grp > 0 ? n / o.grp : 0, nn = n - gi * o.grp;
+                    h[gi * o.stride + a16_index(m, nn, th)] = src[(size_t)m * s.ldo + n];
+                }
+            sg.out = up(h.data(), h.size() * 2);
+            if (s.out_mode == OUT_LERP_A16) {          // all `th` rows exist, as in the engine's activation buffers
+                float* xx = (float*)e->dalloc((size_t)th * s.N * 4, true);
+                float* sx = (float*)e->dalloc((size_t)th * s.N * 4, true);
+                CK(cudaMemcpy(xx, s.lerp_xx + (size_t)l * T * s.N, (size_t)T * s.N * 4, cudaMemcpyHostToDevice));
+                CK(cudaMemcpy(sx, s.lerp_sx + (size_t)l * T * s.N, (size_t)T * s.N * 4, cudaMemcpyHostToDevice));
+                sg.aux0 = xx;
+                sg.aux1 = sx;
+            }
+        }
+    }
+    CK(cudaDeviceSynchronize());                   // every upload has landed before the projection stream starts
+    for (const GemmLaunch& r : runs) e->launch_gemm(r, mt_launch, e->stream, nullptr, split);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(e->stream));
+    for (int l = 0; l < launches; ++l)
+        for (int i = 0; i < nseg; ++i) {
+            const b200rwkv_gemm_seg& s = seg[i];
+            const size_t cells = (size_t)th * s.ldo;
+            if (s.out_mode == OUT_F32) {
+                CK(cudaMemcpy((float*)s.out + l * cells, runs[l].p.seg[i].out, cells * 4, cudaMemcpyDeviceToHost));
+                continue;
+            }
+            const Dst& o = dst[i];
+            std::vector<uint16_t>& h = h16[i];
+            CK(cudaMemcpy(h.data(), runs[l].p.seg[i].out, h.size() * 2, cudaMemcpyDeviceToHost));
+            uint16_t* out = (uint16_t*)s.out + l * cells;
+            for (int m = 0; m < th; ++m)
+                for (int n = 0; n < s.ldo; ++n) {
+                    const int gi = o.grp > 0 ? n / o.grp : 0, nn = n - gi * o.grp;
+                    out[(size_t)m * s.ldo + n] = h[gi * o.stride + a16_index(m, nn, th)];
+                }
+        }
     API_END
 }
 

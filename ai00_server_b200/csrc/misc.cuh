@@ -140,6 +140,17 @@ __global__ void f16_to_f32_kernel(const __half* __restrict__ src, float* __restr
         dst[i] = __half2float(src[i]) * scale + bias;
 }
 
+// f32 rows [T][K] -> a projection operand in the A16 layout of `th` token rows (b200rwkv_op_gemm): f16 rounding, or with `split`
+// the hi / lo pair of common.cuh (hi at row t, lo at row t + 16).  Rows >= T and k >= K are left as they are.
+__global__ void a16_from_f32_kernel(const float* __restrict__ src, int T, int K, int th, bool split, __half* __restrict__ dst) {
+    const size_t n = (size_t)T * K;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const int t = (int)(i / K), k = (int)(i - (size_t)t * K);
+        if (split) split_h(src[i], dst[a16_index(t, k, th)], dst[a16_index(t + 16, k, th)]);
+        else dst[a16_index(t, k, th)] = f2h_sat(src[i]);
+    }
+}
+
 // v5 static decay: w = exp(-exp(time_decay))
 __global__ void decay_table_kernel(const __half* __restrict__ src, float* __restrict__ dst, size_t n) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)

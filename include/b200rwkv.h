@@ -244,6 +244,30 @@ int32_t b200rwkv_op_wkv(int32_t device, int32_t version, int32_t T, int32_t H, c
                         const float* w, const float* u, const float* a, const float* k_k, const float* k_a, const float* r_k,
                         const float* g, const float* lnx_w, const float* lnx_b, float* state, float* out);
 
+/* Operator-level entry (parity tests): one projection launch -- the engine's planner (stream-K cuts, forced grids, Int8 / NF4
+ * quantisation at load) and its projection kernels -- over caller-supplied matrices, no model.  Segment i computes
+ * act(x W^T + bias) with W [N, K] (row-major f16 bits) and x [launches][T][K] f32, rounded to the f16 operand on the device
+ * (precision 0) or split into an f16 hi + lo pair (precision 1: T <= 16, f16 weights).  act: 0 none, 1 tanh, 2 sigmoid,
+ * 3 silu, 4 relu^2, 5 exp(-exp), 6 v7 decay.  out_mode: 0 f32 rows; 1 f16 (the operand layout of a following projection,
+ * `grp` columns per destination matrix, 0 = one matrix); 2 f16 ddlerp  lerp_xx + lerp_sx * (lerp_mu + y)  with lerp_xx /
+ * lerp_sx [launches][T][N] and lerp_mu [N].  out: [launches][rows][ldo], rows = 16 x token tiles (16 / 32 / 64 / 128 by T;
+ * 32 with precision 1, where f16 outputs hold the hi halves in rows 0-15 and the lo halves in rows 16-31), f32 or f16 bits,
+ * de-tiled.  The caller's contents are uploaded first: cells the kernel does not write come back unchanged.
+ * grid 0 = the production plan, > 0 = forced; the plan runs `launches` times back to back on one stream, launch l on input
+ * slice l into output slice l.  plan_out (may be NULL): grid launched, stage blocks, tiles, most CTAs contributing to one tile. */
+typedef struct {
+    int32_t N, K;
+    const uint16_t* w;
+    const float* x;
+    const float* bias;             /* [N] or NULL */
+    int32_t act, out_mode, grp;
+    const float *lerp_xx, *lerp_sx, *lerp_mu;
+    int32_t ldo;                   /* >= N */
+    void* out;
+} b200rwkv_gemm_seg;
+int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t quant_type, int32_t grid, int32_t launches,
+                         int32_t nseg, const b200rwkv_gemm_seg* seg, int32_t* plan_out);
+
 /* Kernels launched by this engine's forward steps since creation (graph replays counted by their kernel nodes). */
 int32_t b200rwkv_launch_count(b200rwkv_engine*, int64_t* total);
 

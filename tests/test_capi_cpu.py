@@ -197,13 +197,70 @@ def test_ctypes_structs_match_the_header(tmp_path):
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     src = tmp_path / "sz.c"
     src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "b200rwkv.h"\n'
-                   'int main(void) { printf("%zu %zu %zu %zu %zu\\n", sizeof(b200rwkv_options), offsetof(b200rwkv_options, devices),\n'
-                   '  offsetof(b200rwkv_options, lora_st), offsetof(b200rwkv_options, quant_layers), sizeof(b200rwkv_info)); return 0; }\n')
+                   'int main(void) { printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b200rwkv_options), offsetof(b200rwkv_options, devices),\n'
+                   '  offsetof(b200rwkv_options, lora_st), offsetof(b200rwkv_options, quant_layers), sizeof(b200rwkv_info),\n'
+                   '  sizeof(b200rwkv_gemm_seg), offsetof(b200rwkv_gemm_seg, act), offsetof(b200rwkv_gemm_seg, lerp_xx),\n'
+                   '  offsetof(b200rwkv_gemm_seg, out)); return 0; }\n')
     exe = tmp_path / "sz"
     subprocess.run([gcc, "-std=c99", "-Wall", "-Werror", "-I", os.path.join(root, "include"), str(src), "-o", str(exe)], check=True)
     got = [int(x) for x in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
-    O = capi.Options
-    assert got == [C.sizeof(O), O.devices.offset, O.lora_st.offset, O.quant_layers.offset, C.sizeof(capi.Info)]
+    O, G = capi.Options, capi.GemmSeg
+    assert got == [C.sizeof(O), O.devices.offset, O.lora_st.offset, O.quant_layers.offset, C.sizeof(capi.Info),
+                   C.sizeof(G), G.act.offset, G.lerp_xx.offset, G.out.offset]
+
+
+def test_op_gemm_refuses_bad_arguments_without_a_gpu():
+    """b200rwkv_op_gemm checks every argument before its first CUDA call, so each refusal returns its status on a machine
+    without a GPU: ERR_INVALID for malformed arguments, ERR_UNSUPPORTED for combinations the projection kernels do not run."""
+    N, K, T = 64, 256, 4
+    w = np.zeros((N, K), np.float16)
+    x = np.zeros((1, T, K), np.float32)
+    out = np.zeros((1, 16, N), np.float32)
+    v = np.zeros((1, T, N), np.float32)
+
+    def seg(**kw):
+        s = capi.GemmSeg(N, K, capi.ptr(w), capi.ptr(x), None, capi.ACT_NONE, capi.OUT_F32, 0, None, None, None, N, capi.ptr(out))
+        for k, val in kw.items():
+            setattr(s, k, val)
+        return s
+
+    def call(segs=None, T=T, precision=0, quant=capi.QUANT_NONE, grid=0, launches=1, nseg=None):
+        segs = [seg()] if segs is None else segs
+        arr = (capi.GemmSeg * len(segs))(*segs)
+        return capi.lib().b200rwkv_op_gemm(0, T, precision, quant, grid, launches, len(segs) if nseg is None else nseg, arr, None)
+
+    INV, UNS = capi.ERR_INVALID, capi.ERR_UNSUPPORTED
+    cases = {
+        "null segment array": (capi.lib().b200rwkv_op_gemm(0, T, 0, 0, 0, 1, 1, None, None), INV),
+        "no segment": (call(nseg=0), INV),
+        "nine segments": (call([seg()] * 9), INV),
+        "T = 0": (call(T=0), INV),
+        "T = 129": (call(T=129), INV),
+        "precision 2": (call(precision=2), INV),
+        "negative grid": (call(grid=-1), INV),
+        "no launch": (call(launches=0), INV),
+        "quant_type 3": (call(quant=3), UNS),
+        "precision 1 at T = 17": (call(T=17, precision=1), UNS),
+        "precision 1 over Int8": (call(T=4, precision=1, quant=capi.QUANT_INT8), UNS),
+        "null weight": (call([seg(w=None)]), INV),
+        "null input": (call([seg(x=None)]), INV),
+        "null output": (call([seg(out=None)]), INV),
+        "N = 0": (call([seg(N=0)]), INV),
+        "ldo < N": (call([seg(ldo=N - 1)]), INV),
+        "unknown activation": (call([seg(act=7)]), INV),
+        "unknown out_mode": (call([seg(out_mode=3)]), INV),
+        "negative grp": (call([seg(out_mode=capi.OUT_A16, grp=-8)]), INV),
+        "ddlerp without mu": (call([seg(out_mode=capi.OUT_LERP_A16, lerp_xx=capi.ptr(v), lerp_sx=capi.ptr(v))]), INV),
+        "f16 output, N % 8": (call([seg(N=60, out_mode=capi.OUT_A16)]), UNS),
+        "f16 output, grp % 8": (call([seg(out_mode=capi.OUT_A16, grp=12)]), UNS),
+        "Int8, K % 128": (call([seg(K=200)], quant=capi.QUANT_INT8), UNS),
+        "NF4, K % 128": (call([seg(), seg(K=96)], quant=capi.QUANT_NF4), UNS),
+        "a bad second segment": (call([seg(), seg(ldo=0)]), INV),
+    }
+    for name, (got, want) in cases.items():
+        assert got == want, name
+    if not _has_gpu():                       # well-formed arguments reach the device, and there is none: no CPU fallback
+        assert call() == capi.ERR_CUDA
 
 
 def test_c_host_program_links_and_calls_the_library(tmp_path):
