@@ -50,6 +50,15 @@ class GemmSeg(C.Structure):
                 ("lerp_xx", C.c_void_p), ("lerp_sx", C.c_void_p), ("lerp_mu", C.c_void_p), ("ldo", C.c_int32), ("out", C.c_void_p)]
 
 
+class WkvArgs(C.Structure):
+    """b200rwkv_wkv_args (include/b200rwkv.h)."""
+    _fields_ = [("version", C.c_int32), ("H", C.c_int32), ("S", C.c_int32), ("nslot", C.c_int32), ("slot", C.c_void_p),
+                ("count", C.c_void_p), ("precision", C.c_int32)] + [
+                (n, C.c_void_p) for n in ("r", "k", "v", "g", "w", "u", "lnx_w", "lnx_b", "a", "k_k", "k_a", "r_k", "nu")] + [
+                ("layer0", C.c_int32), ("v_first", C.c_void_p), ("d1", C.c_void_p), ("time_decay_w2", C.c_void_p),
+                ("decay_bias", C.c_void_p), ("Dd", C.c_int32), ("state", C.c_void_p), ("out", C.c_void_p)]
+
+
 ACT_NONE, ACT_TANH, ACT_SIGMOID, ACT_SILU, ACT_RELU2, ACT_EXPNEGEXP, ACT_V7DECAY = range(7)
 OUT_F32, OUT_A16, OUT_LERP_A16 = 0, 1, 2
 
@@ -92,7 +101,7 @@ SYMBOLS = [
     ("b200rwkv_profile_step", C.c_int32, [_P, C.c_int32, _P, _P, C.POINTER(C.c_float * 4), C.POINTER(C.c_int32 * 4), C.POINTER(C.c_int64)]),
     ("b200rwkv_profile_insitu", C.c_int32, [_P, C.c_int32, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, C.POINTER(C.c_double)]),
     ("b200rwkv_op_quantize", C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P]),
-    ("b200rwkv_op_wkv", C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32] + [_P] * 14),
+    ("b200rwkv_op_wkv", C.c_int32, [C.c_int32, C.POINTER(WkvArgs)]),
     ("b200rwkv_op_gemm", C.c_int32, [C.c_int32] * 7 + [C.POINTER(GemmSeg), C.POINTER(C.c_int32 * 4)]),
     ("b200rwkv_launch_count", C.c_int32, [_P, C.POINTER(C.c_int64)]),
     ("b200rwkv_keep_hidden", C.c_int32, [_P, C.c_int32]),
@@ -170,19 +179,42 @@ def op_quantize(quant_type: int, w16, device: int = 0):
     return (codes, p0, p1) if quant_type == QUANT_INT8 else (codes, p0)
 
 
+def op_wkv_step(version: int, slots, counts, state, out, r, k, v, g, lnx_w, lnx_b, w=None, u=None, a=None, k_k=None, k_a=None,
+                r_k=None, nu=None, layer0: bool = True, v_first=None, d1=None, time_decay_w2=None, decay_bias=None, precision: int = 0,
+                device: int = 0):
+    """One WKV launch of a step (b200rwkv_op_wkv) over a pool of S slots: entry i feeds counts[i] tokens to pool slot slots[i].
+    state [S, H, 64, 64] f32 (M[value][key]), out [gemm_rows(T, precision), H*64] uint16 f16 bits and v7's v_first [T, H*64]
+    f32 are updated in place.  Per-token arrays are [T, H*64] (or [T, H, 64]) f32, per-channel ones [H*64]; d1 [T, Dd] f32 and
+    time_decay_w2 [H*64, Dd] f16 turn on the v6 decay fold."""
+    S, H = state.shape[:2]
+    assert state.dtype == np.float32 and state.flags.c_contiguous and state.shape[2:] == (64, 64)
+    assert out.dtype == np.uint16 and out.flags.c_contiguous and out.shape == (gemm_rows(sum(counts), precision), H * 64)
+    assert v_first is None or (v_first.dtype == np.float32 and v_first.flags.c_contiguous)
+    f32 = lambda x: None if x is None else np.ascontiguousarray(x, np.float32)
+    keep = [np.ascontiguousarray(slots, np.int32), np.ascontiguousarray(counts, np.int32)]
+    keep += [f32(x) for x in (r, k, v, g, w, u, lnx_w, lnx_b, a, k_k, k_a, r_k, nu, d1, decay_bias)]
+    w2 = None if time_decay_w2 is None else np.ascontiguousarray(time_decay_w2, np.float16)
+    p = lambda x: None if x is None else ptr(x)
+    sl, cn, r, k, v, g, w, u, lnx_w, lnx_b, a, k_k, k_a, r_k, nu, d1, decay_bias = keep
+    args = WkvArgs(version, H, S, len(sl), p(sl), p(cn), precision, p(r), p(k), p(v), p(g), p(w), p(u), p(lnx_w), p(lnx_b), p(a),
+                   p(k_k), p(k_a), p(r_k), p(nu), int(layer0), p(v_first), p(d1), p(w2), p(decay_bias),
+                   0 if d1 is None else d1.shape[1], ptr(state), ptr(out))
+    check(lib().b200rwkv_op_wkv(device, C.byref(args)))
+
+
 def op_wkv(version: int, r, k, v, w, state, u=None, a=None, k_k=None, k_a=None, r_k=None, g=None, lnx_w=None, lnx_b=None, device: int = 0):
-    """One launch of the WKV kernel (b200rwkv_op_wkv).  r, k, v: [T, H, 64]; state [H, 64, 64] = M[value][key] (updated copy
-    returned).  Returns (out [T, H, 64] f32, state)."""
+    """One sequence through the WKV kernel (op_wkv_step with one slot; v7 at layer 0).  r, k, v: [T, H, 64]; g None = 1, lnx_w /
+    lnx_b None = 1 / 0; state [H, 64, 64] = M[value][key] (updated copy returned).  Returns (out [T, H, 64] f32, state)."""
     r = np.ascontiguousarray(r, np.float32)
     T, H, _ = r.shape
-    f = lambda x: None if x is None else np.ascontiguousarray(x, np.float32)
-    k, v, w, u, a, k_k, k_a, r_k, g, lnx_w, lnx_b = map(f, (k, v, w, u, a, k_k, k_a, r_k, g, lnx_w, lnx_b))
-    st = np.array(state, np.float32, copy=True, order="C")
-    out = np.empty((T, H, 64), np.float32)
-    p = lambda x: None if x is None else ptr(x)
-    check(lib().b200rwkv_op_wkv(device, version, T, H, p(r), p(k), p(v), p(w), p(u), p(a), p(k_k), p(k_a), p(r_k), p(g), p(lnx_w),
-                                p(lnx_b), p(st), p(out)))
-    return out, st
+    ones = np.ones(H * 64, np.float32)
+    st = np.array(state, np.float32, copy=True, order="C")[None]
+    out = np.zeros((gemm_rows(T), H * 64), np.uint16)
+    v_first = np.zeros((T, H * 64), np.float32) if version == 7 else None
+    op_wkv_step(version, [0], [T], st, out, r, k, v, np.ones((T, H * 64), np.float32) if g is None else g,
+                ones if lnx_w is None else lnx_w, ones * 0 if lnx_b is None else lnx_b, w=w, u=u, a=a, k_k=k_k, k_a=k_a, r_k=r_k,
+                v_first=v_first, device=device)
+    return out[:T].view(np.float16).astype(np.float32).reshape(T, H, 64), st[0]
 
 
 def gemm_rows(T: int, precision: int = 0) -> int:

@@ -53,9 +53,12 @@ __device__ __forceinline__ __half f2h_sat(float v) {
 // Split operand (precision 1 = f32 activations, DESIGN.md §2): a projection input v travels as two f16 numbers hi + lo = v
 // (to ~2^-22 relative); hi sits at token row t, lo at row t + 16 of the same A16 buffer (the second 16-token tile), the
 // projection multiplies both tiles and its epilogue adds the two accumulator tiles.
+// Above |v| = 65504 hi saturates and lo carries the rest; lo saturates as well, so that a finite v never becomes an infinite
+// operand: the pair saturates at +-131008 as the f16 operand does at +-65504.  NaN stays NaN in lo.
 __device__ __forceinline__ void split_h(const float v, __half& hi, __half& lo) {
     hi = f2h_sat(v);
-    lo = __float2half_rn(v - __half2float(hi));
+    const float rest = v - __half2float(hi);
+    lo = __float2half_rn(fabsf(rest) > 65504.f ? copysignf(65504.f, rest) : rest);
 }
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
     __half2 h = __halves2half2(f2h_sat(a), f2h_sat(b));

@@ -536,6 +536,7 @@ struct b200rwkv_engine {
         return d_step_trace + (size_t)STEP_TRACE_ROW * launches_last_step;
     }
     void launch_gemm(const GemmLaunch& g, int MT, cudaStream_t s, Profiler* prof, bool split = false);
+    void launch_wkv(const WkvParams& p, int rows, int th, bool split, cudaStream_t s, Profiler* prof);
     void enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* prof);
     void run_step(int MT, int MTR);
     int fill_meta(int* m, const std::vector<int>& slots, const std::vector<int>& counts, const std::vector<const uint32_t*>& toks,
@@ -834,6 +835,24 @@ void b200rwkv_engine::launch_gemm(const GemmLaunch& g, int MT, cudaStream_t s, P
     }
 }
 
+// The WKV launch of one step of `rows` token rows (16 x token tiles) whose A16 operands hold `th` rows: one CTA per (head, step
+// entry) over min(S, rows) entries (a step has at most one entry per token; CTAs past the step's entries exit), decay rows and
+// staged rows sized by the step shape, since a slot cannot hold more tokens than the step.  `split`: hi + lo output rows.
+void b200rwkv_engine::launch_wkv(const WkvParams& p, int rows, int th, bool split, cudaStream_t s, Profiler* prof) {
+    WkvParams wp = p;
+    wp.kq_tile = th; wp.d1_kq = th;
+    const dim3 grid(wp.H, std::min(S, rows));
+    const size_t sm_b = wkv_smem_bytes(wp.version, wp.version == 6 && wp.wd2t, wp.Dd, rows, split);
+    switch (wp.version * 2 + (split ? 1 : 0)) {
+        case 10: launch_k(wkv_kernel<5>, grid, dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
+        case 11: launch_k(wkv_kernel<5, true>, grid, dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
+        case 12: launch_k(wkv_kernel<6>, grid, dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
+        case 13: launch_k(wkv_kernel<6, true>, grid, dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
+        case 14: launch_k(wkv_kernel<7>, grid, dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
+        default: launch_k(wkv_kernel<7, true>, grid, dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
+    }
+}
+
 // static split-K factor of a row-parallel projection: the S <= 8 / world (partial buffers the LN stages sum) that cuts K
 // into whole 128-wide blocks, gives every CTA whole tiles and puts the most SMs to work.  (Measured, round 2: with the
 // old cap of 4 the 3B channel-mix value projection ran on 40 CTAs, 22 us for 43 MB; 7 slices -> 140 CTAs.)
@@ -862,6 +881,28 @@ static void gemm_smem_limits(int qtype) {
     }
 }
 
+// dynamic shared memory limit of every WKV kernel launch_wkv can pick: prefill steps of up to 128 tokens, the decay-LoRA slice
+// of the v6 fold and the staged rows live there
+static void wkv_smem_limits() {
+    const int wkv_smem_max = 96 * 1024;
+    CK(cudaFuncSetAttribute(wkv_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
+    CK(cudaFuncSetAttribute(wkv_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
+    CK(cudaFuncSetAttribute(wkv_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
+    CK(cudaFuncSetAttribute(wkv_kernel<5, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
+    CK(cudaFuncSetAttribute(wkv_kernel<6, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
+    CK(cudaFuncSetAttribute(wkv_kernel<7, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
+}
+
+// k-major copy of the time_decay_w2 rows c0 .. c0 + 64 Hl - 1 (w2: [C][Dd] f16 as stored), one contiguous [Dd][64] slice per
+// head: the operand of the v6 decay fold inside the WKV kernel
+static std::vector<__half> wd2_k_major(const __half* w2, int c0, int Hl, int Dd) {
+    std::vector<__half> t((size_t)Hl * Dd * 64);
+    for (int h = 0; h < Hl; ++h)
+        for (int k = 0; k < Dd; ++k)
+            for (int c = 0; c < 64; ++c) t[((size_t)h * Dd + k) * 64 + c] = w2[(size_t)(c0 + h * 64 + c) * Dd + k];
+    return t;
+}
+
 // -----------------------------------------------------------------------------------------
 // model build
 // -----------------------------------------------------------------------------------------
@@ -886,15 +927,7 @@ void b200rwkv_engine::build(const StFile& st) {
         REQUIRE(precision == 0, B200RWKV_ERR_UNSUPPORTED, "quantised layers run with precision 0 (f16 operands)");
     }
     gemm_smem_limits(quant_layers > 0 ? quant_type : (int)QT_NONE);
-    {   // prefill steps of up to 128 tokens: per-token decay rows of a slot live in dynamic shared memory
-        const int wkv_smem_max = 96 * 1024;
-        CK(cudaFuncSetAttribute(wkv_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
-        CK(cudaFuncSetAttribute(wkv_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
-        CK(cudaFuncSetAttribute(wkv_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
-        CK(cudaFuncSetAttribute(wkv_kernel<5, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
-        CK(cudaFuncSetAttribute(wkv_kernel<6, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
-        CK(cudaFuncSetAttribute(wkv_kernel<7, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
-    }
+    wkv_smem_limits();
     if (precision == 1) split_act = true;         // f32-activation mode (web-rwkv `Bundle::<f32>`): no activation is rounded to f16
     if (const char* v = dbg_env("B200RWKV_PREFETCH_BLOCKS")) prefetch_blocks = std::max(0, atoi(v));
     if (const char* v = dbg_env("B200RWKV_FUSED_PRE")) fused_pre = atoi(v) != 0;
@@ -1130,11 +1163,7 @@ void b200rwkv_engine::build(const StFile& st) {
                 // k-major copy of this rank's time_decay_w2 rows, one contiguous [Dd][64] slice per head: the WKV
                 // kernels evaluate the decay LoRA stage 2 themselves (one launch / phase less per layer)
                 const StTensor& t = st.get(a + "time_decay_w2");
-                const __half* src = reinterpret_cast<const __half*>(t.data);
-                std::vector<__half> tmp((size_t)Hl * Dd * 64);
-                for (int h = 0; h < Hl; ++h)
-                    for (int k = 0; k < Dd; ++k)
-                        for (int c = 0; c < 64; ++c) tmp[((size_t)h * Dd + k) * 64 + c] = src[(size_t)(c0 + h * 64 + c) * Dd + k];
+                const std::vector<__half> tmp = wd2_k_major(reinterpret_cast<const __half*>(t.data), c0, Hl, Dd);
                 __half* dw = (__half*)dalloc(tmp.size() * 2, false);
                 CK(cudaMemcpy(dw, tmp.data(), tmp.size() * 2, cudaMemcpyHostToDevice));
                 wk.wd2t = dw;
@@ -1404,7 +1433,6 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* pr
             launch_k(ln_mix_kernel, dim3(rows), dim3(LN_THREADS), 0, lp, KC_LN, s, prof);
         }
     };
-    const int wkv_slots = std::min(S, rows);
     for (int l = 0; l < L; ++l) {
         Layer& ly = layers[l];
         const bool fused = fused_pre_ok && MT == 1 && ly.w1_raw;
@@ -1434,20 +1462,9 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* pr
         for (int gi = 0; gi < (int)ly.pre.size(); ++gi)
             if (!pre_skipped(ly, gi)) gemm(ly.pre[gi]);
         {
-            // decays / staged rows are sized by the step shape: a slot cannot hold more tokens than the step
             WkvParams wp = ly.wkv;
             wp.trace = tr_next(2);
-            wp.kq_tile = th; wp.d1_kq = th;
-            const bool sp = split_on && MT == 1;
-            const size_t sm_b = wkv_smem_bytes(info.version, fold_wd2, info.time_decay_adapter, rows, sp);
-            switch (info.version * 2 + (sp ? 1 : 0)) {
-                case 10: launch_k(wkv_kernel<5>, dim3(Hl, wkv_slots), dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
-                case 11: launch_k(wkv_kernel<5, true>, dim3(Hl, wkv_slots), dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
-                case 12: launch_k(wkv_kernel<6>, dim3(Hl, wkv_slots), dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
-                case 13: launch_k(wkv_kernel<6, true>, dim3(Hl, wkv_slots), dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
-                case 14: launch_k(wkv_kernel<7>, dim3(Hl, wkv_slots), dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
-                default: launch_k(wkv_kernel<7, true>, dim3(Hl, wkv_slots), dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
-            }
+            launch_wkv(wp, rows, th, split_on && MT == 1, s, prof);
         }
         gemm(ly.o);
         if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
@@ -2533,74 +2550,121 @@ int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int3
     API_END
 }
 
-// Operator-level entry for the parity tests: ONE launch of the WKV kernel (recurrence + GroupNorm + bonus + gate) on caller
-// supplied head vectors and state, no model around it.  This is how the committed fla fixtures (tests/golden/wkv6_fla.npz,
-// wkv7_fla.npz: independent pins of the recurrences) reach the CUDA kernels.
-int32_t b200rwkv_op_wkv(int32_t device, int32_t version, int32_t T, int32_t H, const float* r, const float* k, const float* v,
-                        const float* w, const float* u, const float* a, const float* k_k, const float* k_a, const float* r_k,
-                        const float* g, const float* lnx_w, const float* lnx_b, float* state, float* out) {
+// Operator-level entry for the parity tests: ONE WKV launch of a step (recurrence + GroupNorm + bonus + gate) on caller-supplied
+// head vectors and state pool, no model around it.  The step metadata comes from the engine's fill_meta on a temporary engine
+// object, the launch from launch_wkv (kernel per version and output form, grid, shared memory, programmatic dependent launch),
+// the k-major decay slice from wd2_k_major and the d1 operand from the f16 conversion of the projection operands: a step runs
+// exactly this.  The committed fla fixtures (tests/golden/wkv6_fla.npz, wkv7_fla.npz) and the float64 reference of
+// tests/test_gpu_wkv.py reach the CUDA kernels through it.
+int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args) {
     API_BEGIN((b200rwkv_engine*)nullptr)
+    REQUIRE(args, B200RWKV_ERR_INVALID, "null arguments");
+    const b200rwkv_wkv_args& x = *args;
+    const int version = x.version;
     REQUIRE(version == 5 || version == 6 || version == 7, B200RWKV_ERR_UNSUPPORTED, "version must be 5, 6 or 7");
-    REQUIRE(T >= 1 && T <= 64 && H >= 1 && H <= 1024 && r && k && v && w && state && out, B200RWKV_ERR_INVALID, "bad argument");
-    REQUIRE(version == 7 ? (a && k_k && k_a && r_k) : (u != nullptr), B200RWKV_ERR_INVALID, "missing per-version operand");
+    REQUIRE(x.H >= 1 && x.H <= 128, B200RWKV_ERR_INVALID, "H must be 1..128 (num_emb <= 8192)");
+    REQUIRE(x.S >= 1 && x.S <= 1024, B200RWKV_ERR_INVALID, "S must be 1..1024 (max_batch)");
+    REQUIRE(x.nslot >= 1 && x.nslot <= x.S && x.slot && x.count, B200RWKV_ERR_INVALID, "nslot must be 1..S with slot and count");
+    REQUIRE(x.precision == 0 || x.precision == 1, B200RWKV_ERR_INVALID, "precision must be 0 or 1");
+    std::vector<char> seen(x.S, 0);
+    int T = 0;
+    for (int i = 0; i < x.nslot; ++i) {
+        REQUIRE(x.slot[i] >= 0 && x.slot[i] < x.S, B200RWKV_ERR_STATE, "slot out of range");
+        REQUIRE(!seen[x.slot[i]], B200RWKV_ERR_INVALID, "duplicate slot in one step");
+        seen[x.slot[i]] = 1;
+        REQUIRE(x.count[i] >= 1 && x.count[i] <= A16_MAX_ROWS - T, B200RWKV_ERR_INVALID, "counts must be >= 1 and sum to <= 128");
+        T += x.count[i];
+    }
+    const bool split = x.precision == 1;
+    REQUIRE(!split || T <= 16, B200RWKV_ERR_UNSUPPORTED, "precision 1 runs decode-shaped steps (T <= 16)");
+    REQUIRE(x.r && x.k && x.v && x.g && x.lnx_w && x.lnx_b && x.state && x.out, B200RWKV_ERR_INVALID, "null r, k, v, g, ln_x, state or out");
+    const bool fold = version == 6 && (x.d1 || x.time_decay_w2 || x.decay_bias);
+    if (fold) {
+        REQUIRE(x.d1 && x.time_decay_w2 && x.decay_bias, B200RWKV_ERR_INVALID, "the decay fold needs d1, time_decay_w2 and decay_bias");
+        REQUIRE(x.Dd >= 8 && x.Dd <= 128 && x.Dd % 8 == 0, B200RWKV_ERR_UNSUPPORTED, "the decay fold needs Dd <= 128 and Dd % 8 == 0");
+    }
+    if (version == 5) REQUIRE(x.w && x.u, B200RWKV_ERR_INVALID, "v5 needs w (static) and u");
+    if (version == 6) REQUIRE((x.w || fold) && x.u, B200RWKV_ERR_INVALID, "v6 needs u and w or the decay fold");
+    if (version == 7) {
+        REQUIRE(x.w && x.a && x.k_k && x.k_a && x.r_k && x.v_first, B200RWKV_ERR_INVALID, "v7 needs w, a, k_k, k_a, r_k and v_first");
+        REQUIRE(x.layer0 || x.nu, B200RWKV_ERR_INVALID, "v7 layers after 0 need nu");
+    }
+
+    const int H = x.H, S = x.S, Cc = H * 64;
+    const int MT = mt_bucket(T), rows = 16 * MT;   // what enqueue_step derives from the step's token count
+    const int th = split ? 32 : rows;
     CK(cudaSetDevice(device));
-    const int Cc = H * 64;
-    const size_t TC = (size_t)T * Cc;
-    std::vector<DevTmp*> keep;
-    struct Guard { std::vector<DevTmp*>& v; ~Guard() { for (auto* p : v) delete p; } } guard{keep};
-    auto up = [&](const float* h, size_t n, float fill) -> float* {
-        keep.push_back(new DevTmp(n * 4));
-        float* d = (float*)keep.back()->p;
-        if (h) CK(cudaMemcpy(d, h, n * 4, cudaMemcpyHostToDevice));
-        else {
-            std::vector<float> tmp(n, fill);
-            CK(cudaMemcpy(d, tmp.data(), n * 4, cudaMemcpyHostToDevice));
-        }
+    std::unique_ptr<b200rwkv_engine> e(new b200rwkv_engine());
+    e->dev = device;
+    e->S = S;                                      // e->maxT stays A16_MAX_ROWS: the metadata layout of every engine
+    CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
+    wkv_smem_limits();
+
+    std::vector<int> slots(x.slot, x.slot + x.nslot), counts(x.count, x.count + x.nslot), outmode(x.nslot, 0);
+    std::vector<uint32_t> tok0(A16_MAX_ROWS, 0);
+    std::vector<const uint32_t*> toks(x.nslot, tok0.data());
+    std::vector<int> meta(MetaView::ints(e->maxT, S), 0);
+    int R = 0;
+    REQUIRE(e->fill_meta(meta.data(), slots, counts, toks, outmode, &R) == T, B200RWKV_ERR_INVALID, "internal: step metadata");
+    e->d_meta = (int*)e->dalloc(meta.size() * 4, false);
+    CK(cudaMemcpy(e->d_meta, meta.data(), meta.size() * 4, cudaMemcpyHostToDevice));
+
+    auto up = [&](const void* h, size_t bytes) {
+        void* d = e->dalloc(bytes, false);
+        CK(cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice));
         return d;
     };
-    const int maxT = 64, maxS = 1;
-    std::vector<int> meta(MetaView::ints(maxT, maxS), 0);
-    meta[0] = T; meta[1] = 1; meta[2] = 0;
-    for (int t = 0; t < T; ++t) {
-        meta[8 + maxT + t] = 0;                       // tok_slot
-        meta[8 + 2 * maxT + t] = t == 0 ? -1 : t - 1; // tok_prev
-        meta[8 + 3 * maxT + t] = t == T - 1;          // tok_last
-        meta[8 + 5 * maxT + t] = -1;                  // tok_outrow
-    }
-    meta[8 + 6 * maxT] = 0; meta[8 + 6 * maxT + maxS] = 0; meta[8 + 6 * maxT + 2 * maxS] = T;
-    keep.push_back(new DevTmp(meta.size() * 4));
-    int* d_meta = (int*)keep.back()->p;
-    CK(cudaMemcpy(d_meta, meta.data(), meta.size() * 4, cudaMemcpyHostToDevice));
+    // per-token rows as the engine's activation buffers hold them: `rows` rows, the ones past T filled with NaN so that a read
+    // outside the step shows in the output
+    auto rows_up = [&](const float* h) -> float* {
+        if (!h) return nullptr;
+        float* d = (float*)e->dalloc((size_t)rows * Cc * 4, false);
+        CK(cudaMemset(d, 0xFF, (size_t)rows * Cc * 4));
+        CK(cudaMemcpy(d, h, (size_t)T * Cc * 4, cudaMemcpyHostToDevice));
+        return d;
+    };
+    auto vec_up = [&](const float* h) { return h ? (const float*)up(h, (size_t)Cc * 4) : nullptr; };
     WkvParams p;
     memset(&p, 0, sizeof(p));
-    p.version = version; p.ld = Cc; p.meta = MetaView{d_meta, maxT, maxS}; p.H = H;
-    p.state = up(state, (size_t)H * 64 * 64, 0.f);
-    p.r = up(r, TC, 0.f); p.k = up(k, TC, 0.f); p.v = up(v, TC, 0.f); p.g = up(g, TC, 1.f);
-    if (version == 5) p.w_static = up(w, Cc, 0.f); else p.w = up(w, TC, 0.f);
-    p.lnx_w = up(lnx_w, Cc, 1.f); p.lnx_b = up(lnx_b, Cc, 0.f);
-    if (version != 7) p.u = up(u, Cc, 0.f);
-    else {
-        p.a = up(a, TC, 0.f); p.nu = up(nullptr, TC, 0.f); p.v_first = up(nullptr, TC, 0.f); p.layer0 = 1;
-        p.k_k = up(k_k, Cc, 0.f); p.k_a = up(k_a, Cc, 0.f); p.r_k = up(r_k, Cc, 0.f);
+    p.version = version; p.ld = Cc; p.meta = MetaView{e->d_meta, e->maxT, S}; p.H = H;
+    const size_t state_bytes = (size_t)S * H * 64 * 64 * 4;
+    p.state = (float*)up(x.state, state_bytes);
+    p.r = rows_up(x.r); p.k = rows_up(x.k); p.v = rows_up(x.v); p.g = rows_up(x.g);
+    if (version == 5) p.w_static = vec_up(x.w);
+    else if (!fold) p.w = rows_up(x.w);
+    p.u = version != 7 ? vec_up(x.u) : nullptr;
+    p.lnx_w = vec_up(x.lnx_w); p.lnx_b = vec_up(x.lnx_b);
+    if (version == 7) {
+        p.a = rows_up(x.a); p.nu = x.layer0 ? nullptr : rows_up(x.nu);
+        p.v_first = rows_up(x.v_first); p.layer0 = x.layer0 != 0;
+        p.k_k = vec_up(x.k_k); p.k_a = vec_up(x.k_a); p.r_k = vec_up(x.r_k);
     }
-    const size_t halves = (size_t)(rup(Cc, GEMM_BK) / GEMM_BK) * A16_KB_HALVES;
-    keep.push_back(new DevTmp(halves * 2));
-    p.out = (__half*)keep.back()->p;
-    p.kq_tile = 64;                       // token rows of the A16 output: any value >= T the reader below agrees on
-    CK(cudaMemset(p.out, 0, halves * 2));
-    const size_t smem = wkv_smem_bytes(version, false, 0, maxT);
-    switch (version) {
-        case 5: wkv_kernel<5><<<dim3(H, 1), WKV_SA_THREADS, smem>>>(p, maxT); break;
-        case 6: wkv_kernel<6><<<dim3(H, 1), WKV_SA_THREADS, smem>>>(p, maxT); break;
-        default: wkv_kernel<7><<<dim3(H, 1), WKV_SA_THREADS, smem>>>(p, maxT); break;
+    if (fold) {
+        const std::vector<__half> wt = wd2_k_major(reinterpret_cast<const __half*>(x.time_decay_w2), 0, H, x.Dd);
+        p.wd2t = (const __half*)up(wt.data(), wt.size() * 2);
+        p.decay_bias = vec_up(x.decay_bias);
+        p.Dd = x.Dd;
+        float* d1 = (float*)up(x.d1, (size_t)T * x.Dd * 4);
+        __half* a16 = (__half*)e->dalloc((size_t)cdiv(x.Dd, GEMM_BK) * A16_KB_HALVES * 2, true);
+        a16_from_f32_kernel<<<cdiv(T * x.Dd, 256), 256>>>(d1, T, x.Dd, th, split, a16);
+        CK(cudaGetLastError());
+        p.d1 = a16;
     }
+    // the output in the A16 layout of `th` token rows, the caller's contents first
+    const size_t halves = (size_t)cdiv(Cc, GEMM_BK) * A16_KB_HALVES;
+    std::vector<uint16_t> h16(halves, 0);
+    for (int m = 0; m < th; ++m)
+        for (int c = 0; c < Cc; ++c) h16[a16_index(m, c, th)] = x.out[(size_t)m * Cc + c];
+    p.out = (__half*)up(h16.data(), halves * 2);
+    CK(cudaDeviceSynchronize());                   // every upload has landed before the launch
+    e->launch_wkv(p, rows, th, split, e->stream, nullptr);
     CK(cudaGetLastError());
-    CK(cudaDeviceSynchronize());
-    std::vector<__half> ho(halves);
-    CK(cudaMemcpy(ho.data(), p.out, halves * 2, cudaMemcpyDeviceToHost));
-    for (int t = 0; t < T; ++t)
-        for (int c = 0; c < Cc; ++c) out[(size_t)t * Cc + c] = __half2float(ho[a16_index(t, c, 64)]);
-    CK(cudaMemcpy(state, p.state, (size_t)H * 64 * 64 * 4, cudaMemcpyDeviceToHost));
+    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaMemcpy(h16.data(), p.out, halves * 2, cudaMemcpyDeviceToHost));
+    for (int m = 0; m < th; ++m)
+        for (int c = 0; c < Cc; ++c) x.out[(size_t)m * Cc + c] = h16[a16_index(m, c, th)];
+    CK(cudaMemcpy(x.state, p.state, state_bytes, cudaMemcpyDeviceToHost));
+    if (version == 7) CK(cudaMemcpy(x.v_first, p.v_first, (size_t)T * Cc * 4, cudaMemcpyDeviceToHost));
     API_END
 }
 

@@ -5,31 +5,26 @@
 // dispatches under `Runtime::infer` (reference run.rs:1143; SURVEY.md §2.2 K6/K6'/K7, math in
 // App. A / App. B).
 //
-// One 256-thread group per (head, slot).  The 64x64 f32 head state (16 KB) lives in HBM as
+// One 128-thread CTA per (head, step entry).  The 64x64 f32 head state (16 KB) lives in HBM as
 // M[value][key] for every version (v6's S[key][value] is stored transposed; the API layout is
 // restored by the state import/export kernels), so that
-//   * each thread owns a 4(value) x 4(key) patch: 4 coalesced 16-byte accesses, rows moved as full
+//   * each thread owns a 4(value) x 8(key) patch: 8 coalesced 16-byte accesses, rows moved as full
 //     256-byte runs;
-//   * every reduction of the recurrence runs over the KEY index = across the 16 lanes of a
-//     half-warp -> pure shuffles, no shared-memory round trip:
+//   * every reduction of the recurrence runs over the KEY index = across the 8 lanes that share a
+//     value row -> pure shuffles, no shared-memory round trip:
 //       v5/v6: out[v] = sum_k r[k] * (u[k] k[k] v[v] + M[v][k]);  M[v][k] = k[k] v[v] + w[k] M[v][k]
 //       v7:    sa[v]  = sum_k M[v][k] * (-kk[k]);
 //              M[v][k] = M[v][k] w[k] + sa[v] (kk[k] a[k]) + v[v] k[k];   out[v] = sum_k M[v][k] r[k]
 //   * state is read once and written once per step, the recurrence loops over the slot's tokens
 //     with the state in registers (prefill chunks).
-// Output: f16( GroupNorm(out) [+ bonus] * gate ) written straight into the A16 operand of the
-// output projection.
-//
-// Two callers share `wkv_slot`: the stand-alone kernel below (one CTA per (head, slot), state
-// through coalesced vector loads) and the persistent whole-step kernel (mega.cuh), where the
-// state tiles arrive through the bulk-TMA stage ring and the v6 decay LoRA is evaluated in place.
+// Output: f16( GroupNorm(out) [+ bonus] * gate ) (or its hi + lo split) written straight into the
+// A16 operand of the output projection.
 #pragma once
 #include "common.cuh"
 
 namespace b200 {
 
-constexpr int WKV_THREADS = 256;
-constexpr int WKV_N = 64;            // head size (all supported RWKV v5/v6/v7 models)
+constexpr int WKV_N = 64;          // head size (all supported RWKV v5/v6/v7 models)
 constexpr float GN_EPS = 64e-5f;
 
 struct WkvParams {
@@ -57,8 +52,8 @@ struct WkvParams {
     const float* r_k;
     __half* out;            // A16 [T, ld]
     int kq_tile;
-    // v6, whole-step kernel only: decay LoRA stage 2 evaluated inside the WKV phase
-    const __half* wd2t;     // [H][Dd][64] f16: time_decay_w2 rows of each head, k-major
+    // v6 decay fold (null wd2t: off): decay LoRA stage 2 evaluated inside the WKV kernel
+    const __half* wd2t;    // [H][Dd][64] f16: time_decay_w2 rows of each head, k-major
     const float* decay_bias;    // [ld] time_decay
     const __half* d1;       // A16 [T, Dd]: tanh(time_decay_w1 @ xw)
     int d1_kq;
@@ -72,11 +67,11 @@ struct WkvShared {
 };
 
 // Runs the recurrence for `nt` tokens starting at token index t0 on head h with the state patch
-// m[4] (rows 4*ig+e, cols 4*j4..) in registers.  `w_local`: optional shared-memory decay rows
-// [token][64] (whole-step kernel, v6) indexed from local token `lt0`.
+// m[4][KC] in registers.  `w_local`: optional shared-memory decay rows [token][64] (the v6 decay
+// fold) indexed from local token `lt0`.
 // `pre`: optional shared-memory copy of the head's per-token vectors, [array][token][64] with arrays
-// r, k, v, g (, w, a, nu for v7) and `pre_stride` floats between arrays (whole-step kernel: gathered
-// once per WKV unit so the per-token loop never waits on L2).
+// r, k, v, g (, w, a, nu for v7) and `pre_stride` floats between arrays (staged runs: gathered in
+// one batch of loads so the per-token loop never waits on L2).
 // KC: key columns per thread (8: 128 threads per head); the thread's patch is m[e][f] = M[4*ig + e][KC*j4 + f].
 template <int VER, int KC = 8, bool SPLIT = false>
 __device__ __forceinline__ void wkv_slot(const WkvParams& p, const int h, const int t0, const int nt, float (&m)[4][KC],

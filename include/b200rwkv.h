@@ -226,13 +226,6 @@ int32_t b200rwkv_profile_insitu(b200rwkv_engine*, int32_t nslot, const int32_t* 
                                 int32_t cap, int32_t* n_out, int32_t* types, double* start_us, double* end_us, int64_t* bytes,
                                 double* step_us);
 
-/* Operator-level entry (parity tests): one launch of the WKV kernel -- recurrence + per-head GroupNorm (eps 64e-5) (+ v7
- * bonus) * gate -- on caller-supplied head vectors, for one sequence of T <= 64 tokens with H heads of size 64; no model.
- * r, k, v, g: [T, H*64] (g NULL = 1); w: decay in (0, 1), [T, H*64] (v5: static [H*64]); u: v5/v6 time_first [H*64];
- * v7: a [T, H*64], k_k / k_a / r_k [H*64] (kk = normalize_head(k * k_k), k <- k * (1 + (a - 1) * k_a), value-residual off);
- * lnx_w / lnx_b [H*64] (NULL = 1 / 0); state: in/out [H][64][64] in the device orientation M[value][key] (v5/v6: the
- * transpose of S[key][value]); out: [T, H*64], the f16 values the kernel hands to the output projection.  The committed
- * flash-linear-attention fixtures (tests/golden/wkv6_fla.npz, wkv7_fla.npz) are checked through this entry. */
 /* Operator-level entry (parity tests): the load-time quantiser on a caller-supplied row-major f16 matrix [N, K] (K % 128 == 0),
  * returned in plain order: codes [N, K] (one byte per element: Int8 code, or NF4 level index 0..15), p0 [N, K/block] (Int8: block
  * minimum, NF4: block absmax), p1 [N, K/block] (Int8: the scale f16((max - min) / 255); NF4: unused, may be NULL).  p0 / p1 are f16
@@ -240,9 +233,39 @@ int32_t b200rwkv_profile_insitu(b200rwkv_engine*, int32_t nslot, const int32_t* 
 int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int32_t K, const uint16_t* w_f16, uint8_t* codes,
                              uint16_t* p0, uint16_t* p1);
 
-int32_t b200rwkv_op_wkv(int32_t device, int32_t version, int32_t T, int32_t H, const float* r, const float* k, const float* v,
-                        const float* w, const float* u, const float* a, const float* k_k, const float* k_a, const float* r_k,
-                        const float* g, const float* lnx_w, const float* lnx_b, float* state, float* out);
+/* Operator-level entry (parity tests): one WKV launch of a forward step -- recurrence + per-head GroupNorm (eps 64e-5)
+ * (+ v7 bonus) * gate, with the step's metadata, grid, kernel choice and launch attributes -- on caller-supplied head vectors
+ * and a state pool, no model.  H heads of size 64 (C = H*64 channels), a pool of S slots, and `nslot` step entries: entry i
+ * feeds count[i] >= 1 tokens to pool slot slot[i] (distinct slots); its tokens are rows sum(count[0..i]) .. of every per-token
+ * array, T = sum(count) <= 128.
+ *   r, k, v, g: [T][C] f32 (g is the gate the output is multiplied by); w: decay in (0, 1), [T][C] (v5: static [C]; v6 with
+ *   the fold: unused); u: v5 / v6 time_first [C]; lnx_w / lnx_b [C]: ln_x weight and bias.
+ *   v7: a [T][C], k_k / k_a / r_k [C] (kk = normalize_head(k * k_k), k <- k * (1 + (a - 1) * k_a), bonus = sum_head(r k r_k));
+ *   v_first [T][C] in/out: layer0 != 0 writes v into it, later layers mix v <- v + (v_first - v) * nu with nu [T][C].
+ *   v6 decay fold (what the engine runs when the decay LoRA rank Dd <= 128, Dd % 8 == 0): pass d1 [T][Dd] f32 (the LoRA's
+ *   tanh stage, rounded to the f16 operand on the device, or hi + lo with precision 1), time_decay_w2 [C][Dd] f16 bits as
+ *   stored in the model, decay_bias [C] (time_decay) and Dd; then w = exp(-exp(decay_bias + time_decay_w2 . d1)).
+ *   state: in/out [S][H][64][64] in the device orientation M[value][key] (v5/v6: the transpose of S[key][value]).
+ *   precision 0: out holds f16 outputs; 1 (T <= 16): split outputs, hi at row t and lo at row t + 16.
+ *   out: [rows][C] f16 bits, de-tiled, rows = 16 x token tiles of the step (16 / 32 / 64 / 128 by T; 32 with precision 1).
+ *   The caller's contents are uploaded first: cells the kernel does not write come back unchanged. */
+typedef struct {
+    int32_t version, H, S, nslot;
+    const int32_t *slot, *count;
+    int32_t precision;
+    const float *r, *k, *v, *g, *w, *u;
+    const float *lnx_w, *lnx_b;
+    const float *a, *k_k, *k_a, *r_k, *nu;
+    int32_t layer0;
+    float* v_first;
+    const float* d1;
+    const uint16_t* time_decay_w2;
+    const float* decay_bias;
+    int32_t Dd;
+    float* state;
+    uint16_t* out;
+} b200rwkv_wkv_args;
+int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args);
 
 /* Operator-level entry (parity tests): one projection launch -- the engine's planner (stream-K cuts, forced grids, Int8 / NF4
  * quantisation at load) and its projection kernels -- over caller-supplied matrices, no model.  Segment i computes

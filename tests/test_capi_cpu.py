@@ -200,13 +200,19 @@ def test_ctypes_structs_match_the_header(tmp_path):
                    'int main(void) { printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b200rwkv_options), offsetof(b200rwkv_options, devices),\n'
                    '  offsetof(b200rwkv_options, lora_st), offsetof(b200rwkv_options, quant_layers), sizeof(b200rwkv_info),\n'
                    '  sizeof(b200rwkv_gemm_seg), offsetof(b200rwkv_gemm_seg, act), offsetof(b200rwkv_gemm_seg, lerp_xx),\n'
-                   '  offsetof(b200rwkv_gemm_seg, out)); return 0; }\n')
+                   '  offsetof(b200rwkv_gemm_seg, out));\n'
+                   '  printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b200rwkv_wkv_args), offsetof(b200rwkv_wkv_args, slot),\n'
+                   '  offsetof(b200rwkv_wkv_args, precision), offsetof(b200rwkv_wkv_args, r), offsetof(b200rwkv_wkv_args, nu),\n'
+                   '  offsetof(b200rwkv_wkv_args, layer0), offsetof(b200rwkv_wkv_args, v_first), offsetof(b200rwkv_wkv_args, Dd),\n'
+                   '  offsetof(b200rwkv_wkv_args, out)); return 0; }\n')
     exe = tmp_path / "sz"
     subprocess.run([gcc, "-std=c99", "-Wall", "-Werror", "-I", os.path.join(root, "include"), str(src), "-o", str(exe)], check=True)
     got = [int(x) for x in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
-    O, G = capi.Options, capi.GemmSeg
+    O, G, W = capi.Options, capi.GemmSeg, capi.WkvArgs
     assert got == [C.sizeof(O), O.devices.offset, O.lora_st.offset, O.quant_layers.offset, C.sizeof(capi.Info),
-                   C.sizeof(G), G.act.offset, G.lerp_xx.offset, G.out.offset]
+                   C.sizeof(G), G.act.offset, G.lerp_xx.offset, G.out.offset,
+                   C.sizeof(W), W.slot.offset, W.precision.offset, W.r.offset, W.nu.offset, W.layer0.offset, W.v_first.offset,
+                   W.Dd.offset, W.out.offset]
 
 
 def test_op_gemm_refuses_bad_arguments_without_a_gpu():
@@ -261,6 +267,78 @@ def test_op_gemm_refuses_bad_arguments_without_a_gpu():
         assert got == want, name
     if not _has_gpu():                       # well-formed arguments reach the device, and there is none: no CPU fallback
         assert call() == capi.ERR_CUDA
+
+
+def test_op_wkv_refuses_bad_arguments_without_a_gpu():
+    """b200rwkv_op_wkv checks every argument before its first CUDA call: ERR_INVALID for malformed arguments, ERR_STATE for a
+    slot outside the pool, ERR_UNSUPPORTED for what the WKV kernels do not run."""
+    H, S, T, Dd = 2, 4, 5, 64
+    Cc = H * 64
+    tok = np.zeros((T, Cc), np.float32)
+    vec = np.zeros(Cc, np.float32)
+    state = np.zeros((S, H, 64, 64), np.float32)
+    out = np.zeros((16, Cc), np.uint16)
+    d1 = np.zeros((T, Dd), np.float32)
+    w2 = np.zeros((Cc, Dd), np.float16)
+    P = capi.ptr
+
+    def args(slots=(1, 3), counts=(2, 3), **kw):
+        sl, cn = np.array(slots, np.int32), np.array(counts, np.int32)
+        a = capi.WkvArgs(version=6, H=H, S=S, nslot=len(sl), slot=P(sl), count=P(cn), precision=0, r=P(tok), k=P(tok), v=P(tok),
+                         g=P(tok), w=P(tok), u=P(vec), lnx_w=P(vec), lnx_b=P(vec), a=P(tok), k_k=P(vec), k_a=P(vec), r_k=P(vec),
+                         nu=P(tok), layer0=1, v_first=P(tok), state=P(state), out=P(out))
+        for k, val in kw.items():
+            setattr(a, k, val)
+        a._keep = (sl, cn)
+        return a
+
+    def call(a):
+        return capi.lib().b200rwkv_op_wkv(0, C.byref(a))
+
+    fold = dict(w=None, d1=P(d1), time_decay_w2=P(w2), decay_bias=P(vec), Dd=Dd)
+    INV, UNS, STA = capi.ERR_INVALID, capi.ERR_UNSUPPORTED, capi.ERR_STATE
+    cases = {
+        "null arguments": (capi.lib().b200rwkv_op_wkv(0, None), INV),
+        "version 4": (call(args(version=4)), UNS),
+        "H = 0": (call(args(H=0)), INV),
+        "H = 129": (call(args(H=129)), INV),
+        "S = 0": (call(args(S=0)), INV),
+        "no entry": (call(args(nslot=0)), INV),
+        "more entries than slots": (call(args(slots=(0, 1, 2, 3, 4), counts=(1,) * 5)), INV),
+        "null slot ids": (call(args(slot=None)), INV),
+        "null counts": (call(args(count=None)), INV),
+        "slot = S": (call(args(slots=(1, 4))), STA),
+        "negative slot": (call(args(slots=(-1, 3))), STA),
+        "duplicate slot": (call(args(slots=(3, 3))), INV),
+        "count 0": (call(args(counts=(2, 0))), INV),
+        "129 tokens": (call(args(counts=(64, 65))), INV),
+        "precision 2": (call(args(precision=2)), INV),
+        "precision 1 at T = 17": (call(args(counts=(8, 9), precision=1)), UNS),
+        "null r": (call(args(r=None)), INV),
+        "null g": (call(args(g=None)), INV),
+        "null ln_x bias": (call(args(lnx_b=None)), INV),
+        "null state": (call(args(state=None)), INV),
+        "null out": (call(args(out=None)), INV),
+        "v5 without u": (call(args(version=5, u=None)), INV),
+        "v5 without w": (call(args(version=5, w=None)), INV),
+        "v6 without w or fold": (call(args(w=None)), INV),
+        "v6 without u": (call(args(u=None)), INV),
+        "fold without decay_bias": (call(args(**dict(fold, decay_bias=None))), INV),
+        "fold without d1": (call(args(**dict(fold, d1=None))), INV),
+        "fold Dd = 0": (call(args(**dict(fold, Dd=0))), UNS),
+        "fold Dd % 8": (call(args(**dict(fold, Dd=60))), UNS),
+        "fold Dd = 136": (call(args(**dict(fold, Dd=136))), UNS),
+        "v7 without a": (call(args(version=7, a=None)), INV),
+        "v7 without w": (call(args(version=7, w=None)), INV),
+        "v7 without r_k": (call(args(version=7, r_k=None)), INV),
+        "v7 without v_first": (call(args(version=7, v_first=None)), INV),
+        "v7 after layer 0 without nu": (call(args(version=7, layer0=0, nu=None)), INV),
+    }
+    for name, (got, want) in cases.items():
+        assert got == want, name
+    if not _has_gpu():                       # well-formed arguments reach the device, and there is none: no CPU fallback
+        for ok in (args(), args(**fold), args(version=5), args(version=7, layer0=0), args(counts=(8, 8), precision=1)):
+            assert call(ok) == capi.ERR_CUDA
 
 
 def test_c_host_program_links_and_calls_the_library(tmp_path):
