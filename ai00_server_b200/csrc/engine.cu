@@ -517,7 +517,11 @@ struct b200rwkv_engine {
     unsigned step_seq = 0;        // step sequence number uploaded as meta[4]
     bool split_on = false;        // precision 1: split (hi + lo f16) projection operands, every step decode-shaped
     bool split_act = false;
-    int prefetch_blocks = 16;     // L2 prefetch depth (32 KB blocks per CTA) into the next projection launch
+    // L2 prefetch depth (32 KB blocks per CTA) into the next projection launch.  Off: on an H100 (50 MB L2, 132 CTAs) every
+    // depth measured made the 7B batch-16 decode step slower -- 7.02 ms/step at 0, 7.29 / 7.45 / 7.53 / 7.59 ms at 4 / 8 / 12 /
+    // 16 blocks (H100 80GB HBM3, 700 W power limit).  16 blocks x 132 CTAs = 69 MB was sized for a 126 MB L2; even 4 blocks
+    // (17 MB) cost the launches more HBM time than the prefetch saves.  The debug build's B200RWKV_PREFETCH_BLOCKS turns it on.
+    int prefetch_blocks = 0;
     bool fused_pre = true, ln_cluster = true;     // decode-shaped cluster kernels of pre6.cuh
     bool fused_pre_ok = false, ln_cluster_ok = false;
     unsigned* pre_gbar = nullptr;
