@@ -17,6 +17,7 @@ LIB_PATH = os.path.join(_HERE, "libb200rwkv.so")
 OK = 0
 ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA, ERR_STATE = -1, -2, -3, -4
 OPTION_LAST, OPTION_FULL, OPTION_NONE = 0, 1, 2
+OPTION_SCORE = 3                # b200rwkv_infer_ex only: per-token log-probabilities and argmax ids, no logits rows
 TP_HANDLE_BYTES = 128
 
 
@@ -63,6 +64,13 @@ ACT_NONE, ACT_TANH, ACT_SIGMOID, ACT_SILU, ACT_RELU2, ACT_EXPNEGEXP, ACT_V7DECAY
 OUT_F32, OUT_A16, OUT_LERP_A16 = 0, 1, 2
 
 
+class InferArgs(C.Structure):
+    """b200rwkv_infer_args (include/b200rwkv.h)."""
+    _fields_ = [("struct_bytes", C.c_uint32), ("nslot", C.c_int32), ("slot", C.c_void_p), ("ntok", C.c_void_p),
+                ("tokens", C.c_void_p), ("option", C.c_void_p), ("logits_out", C.c_void_p), ("logits_cap", C.c_size_t),
+                ("rows_out", C.c_void_p), ("score_out", C.c_void_p), ("argmax_out", C.c_void_p)]
+
+
 class B200Error(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"b200rwkv error {code}: {msg}")
@@ -82,6 +90,7 @@ SYMBOLS = [
     ("b200rwkv_destroy", None, [_P]),
     ("b200rwkv_get_info", C.c_int32, [_P, C.POINTER(Info)]),
     ("b200rwkv_infer", C.c_int32, [_P, C.c_int32, _P, _P, _P, _P, _P, C.c_size_t, _P]),
+    ("b200rwkv_infer_ex", C.c_int32, [_P, C.POINTER(InferArgs)]),
     ("b200rwkv_state_shape", C.c_int32, [_P, C.POINTER(C.c_int64 * 4)]),
     ("b200rwkv_state_init", C.c_int32, [_P, _P]),
     ("b200rwkv_state_load", C.c_int32, [_P, C.c_int32, _P]),

@@ -482,6 +482,10 @@ struct b200rwkv_engine {
     unsigned* tk_out_id = nullptr; float* tk_out_p = nullptr;
     uint8_t *tk_dev = nullptr, *tk_host = nullptr;
     size_t tk_cap = 0;
+    // scoring (b200rwkv_infer_ex, OPTION_SCORE): [ScoreRow x n | score f32 x n | argmax u32 x n], pinned host and device,
+    // n = the call's scored tokens; grown on demand
+    uint8_t *sc_dev = nullptr, *sc_host = nullptr;
+    size_t sc_cap = 0;
     void enqueue_keep(cudaStream_t s, int MTR);
     void sample_topk(int nrows, const int32_t* slots, const int32_t* pen_off, const uint32_t* pen_tok, const float* pen_val,
                      const uint32_t* allow_bits, const int32_t* bias_off, const uint32_t* bias_tok, const float* bias_val,
@@ -545,8 +549,10 @@ struct b200rwkv_engine {
     void run_step(int MT, int MTR);
     int fill_meta(int* m, const std::vector<int>& slots, const std::vector<int>& counts, const std::vector<const uint32_t*>& toks,
                   const std::vector<int>& outmode /*0 none,1 last,2 full*/, int* R_out);
+    // score == nullptr: b200rwkv_infer, which refuses OPTION_SCORE
+    struct ScoreOut { float* score; uint32_t* argmax; };
     void infer(int nslot, const int32_t* slot, const int32_t* ntok, const uint32_t* tokens, const int32_t* option,
-               float* logits_out, size_t cap, int32_t* rows_out);
+               float* logits_out, size_t cap, int32_t* rows_out, const ScoreOut* score = nullptr);
     void state_xform(int slot, bool import, float* snap = nullptr);
 };
 
@@ -564,6 +570,8 @@ b200rwkv_engine::~b200rwkv_engine() {
     if (h_meta) cudaFreeHost(h_meta);
     if (tk_dev) cudaFree(tk_dev);
     if (tk_host) cudaFreeHost(tk_host);
+    if (sc_dev) cudaFree(sc_dev);
+    if (sc_host) cudaFreeHost(sc_host);
     if (step_done) cudaEventDestroy(step_done);
     for (auto& ev : meta_ev) if (ev) cudaEventDestroy(ev);
     if (d_hidden_all) cudaFree(d_hidden_all);
@@ -1490,7 +1498,7 @@ static inline int mt_bucket(int rows) { return rows <= 16 ? 1 : (rows <= 32 ? 2 
 
 // last logits row of every slot of this step -> keep[slot] (rank 0 gathers the vocabulary shards); see sample.cuh
 void b200rwkv_engine::enqueue_keep(cudaStream_t s, int MTR) {
-    if (MTR <= 0 || rank != 0 || !d_keep || Vl % 4 != 0) return;
+    if (MTR <= 0 || rank != 0 || !d_keep) return;
     KeepParams kp;
     memset(&kp, 0, sizeof(kp));
     for (int q = 0; q < world; ++q) kp.shard[q] = (const float*)(peer_base[q] + off_logits);
@@ -1566,22 +1574,27 @@ int b200rwkv_engine::fill_meta(int* m, const std::vector<int>& slots, const std:
 }
 
 void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok, const uint32_t* tokens, const int32_t* option,
-                            float* logits_out, size_t cap, int32_t* rows_out) {
+                            float* logits_out, size_t cap, int32_t* rows_out, const ScoreOut* score) {
     REQUIRE(nslot >= 0 && (nslot == 0 || (slot && ntok && option)), B200RWKV_ERR_INVALID, "infer: null argument");
     REQUIRE(connected, B200RWKV_ERR_INVALID, "tensor-parallel engine is not connected (b200rwkv_tp_connect)");
+    const int max_option = score ? B200RWKV_OPTION_SCORE : B200RWKV_OPTION_NONE;
     std::vector<char> seen(S, 0);
-    size_t total_rows = 0, total_tok = 0;
+    size_t total_rows = 0, total_tok = 0, total_score = 0;
     for (int i = 0; i < nslot; ++i) {
         REQUIRE(slot[i] >= 0 && slot[i] < S, B200RWKV_ERR_STATE, "infer: slot out of range");
         REQUIRE(!seen[slot[i]], B200RWKV_ERR_INVALID, "infer: duplicate slot in one call");
         seen[slot[i]] = 1;
         REQUIRE(ntok[i] >= 0, B200RWKV_ERR_INVALID, "infer: negative token count");
-        REQUIRE(option[i] >= B200RWKV_OPTION_LAST && option[i] <= B200RWKV_OPTION_NONE, B200RWKV_ERR_INVALID, "infer: bad option");
+        REQUIRE(option[i] >= B200RWKV_OPTION_LAST && option[i] <= max_option, B200RWKV_ERR_INVALID, "infer: bad option");
         const int r = (option[i] == B200RWKV_OPTION_FULL) ? ntok[i] : ((option[i] == B200RWKV_OPTION_LAST && ntok[i] > 0) ? 1 : 0);
         if (rows_out) rows_out[i] = r;
         total_rows += (size_t)r;
         total_tok += (size_t)ntok[i];
+        if (option[i] == B200RWKV_OPTION_SCORE) total_score += (size_t)ntok[i];
     }
+    const bool any_score = score && std::any_of(option, option + nslot, [](int32_t o) { return o == B200RWKV_OPTION_SCORE; });
+    REQUIRE(!any_score || score->score, B200RWKV_ERR_INVALID, "infer_ex: score_out is NULL but the call has SCORE entries");
+    REQUIRE(!any_score || world == 1, B200RWKV_ERR_UNSUPPORTED, "infer_ex: OPTION_SCORE is not supported under tensor parallelism");
     REQUIRE(total_tok == 0 || tokens, B200RWKV_ERR_INVALID, "infer: null tokens");
     for (size_t i = 0; i < total_tok; ++i)
         REQUIRE(tokens[i] < (uint32_t)V, B200RWKV_ERR_INVALID, "infer: token id " + std::to_string(tokens[i]) + " is outside the vocabulary");
@@ -1601,6 +1614,42 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         const int r = (option[i] == B200RWKV_OPTION_FULL) ? ntok[i] : ((option[i] == B200RWKV_OPTION_LAST && ntok[i] > 0) ? 1 : 0);
         row_base[i + 1] = row_base[i] + (size_t)r;
     }
+    // SCORE entries: score index of token j of entry i is score_base[i] + j.  Token 0 is scored from the slot's kept row,
+    // token j >= 1 from the row the step produced after token j - 1 (the entry's last row gets no target).  Each scoring
+    // launch reads its own slice of the pinned row list (never rewritten within the call).
+    std::vector<size_t> score_base(nslot + 1, 0);
+    for (int i = 0; i < nslot; ++i) score_base[i + 1] = score_base[i] + (option[i] == B200RWKV_OPTION_SCORE ? (size_t)ntok[i] : 0);
+    ScoreRow* sc_rows = nullptr;
+    size_t sc_used = 0;
+    auto launch_score = [&](size_t first, size_t n) {
+        if (n == 0) return;
+        ScoreParams sp;
+        sp.rows = reinterpret_cast<const ScoreRow*>(sc_dev) + first;
+        sp.V = V;
+        sp.score = reinterpret_cast<float*>(sc_dev + total_score * sizeof(ScoreRow));
+        sp.argmax = reinterpret_cast<unsigned*>(sc_dev + total_score * (sizeof(ScoreRow) + 4));
+        CK(cudaMemcpyAsync(sc_dev + first * sizeof(ScoreRow), sc_rows + first, n * sizeof(ScoreRow), cudaMemcpyHostToDevice, stream));
+        score_rows_kernel<<<(unsigned)n, SCORE_THREADS, 0, stream>>>(sp);
+        CK(cudaGetLastError());
+    };
+    if (total_score > 0) {
+        const size_t want = total_score * (sizeof(ScoreRow) + 8);
+        if (want > sc_cap) {
+            if (sc_dev) { CK(cudaFree(sc_dev)); sc_dev = nullptr; }
+            if (sc_host) { CK(cudaFreeHost(sc_host)); sc_host = nullptr; }
+            sc_cap = 0;
+            const size_t bytes = std::max<size_t>(want, 256 * (sizeof(ScoreRow) + 8));
+            CK(cudaMalloc(&sc_dev, bytes));
+            CK(cudaMallocHost(&sc_host, bytes));
+            sc_cap = bytes;
+        }
+        sc_rows = reinterpret_cast<ScoreRow*>(sc_host);
+        std::lock_guard<std::mutex> lk(keep_mu);
+        for (int i = 0; i < nslot; ++i)
+            if (option[i] == B200RWKV_OPTION_SCORE && ntok[i] > 0)
+                sc_rows[sc_used++] = {keep_valid[slot[i]] ? d_keep + (size_t)slot[i] * V : nullptr, tokens[base[i]], (unsigned)score_base[i]};
+    }
+    launch_score(0, sc_used);          // before the first step replaces the kept rows
     if (hidden_keep && total_tok > hidden_cap_rows) {
         if (d_hidden_all) { CK(cudaFree(d_hidden_all)); d_hidden_all = nullptr; hidden_cap_rows = 0; }
         const size_t want = std::max<size_t>(total_tok, 256);
@@ -1638,8 +1687,12 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
             s_slots.push_back(slot[i]);
             s_toks.push_back(tokens + base[i] + pos[i]);
             const bool finishes = (pos[i] + s_counts[j] == ntok[i]);
-            s_out.push_back(option[i] == B200RWKV_OPTION_FULL ? 2 : ((finishes && option[i] == B200RWKV_OPTION_LAST) ? 1 : 0));
+            // SCORE runs the head exactly as FULL does (same step graph, same kept row): only where the rows go differs
+            const bool all_rows = option[i] == B200RWKV_OPTION_FULL || option[i] == B200RWKV_OPTION_SCORE;
+            s_out.push_back(all_rows ? 2 : ((finishes && option[i] == B200RWKV_OPTION_LAST) ? 1 : 0));
         }
+        auto dev_rows = [&](size_t j) { return s_out[j] == 2 ? s_counts[j] : (s_out[j] == 1 ? 1 : 0); };
+        auto scored = [&](size_t j) { return option[s_entry[j]] == B200RWKV_OPTION_SCORE; };
         // pinned metadata ring: a buffer is rewritten only after the copy that read it has completed
         const int mb = step_no % META_RING;
         if (step_no >= META_RING) CK(cudaEventSynchronize(meta_ev[mb]));
@@ -1659,6 +1712,21 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
                 t0 += s_counts[j];
             }
         }
+        if (sc_rows) {       // this step's SCORE rows, scored against each entry's next token
+            const size_t first = sc_used;
+            int r = 0;
+            for (size_t j = 0; j < s_entry.size(); ++j) {
+                const int i = s_entry[j];
+                if (scored(j))
+                    for (int t = 0; t < s_counts[j]; ++t) {
+                        const int p = pos[i] + t;
+                        if (p + 1 < ntok[i])
+                            sc_rows[sc_used++] = {d_logits + (size_t)(r + t) * V, tokens[base[i] + p + 1], (unsigned)(score_base[i] + p + 1)};
+                    }
+                r += dev_rows(j);
+            }
+            launch_score(first, sc_used - first);
+        }
         CK(cudaEventRecord(step_done, stream));
         if (R > 0) {
             std::lock_guard<std::mutex> lk(keep_mu);
@@ -1667,21 +1735,23 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         }
         if (R > 0 && copy_logits) {
             // rows of this step sit in entry order in d_logits; an entry's rows land at its own place of the entry-major
-            // output, runs that are contiguous on both sides go out as one copy
+            // output, runs that are contiguous on both sides go out as one copy (SCORE rows stay on the device)
             int r0 = 0;
             size_t j = 0;
             while (j < s_entry.size()) {
                 const int i = s_entry[j];
-                int nr = s_out[j] == 2 ? s_counts[j] : (s_out[j] == 1 ? 1 : 0);
+                int nr = dev_rows(j);
                 if (nr == 0) { ++j; continue; }
+                if (scored(j)) { r0 += nr; ++j; continue; }
                 const size_t dst = row_base[i] + (size_t)rows_done[i];
                 int run = nr;
                 rows_done[i] += nr;
                 size_t k = j + 1;
                 while (k < s_entry.size()) {
                     const int i2 = s_entry[k];
-                    const int nr2 = s_out[k] == 2 ? s_counts[k] : (s_out[k] == 1 ? 1 : 0);
+                    const int nr2 = dev_rows(k);
                     if (nr2 == 0) { ++k; continue; }
+                    if (scored(k)) break;
                     if (row_base[i2] + (size_t)rows_done[i2] != dst + (size_t)run) break;
                     rows_done[i2] += nr2;
                     run += nr2;
@@ -1702,7 +1772,14 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         for (size_t j = 0; j < s_entry.size(); ++j) pos[s_entry[j]] += s_counts[j];
         ++step_no;
     }
+    if (total_score > 0)      // scores and argmax ids of the whole call: one copy
+        CK(cudaMemcpyAsync(sc_host + total_score * sizeof(ScoreRow), sc_dev + total_score * sizeof(ScoreRow), total_score * 8,
+                           cudaMemcpyDeviceToHost, stream));
     CK(cudaStreamSynchronize(stream));
+    if (total_score > 0) {
+        memcpy(score->score, sc_host + total_score * sizeof(ScoreRow), total_score * 4);
+        if (score->argmax) memcpy(score->argmax, sc_host + total_score * (sizeof(ScoreRow) + 4), total_score * 4);
+    }
     if (hidden_keep) hidden_rows = (int)total_tok;
 }
 
@@ -2061,12 +2138,13 @@ int32_t b200rwkv_get_info(b200rwkv_engine* e, b200rwkv_info* out) {
 }
 
 static int32_t rank_infer(b200rwkv_engine* e, int32_t nslot, const int32_t* slot, const int32_t* ntok, const uint32_t* tokens,
-                       const int32_t* option, float* logits_out, size_t logits_cap, int32_t* rows_out) {
+                       const int32_t* option, float* logits_out, size_t logits_cap, int32_t* rows_out,
+                       const b200rwkv_engine::ScoreOut* score = nullptr) {
     API_BEGIN(e)
     REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
     std::lock_guard<std::mutex> lk(e->mu);
     CK(cudaSetDevice(e->dev));
-    e->infer(nslot, slot, ntok, tokens, option, logits_out, logits_cap, rows_out);
+    e->infer(nslot, slot, ntok, tokens, option, logits_out, logits_cap, rows_out, score);
     API_END
 }
 
@@ -3095,6 +3173,21 @@ int32_t b200rwkv_infer(b200rwkv_engine* e, int32_t nslot, const int32_t* slot, c
                        const int32_t* option, float* logits_out, size_t logits_cap, int32_t* rows_out) {
     return RANKS(e, rank_infer(er, nslot, slot, ntok, tokens, option, r_ == 0 ? logits_out : nullptr, r_ == 0 ? logits_cap : 0,
                                r_ == 0 ? rows_out : nullptr));
+}
+static int32_t check_infer_args(const b200rwkv_infer_args* a) {
+    API_BEGIN((b200rwkv_engine*)nullptr)
+    REQUIRE(a, B200RWKV_ERR_INVALID, "infer_ex: null args");
+    REQUIRE(a->struct_bytes == sizeof(b200rwkv_infer_args), B200RWKV_ERR_INVALID,
+            "infer_ex: struct_bytes is " + std::to_string(a->struct_bytes) + ", expected sizeof(b200rwkv_infer_args) = " +
+            std::to_string(sizeof(b200rwkv_infer_args)));
+    API_END
+}
+int32_t b200rwkv_infer_ex(b200rwkv_engine* e, const b200rwkv_infer_args* a) {
+    const int32_t st = check_infer_args(a);
+    if (st < 0) return st;
+    const b200rwkv_engine::ScoreOut sc{a->score_out, a->argmax_out};
+    return RANKS(e, rank_infer(er, a->nslot, a->slot, a->ntok, a->tokens, a->option, r_ == 0 ? a->logits_out : nullptr,
+                               r_ == 0 ? a->logits_cap : 0, r_ == 0 ? a->rows_out : nullptr, &sc));
 }
 int32_t b200rwkv_state_load(b200rwkv_engine* e, int32_t slot, const float* in) { return RANKS(e, rank_state_load(er, slot, in)); }
 

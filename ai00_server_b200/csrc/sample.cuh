@@ -203,11 +203,104 @@ __global__ void __launch_bounds__(KEEP_THREADS) keep_rows_kernel(const __grid_co
     pdl_wait();
     if (!live) return;
     float* dst = p.keep + (size_t)slot * p.V;
-    const int n4 = p.Vl >> 2;       // Vl % 4 == 0 is checked by the host
+    const int n4 = p.Vl >> 2;
+    const int i0 = blockIdx.y * KEEP_THREADS + threadIdx.x;
     for (int q = 0; q < p.world; ++q) {
-        const float4* src = reinterpret_cast<const float4*>(p.shard[q] + (size_t)r * p.Vl);
-        float4* d4 = reinterpret_cast<float4*>(dst + (size_t)q * p.Vl);
-        for (int i = blockIdx.y * KEEP_THREADS + threadIdx.x; i < n4; i += KEEP_CHUNKS * KEEP_THREADS) d4[i] = __ldcg(src + i);
+        const float* s = p.shard[q] + (size_t)r * p.Vl;
+        float* d = dst + (size_t)q * p.Vl;
+        // Vl % 4 == 0: every row is 16-byte aligned on both sides.  Otherwise rows start anywhere: float4 loads, scalar stores
+        // where the destination row is not aligned the same way, scalar loads where the source row is not aligned at all.
+        const bool s_al = (reinterpret_cast<uintptr_t>(s) & 15) == 0, d_al = (reinterpret_cast<uintptr_t>(d) & 15) == 0;
+        for (int i = i0; i < n4; i += KEEP_CHUNKS * KEEP_THREADS) {
+            const float4 v = s_al ? __ldcg(reinterpret_cast<const float4*>(s) + i)
+                                  : make_float4(__ldcg(s + 4 * i), __ldcg(s + 4 * i + 1), __ldcg(s + 4 * i + 2), __ldcg(s + 4 * i + 3));
+            if (d_al) reinterpret_cast<float4*>(d)[i] = v;
+            else { d[4 * i] = v.x; d[4 * i + 1] = v.y; d[4 * i + 2] = v.z; d[4 * i + 3] = v.w; }
+        }
+        if (i0 < (p.Vl & 3)) d[4 * n4 + i0] = __ldcg(s + 4 * n4 + i0);      // scalar tail
+    }
+}
+
+// ---------------------------------------------------------------------------------------
+// Scoring (b200rwkv_infer_ex, B200RWKV_OPTION_SCORE): for each listed row, log softmax(row)[target] and the row's argmax
+// (lowest id on ties, the sample_topk order), so a caller that wants the probability of a known continuation -- the
+// reference's perplexity() and choose paths, run.rs:699-755 / 936-983 -- receives 8 bytes per token instead of a num_vocab
+// f32 row.  One CTA per row; the row was just written by the head (L2 resident) or is a slot's kept row, and is read once.
+//   score = (x_t - m) - logf(sum expf(x - m)),  m = row max   (the reference's exp(x) / sum exp(x), run.rs:738, overflows in
+//   f32 above a logit of about 88; elsewhere the two agree to f32 rounding)
+// Element i of the row always goes to thread (i / 4) % SCORE_THREADS, in the same order, whatever the row's address: the
+// result of a row does not depend on where it sits in d_logits or which rows share the launch.  src == nullptr (a slot with
+// no kept row): NaN and UINT32_MAX.
+// ---------------------------------------------------------------------------------------
+struct ScoreRow {
+    const float* src;           // [V]
+    unsigned target;            // token whose log-probability is wanted
+    unsigned dst;               // index into score / argmax
+};
+struct ScoreParams {
+    const ScoreRow* rows;
+    int V;
+    float* score;
+    unsigned* argmax;
+};
+constexpr int SCORE_THREADS = 256;
+
+struct ScoreAcc {
+    float m, s;                 // running max, sum expf(x - m)
+    float bx;                   // best logit, its lowest id
+    unsigned bi;
+    __device__ __forceinline__ void add(const float x, const unsigned i) {
+        if (x > m) { s = s * expf(m - x) + 1.f; m = x; }
+        else if (x > -INFINITY) s += expf(x - m);
+        if (x > bx || (x == bx && i < bi)) { bx = x; bi = i; }
+    }
+    __device__ __forceinline__ void merge(const ScoreAcc& o) {
+        const float M = fmaxf(m, o.m);
+        if (M > -INFINITY) s = (m > -INFINITY ? s * expf(m - M) : 0.f) + (o.m > -INFINITY ? o.s * expf(o.m - M) : 0.f);
+        m = M;
+        if (o.bx > bx || (o.bx == bx && o.bi < bi)) { bx = o.bx; bi = o.bi; }
+    }
+    __device__ __forceinline__ ScoreAcc shfl_xor(const int lane_mask) const {
+        return {__shfl_xor_sync(0xffffffffu, m, lane_mask), __shfl_xor_sync(0xffffffffu, s, lane_mask),
+                __shfl_xor_sync(0xffffffffu, bx, lane_mask), __shfl_xor_sync(0xffffffffu, bi, lane_mask)};
+    }
+};
+
+__global__ void __launch_bounds__(SCORE_THREADS) score_rows_kernel(const __grid_constant__ ScoreParams p) {
+    __shared__ ScoreAcc red[SCORE_THREADS / 32];
+    const ScoreRow rw = p.rows[blockIdx.x];
+    const int tid = threadIdx.x;
+    if (rw.src == nullptr) {
+        if (tid == 0) { p.score[rw.dst] = __int_as_float(0x7fc00000); p.argmax[rw.dst] = 0xFFFFFFFFu; }
+        return;
+    }
+    ScoreAcc a{-INFINITY, 0.f, -INFINITY, 0xFFFFFFFFu};
+    const int n4 = p.V >> 2;
+    const float* s = rw.src;
+    if ((reinterpret_cast<uintptr_t>(s) & 15) == 0) {
+        const float4* s4 = reinterpret_cast<const float4*>(s);
+        for (int g = tid; g < n4; g += SCORE_THREADS) {
+            const float4 v = __ldcg(s4 + g);
+            a.add(v.x, 4 * g); a.add(v.y, 4 * g + 1); a.add(v.z, 4 * g + 2); a.add(v.w, 4 * g + 3);
+        }
+    } else {
+        for (int g = tid; g < n4; g += SCORE_THREADS)
+            for (int k = 0; k < 4; ++k) a.add(__ldcg(s + 4 * g + k), 4 * g + k);
+    }
+    if (tid < (p.V & 3)) a.add(__ldcg(s + 4 * n4 + tid), 4 * n4 + tid);      // scalar tail
+    // fixed-order combine: xor tree inside each warp, then warp 0 over the warps' results
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a.merge(a.shfl_xor(o));
+    if ((tid & 31) == 0) red[tid >> 5] = a;
+    __syncthreads();
+    if (tid < 32) {
+        a = (tid < SCORE_THREADS / 32) ? red[tid] : ScoreAcc{-INFINITY, 0.f, -INFINITY, 0xFFFFFFFFu};
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a.merge(a.shfl_xor(o));
+        if (tid == 0) {
+            p.score[rw.dst] = (__ldcg(s + rw.target) - a.m) - logf(a.s);
+            p.argmax[rw.dst] = a.bi;
+        }
     }
 }
 

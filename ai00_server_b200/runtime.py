@@ -313,6 +313,53 @@ class Model:
             off += r
         return res
 
+    # ---- raw call with scoring: one b200rwkv_infer_ex ----
+    def infer_ex(self, slots, ntok, tokens, options):
+        """b200rwkv_infer_ex: `options` may also hold capi.OPTION_SCORE.  Returns (rows, scores): rows per entry as infer_raw
+        returns them (0 rows for SCORE entries); scores[i] is (log-probabilities f32 [ntok[i]], argmax ids uint32 [ntok[i]])
+        for a SCORE entry, None otherwise.  Token 0 of a SCORE entry is scored from the slot's kept row (NaN if it has none)."""
+        V = self.info["num_vocab"]
+        n = len(slots)
+        total = sum(nt if o == capi.OPTION_FULL else (1 if (o == capi.OPTION_LAST and nt > 0) else 0)
+                    for nt, o in zip(ntok, options))
+        nscore = sum(nt for nt, o in zip(ntok, options) if o == capi.OPTION_SCORE)
+        out = np.empty((max(total, 1), V), np.float32)
+        score = np.empty(max(nscore, 1), np.float32)
+        argmax = np.empty(max(nscore, 1), np.uint32)
+        a_slot, a_ntok = np.asarray(slots, np.int32), np.asarray(ntok, np.int32)
+        a_tok, a_opt = np.asarray(tokens, np.uint32), np.asarray(options, np.int32)
+        a_rows = np.zeros(max(n, 1), np.int32)
+        args = capi.InferArgs(C.sizeof(capi.InferArgs), n, capi.ptr(a_slot).value, capi.ptr(a_ntok).value, capi.ptr(a_tok).value,
+                              capi.ptr(a_opt).value, capi.ptr(out).value, out.size, capi.ptr(a_rows).value, capi.ptr(score).value,
+                              capi.ptr(argmax).value)
+        capi.check(capi.lib().b200rwkv_infer_ex(self._h, C.byref(args)), self._h)
+        rows, scores, off, soff = [], [], 0, 0
+        for i in range(n):
+            r = int(a_rows[i])
+            rows.append(out[off:off + r])
+            off += r
+            if options[i] == capi.OPTION_SCORE:
+                scores.append((score[soff:soff + ntok[i]], argmax[soff:soff + ntok[i]]))
+                soff += ntok[i]
+            else:
+                scores.append(None)
+        return rows, scores
+
+    def perplexity(self, slot: int, tokens, head: float | None = None) -> float:
+        """The reference's `perplexity()` (run.rs:699-755) on one SCORE call, quirks included: without `head` a token 0 is
+        fed first (its own score is not used) and the sum is divided by len(tokens) + 1; with `head` (the probability of
+        tokens[0] the caller already holds) the first term is ln(head), the kept row's score of tokens[0] is not used, and the
+        divisor is len(tokens).  Run on the slot's current state, which it advances like the reference's Full run does."""
+        tokens = [int(t) for t in tokens]
+        fed = tokens if head is not None else [0] + tokens
+        _, scores = self.infer_ex([slot], [len(fed)], fed, [capi.OPTION_SCORE])
+        logp = [np.float32(np.log(np.float32(head)))] if head is not None else []
+        logp += [np.float32(x) for x in scores[0][0][1:len(fed)]]
+        total = np.float32(0.0)
+        for x in logp:                         # `.sum()` over f32 in order, as the iterator does
+            total = np.float32(total + x)
+        return float(np.float32(-total / np.float32(len(fed))))
+
     def softmax(self, tensors):
         """`softmax(&context, Vec<TensorCpu<f32>>)`: list of [V] rows in, list out."""
         if not tensors:

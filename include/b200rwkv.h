@@ -145,6 +145,33 @@ int32_t b200rwkv_infer(b200rwkv_engine*, int32_t nslot, const int32_t* slot, con
                        const uint32_t* tokens, const int32_t* option, float* logits_out,
                        size_t logits_cap, int32_t* rows_out);
 
+/* b200rwkv_infer plus scoring on the device: what the reference's perplexity() and choose path (run.rs:699-755, 936-983)
+ * compute from RnnOption::Full rows, without moving those rows to the host.  A SCORE entry i with tokens x_0 .. x_{n-1}:
+ *   - consumes its tokens as FULL does: the slot's state and kept row (the last row, what b200rwkv_sample_topk reads) are
+ *     bit-identical to the same call with FULL;
+ *   - rows_out[i] = 0: no logits row goes to `logits_out`;
+ *   - score_out[j] = log softmax(row predicting x_j)[x_j] in f32, computed as (x_t - m) - logf(sum expf(x - m)), m the row
+ *     maximum; the row predicting x_j is the row after x_{j-1} for j >= 1, and the slot's kept row for j = 0 (from the
+ *     previous infer call, or from b200rwkv_state_write of a snapshot that carries a row; none: NaN);
+ *   - argmax_out[j] = id of the largest logit of that row, lowest id on ties (UINT32_MAX if there is no row).
+ * score_out / argmax_out hold sum(ntok) over the SCORE entries, in entry order; argmax_out may be NULL.  LAST, FULL, NONE and
+ * SCORE entries mix freely in one call.  Every argument is checked before the first CUDA call.  Tensor parallel engines answer
+ * B200RWKV_ERR_UNSUPPORTED for SCORE entries.  b200rwkv_infer refuses option 3. */
+#define B200RWKV_OPTION_SCORE 3
+typedef struct {
+    uint32_t struct_bytes;          /* = sizeof(b200rwkv_infer_args) */
+    int32_t nslot;
+    const int32_t *slot, *ntok;
+    const uint32_t* tokens;
+    const int32_t* option;
+    float* logits_out;              /* exactly as b200rwkv_infer */
+    size_t logits_cap;
+    int32_t* rows_out;
+    float* score_out;               /* [sum of ntok over SCORE entries], entry order */
+    uint32_t* argmax_out;           /* same shape, may be NULL */
+} b200rwkv_infer_args;
+int32_t b200rwkv_infer_ex(b200rwkv_engine*, const b200rwkv_infer_args* args);
+
 /* `State` trait object — crates/ai00-core/src/lib.rs:399,494; uses at run.rs:477,1099-1107.
  * The host-visible state of one slot is an f32 tensor of web-rwkv shape [C, N+2, L, 1]
  * (x fastest; run.rs:987): row 0 time-mix shift, rows 1..N WKV, row N+1 channel-mix shift. */
