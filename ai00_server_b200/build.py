@@ -9,7 +9,6 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200rwkv.so")
-LIB_DEBUG = os.path.join(HERE, "libb200rwkv_dbg.so")      # -DB200RWKV_DEBUG: micro-benchmarks + environment switches
 SYNTH = os.path.join(HERE, "_synthfill.so")
 ORACLE_C = os.path.join(ROOT, "oracle", "liboracle_ref.so")
 
@@ -31,16 +30,14 @@ def _run(cmd: list[str]) -> None:
     subprocess.check_call(cmd)
 
 
-def build_engine(force: bool = False, verbose_ptxas: bool = False, debug: bool = False) -> str:
+def build_engine(force: bool = False, verbose_ptxas: bool = False) -> str:
     srcs = [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC)) if f.endswith((".cu", ".cuh"))]
     srcs.append(os.path.join(ROOT, "include", "b200rwkv.h"))
-    target = LIB_DEBUG if debug else LIB
-    if force or not _newer(target, srcs):
+    if force or not _newer(LIB, srcs):
         nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-        cmd = [nvcc] + NVCC_FLAGS + (["-DB200RWKV_DEBUG"] if debug else []) + (["-Xptxas", "-v"] if verbose_ptxas else []) + [
-            os.path.join(CSRC, "engine.cu"), "-o", target]
+        cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose_ptxas else []) + [os.path.join(CSRC, "engine.cu"), "-o", LIB]
         _run(cmd)
-    return target
+    return LIB
 
 
 def build_synth(force: bool = False) -> str:
@@ -67,5 +64,3 @@ def build_all(force: bool = False) -> None:
 
 if __name__ == "__main__":
     build_all(force="--force" in sys.argv)
-    if "--debug" in sys.argv:
-        build_engine(force="--force" in sys.argv, debug=True)

@@ -121,24 +121,7 @@ SYMBOLS = [
     ("b200rwkv_last_error", C.c_char_p, [_P]),
 ]
 
-# debug build only (libb200rwkv_dbg.so): micro-benchmarks; the B200RWKV_* environment switches are honoured there
-DEBUG_SYMBOLS = [
-    ("b200rwkv_debug_stream", C.c_int32, [C.c_int32, C.c_int32, C.c_double, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float)]),
-    ("b200rwkv_debug_prefetch", C.c_int32, [C.c_int32, C.c_double, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_int32, C.POINTER(C.c_float)]),
-]
-DEBUG_LIB_PATH = os.path.join(_HERE, "libb200rwkv_dbg.so")
-
 _lib = None
-
-
-def debug_lib() -> C.CDLL:
-    """The debug build (python -m ai00_server_b200.build --debug): micro-benchmarks and environment switches."""
-    l = C.CDLL(DEBUG_LIB_PATH)
-    for name, res, args in SYMBOLS + DEBUG_SYMBOLS:
-        fn = getattr(l, name)
-        fn.restype = res
-        fn.argtypes = args
-    return l
 
 
 def lib() -> C.CDLL:

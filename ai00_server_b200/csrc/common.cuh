@@ -145,10 +145,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, unsigne
     SpinGuard g;
     while (!mbar_try(bar, parity)) g.poll(WD_MBAR, bar, parity, tag);
 }
-// fire-and-forget request to bring [p, p + bytes) into L2 (bytes % 16 == 0)
-__device__ __forceinline__ void bulk_prefetch_l2(const void* p, uint32_t bytes) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
-}
 // L2 policy for streamed-once weights
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
     uint64_t pol;

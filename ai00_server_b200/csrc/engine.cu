@@ -26,9 +26,6 @@
 #include "sample.cuh"
 #include "misc.cuh"
 #include "mix.cuh"
-#ifdef B200RWKV_DEBUG
-#include "streamtest.cuh"
-#endif
 #include "wkv.cuh"
 
 namespace b200 {
@@ -53,17 +50,6 @@ struct Error : std::runtime_error {
     } while (0)
 
 static thread_local std::string g_err;
-
-// Bring-up switches exist only in the debug build (-DB200RWKV_DEBUG, `python -m ai00_server_b200.build --debug` ->
-// libb200rwkv_dbg.so): the product library ignores the environment entirely.
-static inline const char* dbg_env(const char* name) {
-#ifdef B200RWKV_DEBUG
-    return getenv(name);
-#else
-    (void)name;
-    return nullptr;
-#endif
-}
 
 // watchdog record in mapped pinned host memory (see common.cuh)
 static unsigned* g_wd_host = nullptr;
@@ -418,7 +404,6 @@ struct b200rwkv_engine {
     int dev = 0, rank = 0, world = 1, num_sms = 132;
     int S = 0, chunk = 0, maxT = A16_MAX_ROWS, precision = 0;      // steps of up to 128 tokens
     int L = 0, C = 0, F = 0, V = 0, H = 0, N = 64, Cl = 0, Hl = 0, Fl = 0, Vl = 0;
-    bool use_graph = true, use_pdl = true;
     int split_att = 1, split_ffn = 1;
     // tensor parallel: one symmetric comm block per rank (partials, gate block, logits shard, flags)
     uint8_t* comm_base = nullptr;
@@ -518,19 +503,12 @@ struct b200rwkv_engine {
     void launch_k(void (*kern)(P, X...), dim3 grid, dim3 block, size_t smem, const P& params, int cls, cudaStream_t s, Profiler* prof,
                   X... extra);
     bool fold_wd2 = false;
-    unsigned step_seq = 0;        // step sequence number uploaded as meta[4]
     bool split_on = false;        // precision 1: split (hi + lo f16) projection operands, every step decode-shaped
     bool split_act = false;
-    // L2 prefetch depth (32 KB blocks per CTA) into the next projection launch.  Off: on an H100 (50 MB L2, 132 CTAs) every
-    // depth measured made the 7B batch-16 decode step slower -- 7.02 ms/step at 0, 7.29 / 7.45 / 7.53 / 7.59 ms at 4 / 8 / 12 /
-    // 16 blocks (H100 80GB HBM3, 700 W power limit).  16 blocks x 132 CTAs = 69 MB was sized for a 126 MB L2; even 4 blocks
-    // (17 MB) cost the launches more HBM time than the prefetch saves.  The debug build's B200RWKV_PREFETCH_BLOCKS turns it on.
-    int prefetch_blocks = 0;
-    bool fused_pre = true, ln_cluster = true;     // decode-shaped cluster kernels of pre6.cuh
-    bool fused_pre_ok = false, ln_cluster_ok = false;
+    bool fused_pre_ok = false, ln_cluster_ok = false;     // decode-shaped cluster kernels of pre6.cuh fit the model
     unsigned* pre_gbar = nullptr;
     int launch_cluster = 0;                       // consumed by the next launch_k
-    // profiling aid (B200RWKV_STEP_TRACE=1): 8 globaltimer stamps of CTA 0 per launch of the per-op chain
+    // profiling aid (b200rwkv_profile_insitu): 8 globaltimer stamps of CTA 0 per launch of the per-op chain
     unsigned long long* d_step_trace = nullptr;
     std::vector<int> step_trace_types;
     static constexpr int STEP_TRACE_MAX = 1024;
@@ -686,8 +664,6 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
     GemmLaunch g;
     memset(&g.p, 0, sizeof(g.p));
     g.qtype = qtype;
-    g.p.qvar = 1;
-    if (const char* v = dbg_env("B200RWKV_QVAR")) g.p.qvar = atoi(v);
     const size_t blk_bytes = (size_t)q_block_bytes(qtype);
     int blk = 0, tile = 0, kbmax = 0;
     for (size_t i = 0; i < segs.size(); ++i) {
@@ -801,7 +777,7 @@ void b200rwkv_engine::launch_k(void (*kern)(P, X...), dim3 grid, dim3 block, siz
         ++na;
         launch_cluster = 0;
     }
-    if (use_pdl && !prof) {
+    if (!prof) {
         at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         at[na].val.programmaticStreamSerializationAllowed = 1;
         ++na;
@@ -869,7 +845,6 @@ void b200rwkv_engine::launch_wkv(const WkvParams& p, int rows, int th, bool spli
 // into whole 128-wide blocks, gives every CTA whole tiles and puts the most SMs to work.  (Measured, round 2: with the
 // old cap of 4 the 3B channel-mix value projection ran on 40 CTAs, 22 us for 43 MB; 7 slices -> 140 CTAs.)
 int b200rwkv_engine::pick_split(int K, int tiles) const {
-    if (dbg_env("B200RWKV_NOSPLIT")) return 1;
     const int kb = K / GEMM_BK;
     if (K % GEMM_BK != 0) return 1;
     int best = 1;
@@ -941,9 +916,6 @@ void b200rwkv_engine::build(const StFile& st) {
     gemm_smem_limits(quant_layers > 0 ? quant_type : (int)QT_NONE);
     wkv_smem_limits();
     if (precision == 1) split_act = true;         // f32-activation mode (web-rwkv `Bundle::<f32>`): no activation is rounded to f16
-    if (const char* v = dbg_env("B200RWKV_PREFETCH_BLOCKS")) prefetch_blocks = std::max(0, atoi(v));
-    if (const char* v = dbg_env("B200RWKV_FUSED_PRE")) fused_pre = atoi(v) != 0;
-    if (const char* v = dbg_env("B200RWKV_LN_CLUSTER")) ln_cluster = atoi(v) != 0;
 
     // ---- step metadata ----
     meta_ints = MetaView::ints(maxT, S);
@@ -985,11 +957,7 @@ void b200rwkv_engine::build(const StFile& st) {
         d_logits = (float*)(comm_base + off_logits);
         d_epoch = (unsigned*)dalloc(16, true);
         pre_gbar = (unsigned*)dalloc(256, true);
-        if (dbg_env("B200RWKV_STEP_TRACE")) {
-            d_step_trace = (unsigned long long*)dalloc((size_t)STEP_TRACE_MAX * STEP_TRACE_ROW * 8, true);
-            trace_capture = true;
-        }
-        ln_cluster_ok = ln_cluster && C % (4 * PRE_CLUSTER) == 0 && C / (4 * PRE_CLUSTER) <= PRE_THREADS;
+        ln_cluster_ok = C % (4 * PRE_CLUSTER) == 0 && C / (4 * PRE_CLUSTER) <= PRE_THREADS;
         split_on = split_act && ln_cluster_ok;
         REQUIRE(precision != 1 || split_on, B200RWKV_ERR_UNSUPPORTED, "precision 1 needs num_emb to be a multiple of 32 and <= 8192");
     }
@@ -1133,7 +1101,7 @@ void b200rwkv_engine::build(const StFile& st) {
                         "time_mix_w2 must be [5, C, Dm]");
                 REQUIRE(d2.shape.size() == 2 && d2.shape[0] == C && d2.shape[1] == Dd, B200RWKV_ERR_INVALID, "time_decay_w2 must be [C, Dd]");
             }
-            if (fused_pre && (Dm == 32 || Dm == 64) && C % 128 == 0 && C <= PRE_MAX_C) {
+            if ((Dm == 32 || Dm == 64) && C % 128 == 0 && C <= PRE_MAX_C) {
                 auto upload_raw = [&](const StTensor& t) {
                     __half* d = (__half*)dalloc(t.nbytes, false);
                     CK(cudaMemcpy(d, t.data, t.nbytes, cudaMemcpyHostToDevice));
@@ -1171,7 +1139,7 @@ void b200rwkv_engine::build(const StFile& st) {
                 ly.wd2_index = (int)ly.pre.size();
                 ly.pre.push_back(make_launch(sv));
             }
-            if (Dd <= 128 && Dd % 8 == 0 && !dbg_env("B200RWKV_NOFOLD")) {
+            if (Dd <= 128 && Dd % 8 == 0) {
                 // k-major copy of this rank's time_decay_w2 rows, one contiguous [Dd][64] slice per head: the WKV
                 // kernels evaluate the decay LoRA stage 2 themselves (one launch / phase less per layer)
                 const StTensor& t = st.get(a + "time_decay_w2");
@@ -1397,41 +1365,17 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* pr
         if (fold_wd2 && gi == ly.wd2_index) return true;                 // the WKV kernel evaluates the decay LoRA stage 2
         return fused_pre_ok && MT == 1 && ly.w1_raw && gi < 2;           // the front-half kernel holds both ddlerp LoRA stages
     };
-    // projection launches of this step in stream order: each one prefetches the head of the next into L2 (the last one
-    // wraps around to the first launch of the next step)
-    std::vector<const GemmLaunch*> seq;
-    if (prefetch_blocks > 0) {
-        for (int l = 0; l < L; ++l) {
-            const Layer& ly = layers[l];
-            for (int gi = 0; gi < (int)ly.pre.size(); ++gi)
-                if (!pre_skipped(ly, gi)) seq.push_back(&ly.pre[gi]);
-            seq.push_back(&ly.o);
-            for (auto& g : ly.ffn) seq.push_back(&g);
-        }
-        if (MTR > 0) seq.push_back(&head);
-    }
-    size_t seq_pos = 0;
-    auto launch_gemm_chained = [&](const GemmLaunch& g, int mt) {
+    auto gemm = [&](const GemmLaunch& g, int mt) {
         GemmLaunch g2 = g;
         if (d_step_trace && trace_capture) {
             g2.p.trace = tr_next(1000000 + (int)(g.weight_bytes >> 20));
             if ((long long)step_trace_bytes.size() <= launches_last_step) step_trace_bytes.resize(launches_last_step + 1, 0);
             step_trace_bytes[launches_last_step] = (long long)g.weight_bytes;
         }
-        if (!seq.empty()) {
-            REQUIRE(seq_pos < seq.size() && seq[seq_pos] == &g, B200RWKV_ERR_INVALID, "internal: projection launch order");
-            const GemmLaunch& nx = *seq[(seq_pos + 1) % seq.size()];
-            ++seq_pos;
-            g2.p.next_W = nx.qtype == QT_NONE ? nx.p.W : nullptr;     // the L2 prefetch walks 32 KB f16 blocks
-            g2.p.next_blocks = nx.p.total_blocks;
-            g2.p.next_grid = mt >= 4 ? nx.grid_wide : nx.grid;
-            g2.p.prefetch_blocks = prefetch_blocks;
-        }
         for (int i = 0; i < g2.p.nseg; ++i)
             if (g2.p.seg[i].out_mode != OUT_F32) g2.p.seg[i].ldo = th;      // A16 outputs feed a projection of this step
         launch_gemm(g2, mt, s, prof, split_on && MT == 1);      // split operands only when the whole step is decode-shaped
     };
-    auto gemm = [&](const GemmLaunch& g) { launch_gemm_chained(g, MT); };
     launch_k(embed_ln0_kernel, dim3(rows), dim3(LN_THREADS), 0, embed, KC_LN, s, prof);
     auto launch_ln = [&](const LnMixParams& lp0) {
         LnMixParams lp = lp0;
@@ -1472,16 +1416,16 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* pr
             launch_ln(ly.ln1);
         }
         for (int gi = 0; gi < (int)ly.pre.size(); ++gi)
-            if (!pre_skipped(ly, gi)) gemm(ly.pre[gi]);
+            if (!pre_skipped(ly, gi)) gemm(ly.pre[gi], MT);
         {
             WkvParams wp = ly.wkv;
             wp.trace = tr_next(2);
             launch_wkv(wp, rows, th, split_on && MT == 1, s, prof);
         }
-        gemm(ly.o);
+        gemm(ly.o, MT);
         if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
         launch_ln(ly.ln2);
-        for (auto& g : ly.ffn) gemm(g);
+        for (auto& g : ly.ffn) gemm(g, MT);
         if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
     }
     {
@@ -1490,7 +1434,7 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* pr
         if (split_on && MT == 1) launch_k(ln_out_kernel<true>, dim3(rows), dim3(LN_THREADS), 0, lo, KC_LN, s, prof);
         else launch_k(ln_out_kernel<false>, dim3(rows), dim3(LN_THREADS), 0, lo, KC_LN, s, prof);
     }
-    if (MTR > 0) launch_gemm_chained(head, MTR);
+    if (MTR > 0) gemm(head, MTR);
     if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
 }
 
@@ -1509,12 +1453,6 @@ void b200rwkv_engine::enqueue_keep(cudaStream_t s, int MTR) {
 }
 
 void b200rwkv_engine::run_step(int MT, int MTR) {
-    if (!use_graph) {
-        enqueue_step(stream, MT, MTR, nullptr);
-        enqueue_keep(stream, MTR);
-        launch_total += launches_last_step;
-        return;
-    }
     const int key = MT * 8 + MTR;
     auto it = graphs.find(key);
     if (it == graphs.end()) {
@@ -1568,7 +1506,6 @@ int b200rwkv_engine::fill_meta(int* m, const std::vector<int>& slots, const std:
         }
     }
     m[0] = T; m[1] = (int)slots.size(); m[2] = R;
-    m[4] = (int)++step_seq;   // identical on every rank (SPMD): epoch base of the folded rendezvous
     *R_out = R;
     return T;
 }
@@ -2027,8 +1964,6 @@ static int32_t create_rank(const uint8_t* st, size_t len, int32_t device, int32_
     REQUIRE(quant_layers >= 0 && quant_type >= 0, B200RWKV_ERR_INVALID, "bad quant_layers / quant_type");
     e->quant_layers = quant_type == QT_NONE ? 0 : quant_layers;
     e->quant_type = quant_layers == 0 ? (int)QT_NONE : quant_type;
-    if (const char* v = dbg_env("B200RWKV_GRAPH")) e->use_graph = atoi(v) != 0;
-    if (const char* v = dbg_env("B200RWKV_PDL")) e->use_pdl = atoi(v) != 0;
     e->build(f);
     e->loras.clear();            // the LoRA images are only borrowed during the build
     *out = e.release();
@@ -2518,7 +2453,6 @@ static int32_t rank_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int3
     CK(cudaMemcpyAsync(e->d_meta, all.data(), e->meta_ints * 4, cudaMemcpyHostToDevice, e->stream));
     const int MT = mt_bucket(nslot);
     // traced copy of the step graph (the production graphs carry null trace pointers)
-    const bool was = e->trace_capture;
     e->trace_capture = true;
     e->step_trace_types.clear();
     e->step_trace_bytes.clear();
@@ -2530,10 +2464,10 @@ static int32_t rank_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int3
     } catch (...) {
         cudaStreamEndCapture(e->stream, &g);
         if (g) cudaGraphDestroy(g);
-        e->trace_capture = was;
+        e->trace_capture = false;
         throw;
     }
-    e->trace_capture = was;
+    e->trace_capture = false;
     CK(cudaStreamEndCapture(e->stream, &g));
     CK(cudaGraphInstantiate(&ge, g, 0));
     CK(cudaGraphDestroy(g));
@@ -2545,8 +2479,6 @@ static int32_t rank_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int3
     e->step_trace_bytes.resize(n, 0);
     for (int r = 0; r < reps + 1; ++r) {        // first replay is warm-up
         CK(cudaMemsetAsync(e->d_step_trace, 0, (size_t)n * row * 8, e->stream));
-        build_decode_metas(e, nslot, slot, tokens, 1, all);      // a fresh step sequence number: the folded rendezvous keys on it
-        CK(cudaMemcpyAsync(e->d_meta, all.data(), e->meta_ints * 4, cudaMemcpyHostToDevice, e->stream));
         CK(cudaGraphLaunch(ge, e->stream));
         CK(cudaStreamSynchronize(e->stream));
         if (r == 0) continue;
@@ -3070,101 +3002,6 @@ int32_t b200rwkv_debug_gemm_time(b200rwkv_engine* e, int32_t which, int32_t reps
     *bytes_out = (int64_t)pick(0).weight_bytes;
     API_END
 }
-
-#ifdef B200RWKV_DEBUG
-// Streaming micro-benchmark (see streamtest.cuh).  kind 0: vector loads; kind 1: bulk-TMA ring.
-int32_t b200rwkv_debug_stream(int32_t device, int32_t kind, double gbytes, int32_t stage_bytes, int32_t nstage, int32_t use_hint,
-                              int32_t split, int32_t producers, int32_t reps, float* ms_out) {
-    int32_t extra = 0;
-    if (stage_bytes % 16384 != 0 && stage_bytes > 16384) { extra = stage_bytes % 16384; }
-    API_BEGIN((b200rwkv_engine*)nullptr)
-    REQUIRE(ms_out && reps >= 1, B200RWKV_ERR_INVALID, "bad argument");
-    CK(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    CK(cudaGetDeviceProperties(&prop, device));
-    const int G = prop.multiProcessorCount;
-    size_t per_cta = (size_t)(gbytes * 1e9 / G);
-    per_cta = per_cta / stage_bytes * stage_bytes;
-    const size_t total = per_cta * G;
-    uint8_t* buf = nullptr;
-    unsigned* sink = nullptr;
-    CK(cudaMalloc(&buf, total + 1024));
-    CK(cudaMalloc(&sink, 4));
-    CK(cudaMemset(buf, 0, total));
-    cudaEvent_t a, b;
-    CK(cudaEventCreate(&a));
-    CK(cudaEventCreate(&b));
-    StreamParams sp;
-    sp.src = buf; sp.bytes_per_cta = per_cta; sp.stage_bytes = stage_bytes; sp.nstage = nstage; sp.use_hint = use_hint;
-    sp.split = split; sp.producers = producers; sp.extra = extra;
-    const size_t smem = (size_t)nstage * stage_bytes + 2 * nstage * 8 + 64;
-    if (kind == 1) CK(cudaFuncSetAttribute(stream_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    for (int r = 0; r < reps + 1; ++r) {
-        if (r == 1) CK(cudaEventRecord(a));
-        if (kind == 0) stream_ldg_kernel<<<G * 8, 256>>>(reinterpret_cast<const uint4*>(buf), total / 16, sink);
-        else stream_ring_kernel<<<G, 128, smem>>>(sp);
-        CK(cudaGetLastError());
-    }
-    CK(cudaEventRecord(b));
-    CK(cudaDeviceSynchronize());
-    float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, a, b));
-    *ms_out = ms / reps;
-    CK(cudaFree(buf));
-    CK(cudaFree(sink));
-    API_END
-}
-
-// L2 prefetch micro-benchmark (streamtest.cuh): per rep { flush L2 by streaming another buffer; prefetch kernel (+ idle);
-// timed streaming kernel }.  ms_out[0] = streaming kernel alone (events around it), ms_out[1] = prefetch + idle + stream.
-int32_t b200rwkv_debug_prefetch(int32_t device, double mbytes, int32_t consumers, int32_t pf_grid, int32_t skip, int32_t nblk,
-                                int32_t mode, double idle_us, int32_t reps, float* ms_out) {
-    API_BEGIN((b200rwkv_engine*)nullptr)
-    REQUIRE(ms_out && reps >= 1 && consumers >= 1 && pf_grid >= 1, B200RWKV_ERR_INVALID, "bad argument");
-    CK(cudaSetDevice(device));
-    const int stage = 32768, nstage = 5;
-    size_t per_cta = (size_t)(mbytes * 1e6 / consumers) / stage * stage;
-    const size_t total = per_cta * consumers;
-    int nsm = 0;
-    CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
-    const size_t flush_bytes = (size_t)nsm * stage * 64;       // 2 MB per SM through the same ring kernel, several times the L2
-    uint8_t *buf = nullptr, *fl = nullptr;
-    CK(cudaMalloc(&buf, total + 1024));
-    CK(cudaMalloc(&fl, flush_bytes + 1024));
-    CK(cudaMemset(buf, 0, total));
-    CK(cudaMemset(fl, 0, flush_bytes));
-    const size_t smem = (size_t)nstage * stage + 2 * nstage * 8 + 64;
-    CK(cudaFuncSetAttribute(stream_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    StreamParams sp;
-    memset(&sp, 0, sizeof(sp));
-    sp.src = buf; sp.bytes_per_cta = per_cta; sp.stage_bytes = stage; sp.nstage = nstage; sp.use_hint = 1; sp.split = 1; sp.producers = 1;
-    StreamParams fp = sp;
-    fp.src = fl; fp.bytes_per_cta = (size_t)stage * 64;
-    cudaEvent_t a, b, c;
-    CK(cudaEventCreate(&a)); CK(cudaEventCreate(&b)); CK(cudaEventCreate(&c));
-    double s0 = 0, s1 = 0;
-    for (int r = 0; r < reps + 1; ++r) {
-        stream_ring_kernel<<<nsm, 128, smem>>>(fp);
-        CK(cudaEventRecord(a));
-        prefetch_probe_kernel<<<pf_grid, 128>>>(buf, per_cta, consumers, skip, nblk, mode, (unsigned long long)(idle_us * 1e3));
-        CK(cudaEventRecord(b));
-        stream_ring_kernel<<<consumers, 128, smem>>>(sp);
-        CK(cudaEventRecord(c));
-        CK(cudaDeviceSynchronize());
-        CK(cudaGetLastError());
-        float m0 = 0.f, m1 = 0.f;
-        CK(cudaEventElapsedTime(&m0, b, c));
-        CK(cudaEventElapsedTime(&m1, a, c));
-        if (r > 0) { s0 += m0; s1 += m1; }
-    }
-    ms_out[0] = (float)(s0 / reps);
-    ms_out[1] = (float)(s1 / reps);
-    CK(cudaFree(buf)); CK(cudaFree(fl));
-    cudaEventDestroy(a); cudaEventDestroy(b); cudaEventDestroy(c);
-    API_END
-}
-
-#endif   // B200RWKV_DEBUG
 
 // ---- exported SPMD entries: one rank, or all ranks of an in-process tensor-parallel engine at once ----
 #define RANKS(e, call_r) ((e) && (e)->group ? (e)->group->spmd([&](int r_) -> int32_t { b200rwkv_engine* er = (e)->group->ranks[r_]; (void)er; return call_r; }) : [&]() -> int32_t { b200rwkv_engine* er = (e); const int r_ = 0; (void)r_; return call_r; }())

@@ -88,12 +88,6 @@ struct GemmParams {
     const int* nrows;       // device: valid token rows
     uint32_t w_lbo, w_sbo, a_lbo, a_sbo;   // wgmma descriptor strides (bytes)
     unsigned long long* trace;             // profiling aid: 8 globaltimer stamps of CTA 0 (null in production)
-    // L2 prefetch of the NEXT projection launch of the step (set per launch by the engine): when this CTA's producer
-    // has requested its last block it asks L2 for the first `prefetch_blocks` blocks the same CTA index will stream in
-    // that launch, so HBM keeps working through this launch's tail, the launch boundary and any small kernel between
-    const uint8_t* next_W;
-    int next_blocks, next_grid, prefetch_blocks;
-    int qvar;               // qgemm.cuh: hand-off variant / diagnostic switches (bit 0 set in production)
     GemmSeg seg[GEMM_MAX_SEG];
 };
 
@@ -540,12 +534,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, RING == 1 ? 2 : 1) gemm_kernel(c
                     kb = 0;
                     blocks_left_in_seg = sg->tiles * sg->KB;
                 }
-            }
-            if (p.next_W && cta < p.next_grid) {
-                const int n0 = (int)((long long)cta * p.next_blocks / p.next_grid);
-                const int n1 = (int)((long long)(cta + 1) * p.next_blocks / p.next_grid);
-                const int np = min(n1 - n0, p.prefetch_blocks);
-                for (int i = 0; i < np; ++i) bulk_prefetch_l2(p.next_W + (size_t)(n0 + i) * GEMM_WBYTES, GEMM_WBYTES);
             }
         }
     } else {

@@ -151,17 +151,6 @@ __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_co
     const int b0 = (int)((long long)cta * TB / G);
     const int b1 = (int)((long long)(cta + 1) * TB / G);
     unsigned long long* const tr = (p.trace && cta == 0) ? p.trace : nullptr;
-    // hand-off variant (bit 0: one arrival per expansion warp, set in production).  The timing diagnostics (bits 1-3: skip the
-    // expansion, the MMAs, the proxy fence; results are wrong with those set) exist in the debug build only, so that the
-    // product kernel's MMA issue is unconditional.
-    const int qv = p.qvar;
-    const bool q_elect = qv & 1;
-#ifdef B200RWKV_DEBUG
-    const bool q_noexpand = qv & 2, q_nomma = qv & 4, q_nofence = qv & 8;
-#else
-    constexpr bool q_noexpand = false, q_nomma = false, q_nofence = false;
-#endif
-    constexpr int QTR = 460;          // CTA 0's cycle accounts live behind the per-CTA stamps of the trace row
     constexpr int EXP_WARP0 = GEMM_THREADS / 32;
 
     if (tid == 0) {
@@ -171,7 +160,7 @@ __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_co
             mbar_init(empty_bar + s * 8, GEMM_EPI_WARPS);
         }
         for (int s = 0; s < NBUF; ++s) {
-            mbar_init(dfull_bar + s * 8, q_elect ? Q_DQ_WARPS : Q_DQ_THREADS);
+            mbar_init(dfull_bar + s * 8, Q_DQ_WARPS);          // one arrival per expansion warp
             mbar_init(dfree_bar + s * 8, GEMM_EPI_WARPS);
         }
         mbar_fence_init();
@@ -206,15 +195,11 @@ __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_co
             int blocks_left_in_seg = sg->blk_begin + sg->tiles * sg->KB - b0;
             int stage = 0;
             uint32_t ephase = 1;
-            long long c_wait = 0;
-            const long long c_begin = clock64();
             for (int b = b0, it = 0; b < b1; ++b, ++it) {
                 const uint32_t st = ring_base + stage * STAGE_BYTES;
                 const uint32_t fb = full_bar + stage * 8;
                 if (it >= NSTAGE) {
-                    const long long c0 = tr ? clock64() : 0;
                     mbar_wait(empty_bar + stage * 8, ephase, 14);
-                    if (tr) c_wait += clock64() - c0;
                     mbar_expect_tx(fb, STAGE_BYTES);
                     bulk_g2s_hint(st, p.W + (size_t)b * RAW_W, RAW_W, fb, pol_w);
                 }
@@ -228,37 +213,21 @@ __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_co
                     blocks_left_in_seg = sg->tiles * sg->KB;
                 }
             }
-            if (tr) { tr[QTR + 10] = (unsigned long long)c_wait; tr[QTR + 11] = (unsigned long long)(clock64() - c_begin); }
         }
     } else if (warp >= EXP_WARP0) {
         // ===================== expansion: 4 warps =====================
         const int r = tid - GEMM_THREADS;
         RingPos rp{0, 0u};
-        const bool acct = tr && warp == EXP_WARP0 && lane == 0;
-        long long c_full = 0, c_dfree = 0, c_expand = 0, c_hand = 0;
         for (int b = b0, it = 0; b < b1; ++b, ++it) {
             const int d = it % NBUF;
             const int u = it / NBUF;
-            const long long c0 = acct ? clock64() : 0;
             mbar_wait(full_bar + rp.stage * 8, rp.phase, 16);
-            const long long c1 = acct ? clock64() : 0;
             if (u > 0) mbar_wait(dfree_bar + d * 8, (unsigned)(u - 1) & 1u, 17);          // the MMAs that read this buffer retired
-            const long long c2 = acct ? clock64() : 0;
-            if (!q_noexpand) q_expand_block<QT>(ring_base + rp.stage * STAGE_BYTES, dq_base + d * GEMM_WBYTES, lut_base, r, lane);
-            const long long c3 = acct ? clock64() : 0;
-            if (!q_nofence) fence_proxy_async();     // generic-proxy stores -> visible to the tensor core's async-proxy reads
-            if (q_elect) {
-                __syncwarp();                        // the other lanes' (fenced) stores happen before lane 0's release
-                if (lane == 0) mbar_arrive(dfull_bar + d * 8);
-            } else {
-                mbar_arrive(dfull_bar + d * 8);
-            }
-            if (acct) { const long long c4 = clock64(); c_full += c1 - c0; c_dfree += c2 - c1; c_expand += c3 - c2; c_hand += c4 - c3; }
+            q_expand_block<QT>(ring_base + rp.stage * STAGE_BYTES, dq_base + d * GEMM_WBYTES, lut_base, r, lane);
+            fence_proxy_async();                     // generic-proxy stores -> visible to the tensor core's async-proxy reads
+            __syncwarp();                            // the other lanes' (fenced) stores happen before lane 0's release
+            if (lane == 0) mbar_arrive(dfull_bar + d * 8);
             rp.advance<NSTAGE>(1);
-        }
-        if (acct) {
-            tr[QTR + 0] = (unsigned long long)c_full; tr[QTR + 1] = (unsigned long long)c_dfree; tr[QTR + 2] = (unsigned long long)c_expand;
-            tr[QTR + 3] = (unsigned long long)c_hand; tr[QTR + 4] = (unsigned long long)(b1 - b0);
         }
     } else {
         // ===================== consumer warpgroup: MMA + epilogue =====================
@@ -266,8 +235,6 @@ __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_co
         constexpr uint32_t a_lbo = 16 * MT * 16;
         RingPos rp{0, 0u};
         int it = 0;
-        long long c_full = 0, c_dfull = 0;
-        const long long c_begin = clock64();
         SegWalk w;
         w.init(p, b0, b1);
         while (!w.done()) {
@@ -280,24 +247,19 @@ __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_co
             int prev_stage = -1, prev_d = -1;
             for (int i = 0; i < nblk; ++i, ++it) {
                 const int d = it % NBUF;
-                const long long c0 = tr ? clock64() : 0;
                 mbar_wait(full_bar + rp.stage * 8, rp.phase, 12);                     // token operand landed
-                const long long c1 = tr ? clock64() : 0;
                 mbar_wait(dfull_bar + d * 8, (unsigned)(it / NBUF) & 1u, 15);         // weights expanded
-                if (tr) { c_full += c1 - c0; c_dfull += clock64() - c1; }
                 const uint32_t wst = dq_base + d * GEMM_WBYTES;
                 const uint32_t ast = ring_base + rp.stage * STAGE_BYTES + RAW_W;
                 wgmma_fence_operand(acc[0]);
                 wgmma_fence_operand(acc[1]);
                 wgmma_fence();
-                if (!q_nomma) {
 #pragma unroll
-                    for (int k16 = 0; k16 < GEMM_BK / 16; ++k16) {
-                        const uint64_t bdesc = gmma_desc(ast + k16 * 2 * a_lbo, a_lbo, GEMM_A_SBO);
+                for (int k16 = 0; k16 < GEMM_BK / 16; ++k16) {
+                    const uint64_t bdesc = gmma_desc(ast + k16 * 2 * a_lbo, a_lbo, GEMM_A_SBO);
 #pragma unroll
-                        for (int h = 0; h < 2; ++h)
-                            wgmma_f16<16 * MT>(acc[h], gmma_desc(wst + h * 8 * GEMM_W_SBO + k16 * 2 * GEMM_W_LBO, GEMM_W_LBO, GEMM_W_SBO), bdesc);
-                    }
+                    for (int h = 0; h < 2; ++h)
+                        wgmma_f16<16 * MT>(acc[h], gmma_desc(wst + h * 8 * GEMM_W_SBO + k16 * 2 * GEMM_W_LBO, GEMM_W_LBO, GEMM_W_SBO), bdesc);
                 }
                 wgmma_commit();
                 wgmma_wait<1>();                     // the previous block's MMAs retired: its ring slot and buffer go back
@@ -318,10 +280,6 @@ __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_co
             gemm_acc_to_rows<MT>(acc, v, s_x);
             gemm_epilogue_tile<MT, false>(p, w, cta, G, v, *p.nrows, &s_last, reinterpret_cast<__half*>(s_x));
             w.next();
-        }
-        if (tr && tid == 0) {
-            tr[QTR + 5] = (unsigned long long)c_full; tr[QTR + 6] = (unsigned long long)c_dfull;
-            tr[QTR + 7] = 0; tr[QTR + 8] = (unsigned long long)(clock64() - c_begin);
         }
     }
     __syncthreads();

@@ -342,16 +342,6 @@ int32_t b200rwkv_debug_trace(b200rwkv_engine*, uint64_t* out, size_t cap, int32_
 int32_t b200rwkv_debug_gemm_time(b200rwkv_engine*, int32_t which, int32_t reps, float* ms_out, int64_t* bytes_out,
                                  uint64_t* trace_out);
 
-#ifdef B200RWKV_DEBUG
-/* Debug build only (libb200rwkv_dbg.so, `python -m ai00_server_b200.build --debug`): HBM streaming and L2 prefetch
- * micro-benchmarks (csrc/streamtest.cuh).  The debug build also honours the B200RWKV_* bring-up environment switches;
- * the product library ignores the environment. */
-int32_t b200rwkv_debug_stream(int32_t device, int32_t kind, double gbytes, int32_t stage_bytes, int32_t nstage,
-                              int32_t use_hint, int32_t split, int32_t producers, int32_t reps, float* ms_out);
-int32_t b200rwkv_debug_prefetch(int32_t device, double mbytes, int32_t consumers, int32_t pf_grid, int32_t skip, int32_t nblk,
-                                int32_t mode, double idle_us, int32_t reps, float* ms_out);
-#endif
-
 const char* b200rwkv_last_error(b200rwkv_engine*);
 
 #ifdef __cplusplus

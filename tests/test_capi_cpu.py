@@ -18,11 +18,11 @@ def _has_gpu():
     return torch.cuda.is_available()
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_exactly_the_declared_symbols():
+    import shutil
+    import subprocess
     hdr = open(os.path.join(ROOT, "include", "b200rwkv.h")).read()
-    # the debug-build section (#ifdef B200RWKV_DEBUG ... #endif) is not part of the product library
-    product_hdr = re.sub(r"#ifdef B200RWKV_DEBUG.*?#endif", "", hdr, flags=re.S)
-    declared = set(re.findall(r"\b(b200rwkv_[a-z0-9_]+)\s*\(", product_hdr))
+    declared = set(re.findall(r"\b(b200rwkv_[a-z0-9_]+)\s*\(", hdr))
     declared -= {"b200rwkv_status", "b200rwkv_info", "b200rwkv_engine", "b200rwkv_options"}
     assert len(declared) >= 30
     lib = capi.lib()
@@ -30,20 +30,28 @@ def test_library_exports_every_declared_symbol():
     assert declared == bound, (declared ^ bound)
     for name in declared:
         assert getattr(lib, name) is not None
-    for name, _, _ in capi.DEBUG_SYMBOLS:            # and the product library really does not carry the debug entries
+    # and nothing else: the removed HBM-streaming / L2-prefetch micro-benchmark entries in particular
+    for name in ("b200rwkv_debug_stream", "b200rwkv_debug_prefetch"):
         assert not hasattr(lib, name)
+    nm = shutil.which("nm")
+    if nm is not None:
+        out = subprocess.run([nm, "-D", "--defined-only", capi.LIB_PATH], check=True, capture_output=True, text=True).stdout
+        exported = {f[-1] for f in (l.split() for l in out.splitlines()) if f and f[-1].startswith("b200rwkv_")}
+        assert exported == declared, (exported ^ declared)
 
 
 def test_product_library_ignores_the_environment():
-    """The bring-up switches (B200RWKV_*) exist only in the debug build: every getenv in the engine sources sits inside an
-    `#ifdef B200RWKV_DEBUG` block (the CUDA runtime linked into the library reads its own CUDA_* variables)."""
+    """The library reads no environment variable (the CUDA runtime linked into it reads its own CUDA_* variables): no engine
+    source calls getenv, and no source or build recipe names a B200RWKV_DEBUG macro that could compile a switch back in."""
     csrc = os.path.join(ROOT, "ai00_server_b200", "csrc")
-    for f in sorted(os.listdir(csrc)):
-        if not f.endswith((".cu", ".cuh")):
-            continue
-        src = open(os.path.join(csrc, f)).read()
-        outside = re.sub(r"#ifdef B200RWKV_DEBUG.*?#e(?:lse|ndif)", "", src, flags=re.S)
-        assert "getenv(" not in outside, f
+    sources = [os.path.join(csrc, f) for f in sorted(os.listdir(csrc))]
+    sources += [os.path.join(ROOT, "include", f) for f in sorted(os.listdir(os.path.join(ROOT, "include")))]
+    sources.append(os.path.join(ROOT, "ai00_server_b200", "build.py"))
+    for path in sources:
+        src = open(path, errors="replace").read()
+        if path.startswith(csrc):
+            assert "getenv(" not in src, path
+        assert "B200RWKV_DEBUG" not in src, path
 
 
 def test_info_from_st_host_only():
