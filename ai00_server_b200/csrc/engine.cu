@@ -445,6 +445,18 @@ struct b200rwkv_engine {
     float* d_hidden_all = nullptr;
     size_t hidden_cap_rows = 0;
     int hidden_rows = 0;
+    // b200rwkv_keep_hidden_layers: the residual stream after chosen layers for every token of an infer call.  LN1 of layer
+    // l + 1 writes the rows of layer l into the step buffer d_hid_tab[l] points to (null: not recorded); layer L - 1 comes
+    // from ln_out_kernel's d_hidden.  After every step the rows go to their entry's place in hid_all.
+    static constexpr int HID_MAX_LAYERS = 8;
+    std::vector<int> hid_layers;       // recorded layers, in the order the caller gave them
+    float** d_hid_tab = nullptr;       // [L]
+    float* hid_step = nullptr;         // [HID_MAX_LAYERS][maxT][C], step buffer k belongs to hid_layers[k]
+    float* hid_all = nullptr;          // [hid_layers.size()][tokens of the call][C]
+    size_t hid_all_floats = 0;
+    std::vector<int> hid_last;         // layers recorded by the most recent infer call (the layout of hid_all)
+    size_t hid_last_rows = 0;
+    const float* hid_step_src(int k) const { return hid_layers[k] == L - 1 ? d_hidden : hid_step + (size_t)k * maxT * C; }
     int *d_meta = nullptr, *h_meta = nullptr;
     int* d_meta_all = nullptr;
     size_t meta_ints = 0;
@@ -553,6 +565,7 @@ b200rwkv_engine::~b200rwkv_engine() {
     if (step_done) cudaEventDestroy(step_done);
     for (auto& ev : meta_ev) if (ev) cudaEventDestroy(ev);
     if (d_hidden_all) cudaFree(d_hidden_all);
+    if (hid_all) cudaFree(hid_all);
     if (stream) cudaStreamDestroy(stream);
     if (sm_stream) cudaStreamDestroy(sm_stream);
 }
@@ -964,6 +977,7 @@ void b200rwkv_engine::build(const StFile& st) {
     const int S_att = pick_split(Cl, cdiv(C, GEMM_BN)), S_ffn = pick_split(Fl, cdiv(C, GEMM_BN));
     split_att = S_att; split_ffn = S_ffn;
     d_hidden = (float*)dalloc(TC * 4);
+    d_hid_tab = (float**)dalloc((size_t)L * sizeof(float*));
     CK(cudaEventCreateWithFlags(&step_done, cudaEventDisableTiming));
     keep_valid.assign(S, 0);
     if (rank == 0) {
@@ -1037,6 +1051,7 @@ void b200rwkv_engine::build(const StFile& st) {
             if (ver != 7) { n1.n_gate = 1; n1.gate_cl = Cl; n1.gates[0] = f_rr; }
             n1.commit_dst = ffn_shift + (size_t)(l - 1) * S * C;
             n1.commit_src = xx2;
+            n1.hid_slot = d_hid_tab + (l - 1);       // x_out here is the residual stream after layer l - 1
         }
         n1.ln_w = vec_f32(st, b + "ln1.weight", 0, C);
         n1.ln_b = vec_f32(st, b + "ln1.bias", 0, C);
@@ -1594,6 +1609,15 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         hidden_cap_rows = want;
     }
     hidden_rows = 0;
+    const size_t n_hid = hid_layers.size();
+    hid_last.clear();
+    hid_last_rows = 0;
+    if (n_hid * total_tok * C > hid_all_floats) {
+        if (hid_all) { CK(cudaFree(hid_all)); hid_all = nullptr; hid_all_floats = 0; }
+        const size_t want = n_hid * std::max<size_t>(total_tok, 256) * C;
+        CK(cudaMalloc(&hid_all, want * 4));
+        hid_all_floats = want;
+    }
     int step_no = 0;
     for (;;) {
         int n_active = 0;
@@ -1640,15 +1664,18 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         CK(cudaMemcpyAsync(d_meta, hm, meta_ints * 4, cudaMemcpyHostToDevice, stream));
         CK(cudaEventRecord(meta_ev[mb], stream));
         run_step(mt_bucket(T), R > 0 ? mt_bucket(R) : 0);
-        if (hidden_keep) {       // hidden rows of every token of this call (b200rwkv_last_hidden), in entry order
+        // step rows [T][C] -> the rows of every token of this call, in entry order
+        auto gather_rows = [&](float* dst, const float* src) {
             int t0 = 0;
             for (size_t j = 0; j < s_entry.size(); ++j) {
                 const int i = s_entry[j];
-                CK(cudaMemcpyAsync(d_hidden_all + (base[i] + pos[i]) * (size_t)C, d_hidden + (size_t)t0 * C, (size_t)s_counts[j] * C * 4,
+                CK(cudaMemcpyAsync(dst + (base[i] + pos[i]) * (size_t)C, src + (size_t)t0 * C, (size_t)s_counts[j] * C * 4,
                                    cudaMemcpyDeviceToDevice, stream));
                 t0 += s_counts[j];
             }
-        }
+        };
+        if (hidden_keep) gather_rows(d_hidden_all, d_hidden);       // b200rwkv_last_hidden
+        for (size_t k = 0; k < n_hid; ++k) gather_rows(hid_all + k * total_tok * C, hid_step_src((int)k));     // b200rwkv_last_hidden_layer
         if (sc_rows) {       // this step's SCORE rows, scored against each entry's next token
             const size_t first = sc_used;
             int r = 0;
@@ -1718,6 +1745,8 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         if (score->argmax) memcpy(score->argmax, sc_host + total_score * (sizeof(ScoreRow) + 4), total_score * 4);
     }
     if (hidden_keep) hidden_rows = (int)total_tok;
+    hid_last = hid_layers;
+    hid_last_rows = total_tok;
 }
 
 // GPU sampling front half (sample.cuh).  Runs on the softmax stream under the softmax mutex: the reference samples from the
@@ -2881,6 +2910,57 @@ int32_t b200rwkv_last_hidden(b200rwkv_engine* e, float* out, size_t cap) {
     return st < 0 ? st : rows;
 }
 
+int32_t b200rwkv_keep_hidden_layers(b200rwkv_engine* e, int32_t n, const int32_t* layers) {
+    API_BEGIN(e)
+    REQUIRE(n >= 0 && n <= b200rwkv_engine::HID_MAX_LAYERS, B200RWKV_ERR_INVALID,
+            "keep_hidden_layers: n must be in [0, " + std::to_string(b200rwkv_engine::HID_MAX_LAYERS) + "]");
+    REQUIRE(n == 0 || layers, B200RWKV_ERR_INVALID, "keep_hidden_layers: null layers");
+    for (int i = 0; i < n; ++i) {
+        REQUIRE(layers[i] >= 0, B200RWKV_ERR_INVALID, "keep_hidden_layers: negative layer " + std::to_string(layers[i]));
+        REQUIRE(std::find(layers, layers + i, layers[i]) == layers + i, B200RWKV_ERR_INVALID,
+                "keep_hidden_layers: layer " + std::to_string(layers[i]) + " is listed twice");
+    }
+    REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (int i = 0; i < n; ++i)
+        REQUIRE(layers[i] < e->L, B200RWKV_ERR_INVALID,
+                "keep_hidden_layers: layer " + std::to_string(layers[i]) + " is outside [0, " + std::to_string(e->L) + ")");
+    CK(cudaSetDevice(e->dev));
+    if (n > 0 && !e->hid_step) e->hid_step = (float*)e->dalloc((size_t)b200rwkv_engine::HID_MAX_LAYERS * e->maxT * e->C * 4);
+    std::vector<float*> tab(e->L, nullptr);
+    for (int k = 0; k < n; ++k)
+        if (layers[k] < e->L - 1) tab[layers[k]] = e->hid_step + (size_t)k * e->maxT * e->C;
+    // on the engine's stream and complete before returning: the step kernels read the table before griddepcontrol.wait
+    CK(cudaMemcpyAsync(e->d_hid_tab, tab.data(), tab.size() * sizeof(float*), cudaMemcpyHostToDevice, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    e->hid_layers.assign(layers, layers + n);
+    API_END
+}
+
+// returns the number of rows written (negative status on error)
+int32_t b200rwkv_last_hidden_layer(b200rwkv_engine* e, int32_t layer, float* out, size_t cap) {
+    int32_t rows = 0;
+    const int32_t st = [&]() -> int32_t {
+        API_BEGIN(e)
+        REQUIRE(layer >= 0, B200RWKV_ERR_INVALID, "last_hidden_layer: negative layer " + std::to_string(layer));
+        REQUIRE(e && out, B200RWKV_ERR_INVALID, "null argument");
+        std::lock_guard<std::mutex> lk(e->mu);
+        REQUIRE(layer < e->L, B200RWKV_ERR_INVALID,
+                "last_hidden_layer: layer " + std::to_string(layer) + " is outside [0, " + std::to_string(e->L) + ")");
+        const auto it = std::find(e->hid_last.begin(), e->hid_last.end(), layer);
+        REQUIRE(it != e->hid_last.end(), B200RWKV_ERR_STATE,
+                "last_hidden_layer: layer " + std::to_string(layer) + " was not recorded by the most recent infer call");
+        const size_t n = e->hid_last_rows * e->C;
+        REQUIRE(n <= cap, B200RWKV_ERR_INVALID, "last_hidden_layer: buffer too small");
+        CK(cudaSetDevice(e->dev));
+        CK(cudaStreamSynchronize(e->stream));
+        if (n) CK(cudaMemcpy(out, e->hid_all + (size_t)(it - e->hid_last.begin()) * n, n * 4, cudaMemcpyDeviceToHost));
+        rows = (int32_t)e->hid_last_rows;
+        API_END
+    }();
+    return st < 0 ? st : rows;
+}
+
 // Debug aid for the parity tests: copy a named internal activation buffer of the most recent
 // step to the host as f32 row-major [rows, cols]; returns cols (rows = tokens of the last step,
 // capped by `cap`), or a negative status.  Not used on the product path.
@@ -2910,6 +2990,13 @@ int32_t b200rwkv_debug_read(b200rwkv_engine* e, const char* name, float* out, si
                 }
                 return f.cols;
             }
+        if (n.rfind("hid_step", 0) == 0 && n.size() == 9 && n[8] >= '0' && n[8] < '0' + b200rwkv_engine::HID_MAX_LAYERS) {
+            // step buffer k of b200rwkv_keep_hidden_layers (zeros until the first layer is recorded into it)
+            REQUIRE(e->hid_step, B200RWKV_ERR_STATE, "no hidden layer has been recorded yet");
+            REQUIRE((size_t)T * e->C <= cap, B200RWKV_ERR_INVALID, "debug buffer too small");
+            CK(cudaMemcpy(out, e->hid_step + (size_t)(n[8] - '0') * e->maxT * e->C, (size_t)T * e->C * 4, cudaMemcpyDeviceToHost));
+            return e->C;
+        }
         struct A { std::string n; const A16Buf* b; int cols; int mat; };
         std::vector<A> as;
         for (int i = 0; i < 6; ++i) as.push_back({"a_x" + std::to_string(i), &e->a_x[i], e->C, 0});

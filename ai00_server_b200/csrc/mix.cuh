@@ -46,6 +46,10 @@ struct LnMixParams {
     float* commit_dst;      // [S, C] or null
     const float* commit_src;    // [T, C]
     unsigned long long* trace;  // profiling aid (null in production)
+    // LN1 of layer l + 1 only: slot l of the engine's per-layer hidden-row table (b200rwkv_keep_hidden_layers).  The slot
+    // holds a [T, C] buffer that receives x_out (the residual stream after layer l) or null.  It changes only between
+    // host-synchronous infer calls, so kernels read it before griddepcontrol.wait and the step graphs never change.
+    float* const* hid_slot;
 };
 
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
@@ -139,8 +143,9 @@ __device__ __forceinline__ float4 ln_apply(const float4 a, const float mean, con
     return o;
 }
 
+// `hid`: null, or the [T, C] buffer that records this stage's updated residual (LnMixParams::hid_slot)
 template <int NV>
-__device__ __forceinline__ void ln_mix_row_nv(const LnMixParams& p, const int t, float* red, unsigned long long* stamps = nullptr) {
+__device__ __forceinline__ void ln_mix_row_nv(const LnMixParams& p, const int t, float* red, float* hid, unsigned long long* stamps = nullptr) {
     auto stamp = [&](int i) { if (stamps && threadIdx.x == 0) stamps[i] = globaltimer_ns(); };
     stamp(0);
     const int C = p.C;
@@ -167,6 +172,13 @@ __device__ __forceinline__ void ln_mix_row_nv(const LnMixParams& p, const int t,
         for (int j = 0; j < NV; ++j) {
             const int c = 4 * (threadIdx.x + LN_THREADS * j);
             if (c < C) *reinterpret_cast<float4*>(p.x_out + (size_t)t * C + c) = a[j];
+        }
+    }
+    if (hid) {
+#pragma unroll
+        for (int j = 0; j < NV; ++j) {
+            const int c = 4 * (threadIdx.x + LN_THREADS * j);
+            if (c < C) *reinterpret_cast<float4*>(hid + (size_t)t * C + c) = a[j];
         }
     }
     float mean, rstd;
@@ -217,12 +229,12 @@ __device__ __forceinline__ void ln_mix_row_nv(const LnMixParams& p, const int t,
     }
 }
 
-__device__ __forceinline__ void ln_mix_row(const LnMixParams& p, const int t, float* red, unsigned long long* stamps = nullptr) {
+__device__ __forceinline__ void ln_mix_row(const LnMixParams& p, const int t, float* red, float* hid, unsigned long long* stamps = nullptr) {
     const int nv = (p.C + 4 * LN_THREADS - 1) / (4 * LN_THREADS);
-    if (nv <= 1) ln_mix_row_nv<1>(p, t, red);
-    else if (nv == 2) ln_mix_row_nv<2>(p, t, red);
-    else if (nv <= 4) ln_mix_row_nv<4>(p, t, red, stamps);
-    else ln_mix_row_nv<8>(p, t, red);
+    if (nv <= 1) ln_mix_row_nv<1>(p, t, red, hid);
+    else if (nv == 2) ln_mix_row_nv<2>(p, t, red, hid);
+    else if (nv <= 4) ln_mix_row_nv<4>(p, t, red, hid, stamps);
+    else ln_mix_row_nv<8>(p, t, red, hid);
     if (stamps && threadIdx.x == 0) stamps[6] = globaltimer_ns();
 }
 
@@ -230,11 +242,12 @@ __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const __grid_constan
     __shared__ float red[32];
     trace_stamp(p.trace, 0);
     pdl_launch_dependents();
+    float* const hid = p.hid_slot ? *p.hid_slot : nullptr;
     pdl_wait();
     trace_stamp(p.trace, 1);
     const int t = blockIdx.x;
     if (t >= p.meta.T()) return;
-    ln_mix_row(p, t, red);
+    ln_mix_row(p, t, red, hid);
     trace_stamp(p.trace, 7);
 }
 

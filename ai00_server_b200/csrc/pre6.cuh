@@ -152,6 +152,7 @@ struct PreLnStatic {       // operands of phase 1 that no kernel of this step wr
     float4 w, b;
     float4 mu[NMIX];
     int T, slot, prev_t, last;     // step metadata is uploaded before the step's first launch
+    float* hid;                    // hidden-row buffer of this stage (LnMixParams::hid_slot) or null
 };
 
 template <int NMIX>
@@ -162,6 +163,7 @@ __device__ __forceinline__ PreLnStatic<NMIX> pre_ln_static(const LnMixParams& p,
     st.slot = p.meta.tok_slot()[t];
     st.prev_t = p.meta.tok_prev()[t];
     st.last = p.meta.tok_last()[t];
+    st.hid = p.hid_slot ? *p.hid_slot : nullptr;
     const bool act = 4 * (int)threadIdx.x < Cs;
     const int c = act ? (int)rank * Cs + 4 * (int)threadIdx.x : 0;
     const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -190,6 +192,7 @@ __device__ __forceinline__ void pre_ln_slice(const LnMixParams& p, const int t, 
     if (commit) cm = ld4(p.commit_src + (size_t)t * C + c);
     float4 a = act ? residual_vec(r, t, c) : z4;
     if (act && (p.x_out != p.x_in || p.n_parts > 0)) *reinterpret_cast<float4*>(p.x_out + (size_t)t * C + c) = a;
+    if (act && st.hid) *reinterpret_cast<float4*>(st.hid + (size_t)t * C + c) = a;
     float mean, rstd;
     slice_stats(cl, rank, C, act, a, red, xch[0], mean, rstd);
     if (prev_t >= 0) {          // multi-token slot: previous token's LN output, recomputed (uniform over the cluster)

@@ -409,16 +409,41 @@ class Model:
         capi.check(capi.lib().b200rwkv_launch_count(self._h, C.byref(n)), self._h)
         return n.value
 
-    def keep_hidden(self, enable: bool = True) -> None:
-        capi.check(capi.lib().b200rwkv_keep_hidden(self._h, int(enable)), self._h)
+    def keep_hidden(self, enable: bool = True, layers=None) -> None:
+        """keep_hidden(bool): record the residual stream after the last layer for every token of each infer call
+        (b200rwkv_keep_hidden).  keep_hidden(layers=[...]): record it after each listed layer instead (at most 8 distinct
+        layers, b200rwkv_keep_hidden_layers); layers=[] turns that recording off.  The two are independent."""
+        if layers is None:
+            capi.check(capi.lib().b200rwkv_keep_hidden(self._h, int(enable)), self._h)
+            return
+        a = np.asarray(layers, np.int32).reshape(-1)
+        capi.check(capi.lib().b200rwkv_keep_hidden_layers(self._h, a.size, capi.ptr(a) if a.size else None), self._h)
 
-    def last_hidden(self, max_rows: int = 64) -> np.ndarray:
-        """Residual stream after the last layer per token of the most recent infer call (all tokens after keep_hidden())."""
+    def last_hidden(self, max_rows: int = 64, layer: int | None = None) -> np.ndarray:
+        """Residual stream per token of the most recent infer call: after the last layer (all tokens after keep_hidden()),
+        or after `layer`, which that call must have recorded (keep_hidden(layers=[...]))."""
         Cc = self.info["num_emb"]
         buf = np.empty((max_rows, Cc), np.float32)
-        r = capi.lib().b200rwkv_last_hidden(self._h, capi.ptr(buf), buf.size)
+        if layer is None:
+            r = capi.lib().b200rwkv_last_hidden(self._h, capi.ptr(buf), buf.size)
+        else:
+            r = capi.lib().b200rwkv_last_hidden_layer(self._h, int(layer), capi.ptr(buf), buf.size)
         capi.check(r, self._h)
         return buf[:r]
+
+    def embed(self, slot: int, tokens, layer: int) -> np.ndarray:
+        """The embeddings route (reference docs/doc-api/openai.md:376-437): feed `tokens` to `slot` in one infer call with
+        no logits and return the residual stream after `layer` at the last token, [num_emb] f32.  Advances the slot's state;
+        turns layer recording off afterwards."""
+        tokens = [int(t) for t in tokens]
+        if not tokens:
+            raise capi.B200Error(capi.ERR_INVALID, "embed: no tokens")
+        self.keep_hidden(layers=[layer])
+        try:
+            self.infer_raw([slot], [len(tokens)], tokens, [capi.OPTION_NONE])
+            return self.last_hidden(max_rows=len(tokens), layer=layer)[-1].copy()
+        finally:
+            self.keep_hidden(layers=[])
 
     def debug_read(self, name: str, rows: int = 64) -> np.ndarray:
         buf = np.empty(rows * 65536, np.float32)

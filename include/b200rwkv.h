@@ -328,6 +328,20 @@ int32_t b200rwkv_launch_count(b200rwkv_engine*, int64_t* total);
 int32_t b200rwkv_keep_hidden(b200rwkv_engine*, int32_t enable);
 int32_t b200rwkv_last_hidden(b200rwkv_engine*, float* out, size_t cap);
 
+/* The residual stream after any chosen layers: the `layer` parameter of the embeddings route (reference
+ * docs/doc-api/openai.md:376-437).  "Layer l" is the f32 residual stream after block l, l in [0, num_layer - 1], before any
+ * LayerNorm: x_l = x_{l-1} + att_l + ffn_l, with x_{-1} = ln0(emb[token]).  For l = num_layer - 1 the rows are bit-identical
+ * to b200rwkv_last_hidden's.  This is our reading of the documentation's wording; no reference output pins it.
+ * b200rwkv_keep_hidden_layers(e, n, layers) makes every following infer call record the rows of ALL its tokens for the n
+ * listed layers (entry order, like the token array, across internal steps); n = 0 turns recording off.  At most 8 distinct
+ * layers; a layer outside [0, num_layer), a duplicate or n > 8 is B200RWKV_ERR_INVALID, checked before the first CUDA call.
+ * Independent of b200rwkv_keep_hidden.  Recording adds no kernel launch and changes no other output.
+ * b200rwkv_last_hidden_layer copies layer `layer`'s rows of the most recent infer call ([rows][num_emb] f32) and returns the
+ * row count: B200RWKV_ERR_STATE if that call did not record the layer, B200RWKV_ERR_INVALID if `cap` (floats) is too small.
+ * In-process tensor parallelism: the residual stream is replicated over the ranks; rank 0 records it. */
+int32_t b200rwkv_keep_hidden_layers(b200rwkv_engine*, int32_t n, const int32_t* layers);
+int32_t b200rwkv_last_hidden_layer(b200rwkv_engine*, int32_t layer, float* out, size_t cap);
+
 /* Test aid: copy a named internal activation buffer of the most recent step to the host as f32
  * row-major; returns the column count (negative status on error).  Not on the product path. */
 int32_t b200rwkv_debug_read(b200rwkv_engine*, const char* name, float* out, size_t cap);
