@@ -104,6 +104,7 @@ SYMBOLS = [
     ("b200rwkv_read_state", C.c_int32, [C.POINTER(Info), _P, C.c_size_t, _P]),
     ("b200rwkv_softmax", C.c_int32, [_P, C.c_int32, _P, _P]),
     ("b200rwkv_sample_topk", C.c_int32, [_P, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _P, _P]),
+    ("b200rwkv_sample_probs", C.c_int32, [_P, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     ("b200rwkv_host_alloc", C.c_int32, [C.c_size_t, C.POINTER(_P)]),
     ("b200rwkv_host_free", None, [_P]),
     ("b200rwkv_bench_decode", C.c_int32, [_P, C.c_int32, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_int64), _P]),

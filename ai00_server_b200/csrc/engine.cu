@@ -479,14 +479,24 @@ struct b200rwkv_engine {
     unsigned* tk_out_id = nullptr; float* tk_out_p = nullptr;
     uint8_t *tk_dev = nullptr, *tk_host = nullptr;
     size_t tk_cap = 0;
+    // b200rwkv_sample_probs: [nrows][V rounded up to 4] f32 rows | [nrows][segments] float2 statistics; grown on demand
+    uint8_t* sp_dev = nullptr;
+    size_t sp_cap = 0;
     // scoring (b200rwkv_infer_ex, OPTION_SCORE): [ScoreRow x n | score f32 x n | argmax u32 x n], pinned host and device,
     // n = the call's scored tokens; grown on demand
     uint8_t *sc_dev = nullptr, *sc_host = nullptr;
     size_t sc_cap = 0;
     void enqueue_keep(cudaStream_t s, int MTR);
+    void check_sample_slots(int nrows, const int32_t* slots, const char* who);
+    SampleAdjust stage_sample_args(int nrows, const int32_t* slots, const int32_t* pen_off, const uint32_t* pen_tok,
+                                   const float* pen_val, const uint32_t* allow_bits, const int32_t* bias_off,
+                                   const uint32_t* bias_tok, const float* bias_val);
     void sample_topk(int nrows, const int32_t* slots, const int32_t* pen_off, const uint32_t* pen_tok, const float* pen_val,
                      const uint32_t* allow_bits, const int32_t* bias_off, const uint32_t* bias_tok, const float* bias_val,
                      int top_k, uint32_t* ids_out, float* probs_out);
+    void sample_probs(int nrows, const int32_t* slots, const int32_t* pen_off, const uint32_t* pen_tok, const float* pen_val,
+                      const uint32_t* allow_bits, const int32_t* bias_off, const uint32_t* bias_tok, const float* bias_val,
+                      float* probs_out);
 
     std::mutex mu, sm_mu;
 
@@ -560,6 +570,7 @@ b200rwkv_engine::~b200rwkv_engine() {
     if (h_meta) cudaFreeHost(h_meta);
     if (tk_dev) cudaFree(tk_dev);
     if (tk_host) cudaFreeHost(tk_host);
+    if (sp_dev) cudaFree(sp_dev);
     if (sc_dev) cudaFree(sc_dev);
     if (sc_host) cudaFreeHost(sc_host);
     if (step_done) cudaEventDestroy(step_done);
@@ -1752,30 +1763,39 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
 // GPU sampling front half (sample.cuh).  Runs on the softmax stream under the softmax mutex: the reference samples from the
 // task that owns softmax (run.rs:1237), concurrently with the infer task; the per-slot rows it reads are only rewritten by a
 // step that contains the slot, which the host cannot submit before this call returned the slot's token.
-void b200rwkv_engine::sample_topk(int nrows, const int32_t* slots, const int32_t* pen_off, const uint32_t* pen_tok, const float* pen_val,
-                                  const uint32_t* allow_bits, const int32_t* bias_off, const uint32_t* bias_tok, const float* bias_val,
-                                  int top_k, uint32_t* ids_out, float* probs_out) {
-    REQUIRE(rank == 0, B200RWKV_ERR_INVALID, "sample_topk: only rank 0 holds the gathered logits");
-    REQUIRE(tk_cand_x, B200RWKV_ERR_UNSUPPORTED, "sample_topk: num_vocab > 65536 is not supported");
-    REQUIRE(nrows >= 1 && nrows <= S && slots && ids_out && probs_out, B200RWKV_ERR_INVALID, "sample_topk: bad argument");
-    REQUIRE(top_k >= 1 && top_k <= TOPK_MAX, B200RWKV_ERR_INVALID, "sample_topk: top_k must be in [1, 128]");
-    {
-        std::lock_guard<std::mutex> lk(keep_mu);
-        std::vector<char> seen(S, 0);
-        for (int i = 0; i < nrows; ++i) {
-            REQUIRE(slots[i] >= 0 && slots[i] < S, B200RWKV_ERR_STATE, "sample_topk: slot out of range");
-            REQUIRE(!seen[slots[i]], B200RWKV_ERR_INVALID, "sample_topk: duplicate slot");
-            seen[slots[i]] = 1;
-            REQUIRE(keep_valid[slots[i]], B200RWKV_ERR_STATE, "sample_topk: slot " + std::to_string(slots[i]) + " has produced no logits row yet");
-        }
-    }
+// Argument checks of the sampling entries (sample_topk, sample_probs) that need no engine: the adjustment lists.
+static void check_sample_lists(int nrows, const int32_t* pen_off, const uint32_t* pen_tok, const float* pen_val, const int32_t* bias_off,
+                               const uint32_t* bias_tok, const float* bias_val, const char* who) {
+    const std::string w(who);
     const int npen = pen_off ? pen_off[nrows] : 0, nbias = bias_off ? bias_off[nrows] : 0;
     REQUIRE(npen >= 0 && nbias >= 0 && (npen == 0 || (pen_tok && pen_val)) && (nbias == 0 || (bias_tok && bias_val)), B200RWKV_ERR_INVALID,
-            "sample_topk: bad adjustment lists");
+            w + ": bad adjustment lists");
     for (int i = 0; i < nrows; ++i) {
-        REQUIRE(!pen_off || (pen_off[i] >= 0 && pen_off[i] <= pen_off[i + 1]), B200RWKV_ERR_INVALID, "sample_topk: penalty offsets must ascend");
-        REQUIRE(!bias_off || (bias_off[i] >= 0 && bias_off[i] <= bias_off[i + 1]), B200RWKV_ERR_INVALID, "sample_topk: bias offsets must ascend");
+        REQUIRE(!pen_off || (pen_off[i] >= 0 && pen_off[i] <= pen_off[i + 1]), B200RWKV_ERR_INVALID, w + ": penalty offsets must ascend");
+        REQUIRE(!bias_off || (bias_off[i] >= 0 && bias_off[i] <= bias_off[i + 1]), B200RWKV_ERR_INVALID, w + ": bias offsets must ascend");
     }
+}
+
+// The slot checks of the sampling entries: nrows in [1, max_batch], every slot in range, listed once, with a kept row.
+void b200rwkv_engine::check_sample_slots(int nrows, const int32_t* slots, const char* who) {
+    const std::string w(who);
+    REQUIRE(nrows >= 1 && nrows <= S && slots, B200RWKV_ERR_INVALID, w + ": bad argument");
+    std::lock_guard<std::mutex> lk(keep_mu);
+    std::vector<char> seen(S, 0);
+    for (int i = 0; i < nrows; ++i) {
+        REQUIRE(slots[i] >= 0 && slots[i] < S, B200RWKV_ERR_STATE, w + ": slot out of range");
+        REQUIRE(!seen[slots[i]], B200RWKV_ERR_INVALID, w + ": duplicate slot");
+        seen[slots[i]] = 1;
+        REQUIRE(keep_valid[slots[i]], B200RWKV_ERR_STATE, w + ": slot " + std::to_string(slots[i]) + " has produced no logits row yet");
+    }
+}
+
+// Stages the slots and adjustment lists (checked) in one blob, uploads it on the softmax stream after the most recent step,
+// and returns the device view.
+SampleAdjust b200rwkv_engine::stage_sample_args(int nrows, const int32_t* slots, const int32_t* pen_off, const uint32_t* pen_tok,
+                                                const float* pen_val, const uint32_t* allow_bits, const int32_t* bias_off,
+                                                const uint32_t* bias_tok, const float* bias_val) {
+    const int npen = pen_off ? pen_off[nrows] : 0, nbias = bias_off ? bias_off[nrows] : 0;
     const size_t words = (size_t)(V + 31) / 32;
     auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
     // one staging blob: slot[n] | pen_off[n+1] | bias_off[n+1] | pen_tok | pen_val | bias_tok | bias_val | allow
@@ -1801,13 +1821,27 @@ void b200rwkv_engine::sample_topk(int nrows, const int32_t* slots, const int32_t
     if (allow_bits) memcpy(tk_host + o_al, allow_bits, (size_t)nrows * words * 4);
     CK(cudaStreamWaitEvent(sm_stream, step_done, 0));
     CK(cudaMemcpyAsync(tk_dev, tk_host, total, cudaMemcpyHostToDevice, sm_stream));
+    SampleAdjust a;
+    a.slot = (const int*)(tk_dev + o_slot);
+    a.pen_off = (const int*)(tk_dev + o_po); a.pen_tok = (const unsigned*)(tk_dev + o_pt); a.pen_val = (const float*)(tk_dev + o_pv);
+    a.bias_off = (const int*)(tk_dev + o_bo); a.bias_tok = (const unsigned*)(tk_dev + o_bt); a.bias_val = (const float*)(tk_dev + o_bv);
+    a.allow = allow_bits ? (const unsigned*)(tk_dev + o_al) : nullptr;
+    return a;
+}
+
+void b200rwkv_engine::sample_topk(int nrows, const int32_t* slots, const int32_t* pen_off, const uint32_t* pen_tok, const float* pen_val,
+                                  const uint32_t* allow_bits, const int32_t* bias_off, const uint32_t* bias_tok, const float* bias_val,
+                                  int top_k, uint32_t* ids_out, float* probs_out) {
+    REQUIRE(rank == 0, B200RWKV_ERR_INVALID, "sample_topk: only rank 0 holds the gathered logits");
+    REQUIRE(tk_cand_x, B200RWKV_ERR_UNSUPPORTED, "sample_topk: num_vocab > 65536 is not supported");
+    REQUIRE(ids_out && probs_out, B200RWKV_ERR_INVALID, "sample_topk: bad argument");
+    REQUIRE(top_k >= 1 && top_k <= TOPK_MAX, B200RWKV_ERR_INVALID, "sample_topk: top_k must be in [1, 128]");
+    check_sample_slots(nrows, slots, "sample_topk");
+    check_sample_lists(nrows, pen_off, pen_tok, pen_val, bias_off, bias_tok, bias_val, "sample_topk");
     TopkParams tp;
     memset(&tp, 0, sizeof(tp));
     tp.keep = d_keep; tp.V = V; tp.nseg = cdiv(V, TOPK_SEG);
-    tp.slot = (const int*)(tk_dev + o_slot);
-    tp.pen_off = (const int*)(tk_dev + o_po); tp.pen_tok = (const unsigned*)(tk_dev + o_pt); tp.pen_val = (const float*)(tk_dev + o_pv);
-    tp.bias_off = (const int*)(tk_dev + o_bo); tp.bias_tok = (const unsigned*)(tk_dev + o_bt); tp.bias_val = (const float*)(tk_dev + o_bv);
-    tp.allow = allow_bits ? (const unsigned*)(tk_dev + o_al) : nullptr;
+    tp.adj = stage_sample_args(nrows, slots, pen_off, pen_tok, pen_val, allow_bits, bias_off, bias_tok, bias_val);
     tp.cand_x = tk_cand_x; tp.cand_id = tk_cand_id; tp.stats = tk_stats;
     tp.top_k = top_k; tp.out_id = tk_out_id; tp.out_p = tk_out_p;
     topk_segment_kernel<<<dim3(tp.nseg, nrows), TOPK_SEG_THREADS, 0, sm_stream>>>(tp);
@@ -1816,6 +1850,37 @@ void b200rwkv_engine::sample_topk(int nrows, const int32_t* slots, const int32_t
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(ids_out, tk_out_id, (size_t)nrows * top_k * 4, cudaMemcpyDeviceToHost, sm_stream));
     CK(cudaMemcpyAsync(probs_out, tk_out_p, (size_t)nrows * top_k * 4, cudaMemcpyDeviceToHost, sm_stream));
+    CK(cudaStreamSynchronize(sm_stream));
+}
+
+// The whole adjusted distribution of each listed slot's kept row (sample.cuh, probs_*_kernel).  Same thread contract as
+// sample_topk; the caller has checked the adjustment lists, probs_out and nrows >= 1.  The kept rows are only read.
+void b200rwkv_engine::sample_probs(int nrows, const int32_t* slots, const int32_t* pen_off, const uint32_t* pen_tok, const float* pen_val,
+                                   const uint32_t* allow_bits, const int32_t* bias_off, const uint32_t* bias_tok, const float* bias_val,
+                                   float* probs_out) {
+    REQUIRE(rank == 0, B200RWKV_ERR_INVALID, "sample_probs: only rank 0 holds the gathered logits");
+    check_sample_slots(nrows, slots, "sample_probs");
+    CK(cudaSetDevice(dev));
+    ProbsParams pp;
+    memset(&pp, 0, sizeof(pp));
+    pp.keep = d_keep; pp.V = V; pp.nseg = cdiv(V, TOPK_SEG); pp.ld = (V + 3) & ~3;
+    const size_t row_bytes = (size_t)nrows * pp.ld * 4, need = row_bytes + (size_t)nrows * pp.nseg * sizeof(float2);
+    if (need > sp_cap) {
+        if (sp_dev) { CK(cudaFree(sp_dev)); sp_dev = nullptr; }
+        sp_cap = 0;
+        const size_t want = std::min(std::max<size_t>(need * 2, 1 << 20), (size_t)S * (pp.ld * 4 + pp.nseg * sizeof(float2)));
+        CK(cudaMalloc(&sp_dev, want));
+        sp_cap = want;
+    }
+    pp.adj = stage_sample_args(nrows, slots, pen_off, pen_tok, pen_val, allow_bits, bias_off, bias_tok, bias_val);
+    pp.out = (float*)sp_dev;
+    pp.stats = (float2*)(sp_dev + row_bytes);
+    probs_stats_kernel<<<dim3(pp.nseg, nrows), TOPK_SEG_THREADS, 0, sm_stream>>>(pp);
+    CK(cudaGetLastError());
+    probs_write_kernel<<<dim3(pp.nseg, nrows), TOPK_SEG_THREADS, 0, sm_stream>>>(pp);
+    CK(cudaGetLastError());
+    if (pp.ld == V) CK(cudaMemcpyAsync(probs_out, pp.out, row_bytes, cudaMemcpyDeviceToHost, sm_stream));
+    else CK(cudaMemcpy2DAsync(probs_out, (size_t)V * 4, pp.out, (size_t)pp.ld * 4, (size_t)V * 4, nrows, cudaMemcpyDeviceToHost, sm_stream));
     CK(cudaStreamSynchronize(sm_stream));
 }
 
@@ -2349,6 +2414,19 @@ int32_t b200rwkv_sample_topk(b200rwkv_engine* e, int32_t nrows, const int32_t* s
     CK(cudaSetDevice(e->dev));
     e->sample_topk(nrows, slots, penalty_offset, penalty_token, penalty_value, allow_bits, bias_offset, bias_token, bias_value, top_k,
                    ids_out, probs_out);
+    API_END
+}
+
+int32_t b200rwkv_sample_probs(b200rwkv_engine* e, int32_t nrows, const int32_t* slots, const int32_t* penalty_offset,
+                              const uint32_t* penalty_token, const float* penalty_value, const uint32_t* allow_bits,
+                              const int32_t* bias_offset, const uint32_t* bias_token, const float* bias_value, float* probs_out) {
+    API_BEGIN(e)
+    REQUIRE(nrows >= 1 && slots && probs_out, B200RWKV_ERR_INVALID, "sample_probs: bad argument");
+    REQUIRE(!e || nrows <= e->S, B200RWKV_ERR_INVALID, "sample_probs: nrows exceeds max_batch");
+    check_sample_lists(nrows, penalty_offset, penalty_token, penalty_value, bias_offset, bias_token, bias_value, "sample_probs");
+    REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
+    std::lock_guard<std::mutex> lk(e->sm_mu);
+    e->sample_probs(nrows, slots, penalty_offset, penalty_token, penalty_value, allow_bits, bias_offset, bias_token, bias_value, probs_out);
     API_END
 }
 

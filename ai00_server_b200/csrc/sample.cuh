@@ -32,9 +32,8 @@ constexpr int TOPK_SEG_THREADS = 256;
 constexpr int TOPK_MAX_SEGS = 32;         // => num_vocab <= 65536
 constexpr int TOPK_MERGE_THREADS = 1024;
 
-struct TopkParams {
-    const float* keep;          // [S][V] last logits row of every slot
-    int V, nseg;
+// The rows to sample and their adjustments (run.rs:671-682), staged in one blob by the host; shared by both entry points.
+struct SampleAdjust {
     const int* slot;            // [nrows]
     const int* pen_off;         // [nrows + 1]
     const unsigned* pen_tok;    // logits[tok] -= val   (entries of one row have distinct tokens)
@@ -43,6 +42,12 @@ struct TopkParams {
     const unsigned* bias_tok;   // logits[tok] += val   (distinct tokens within a row)
     const float* bias_val;
     const unsigned* allow;      // optional [nrows][ceil(V / 32)]: bit = 1 -> token allowed; disallowed -> -inf
+};
+
+struct TopkParams {
+    const float* keep;          // [S][V] last logits row of every slot
+    int V, nseg;
+    SampleAdjust adj;
     float* cand_x;              // [nrows][nseg][128]
     unsigned* cand_id;          // [nrows][nseg][128]
     float2* stats;              // [nrows][nseg] (max, sum exp(x - max))
@@ -56,25 +61,17 @@ __device__ __forceinline__ bool cand_before(const float xa, const unsigned ia, c
     return xa > xb || (xa == xb && ia < ib);
 }
 
-__global__ void __launch_bounds__(TOPK_SEG_THREADS) topk_segment_kernel(const __grid_constant__ TopkParams p) {
-    __shared__ float sx[TOPK_SEG];
-    __shared__ unsigned sid[TOPK_SEG];
-    __shared__ float red[32];
-    const int seg = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
-    const int seg0 = seg * TOPK_SEG;
-    const float* src = p.keep + (size_t)p.slot[row] * p.V;
-    const unsigned* allow = p.allow ? p.allow + (size_t)row * ((p.V + 31) / 32) : nullptr;
-#pragma unroll
-    for (int j = 0; j < TOPK_SEG / TOPK_SEG_THREADS; ++j) {
-        const int li = tid + TOPK_SEG_THREADS * j, i = seg0 + li;
-        sx[li] = (i < p.V) ? src[i] : -INFINITY;
-        sid[li] = (i < p.V) ? (unsigned)i : 0xFFFFFFFFu;
-    }
+// Adjusts segment `seg0 .. seg0 + TOPK_SEG` of row `row`, already loaded into sx (-inf past V), in place: penalties, the
+// allowed-token mask, then bias -- the order of run.rs:671-682.  All TOPK_SEG_THREADS threads call it; it synchronises
+// before it reads sx and before it returns.
+__device__ __forceinline__ void adjust_segment(float* sx, const int seg0, const int V, const int row, const SampleAdjust& a) {
+    const int tid = threadIdx.x;
+    const unsigned* allow = a.allow ? a.allow + (size_t)row * ((V + 31) / 32) : nullptr;
     __syncthreads();
     // Sampler::transform: penalties (distinct tokens: race free)
-    for (int e = p.pen_off[row] + tid; e < p.pen_off[row + 1]; e += TOPK_SEG_THREADS) {
-        const unsigned t = p.pen_tok[e];
-        if (t >= (unsigned)seg0 && t < (unsigned)(seg0 + TOPK_SEG) && t < (unsigned)p.V) sx[t - seg0] -= p.pen_val[e];
+    for (int e = a.pen_off[row] + tid; e < a.pen_off[row + 1]; e += TOPK_SEG_THREADS) {
+        const unsigned t = a.pen_tok[e];
+        if (t >= (unsigned)seg0 && t < (unsigned)(seg0 + TOPK_SEG) && t < (unsigned)V) sx[t - seg0] -= a.pen_val[e];
     }
     __syncthreads();
     // Formatter::transform: tokens the grammar does not allow
@@ -82,17 +79,23 @@ __global__ void __launch_bounds__(TOPK_SEG_THREADS) topk_segment_kernel(const __
 #pragma unroll
         for (int j = 0; j < TOPK_SEG / TOPK_SEG_THREADS; ++j) {
             const int li = tid + TOPK_SEG_THREADS * j, i = seg0 + li;
-            if (i < p.V && !((allow[i >> 5] >> (i & 31)) & 1u)) sx[li] = -INFINITY;
+            if (i < V && !((allow[i >> 5] >> (i & 31)) & 1u)) sx[li] = -INFINITY;
         }
         __syncthreads();
     }
     // bias
-    for (int e = p.bias_off[row] + tid; e < p.bias_off[row + 1]; e += TOPK_SEG_THREADS) {
-        const unsigned t = p.bias_tok[e];
-        if (t >= (unsigned)seg0 && t < (unsigned)(seg0 + TOPK_SEG) && t < (unsigned)p.V) sx[t - seg0] += p.bias_val[e];
+    for (int e = a.bias_off[row] + tid; e < a.bias_off[row + 1]; e += TOPK_SEG_THREADS) {
+        const unsigned t = a.bias_tok[e];
+        if (t >= (unsigned)seg0 && t < (unsigned)(seg0 + TOPK_SEG) && t < (unsigned)V) sx[t - seg0] += a.bias_val[e];
     }
     __syncthreads();
-    // segment statistics of the softmax
+}
+
+// Softmax statistics of one adjusted segment in shared memory: (max, sum expf(x - max)), (-inf, 0) if every element is -inf.
+// Element i always goes to thread i % TOPK_SEG_THREADS and the block reductions have a fixed shape, so the result depends
+// only on the segment's values.
+__device__ __forceinline__ float2 segment_stats(const float* sx, float* red) {
+    const int tid = threadIdx.x;
     float mx = -INFINITY;
 #pragma unroll
     for (int j = 0; j < TOPK_SEG / TOPK_SEG_THREADS; ++j) mx = fmaxf(mx, sx[tid + TOPK_SEG_THREADS * j]);
@@ -103,7 +106,26 @@ __global__ void __launch_bounds__(TOPK_SEG_THREADS) topk_segment_kernel(const __
         for (int j = 0; j < TOPK_SEG / TOPK_SEG_THREADS; ++j) s += expf(sx[tid + TOPK_SEG_THREADS * j] - mx);
     }
     s = block_sum_any(s, red);
-    if (tid == 0) p.stats[(size_t)row * p.nseg + seg] = make_float2(mx, s);
+    return make_float2(mx, s);
+}
+
+__global__ void __launch_bounds__(TOPK_SEG_THREADS) topk_segment_kernel(const __grid_constant__ TopkParams p) {
+    __shared__ float sx[TOPK_SEG];
+    __shared__ unsigned sid[TOPK_SEG];
+    __shared__ float red[32];
+    const int seg = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
+    const int seg0 = seg * TOPK_SEG;
+    const float* src = p.keep + (size_t)p.adj.slot[row] * p.V;
+#pragma unroll
+    for (int j = 0; j < TOPK_SEG / TOPK_SEG_THREADS; ++j) {
+        const int li = tid + TOPK_SEG_THREADS * j, i = seg0 + li;
+        sx[li] = (i < p.V) ? src[i] : -INFINITY;
+        sid[li] = (i < p.V) ? (unsigned)i : 0xFFFFFFFFu;
+    }
+    adjust_segment(sx, seg0, p.V, row, p.adj);
+    // segment statistics of the softmax
+    const float2 st = segment_stats(sx, red);
+    if (tid == 0) p.stats[(size_t)row * p.nseg + seg] = st;
     // bitonic sort, best first
     for (int k = 2; k <= TOPK_SEG; k <<= 1) {
         for (int j = k >> 1; j > 0; j >>= 1) {
@@ -175,6 +197,84 @@ __global__ void __launch_bounds__(TOPK_MERGE_THREADS) topk_merge_kernel(const __
         // same expression as softmax_kernel (misc.cuh): exp(x - max) * (1 / sum)
         p.out_id[(size_t)row * p.top_k + tid] = sid[tid];
         p.out_p[(size_t)row * p.top_k + tid] = (sx[tid] > -INFINITY) ? expf(sx[tid] - s_m) * s_inv : 0.f;
+    }
+}
+
+// ---------------------------------------------------------------------------------------
+// Whole adjusted distribution (b200rwkv_sample_probs): for samplers that read every probability (Mirostat, Typical, Nucleus
+// with top_k > 128), the vector run.rs:673-691 hands to Sampler::sample, softmax(logits - penalties, masked, + bias), written
+// from the slot's kept row.  Any num_vocab; same segments, adjustment and segment statistics as topk_segment_kernel.
+//   pass 1 (grid = segments x rows): load, adjust_segment, segment_stats; the adjusted segment goes to `out`;
+//   pass 2 (grid = segments x rows): every CTA combines its row's segment statistics in a fixed order (lane g of warp 0
+//            takes segments g, g + 32, ... in turn, then an xor tree), then writes expf(x - M) * (1 / S) over its segment
+//            with float4 (rows of `out` are 16-byte aligned: ld = V rounded up to 4) and a scalar tail for V % 4.
+// For num_vocab <= 65536 (at most 32 segments, one per lane) the combine and the expression are topk_merge_kernel's, so a
+// candidate's probability from sample_topk equals this row's entry bit for bit.  A disallowed token is exactly 0; a row
+// with every token disallowed is all zeros (sample_topk's probabilities on such a row are 0 as well).
+// ---------------------------------------------------------------------------------------
+struct ProbsParams {
+    const float* keep;          // [S][V] last logits row of every slot
+    int V, nseg, ld;            // ld: row stride of `out` in floats, V rounded up to a multiple of 4
+    SampleAdjust adj;
+    float* out;                 // [nrows][ld]: adjusted logits after pass 1, probabilities after pass 2
+    float2* stats;              // [nrows][nseg] (max, sum exp(x - max))
+};
+
+__global__ void __launch_bounds__(TOPK_SEG_THREADS) probs_stats_kernel(const __grid_constant__ ProbsParams p) {
+    __shared__ float sx[TOPK_SEG];
+    __shared__ float red[32];
+    const int seg = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
+    const int seg0 = seg * TOPK_SEG;
+    const float* src = p.keep + (size_t)p.adj.slot[row] * p.V;
+#pragma unroll
+    for (int j = 0; j < TOPK_SEG / TOPK_SEG_THREADS; ++j) {
+        const int li = tid + TOPK_SEG_THREADS * j, i = seg0 + li;
+        sx[li] = (i < p.V) ? src[i] : -INFINITY;
+    }
+    adjust_segment(sx, seg0, p.V, row, p.adj);
+    const float2 st = segment_stats(sx, red);
+    if (tid == 0) p.stats[(size_t)row * p.nseg + seg] = st;
+    float* dst = p.out + (size_t)row * p.ld;
+#pragma unroll
+    for (int j = 0; j < TOPK_SEG / TOPK_SEG_THREADS; ++j) {
+        const int li = tid + TOPK_SEG_THREADS * j, i = seg0 + li;
+        if (i < p.V) dst[i] = sx[li];
+    }
+}
+
+__global__ void __launch_bounds__(TOPK_SEG_THREADS) probs_write_kernel(const __grid_constant__ ProbsParams p) {
+    __shared__ float s_m, s_inv;
+    const int seg = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
+    if (tid < 32) {
+        const float2* st = p.stats + (size_t)row * p.nseg;
+        float m = -INFINITY;
+        for (int g = tid; g < p.nseg; g += 32) m = fmaxf(m, st[g].x);
+        const float M = warp_max(m);
+        float sc = 0.f;
+        for (int g = tid; g < p.nseg; g += 32) {
+            const float2 v = st[g];
+            sc += (v.x > -INFINITY) ? v.y * expf(v.x - M) : 0.f;
+        }
+        sc = warp_sum(sc);
+        if (tid == 0) { s_m = M; s_inv = 1.0f / sc; }
+    }
+    __syncthreads();
+    const float M = s_m, inv = s_inv;
+    float* x = p.out + (size_t)row * p.ld;
+    float4* x4 = reinterpret_cast<float4*>(x);
+    const int n4 = p.V >> 2;
+    const int q1 = min(n4, (seg + 1) * (TOPK_SEG / 4));
+    for (int q = seg * (TOPK_SEG / 4) + tid; q < q1; q += TOPK_SEG_THREADS) {
+        float4 v = x4[q];
+        v.x = (v.x > -INFINITY) ? expf(v.x - M) * inv : 0.f;
+        v.y = (v.y > -INFINITY) ? expf(v.y - M) * inv : 0.f;
+        v.z = (v.z > -INFINITY) ? expf(v.z - M) * inv : 0.f;
+        v.w = (v.w > -INFINITY) ? expf(v.w - M) * inv : 0.f;
+        x4[q] = v;
+    }
+    if (seg == p.nseg - 1 && tid < (p.V & 3)) {           // scalar tail
+        const float v = x[4 * n4 + tid];
+        x[4 * n4 + tid] = (v > -INFINITY) ? expf(v - M) * inv : 0.f;
     }
 }
 

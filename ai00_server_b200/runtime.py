@@ -369,11 +369,9 @@ class Model:
         capi.check(capi.lib().b200rwkv_softmax(self._h, x.shape[0], capi.ptr(x), capi.ptr(y)), self._h)
         return [y[i] for i in range(y.shape[0])]
 
-    def sample_topk(self, slots, penalties=None, bias=None, allow=None, top_k: int = 128):
-        """GPU front half of sampling (b200rwkv_sample_topk): for each slot the `top_k` most probable tokens of its last
-        logits row after penalties / grammar mask / bias, as (ids [n, top_k] uint32, probs [n, top_k] f32).
-        penalties, bias: per-slot dict token -> value (the reference's HashMaps, nucleus.rs:29, run.rs:679);
-        allow: optional [n, V] bool array (tokens the formatter allows)."""
+    def _sample_args(self, slots, penalties, bias, allow):
+        """The slot list and adjustment lists of the sampling entries as C arrays: (slots, penalty offsets / tokens / values,
+        allow bits or None, bias offsets / tokens / values)."""
         n = len(slots)
         V = self.info["num_vocab"]
 
@@ -396,13 +394,33 @@ class Model:
             padded = np.zeros((n, words * 32), bool)
             padded[:, :V] = a
             bits = np.ascontiguousarray(np.packbits(padded.reshape(n, words, 32), axis=2, bitorder="little").view(np.uint32).reshape(n, words))
+        return np.asarray(slots, np.int32), po, pt, pv, bits, bo, bt, bv
+
+    def sample_topk(self, slots, penalties=None, bias=None, allow=None, top_k: int = 128):
+        """GPU front half of sampling (b200rwkv_sample_topk): for each slot the `top_k` most probable tokens of its last
+        logits row after penalties / grammar mask / bias, as (ids [n, top_k] uint32, probs [n, top_k] f32).
+        penalties, bias: per-slot dict token -> value (the reference's HashMaps, nucleus.rs:29, run.rs:679);
+        allow: optional [n, V] bool array (tokens the formatter allows)."""
+        n = len(slots)
+        a_slot, po, pt, pv, bits, bo, bt, bv = self._sample_args(slots, penalties, bias, allow)
         ids = np.empty((n, top_k), np.uint32)
         probs = np.empty((n, top_k), np.float32)
-        a_slot = np.asarray(slots, np.int32)
         capi.check(capi.lib().b200rwkv_sample_topk(self._h, n, capi.ptr(a_slot), capi.ptr(po), capi.ptr(pt), capi.ptr(pv),
                                                    capi.ptr(bits) if bits is not None else None, capi.ptr(bo), capi.ptr(bt),
                                                    capi.ptr(bv), top_k, capi.ptr(ids), capi.ptr(probs)), self._h)
         return ids, probs
+
+    def sample_probs(self, slots, penalties=None, bias=None, allow=None) -> np.ndarray:
+        """The whole adjusted distribution of each slot's last logits row (b200rwkv_sample_probs): softmax of the row after
+        penalties / grammar mask / bias, [n, V] f32 -- what run.rs:673-691 hands to Sampler::sample, for the samplers that
+        read every probability (Mirostat, Typical, Nucleus with top_k > 128).  Arguments as sample_topk."""
+        n = len(slots)
+        a_slot, po, pt, pv, bits, bo, bt, bv = self._sample_args(slots, penalties, bias, allow)
+        out = np.empty((n, self.info["num_vocab"]), np.float32)
+        capi.check(capi.lib().b200rwkv_sample_probs(self._h, n, capi.ptr(a_slot), capi.ptr(po), capi.ptr(pt), capi.ptr(pv),
+                                                    capi.ptr(bits) if bits is not None else None, capi.ptr(bo), capi.ptr(bt),
+                                                    capi.ptr(bv), capi.ptr(out)), self._h)
+        return out
 
     def launch_count(self) -> int:
         n = C.c_int64(0)

@@ -140,7 +140,7 @@ int32_t b200rwkv_get_info(b200rwkv_engine*, b200rwkv_info* out);
  * ntok[i] rows for FULL, none for NONE; rows_out[i] receives the row count of entry i
  * (== RnnOutputBatch being empty or not, run.rs:1146-1155).  `logits_cap` is in floats.
  * `logits_out` may be NULL: nothing is copied to the host, the last row of every slot stays in HBM for
- * b200rwkv_sample_topk.  Token ids >= num_vocab are B200RWKV_ERR_INVALID. */
+ * b200rwkv_sample_topk / b200rwkv_sample_probs.  Token ids >= num_vocab are B200RWKV_ERR_INVALID. */
 int32_t b200rwkv_infer(b200rwkv_engine*, int32_t nslot, const int32_t* slot, const int32_t* ntok,
                        const uint32_t* tokens, const int32_t* option, float* logits_out,
                        size_t logits_cap, int32_t* rows_out);
@@ -217,12 +217,33 @@ int32_t b200rwkv_softmax(b200rwkv_engine*, int32_t rows, const float* in, float*
  * (tokens distinct within one row's penalty list and within its bias list, as the reference's HashMaps are), with
  * probs = softmax over the whole adjusted row.  Order: logit descending, token id ascending on ties.  ids_out / probs_out:
  * [nrows][top_k].  The draw itself (top_p cut, temperature, RNG, penalty update; nucleus.rs:81-123) stays in the host
- * sampler, now over <= 128 pairs.  Samplers that need the whole distribution (Mirostat, Typical) keep using
- * b200rwkv_infer with a logits buffer + b200rwkv_softmax.  Thread contract: the softmax task's (run.rs:1237). */
+ * sampler, now over <= 128 pairs.  Samplers that need the whole distribution (Mirostat, Typical, Nucleus with top_k > 128)
+ * use b200rwkv_sample_probs below.  A row whose every token is disallowed yields ids 0 .. top_k-1, each with probability 0.
+ * Thread contract: the softmax task's (run.rs:1237). */
 int32_t b200rwkv_sample_topk(b200rwkv_engine*, int32_t nrows, const int32_t* slots, const int32_t* penalty_offset,
                              const uint32_t* penalty_token, const float* penalty_value, const uint32_t* allow_bits,
                              const int32_t* bias_offset, const uint32_t* bias_token, const float* bias_value, int32_t top_k,
                              uint32_t* ids_out, float* probs_out);
+
+/* The whole adjusted distribution on the device, for samplers that read every probability: MirostatSampler
+ * (sampler/mirostat.rs:44-90), TypicalSampler (sampler/typical.rs:70-131) and NucleusSampler with top_k > 128.  Writes, for
+ * each listed slot's most recent logits row (the row b200rwkv_sample_topk reads), exactly the vector run.rs:673-691 hands to
+ * `Sampler::sample`: probs_out[i] = softmax(row adjusted as in b200rwkv_sample_topk), [nrows][num_vocab] f32, the adjustment
+ * lists meaning and validated what they do there (allow_bits may be NULL).  The sampler itself stays on the host, unchanged.
+ *   - probabilities are expf(x - max) * (1 / sum expf(x - max)) in f32; a disallowed token is exactly 0.  For num_vocab <=
+ *     65536 every candidate probability b200rwkv_sample_topk returns for the same row and lists equals probs_out[i][id].
+ *   - a row whose every token is disallowed is all zeros, as b200rwkv_sample_topk's probabilities are on such a row.
+ *   - any num_vocab.  A row's result depends neither on which other rows the call lists nor on their order.
+ *   - every argument is checked before the first CUDA call: nrows outside [1, max_batch], NULL slots / probs_out, a duplicate
+ *     slot or bad adjustment lists are B200RWKV_ERR_INVALID; a slot out of range or without a kept row is B200RWKV_ERR_STATE.
+ *   - the kept rows are not modified.  Tensor parallel engines run it on rank 0, which holds the gathered rows.
+ * With b200rwkv_infer(logits_out = NULL) first, one num_vocab f32 row per slot crosses PCIe per token (256 KiB at 65536)
+ * instead of a logits copy, an upload of the adjusted row and a probabilities copy.  probs_out may be any host memory; pinned
+ * memory (b200rwkv_host_alloc) makes that copy about 4x faster (DESIGN.md §6).  Thread contract: the softmax task's
+ * (run.rs:1237), as b200rwkv_sample_topk. */
+int32_t b200rwkv_sample_probs(b200rwkv_engine*, int32_t nrows, const int32_t* slots, const int32_t* penalty_offset,
+                              const uint32_t* penalty_token, const float* penalty_value, const uint32_t* allow_bits,
+                              const int32_t* bias_offset, const uint32_t* bias_token, const float* bias_value, float* probs_out);
 
 /* Pinned host memory for logits / state buffers (full-rate DMA); optional. */
 int32_t b200rwkv_host_alloc(size_t bytes, void** out);
