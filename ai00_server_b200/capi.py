@@ -60,6 +60,48 @@ class WkvArgs(C.Structure):
                 ("decay_bias", C.c_void_p), ("Dd", C.c_int32), ("state", C.c_void_p), ("out", C.c_void_p)]
 
 
+class LnArgs(C.Structure):
+    """b200rwkv_ln_args (include/b200rwkv.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("stage", "C", "S", "nslot")] + [
+                (n, C.c_void_p) for n in ("slot", "count", "option")] + [
+                ("precision", C.c_int32), ("launches", C.c_int32), ("x_in", C.c_void_p), ("n_parts", C.c_int32),
+                ("n_gate", C.c_int32)] + [
+                (n, C.c_void_p) for n in ("parts", "gates", "ln_w", "ln_b", "shift_state")] + [
+                ("n_mix", C.c_int32)] + [
+                (n, C.c_void_p) for n in ("mu", "commit_src", "commit_dst", "hidden", "x_out", "xx_out", "sx_out", "mix_out")] + [
+                ("Dm", C.c_int32)] + [
+                (n, C.c_void_p) for n in ("W1", "W2", "mu5", "lora_out", "out5", "emb")] + [
+                ("V", C.c_int32), ("tokens", C.c_void_p), ("head_out", C.c_void_p), ("kernel_out", C.c_void_p)]
+
+
+LN_EMBED, LN_MIX, LN_FRONT6, LN_OUT = range(4)                     # b200rwkv_ln_args.stage
+K_EMBED, K_LN_MIX, K_LN_MIX_CLUSTER, K_PRE6, K_LN_OUT = range(5)   # kernel_out[0]
+
+
+def op_ln(stage: int, channels: int, slots, counts, launches: int = 1, precision: int = 0, option=None, device: int = 0, **arrays):
+    """One LN stage of a step (b200rwkv_op_ln), `launches` times back to back.  `arrays` holds the struct's array members by
+    name (numpy arrays of the header's element types; absent = NULL); output arrays are updated in place.  Returns
+    kernel_out: (kernel, variant, split)."""
+    slots, counts = np.ascontiguousarray(slots, np.int32), np.ascontiguousarray(counts, np.int32)
+    keep = [slots, counts]
+    a = LnArgs(stage=stage, C=channels, S=int(arrays.pop("S")), nslot=len(slots), slot=ptr(slots), count=ptr(counts),
+               precision=precision, launches=launches, n_parts=int(arrays.pop("n_parts", 0)), n_gate=int(arrays.pop("n_gate", 0)),
+               n_mix=int(arrays.pop("n_mix", 0)), Dm=int(arrays.pop("Dm", 0)), V=int(arrays.pop("V", 0)))
+    if option is not None:
+        option = np.ascontiguousarray(option, np.int32)
+        keep.append(option)
+        a.option = ptr(option)
+    for name, arr in arrays.items():
+        if arr is None:
+            continue
+        assert isinstance(arr, np.ndarray) and arr.flags.c_contiguous, name
+        setattr(a, name, ptr(arr))
+    kern = np.zeros(3, np.int32)
+    a.kernel_out = ptr(kern)
+    check(lib().b200rwkv_op_ln(device, C.byref(a)))
+    return tuple(int(v) for v in kern)
+
+
 ACT_NONE, ACT_TANH, ACT_SIGMOID, ACT_SILU, ACT_RELU2, ACT_EXPNEGEXP, ACT_V7DECAY = range(7)
 OUT_F32, OUT_A16, OUT_LERP_A16 = 0, 1, 2
 
@@ -112,6 +154,7 @@ SYMBOLS = [
     ("b200rwkv_profile_insitu", C.c_int32, [_P, C.c_int32, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, C.POINTER(C.c_double)]),
     ("b200rwkv_op_quantize", C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P]),
     ("b200rwkv_op_wkv", C.c_int32, [C.c_int32, C.POINTER(WkvArgs)]),
+    ("b200rwkv_op_ln", C.c_int32, [C.c_int32, C.POINTER(LnArgs)]),
     ("b200rwkv_op_gemm", C.c_int32, [C.c_int32] * 7 + [C.POINTER(GemmSeg), C.POINTER(C.c_int32 * 4)]),
     ("b200rwkv_launch_count", C.c_int32, [_P, C.POINTER(C.c_int64)]),
     ("b200rwkv_keep_hidden", C.c_int32, [_P, C.c_int32]),

@@ -372,6 +372,20 @@ struct Profiler {
 
 struct Snapshot { float* buf = nullptr; float* logits = nullptr; size_t bytes = 0; };   // CachedItem {state, output} on the device (run.rs:199-205)
 
+// The LN-stage kernel a launch picked (b200rwkv_ln_args::kernel_out): kernel, its NV (float4 per thread of the per-token
+// kernels) or Dm / 16 (pre6_kernel), and whether it wrote split (hi + lo) operands.
+enum LnKernel { LNK_EMBED = 0, LNK_MIX = 1, LNK_MIX_CLUSTER = 2, LNK_PRE6 = 3, LNK_OUT = 4 };
+struct LnPick { int kernel, variant, split; };
+// float4 per thread of the per-token LN kernels: the NV that ln_mix_row / embed_row / ln_out_row dispatch to
+static inline int ln_nv(int C) {
+    const int nv = (C + 4 * LN_THREADS - 1) / (4 * LN_THREADS);
+    return nv <= 1 ? 1 : nv == 2 ? 2 : nv <= 4 ? 4 : 8;
+}
+// the cluster LN kernels hold one float4 per thread of each of the 8 channel slices
+static inline bool ln_cluster_fits(int C) { return C % (4 * PRE_CLUSTER) == 0 && C / (4 * PRE_CLUSTER) <= PRE_THREADS; }
+// pre6_kernel: LoRA rank Dm as its KD = Dm / 16 instantiations, 16-wide k steps in every 8-way K slice, W1 fragments in registers
+static inline bool pre6_fits(int Dm, int C) { return (Dm == 32 || Dm == 64) && C % 128 == 0 && C <= PRE_MAX_C; }
+
 }  // namespace b200
 
 using namespace b200;
@@ -545,6 +559,11 @@ struct b200rwkv_engine {
     }
     void launch_gemm(const GemmLaunch& g, int MT, cudaStream_t s, Profiler* prof, bool split = false);
     void launch_wkv(const WkvParams& p, int rows, int th, bool split, cudaStream_t s, Profiler* prof);
+    // LN stages of a step; each returns which kernel it launched
+    LnPick launch_embed(const EmbedParams& p, int rows, cudaStream_t s, Profiler* prof);
+    LnPick launch_ln(const LnMixParams& p, int MT, int th, cudaStream_t s, Profiler* prof);
+    LnPick launch_pre6(const Pre6Params& q, int th, cudaStream_t s, Profiler* prof);
+    LnPick launch_ln_out(const LnOutParams& p, int MT, int th_rows, cudaStream_t s, Profiler* prof);
     void enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* prof);
     void run_step(int MT, int MTR);
     int fill_meta(int* m, const std::vector<int>& slots, const std::vector<int>& counts, const std::vector<const uint32_t*>& toks,
@@ -981,7 +1000,7 @@ void b200rwkv_engine::build(const StFile& st) {
         d_logits = (float*)(comm_base + off_logits);
         d_epoch = (unsigned*)dalloc(16, true);
         pre_gbar = (unsigned*)dalloc(256, true);
-        ln_cluster_ok = C % (4 * PRE_CLUSTER) == 0 && C / (4 * PRE_CLUSTER) <= PRE_THREADS;
+        ln_cluster_ok = ln_cluster_fits(C);
         split_on = split_act && ln_cluster_ok;
         REQUIRE(precision != 1 || split_on, B200RWKV_ERR_UNSUPPORTED, "precision 1 needs num_emb to be a multiple of 32 and <= 8192");
     }
@@ -1127,7 +1146,7 @@ void b200rwkv_engine::build(const StFile& st) {
                         "time_mix_w2 must be [5, C, Dm]");
                 REQUIRE(d2.shape.size() == 2 && d2.shape[0] == C && d2.shape[1] == Dd, B200RWKV_ERR_INVALID, "time_decay_w2 must be [C, Dd]");
             }
-            if ((Dm == 32 || Dm == 64) && C % 128 == 0 && C <= PRE_MAX_C) {
+            if (pre6_fits(Dm, C)) {
                 auto upload_raw = [&](const StTensor& t) {
                     __half* d = (__half*)dalloc(t.nbytes, false);
                     CK(cudaMemcpy(d, t.data, t.nbytes, cudaMemcpyHostToDevice));
@@ -1402,18 +1421,11 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* pr
             if (g2.p.seg[i].out_mode != OUT_F32) g2.p.seg[i].ldo = th;      // A16 outputs feed a projection of this step
         launch_gemm(g2, mt, s, prof, split_on && MT == 1);      // split operands only when the whole step is decode-shaped
     };
-    launch_k(embed_ln0_kernel, dim3(rows), dim3(LN_THREADS), 0, embed, KC_LN, s, prof);
-    auto launch_ln = [&](const LnMixParams& lp0) {
+    launch_embed(embed, rows, s, prof);
+    auto ln_stage = [&](const LnMixParams& lp0) {
         LnMixParams lp = lp0;
         lp.trace = tr_next(0);
-        lp.kq_tile = th;
-        if (ln_cluster_ok && MT == 1) {
-            launch_cluster = PRE_CLUSTER;
-            if (split_on) launch_k(ln_mix_cluster_kernel<true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, lp, KC_LN, s, prof);
-            else launch_k(ln_mix_cluster_kernel<false>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, lp, KC_LN, s, prof);
-        } else {
-            launch_k(ln_mix_kernel, dim3(rows), dim3(LN_THREADS), 0, lp, KC_LN, s, prof);
-        }
+        launch_ln(lp, MT, th, s, prof);
     };
     for (int l = 0; l < L; ++l) {
         Layer& ly = layers[l];
@@ -1424,22 +1436,14 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* pr
             memset(&q, 0, sizeof(q));
             q.ln = ly.ln1;
             q.ln.trace = tr_next(6);
-            q.ln.kq_tile = th;
             q.W1 = ly.w1_raw; q.W2 = ly.w2_raw;
             for (int j = 0; j < 5; ++j) { q.mu[j] = ly.mu5[j]; q.out[j] = a_x[j].p; }
             q.lora = a_lora[0].p; q.lora_stride = (int)a_lora[0].halves_per_matrix; q.lora_kq = a_lora[0].kq;
             q.Dm = info.time_mix_adapter;
             q.gbar = pre_gbar;
-            launch_cluster = PRE_CLUSTER;
-            if (split_on) {
-                if (q.Dm == 32) launch_k(pre6_kernel<2, true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
-                else launch_k(pre6_kernel<4, true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
-            } else {
-                if (q.Dm == 32) launch_k(pre6_kernel<2, false>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
-                else launch_k(pre6_kernel<4, false>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
-            }
+            launch_pre6(q, th, s, prof);
         } else {
-            launch_ln(ly.ln1);
+            ln_stage(ly.ln1);
         }
         for (int gi = 0; gi < (int)ly.pre.size(); ++gi)
             if (!pre_skipped(ly, gi)) gemm(ly.pre[gi], MT);
@@ -1450,18 +1454,60 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* pr
         }
         gemm(ly.o, MT);
         if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
-        launch_ln(ly.ln2);
+        ln_stage(ly.ln2);
         for (auto& g : ly.ffn) gemm(g, MT);
         if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
     }
-    {
-        LnOutParams lo = lnout;
-        lo.kq_tile = th_rows;
-        if (split_on && MT == 1) launch_k(ln_out_kernel<true>, dim3(rows), dim3(LN_THREADS), 0, lo, KC_LN, s, prof);
-        else launch_k(ln_out_kernel<false>, dim3(rows), dim3(LN_THREADS), 0, lo, KC_LN, s, prof);
-    }
+    launch_ln_out(lnout, MT, th_rows, s, prof);
     if (MTR > 0) gemm(head, MTR);
     if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
+}
+
+// embedding gather + LN0 of a step of `rows` token rows: one CTA per row, CTAs past T exit
+LnPick b200rwkv_engine::launch_embed(const EmbedParams& p, int rows, cudaStream_t s, Profiler* prof) {
+    launch_k(embed_ln0_kernel, dim3(rows), dim3(LN_THREADS), 0, p, KC_LN, s, prof);
+    return {LNK_EMBED, ln_nv(p.C), 0};
+}
+
+// LN1 / LN2 of a step of MT token tiles whose A16 operands hold `th` rows: the 16 x 8 cluster kernel when the whole step is
+// decode-shaped and the row fits its slices (split operands with precision 1), else one CTA per token row
+LnPick b200rwkv_engine::launch_ln(const LnMixParams& p, int MT, int th, cudaStream_t s, Profiler* prof) {
+    LnMixParams lp = p;
+    lp.kq_tile = th;
+    if (ln_cluster_ok && MT == 1) {
+        launch_cluster = PRE_CLUSTER;
+        if (split_on) launch_k(ln_mix_cluster_kernel<true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, lp, KC_LN, s, prof);
+        else launch_k(ln_mix_cluster_kernel<false>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, lp, KC_LN, s, prof);
+        return {LNK_MIX_CLUSTER, 1, split_on ? 1 : 0};
+    }
+    launch_k(ln_mix_kernel, dim3(MT * 16), dim3(LN_THREADS), 0, lp, KC_LN, s, prof);
+    return {LNK_MIX, ln_nv(p.C), 0};
+}
+
+// RWKV-6 decode front half (LN1 + token shift + ddlerp LoRA) as one launch of 16 clusters x 8; the caller checked
+// pre6_fits(q.Dm, C) and that the step is decode-shaped (th = 16, or 32 with split operands)
+LnPick b200rwkv_engine::launch_pre6(const Pre6Params& q0, int th, cudaStream_t s, Profiler* prof) {
+    Pre6Params q = q0;
+    q.ln.kq_tile = th;
+    launch_cluster = PRE_CLUSTER;
+    if (split_on) {
+        if (q.Dm == 32) launch_k(pre6_kernel<2, true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
+        else launch_k(pre6_kernel<4, true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
+    } else {
+        if (q.Dm == 32) launch_k(pre6_kernel<2, false>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
+        else launch_k(pre6_kernel<4, false>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
+    }
+    return {LNK_PRE6, q.Dm / 16, split_on ? 1 : 0};
+}
+
+// final residual update + ln_out of a step of MT token tiles into the head operand of `th_rows` output rows
+LnPick b200rwkv_engine::launch_ln_out(const LnOutParams& p, int MT, int th_rows, cudaStream_t s, Profiler* prof) {
+    LnOutParams lo = p;
+    lo.kq_tile = th_rows;
+    const bool split = split_on && MT == 1;
+    if (split) launch_k(ln_out_kernel<true>, dim3(MT * 16), dim3(LN_THREADS), 0, lo, KC_LN, s, prof);
+    else launch_k(ln_out_kernel<false>, dim3(MT * 16), dim3(LN_THREADS), 0, lo, KC_LN, s, prof);
+    return {LNK_OUT, ln_nv(p.C), split ? 1 : 0};
 }
 
 static inline int mt_bucket(int rows) { return rows <= 16 ? 1 : (rows <= 32 ? 2 : (rows <= 64 ? 4 : 8)); }
@@ -2786,6 +2832,238 @@ int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args) {
         for (int c = 0; c < Cc; ++c) x.out[(size_t)m * Cc + c] = h16[a16_index(m, c, th)];
     CK(cudaMemcpy(x.state, p.state, state_bytes, cudaMemcpyDeviceToHost));
     if (version == 7) CK(cudaMemcpy(x.v_first, p.v_first, (size_t)T * Cc * 4, cudaMemcpyDeviceToHost));
+    API_END
+}
+
+// Operator-level entry for the parity tests: ONE LN stage of a step (embed + LN0, LN1 / LN2, the RWKV-6 front half or ln_out)
+// on caller-supplied rows and pool, no model.  The step metadata comes from the engine's fill_meta on a temporary engine
+// object, the parameter blocks are the kernels' own, and the launch from launch_embed / launch_ln / launch_pre6 /
+// launch_ln_out (kernel choice, cluster and programmatic-dependent-launch attributes, token rows of the operands): a step runs
+// exactly this.  tests/test_gpu_ln.py holds the LN kernels to a float64 reference through it.
+int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
+    API_BEGIN((b200rwkv_engine*)nullptr)
+    REQUIRE(args, B200RWKV_ERR_INVALID, "null arguments");
+    const b200rwkv_ln_args& x = *args;
+    const int stage = x.stage, C = x.C, S = x.S, NL = x.launches;
+    REQUIRE(stage >= 0 && stage <= 3, B200RWKV_ERR_INVALID, "stage must be 0 (embed), 1 (LN), 2 (front half) or 3 (ln_out)");
+    REQUIRE(C >= 64 && C <= LN_MAXC && C % 64 == 0, B200RWKV_ERR_INVALID, "C must be a multiple of 64 and <= 8192");
+    REQUIRE(S >= 1 && S <= 1024, B200RWKV_ERR_INVALID, "S must be 1..1024 (max_batch)");
+    REQUIRE(x.nslot >= 1 && x.nslot <= S && x.slot && x.count, B200RWKV_ERR_INVALID, "nslot must be 1..S with slot and count");
+    REQUIRE(x.precision == 0 || x.precision == 1, B200RWKV_ERR_INVALID, "precision must be 0 or 1");
+    REQUIRE(NL >= 1 && NL <= 16, B200RWKV_ERR_INVALID, "launches must be 1..16");
+    std::vector<char> seen(S, 0);
+    int T = 0;
+    for (int i = 0; i < x.nslot; ++i) {
+        REQUIRE(x.slot[i] >= 0 && x.slot[i] < S, B200RWKV_ERR_STATE, "slot out of range");
+        REQUIRE(!seen[x.slot[i]], B200RWKV_ERR_INVALID, "duplicate slot in one step");
+        seen[x.slot[i]] = 1;
+        REQUIRE(x.count[i] >= 1 && x.count[i] <= A16_MAX_ROWS - T, B200RWKV_ERR_INVALID, "counts must be >= 1 and sum to <= 128");
+        T += x.count[i];
+    }
+    const bool split = x.precision == 1;
+    REQUIRE(!split || T <= 16, B200RWKV_ERR_UNSUPPORTED, "precision 1 runs decode-shaped steps (T <= 16)");
+    if (stage == 0) {
+        REQUIRE(x.emb && x.V >= 1 && x.tokens && x.ln_w && x.ln_b && x.x_out, B200RWKV_ERR_INVALID,
+                "embed needs emb, V >= 1, tokens, ln_w, ln_b and x_out");
+        for (size_t i = 0; i < (size_t)NL * T; ++i)
+            REQUIRE(x.tokens[i] < (uint32_t)x.V, B200RWKV_ERR_INVALID, "token id " + std::to_string(x.tokens[i]) + " is outside the vocabulary");
+    } else {
+        REQUIRE(x.x_in && x.ln_w && x.ln_b, B200RWKV_ERR_INVALID, "null x_in, ln_w or ln_b");
+        REQUIRE(x.n_parts >= 0 && x.n_parts <= 8 && x.n_gate >= 0 && x.n_gate <= 8, B200RWKV_ERR_INVALID, "n_parts and n_gate must be 0..8");
+        REQUIRE(x.n_parts == 0 || x.parts, B200RWKV_ERR_INVALID, "null parts");
+        REQUIRE(x.n_gate == 0 || x.gates, B200RWKV_ERR_INVALID, "null gates");
+        REQUIRE(x.n_gate == 0 || (C % x.n_gate == 0 && (C / x.n_gate) % 4 == 0), B200RWKV_ERR_INVALID,
+                "gate blocks (C / n_gate columns) must be whole multiples of 4 columns");
+        REQUIRE(!x.commit_src == !x.commit_dst, B200RWKV_ERR_INVALID, "the commit needs both commit_src and commit_dst");
+    }
+    if (stage == 1 || stage == 2) {
+        REQUIRE(x.n_mix >= 1 && x.n_mix <= 6, B200RWKV_ERR_INVALID, "n_mix must be 1..6");
+        REQUIRE(x.shift_state && x.mu && x.mix_out && x.xx_out, B200RWKV_ERR_INVALID, "null shift_state, mu, mix_out or xx_out");
+        REQUIRE(x.x_out || x.n_parts == 0, B200RWKV_ERR_INVALID, "in place (x_out NULL) takes no parts");
+    }
+    if (stage == 2) {
+        REQUIRE(T <= 16 && pre6_fits(x.Dm, C), B200RWKV_ERR_UNSUPPORTED,
+                "the front half runs decode-shaped steps (T <= 16) with Dm 32 or 64, C % 128 == 0 and C <= 4096");
+        REQUIRE(x.n_mix == 1 && x.sx_out && x.W1 && x.W2 && x.mu5 && x.lora_out && x.out5, B200RWKV_ERR_INVALID,
+                "the front half needs n_mix 1, sx_out, W1, W2, mu5, lora_out and out5");
+    }
+    std::vector<int> outmode(x.nslot, 0);
+    if (stage == 3) {
+        REQUIRE(x.option && x.head_out, B200RWKV_ERR_INVALID, "ln_out needs option and head_out");
+        for (int i = 0; i < x.nslot; ++i) {
+            REQUIRE(x.option[i] >= B200RWKV_OPTION_LAST && x.option[i] <= B200RWKV_OPTION_NONE, B200RWKV_ERR_INVALID, "bad option");
+            outmode[i] = x.option[i] == B200RWKV_OPTION_FULL ? 2 : (x.option[i] == B200RWKV_OPTION_LAST ? 1 : 0);
+        }
+    }
+
+    const int MT = mt_bucket(T), rows = 16 * MT;   // what enqueue_step derives from the step's token count
+    const int th = split ? 32 : rows;
+    CK(cudaSetDevice(device));
+    std::unique_ptr<b200rwkv_engine> e(new b200rwkv_engine());
+    e->dev = device;
+    e->S = S;                                      // e->maxT stays A16_MAX_ROWS: the metadata layout of every engine
+    e->ln_cluster_ok = ln_cluster_fits(C);         // as build() decides them for a model of C channels
+    e->split_on = split;
+    CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
+
+    auto up = [&](const void* h, size_t bytes) {
+        void* d = e->dalloc(bytes, false);
+        CK(cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice));
+        return d;
+    };
+    // step metadata of every launch (they differ only in the token ids)
+    std::vector<int> slots(x.slot, x.slot + x.nslot), counts(x.count, x.count + x.nslot);
+    std::vector<int*> metas(NL);
+    int R = 0;
+    for (int l = 0; l < NL; ++l) {
+        std::vector<uint32_t> tk(A16_MAX_ROWS, 0);
+        if (x.tokens) std::copy(x.tokens + (size_t)l * T, x.tokens + (size_t)(l + 1) * T, tk.begin());
+        std::vector<const uint32_t*> toks(x.nslot);
+        for (int i = 0, t0 = 0; i < x.nslot; t0 += counts[i], ++i) toks[i] = tk.data() + t0;
+        std::vector<int> meta(MetaView::ints(e->maxT, S), 0);
+        REQUIRE(e->fill_meta(meta.data(), slots, counts, toks, outmode, &R) == T, B200RWKV_ERR_INVALID, "internal: step metadata");
+        metas[l] = (int*)up(meta.data(), meta.size() * 4);
+    }
+    const int MTR = R > 0 ? mt_bucket(R) : 0;
+    const int th_rows = split ? 32 : 16 * MTR;     // the head operand holds output rows
+    const int hrows = split ? 32 : 16 * std::max(MTR, 1);
+
+    // per-token rows as the engine's activation buffers hold them: `rows` rows, the ones past T filled with NaN so that a read
+    // outside the step shows in the output
+    auto rows_up = [&](const float* h, int cols) -> float* {
+        float* d = (float*)e->dalloc((size_t)rows * cols * 4, false);
+        CK(cudaMemset(d, 0xFF, (size_t)rows * cols * 4));
+        CK(cudaMemcpy(d, h, (size_t)T * cols * 4, cudaMemcpyHostToDevice));
+        return d;
+    };
+    auto rows_down = [&](float* h, const float* d) { CK(cudaMemcpy(h, d, (size_t)T * C * 4, cudaMemcpyDeviceToHost)); };
+    // A16 operands: `nmat` matrices of K columns with `tr` token rows, exchanged with the caller as [nmat][tr][K]
+    auto a16_stride = [](int K) { return (size_t)cdiv(K, GEMM_BK) * A16_KB_HALVES; };
+    auto a16_up = [&](const uint16_t* h, int nmat, int K, int tr) {
+        const size_t st = a16_stride(K);
+        std::vector<uint16_t> b(st * nmat, 0);
+        for (int j = 0; j < nmat; ++j)
+            for (int m = 0; m < tr; ++m)
+                for (int k = 0; k < K; ++k) b[j * st + a16_index(m, k, tr)] = h[((size_t)j * tr + m) * K + k];
+        return (__half*)up(b.data(), b.size() * 2);
+    };
+    auto a16_down = [&](uint16_t* h, const __half* d, int nmat, int K, int tr) {
+        const size_t st = a16_stride(K);
+        std::vector<uint16_t> b(st * nmat);
+        CK(cudaMemcpy(b.data(), d, b.size() * 2, cudaMemcpyDeviceToHost));
+        for (int j = 0; j < nmat; ++j)
+            for (int m = 0; m < tr; ++m)
+                for (int k = 0; k < K; ++k) h[((size_t)j * tr + m) * K + k] = b[j * st + a16_index(m, k, tr)];
+    };
+
+    const size_t TC = (size_t)T * C;
+    const float* ln_w = (const float*)up(x.ln_w, (size_t)C * 4);
+    const float* ln_b = (const float*)up(x.ln_b, (size_t)C * 4);
+    float* cdst = x.commit_dst ? (float*)up(x.commit_dst, (size_t)S * C * 4) : nullptr;
+    unsigned* gbar = (unsigned*)e->dalloc(256, true);      // the front half's barrier counters, shared by every launch
+    float** hid_tab = nullptr;
+    std::vector<float*> hid_rows(NL, nullptr);
+    const int gcl = x.n_gate > 0 ? C / x.n_gate : 0;
+    auto residual = [&](auto& p, int l) {          // LnMixParams / LnOutParams: x_in + gate (.) sum parts of launch l
+        p.x_in = rows_up(x.x_in + l * TC, C);
+        p.C = C;
+        p.meta = MetaView{metas[l], e->maxT, S};
+        p.n_parts = x.n_parts;
+        for (int q = 0; q < x.n_parts; ++q) p.parts[q] = rows_up(x.parts + ((size_t)l * x.n_parts + q) * TC, C);
+        p.n_gate = x.n_gate;
+        p.gate_cl = gcl;
+        for (int q = 0; q < x.n_gate; ++q) p.gates[q] = rows_up(x.gates + ((size_t)l * x.n_gate + q) * T * gcl, gcl);
+        p.ln_w = ln_w; p.ln_b = ln_b;
+        p.commit_dst = cdst;
+        p.commit_src = x.commit_src ? rows_up(x.commit_src + l * TC, C) : nullptr;
+        if (x.hidden) hid_rows[l] = rows_up(x.hidden + l * TC, C);
+    };
+
+    std::vector<EmbedParams> em(NL);
+    std::vector<LnMixParams> lm(NL);
+    std::vector<Pre6Params> pq(NL);
+    std::vector<LnOutParams> lo(NL);
+    if (stage == 0) {
+        const __half* emb = (const __half*)up(x.emb, (size_t)x.V * C * 2);
+        for (int l = 0; l < NL; ++l) {
+            EmbedParams& p = em[l];
+            memset(&p, 0, sizeof(p));
+            p.emb = emb; p.C = C; p.V = x.V; p.meta = MetaView{metas[l], e->maxT, S};
+            p.ln_w = ln_w; p.ln_b = ln_b;
+            p.x_out = rows_up(x.x_out + l * TC, C);
+        }
+    } else if (stage == 1 || stage == 2) {
+        const float* shift = (const float*)up(x.shift_state, (size_t)S * C * 4);
+        const float* mu = (const float*)up(x.mu, (size_t)x.n_mix * C * 4);
+        if (x.hidden) hid_tab = (float**)e->dalloc((size_t)NL * sizeof(float*), true);
+        for (int l = 0; l < NL; ++l) {
+            LnMixParams& p = lm[l];
+            memset(&p, 0, sizeof(p));
+            residual(p, l);
+            p.x_out = x.x_out ? rows_up(x.x_out + l * TC, C) : const_cast<float*>(p.x_in);
+            p.shift_state = shift;
+            p.n_mix = x.n_mix;
+            const __half* mix = a16_up(x.mix_out + (size_t)l * x.n_mix * th * C, x.n_mix, C, th);
+            for (int j = 0; j < x.n_mix; ++j) { p.mu[j] = mu + (size_t)j * C; p.mix_out[j] = const_cast<__half*>(mix) + j * a16_stride(C); }
+            p.xx_out = rows_up(x.xx_out + l * TC, C);
+            p.sx_out = x.sx_out ? rows_up(x.sx_out + l * TC, C) : nullptr;
+            p.hid_slot = hid_tab ? hid_tab + l : nullptr;
+        }
+        if (hid_tab) CK(cudaMemcpy(hid_tab, hid_rows.data(), (size_t)NL * sizeof(float*), cudaMemcpyHostToDevice));
+        if (stage == 2) {
+            const int Dm = x.Dm;
+            const __half* W1 = (const __half*)up(x.W1, (size_t)5 * Dm * C * 2);
+            const __half* W2 = (const __half*)up(x.W2, (size_t)5 * C * Dm * 2);
+            const float* mu5 = (const float*)up(x.mu5, (size_t)5 * C * 4);
+            for (int l = 0; l < NL; ++l) {
+                Pre6Params& q = pq[l];
+                memset(&q, 0, sizeof(q));
+                q.ln = lm[l];
+                q.W1 = W1; q.W2 = W2;
+                const __half* o5 = a16_up(x.out5 + (size_t)l * 5 * th * C, 5, C, th);
+                for (int j = 0; j < 5; ++j) { q.mu[j] = mu5 + (size_t)j * C; q.out[j] = const_cast<__half*>(o5) + j * a16_stride(C); }
+                q.lora = const_cast<__half*>(a16_up(x.lora_out + (size_t)l * 5 * th * Dm, 5, Dm, th));
+                q.lora_stride = (int)a16_stride(Dm); q.lora_kq = rup(Dm, GEMM_BK) / 32;
+                q.Dm = Dm;
+                q.gbar = gbar;
+            }
+        }
+    } else {
+        for (int l = 0; l < NL; ++l) {
+            LnOutParams& p = lo[l];
+            memset(&p, 0, sizeof(p));
+            residual(p, l);
+            p.head_in = const_cast<__half*>(a16_up(x.head_out + (size_t)l * hrows * C, 1, C, hrows));
+            p.hidden_out = hid_rows[l];
+        }
+    }
+    CK(cudaDeviceSynchronize());                   // every upload has landed before the launches
+    LnPick pick{};
+    for (int l = 0; l < NL; ++l) {
+        if (stage == 0) pick = e->launch_embed(em[l], rows, e->stream, nullptr);
+        else if (stage == 1) pick = e->launch_ln(lm[l], MT, th, e->stream, nullptr);
+        else if (stage == 2) pick = e->launch_pre6(pq[l], th, e->stream, nullptr);
+        else pick = e->launch_ln_out(lo[l], MT, th_rows, e->stream, nullptr);
+    }
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(e->stream));
+    for (int l = 0; l < NL; ++l) {
+        if (stage == 0) { rows_down(x.x_out + l * TC, em[l].x_out); continue; }
+        if (x.hidden) rows_down(x.hidden + l * TC, hid_rows[l]);
+        if (stage == 3) { a16_down(x.head_out + (size_t)l * hrows * C, lo[l].head_in, 1, C, hrows); continue; }
+        const LnMixParams& p = lm[l];
+        if (x.x_out) rows_down(x.x_out + l * TC, p.x_out);
+        else rows_down(x.x_in + l * TC, p.x_in);
+        rows_down(x.xx_out + l * TC, p.xx_out);
+        if (x.sx_out) rows_down(x.sx_out + l * TC, p.sx_out);
+        a16_down(x.mix_out + (size_t)l * x.n_mix * th * C, p.mix_out[0], x.n_mix, C, th);
+        if (stage == 2) {
+            a16_down(x.out5 + (size_t)l * 5 * th * C, pq[l].out[0], 5, C, th);
+            a16_down(x.lora_out + (size_t)l * 5 * th * x.Dm, pq[l].lora, 5, x.Dm, th);
+        }
+    }
+    if (cdst) CK(cudaMemcpy(x.commit_dst, cdst, (size_t)S * C * 4, cudaMemcpyDeviceToHost));
+    if (x.kernel_out) { x.kernel_out[0] = pick.kernel; x.kernel_out[1] = pick.variant; x.kernel_out[2] = pick.split; }
     API_END
 }
 

@@ -315,6 +315,57 @@ typedef struct {
 } b200rwkv_wkv_args;
 int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args);
 
+/* Operator-level entry (parity tests): one LN stage of a forward step -- with the step's metadata, kernel choice, cluster
+ * and launch attributes and token-row layout -- on caller-supplied rows and a pool of S slots, no model.  Entries as in
+ * b200rwkv_op_wkv (nslot entries, count[i] >= 1 tokens for distinct pool slot slot[i], T = sum(count) <= 128); C is a
+ * multiple of 64, <= 8192.  `launches` (1..16) runs the stage back to back on one stream; per-token arrays carry a
+ * leading [launches] dimension, the pool arrays (shift_state, commit_dst) and the front half's barrier counters are shared.
+ *   stage 0 embed + LN0:  x_out[t] = LN0(f32(emb[tokens[t]])), emb [V][C] f16 bits, tokens [T] (< V), ln_w / ln_b = ln0.
+ *   stage 1 LN / mix (LN1, LN2):  a = x_in + g (.) sum_p parts[p]  (g: gate block c / (C / n_gate) of column c, 1 without
+ *     gates), x_out = a, xx = LN(a) (eps 1e-5), prev = shift_state[slot] for an entry's first token, else the LN of the
+ *     previous token's a; sx = prev - xx; mix_j = xx + sx mu_j (n_mix 1..6).  commit_dst[slot] <- commit_src[last token of
+ *     the entry] (both or neither); hidden (may be NULL) <- a through a device-resident table cell, as the engine records
+ *     layers; x_out NULL: in place (x_out is x_in, n_parts = 0), x_in then comes back as the device left it.
+ *   stage 2 RWKV-6 front half (T <= 16, Dm 32 or 64, C % 128 == 0, C <= 4096): stage 1 with n_mix = 1 (mu = time_mix_x),
+ *     then lora_j = tanh(W1_j mix_0) and out_j = xx + sx (mu5_j + W2_j lora_j), j < 5; W1 [5 Dm][C], W2 [5][C][Dm] f16 bits.
+ *   stage 3 ln_out:  a as in stage 1, head row option-row(t) = LN(a) for tokens that produce logits (option per entry:
+ *     OPTION_LAST / FULL / NONE), hidden (may be NULL) <- a, the commit as in stage 1.
+ *   n_parts, n_gate 0..8: parts [n_parts][T][C], gates [n_gate][T][C / n_gate] (C / n_gate a multiple of 4).
+ *   Outputs: x_out, xx_out, sx_out, hidden [T][C] f32; mix_out [n_mix][rows][C], lora_out [5][rows][Dm], out5 [5][rows][C],
+ *   head_out [rows][C] f16 bits, de-tiled; rows = 16 x token tiles (16 / 32 / 64 / 128 by T, for head_out by the logits
+ *   rows) or 32 with precision 1 (T <= 16), where hi sits at row t and lo at row t + 16.  The caller's contents are uploaded
+ *   first: cells the kernel does not write come back unchanged.  kernel_out (may be NULL) receives {kernel, variant, split}:
+ *   kernel 0 embed_ln0, 1 ln_mix, 2 ln_mix_cluster, 3 pre6 (variant Dm / 16), 4 ln_out; variant of the other kernels =
+ *   float4 per thread (1 / 2 / 4 / 8; always 1 in ln_mix_cluster). */
+typedef struct {
+    int32_t stage, C, S, nslot;
+    const int32_t *slot, *count;
+    const int32_t* option;
+    int32_t precision, launches;
+    float* x_in;
+    int32_t n_parts, n_gate;
+    const float *parts, *gates;
+    const float *ln_w, *ln_b;
+    const float* shift_state;
+    int32_t n_mix;
+    const float* mu;
+    const float* commit_src;
+    float* commit_dst;
+    float* hidden;
+    float *x_out, *xx_out, *sx_out;
+    uint16_t* mix_out;
+    int32_t Dm;
+    const uint16_t *W1, *W2;
+    const float* mu5;
+    uint16_t *lora_out, *out5;
+    const uint16_t* emb;
+    int32_t V;
+    const uint32_t* tokens;
+    uint16_t* head_out;
+    int32_t* kernel_out;
+} b200rwkv_ln_args;
+int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args);
+
 /* Operator-level entry (parity tests): one projection launch -- the engine's planner (stream-K cuts, forced grids, Int8 / NF4
  * quantisation at load) and its projection kernels -- over caller-supplied matrices, no model.  Segment i computes
  * act(x W^T + bias) with W [N, K] (row-major f16 bits) and x [launches][T][K] f32, rounded to the f16 operand on the device

@@ -212,15 +212,21 @@ def test_ctypes_structs_match_the_header(tmp_path):
                    '  printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b200rwkv_wkv_args), offsetof(b200rwkv_wkv_args, slot),\n'
                    '  offsetof(b200rwkv_wkv_args, precision), offsetof(b200rwkv_wkv_args, r), offsetof(b200rwkv_wkv_args, nu),\n'
                    '  offsetof(b200rwkv_wkv_args, layer0), offsetof(b200rwkv_wkv_args, v_first), offsetof(b200rwkv_wkv_args, Dd),\n'
-                   '  offsetof(b200rwkv_wkv_args, out)); return 0; }\n')
+                   '  offsetof(b200rwkv_wkv_args, out));\n'
+                   '  printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b200rwkv_ln_args), offsetof(b200rwkv_ln_args, slot),\n'
+                   '  offsetof(b200rwkv_ln_args, precision), offsetof(b200rwkv_ln_args, x_in), offsetof(b200rwkv_ln_args, parts),\n'
+                   '  offsetof(b200rwkv_ln_args, n_mix), offsetof(b200rwkv_ln_args, mix_out), offsetof(b200rwkv_ln_args, Dm),\n'
+                   '  offsetof(b200rwkv_ln_args, V), offsetof(b200rwkv_ln_args, kernel_out)); return 0; }\n')
     exe = tmp_path / "sz"
     subprocess.run([gcc, "-std=c99", "-Wall", "-Werror", "-I", os.path.join(root, "include"), str(src), "-o", str(exe)], check=True)
     got = [int(x) for x in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
-    O, G, W = capi.Options, capi.GemmSeg, capi.WkvArgs
+    O, G, W, L = capi.Options, capi.GemmSeg, capi.WkvArgs, capi.LnArgs
     assert got == [C.sizeof(O), O.devices.offset, O.lora_st.offset, O.quant_layers.offset, C.sizeof(capi.Info),
                    C.sizeof(G), G.act.offset, G.lerp_xx.offset, G.out.offset,
                    C.sizeof(W), W.slot.offset, W.precision.offset, W.r.offset, W.nu.offset, W.layer0.offset, W.v_first.offset,
-                   W.Dd.offset, W.out.offset]
+                   W.Dd.offset, W.out.offset,
+                   C.sizeof(L), L.slot.offset, L.precision.offset, L.x_in.offset, L.parts.offset, L.n_mix.offset,
+                   L.mix_out.offset, L.Dm.offset, L.V.offset, L.kernel_out.offset]
 
 
 def test_op_gemm_refuses_bad_arguments_without_a_gpu():
@@ -346,6 +352,100 @@ def test_op_wkv_refuses_bad_arguments_without_a_gpu():
         assert got == want, name
     if not _has_gpu():                       # well-formed arguments reach the device, and there is none: no CPU fallback
         for ok in (args(), args(**fold), args(version=5), args(version=7, layer0=0), args(counts=(8, 8), precision=1)):
+            assert call(ok) == capi.ERR_CUDA
+
+
+def test_op_ln_refuses_bad_arguments_without_a_gpu():
+    """b200rwkv_op_ln checks every argument before its first CUDA call: ERR_INVALID for malformed arguments, ERR_STATE for a
+    slot outside the pool, ERR_UNSUPPORTED for a front half or precision the kernels do not run."""
+    Cc, S, T, Dm, V = 256, 4, 5, 32, 10
+    tok = np.zeros((T, Cc), np.float32)
+    vec = np.zeros(8 * Cc, np.float32)
+    pool = np.zeros((S, Cc), np.float32)
+    a16 = np.zeros((8, 32, Cc), np.uint16)
+    ids = np.zeros(T, np.uint32)
+    bad_ids = np.full(T, V, np.uint32)
+    opt = np.zeros(2, np.int32)
+    bad_opt = np.array([0, 3], np.int32)
+    kern = np.zeros(3, np.int32)
+    P = capi.ptr
+
+    def args(slots=(1, 3), counts=(2, 3), **kw):
+        sl, cn = np.array(slots, np.int32), np.array(counts, np.int32)
+        a = capi.LnArgs(stage=capi.LN_MIX, C=Cc, S=S, nslot=len(sl), slot=P(sl), count=P(cn), option=P(opt), precision=0,
+                        launches=1, x_in=P(tok), n_parts=1, n_gate=1, parts=P(tok), gates=P(tok), ln_w=P(vec), ln_b=P(vec),
+                        shift_state=P(pool), n_mix=2, mu=P(vec), commit_src=P(tok), commit_dst=P(pool), hidden=P(tok),
+                        x_out=P(tok), xx_out=P(tok), sx_out=P(tok), mix_out=P(a16), Dm=Dm, W1=P(a16), W2=P(a16), mu5=P(vec),
+                        lora_out=P(a16), out5=P(a16), emb=P(a16), V=V, tokens=P(ids), head_out=P(a16), kernel_out=P(kern))
+        for k, val in kw.items():
+            setattr(a, k, val)
+        a._keep = (sl, cn)
+        return a
+
+    def call(a):
+        return capi.lib().b200rwkv_op_ln(0, C.byref(a))
+
+    six = dict(stage=capi.LN_FRONT6, n_mix=1)
+    INV, UNS, STA = capi.ERR_INVALID, capi.ERR_UNSUPPORTED, capi.ERR_STATE
+    cases = {
+        "null arguments": (capi.lib().b200rwkv_op_ln(0, None), INV),
+        "stage 4": (call(args(stage=4)), INV),
+        "C = 0": (call(args(C=0)), INV),
+        "C % 64": (call(args(C=96)), INV),
+        "C = 8256": (call(args(C=8256)), INV),
+        "S = 0": (call(args(S=0)), INV),
+        "S = 1025": (call(args(S=1025)), INV),
+        "no entry": (call(args(nslot=0)), INV),
+        "null slot ids": (call(args(slot=None)), INV),
+        "null counts": (call(args(count=None)), INV),
+        "slot = S": (call(args(slots=(1, 4))), STA),
+        "negative slot": (call(args(slots=(-1, 3))), STA),
+        "duplicate slot": (call(args(slots=(3, 3))), INV),
+        "count 0": (call(args(counts=(2, 0))), INV),
+        "129 tokens": (call(args(counts=(64, 65))), INV),
+        "precision 2": (call(args(precision=2)), INV),
+        "precision 1 at T = 17": (call(args(counts=(8, 9), precision=1)), UNS),
+        "no launch": (call(args(launches=0)), INV),
+        "17 launches": (call(args(launches=17)), INV),
+        "null x_in": (call(args(x_in=None)), INV),
+        "null ln_w": (call(args(ln_w=None)), INV),
+        "nine parts": (call(args(n_parts=9)), INV),
+        "negative n_gate": (call(args(n_gate=-1)), INV),
+        "nine gates": (call(args(n_gate=9)), INV),
+        "parts without buffer": (call(args(parts=None)), INV),
+        "gates without buffer": (call(args(gates=None)), INV),
+        "C / n_gate not whole": (call(args(n_gate=3)), INV),
+        "commit_src alone": (call(args(commit_dst=None)), INV),
+        "commit_dst alone": (call(args(commit_src=None)), INV),
+        "n_mix 0": (call(args(n_mix=0)), INV),
+        "n_mix 7": (call(args(n_mix=7)), INV),
+        "null shift_state": (call(args(shift_state=None)), INV),
+        "null mu": (call(args(mu=None)), INV),
+        "null mix_out": (call(args(mix_out=None)), INV),
+        "null xx_out": (call(args(xx_out=None)), INV),
+        "in place with parts": (call(args(x_out=None)), INV),
+        "front half, Dm 16": (call(args(**six, Dm=16)), UNS),
+        "front half, C % 128": (call(args(**six, C=192, n_gate=0)), UNS),
+        "front half, C = 4224": (call(args(**six, C=4224)), UNS),
+        "front half, T = 17": (call(args(**six, counts=(8, 9))), UNS),
+        "front half, two mixes": (call(args(**dict(six, n_mix=2))), INV),
+        "front half without sx_out": (call(args(**six, sx_out=None)), INV),
+        "front half without W1": (call(args(**six, W1=None)), INV),
+        "front half without out5": (call(args(**six, out5=None)), INV),
+        "ln_out without option": (call(args(stage=capi.LN_OUT, option=None)), INV),
+        "ln_out without head": (call(args(stage=capi.LN_OUT, head_out=None)), INV),
+        "ln_out, option 3": (call(args(stage=capi.LN_OUT, option=P(bad_opt))), INV),
+        "embed without emb": (call(args(stage=capi.LN_EMBED, emb=None)), INV),
+        "embed, V = 0": (call(args(stage=capi.LN_EMBED, V=0)), INV),
+        "embed without tokens": (call(args(stage=capi.LN_EMBED, tokens=None)), INV),
+        "embed, token V": (call(args(stage=capi.LN_EMBED, tokens=P(bad_ids))), INV),
+        "embed without x_out": (call(args(stage=capi.LN_EMBED, x_out=None)), INV),
+    }
+    for name, (got, want) in cases.items():
+        assert got == want, name
+    if not _has_gpu():                       # well-formed arguments reach the device, and there is none: no CPU fallback
+        for ok in (args(), args(x_out=None, n_parts=0), args(**six), args(**six, precision=1), args(stage=capi.LN_OUT),
+                   args(stage=capi.LN_EMBED), args(counts=(60, 68), n_gate=8, n_parts=8)):
             assert call(ok) == capi.ERR_CUDA
 
 
