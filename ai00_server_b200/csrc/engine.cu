@@ -376,6 +376,33 @@ struct Snapshot { float* buf = nullptr; float* logits = nullptr; size_t bytes = 
 // kernels) or Dm / 16 (pre6_kernel), and whether it wrote split (hi + lo) operands.
 enum LnKernel { LNK_EMBED = 0, LNK_MIX = 1, LNK_MIX_CLUSTER = 2, LNK_PRE6 = 3, LNK_OUT = 4 };
 struct LnPick { int kernel, variant, split; };
+// The launch shape of one step (b200rwkv_engine::step_shape): MT token tiles of 16 rows and MTR row tiles of the head (0: no
+// output rows), `rows` = 16 * MT rows of the per-token buffers, and the token rows th / th_rows of the step's A16 operands and
+// of the head's operand.  `split`: the operands hold hi + lo f16 rows (th = th_rows = 32).
+struct StepShape { int MT, MTR, rows, th, th_rows; bool split; };
+
+// The A16 layout (common.cuh) on the host.  a16_halves: halves of one matrix of K columns.  a16_pack / a16_unpack move `ncols`
+// columns of token rows between a caller's dense array and consecutive A16 matrices of K columns and `tr` token rows each (the
+// last matrix may be partial): column k of matrix j, row m is dense[j * mat_ld + m * row_ld + k].  a16_pack moves all `tr`
+// rows, a16_unpack the first `nrows` (any nrows <= A16_MAX_ROWS stays inside each matrix).
+static inline size_t a16_halves(int K) { return (size_t)cdiv(K, GEMM_BK) * A16_KB_HALVES; }
+static std::vector<uint16_t> a16_pack(const uint16_t* dense, int ncols, int K, int tr, size_t mat_ld, size_t row_ld) {
+    const size_t st = a16_halves(K);
+    std::vector<uint16_t> b(st * cdiv(ncols, K), 0);
+    for (int c = 0; c < ncols; ++c) {
+        const int j = c / K, k = c - j * K;
+        for (int m = 0; m < tr; ++m) b[j * st + a16_index(m, k, tr)] = dense[j * mat_ld + m * row_ld + k];
+    }
+    return b;
+}
+static void a16_unpack(const std::vector<uint16_t>& b, int ncols, int K, int tr, int nrows, size_t mat_ld, size_t row_ld,
+                       uint16_t* dense) {
+    const size_t st = a16_halves(K);
+    for (int c = 0; c < ncols; ++c) {
+        const int j = c / K, k = c - j * K;
+        for (int m = 0; m < nrows; ++m) dense[j * mat_ld + m * row_ld + k] = b[j * st + a16_index(m, k, tr)];
+    }
+}
 // float4 per thread of the per-token LN kernels: the NV that ln_mix_row / embed_row / ln_out_row dispatch to
 static inline int ln_nv(int C) {
     const int nv = (C + 4 * LN_THREADS - 1) / (4 * LN_THREADS);
@@ -557,15 +584,17 @@ struct b200rwkv_engine {
         step_trace_types[launches_last_step] = label;
         return d_step_trace + (size_t)STEP_TRACE_ROW * launches_last_step;
     }
-    void launch_gemm(const GemmLaunch& g, int MT, cudaStream_t s, Profiler* prof, bool split = false);
-    void launch_wkv(const WkvParams& p, int rows, int th, bool split, cudaStream_t s, Profiler* prof);
+    StepShape step_shape(int T, int R) const;
+    // `head`: the head projection, over the step's output rows
+    void launch_gemm(const GemmLaunch& g, const StepShape& sh, cudaStream_t s, Profiler* prof, bool head = false);
+    void launch_wkv(const WkvParams& p, const StepShape& sh, cudaStream_t s, Profiler* prof);
     // LN stages of a step; each returns which kernel it launched
-    LnPick launch_embed(const EmbedParams& p, int rows, cudaStream_t s, Profiler* prof);
-    LnPick launch_ln(const LnMixParams& p, int MT, int th, cudaStream_t s, Profiler* prof);
-    LnPick launch_pre6(const Pre6Params& q, int th, cudaStream_t s, Profiler* prof);
-    LnPick launch_ln_out(const LnOutParams& p, int MT, int th_rows, cudaStream_t s, Profiler* prof);
-    void enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* prof);
-    void run_step(int MT, int MTR);
+    LnPick launch_embed(const EmbedParams& p, const StepShape& sh, cudaStream_t s, Profiler* prof);
+    LnPick launch_ln(const LnMixParams& p, const StepShape& sh, cudaStream_t s, Profiler* prof);
+    LnPick launch_pre6(const Pre6Params& q, const StepShape& sh, cudaStream_t s, Profiler* prof);
+    LnPick launch_ln_out(const LnOutParams& p, const StepShape& sh, cudaStream_t s, Profiler* prof);
+    void enqueue_step(cudaStream_t s, const StepShape& sh, Profiler* prof);
+    void run_step(const StepShape& sh);
     int fill_meta(int* m, const std::vector<int>& slots, const std::vector<int>& counts, const std::vector<const uint32_t*>& toks,
                   const std::vector<int>& outmode /*0 none,1 last,2 full*/, int* R_out);
     // score == nullptr: b200rwkv_infer, which refuses OPTION_SCORE
@@ -695,9 +724,8 @@ float* b200rwkv_engine::vec_f32(const StFile& st, const std::string& name, size_
 
 A16Buf b200rwkv_engine::a16_alloc(int K, int nmat) {
     A16Buf b;
-    const int Kp = rup(K, GEMM_BK);          // whole 128-wide k blocks, zero padded
-    b.kq = Kp / 32;
-    b.halves_per_matrix = (size_t)(Kp / GEMM_BK) * A16_KB_HALVES;
+    b.kq = rup(K, GEMM_BK) / 32;             // whole 128-wide k blocks, zero padded
+    b.halves_per_matrix = a16_halves(K);
     b.p = (__half*)dalloc(b.halves_per_matrix * 2 * nmat, true);
     return b;
 }
@@ -841,9 +869,10 @@ void b200rwkv_engine::launch_k(void (*kern)(P, X...), dim3 grid, dim3 block, siz
     ++launches_last_step;
 }
 
-void b200rwkv_engine::launch_gemm(const GemmLaunch& g, int MT, cudaStream_t s, Profiler* prof, bool split) {
+void b200rwkv_engine::launch_gemm(const GemmLaunch& g, const StepShape& sh, cudaStream_t s, Profiler* prof, bool head) {
+    const int MT = head ? sh.MTR : sh.MT;
     if (g.qtype != QT_NONE) {
-        REQUIRE(!split, B200RWKV_ERR_UNSUPPORTED, "internal: quantised projections run with f16 activations");
+        REQUIRE(!sh.split, B200RWKV_ERR_UNSUPPORTED, "internal: quantised projections run with f16 activations");
         const int grid = MT >= 4 ? g.grid_wide : g.grid;
 #define QLAUNCH(MT_, QT_) launch_k(qgemm_kernel<MT_, QT_>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<MT_, QT_>::SMEM_BYTES, g.p, KC_GEMM, s, prof)
         if (g.qtype == QT_INT8) {
@@ -857,7 +886,7 @@ void b200rwkv_engine::launch_gemm(const GemmLaunch& g, int MT, cudaStream_t s, P
     // RING 2 = one stage less than fits, so the small kernels around a projection can share its SMs (findings r1 §7)
     switch (MT) {
         case 1:
-            if (split) launch_k(gemm_kernel<2, 2, true>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<2, 2>::SMEM_BYTES, g.p, KC_GEMM, s, prof);
+            if (sh.split) launch_k(gemm_kernel<2, 2, true>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<2, 2>::SMEM_BYTES, g.p, KC_GEMM, s, prof);
             else launch_k(gemm_kernel<1, 2>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<1, 2>::SMEM_BYTES, g.p, KC_GEMM, s, prof);
             break;
         case 2: launch_k(gemm_kernel<2>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<2>::SMEM_BYTES, g.p, KC_GEMM, s, prof); break;
@@ -866,15 +895,16 @@ void b200rwkv_engine::launch_gemm(const GemmLaunch& g, int MT, cudaStream_t s, P
     }
 }
 
-// The WKV launch of one step of `rows` token rows (16 x token tiles) whose A16 operands hold `th` rows: one CTA per (head, step
-// entry) over min(S, rows) entries (a step has at most one entry per token; CTAs past the step's entries exit), decay rows and
-// staged rows sized by the step shape, since a slot cannot hold more tokens than the step.  `split`: hi + lo output rows.
-void b200rwkv_engine::launch_wkv(const WkvParams& p, int rows, int th, bool split, cudaStream_t s, Profiler* prof) {
+// The WKV launch of one step: one CTA per (head, step entry) over min(S, rows) entries (a step has at most one entry per token;
+// CTAs past the step's entries exit), decay rows and staged rows sized by the step shape, since a slot cannot hold more tokens
+// than the step.  Split steps write hi + lo output rows.
+void b200rwkv_engine::launch_wkv(const WkvParams& p, const StepShape& sh, cudaStream_t s, Profiler* prof) {
     WkvParams wp = p;
-    wp.kq_tile = th; wp.d1_kq = th;
+    wp.kq_tile = sh.th; wp.d1_kq = sh.th;
+    const int rows = sh.rows;
     const dim3 grid(wp.H, std::min(S, rows));
-    const size_t sm_b = wkv_smem_bytes(wp.version, wp.version == 6 && wp.wd2t, wp.Dd, rows, split);
-    switch (wp.version * 2 + (split ? 1 : 0)) {
+    const size_t sm_b = wkv_smem_bytes(wp.version, wp.version == 6 && wp.wd2t, wp.Dd, rows, sh.split);
+    switch (wp.version * 2 + (sh.split ? 1 : 0)) {
         case 10: launch_k(wkv_kernel<5>, grid, dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
         case 11: launch_k(wkv_kernel<5, true>, grid, dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
         case 12: launch_k(wkv_kernel<6>, grid, dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
@@ -1399,18 +1429,14 @@ void b200rwkv_engine::finalize_tp() {
 // -----------------------------------------------------------------------------------------
 // one forward step over the tokens described by d_meta
 // -----------------------------------------------------------------------------------------
-void b200rwkv_engine::enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* prof) {
+void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler* prof) {
     launches_last_step = 0;
-    const int rows = MT * 16;
-    // token rows of this step's A16 operands (common.cuh): every producer and consumer of the step uses the same value
-    const int th = (split_on && MT == 1) ? 32 : 16 * MT;
-    const int th_rows = (split_on && MT == 1) ? 32 : 16 * MTR;        // the head's operand holds output rows
-    last_th = th;
+    last_th = sh.th;
     auto pre_skipped = [&](const Layer& ly, int gi) {
         if (fold_wd2 && gi == ly.wd2_index) return true;                 // the WKV kernel evaluates the decay LoRA stage 2
-        return fused_pre_ok && MT == 1 && ly.w1_raw && gi < 2;           // the front-half kernel holds both ddlerp LoRA stages
+        return fused_pre_ok && sh.MT == 1 && ly.w1_raw && gi < 2;        // the front-half kernel holds both ddlerp LoRA stages
     };
-    auto gemm = [&](const GemmLaunch& g, int mt) {
+    auto gemm = [&](const GemmLaunch& g, bool head = false) {
         GemmLaunch g2 = g;
         if (d_step_trace && trace_capture) {
             g2.p.trace = tr_next(1000000 + (int)(g.weight_bytes >> 20));
@@ -1418,18 +1444,18 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* pr
             step_trace_bytes[launches_last_step] = (long long)g.weight_bytes;
         }
         for (int i = 0; i < g2.p.nseg; ++i)
-            if (g2.p.seg[i].out_mode != OUT_F32) g2.p.seg[i].ldo = th;      // A16 outputs feed a projection of this step
-        launch_gemm(g2, mt, s, prof, split_on && MT == 1);      // split operands only when the whole step is decode-shaped
+            if (g2.p.seg[i].out_mode != OUT_F32) g2.p.seg[i].ldo = sh.th;   // A16 outputs feed a projection of this step
+        launch_gemm(g2, sh, s, prof, head);
     };
-    launch_embed(embed, rows, s, prof);
+    launch_embed(embed, sh, s, prof);
     auto ln_stage = [&](const LnMixParams& lp0) {
         LnMixParams lp = lp0;
         lp.trace = tr_next(0);
-        launch_ln(lp, MT, th, s, prof);
+        launch_ln(lp, sh, s, prof);
     };
     for (int l = 0; l < L; ++l) {
         Layer& ly = layers[l];
-        const bool fused = fused_pre_ok && MT == 1 && ly.w1_raw;
+        const bool fused = fused_pre_ok && sh.MT == 1 && ly.w1_raw;
         if (fused) {
             // LN1 + token shift + ddlerp LoRA (W1, tanh, W2, lerps) in one launch
             Pre6Params q;
@@ -1441,76 +1467,88 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, int MT, int MTR, Profiler* pr
             q.lora = a_lora[0].p; q.lora_stride = (int)a_lora[0].halves_per_matrix; q.lora_kq = a_lora[0].kq;
             q.Dm = info.time_mix_adapter;
             q.gbar = pre_gbar;
-            launch_pre6(q, th, s, prof);
+            launch_pre6(q, sh, s, prof);
         } else {
             ln_stage(ly.ln1);
         }
         for (int gi = 0; gi < (int)ly.pre.size(); ++gi)
-            if (!pre_skipped(ly, gi)) gemm(ly.pre[gi], MT);
+            if (!pre_skipped(ly, gi)) gemm(ly.pre[gi]);
         {
             WkvParams wp = ly.wkv;
             wp.trace = tr_next(2);
-            launch_wkv(wp, rows, th, split_on && MT == 1, s, prof);
+            launch_wkv(wp, sh, s, prof);
         }
-        gemm(ly.o, MT);
+        gemm(ly.o);
         if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
         ln_stage(ly.ln2);
-        for (auto& g : ly.ffn) gemm(g, MT);
+        for (auto& g : ly.ffn) gemm(g);
         if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
     }
-    launch_ln_out(lnout, MT, th_rows, s, prof);
-    if (MTR > 0) gemm(head, MTR);
+    launch_ln_out(lnout, sh, s, prof);
+    if (sh.MTR > 0) gemm(head, true);
     if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
 }
 
-// embedding gather + LN0 of a step of `rows` token rows: one CTA per row, CTAs past T exit
-LnPick b200rwkv_engine::launch_embed(const EmbedParams& p, int rows, cudaStream_t s, Profiler* prof) {
-    launch_k(embed_ln0_kernel, dim3(rows), dim3(LN_THREADS), 0, p, KC_LN, s, prof);
+// embedding gather + LN0 of a step: one CTA per token row, CTAs past T exit
+LnPick b200rwkv_engine::launch_embed(const EmbedParams& p, const StepShape& sh, cudaStream_t s, Profiler* prof) {
+    launch_k(embed_ln0_kernel, dim3(sh.rows), dim3(LN_THREADS), 0, p, KC_LN, s, prof);
     return {LNK_EMBED, ln_nv(p.C), 0};
 }
 
-// LN1 / LN2 of a step of MT token tiles whose A16 operands hold `th` rows: the 16 x 8 cluster kernel when the whole step is
-// decode-shaped and the row fits its slices (split operands with precision 1), else one CTA per token row
-LnPick b200rwkv_engine::launch_ln(const LnMixParams& p, int MT, int th, cudaStream_t s, Profiler* prof) {
+// LN1 / LN2 of a step: the 16 x 8 cluster kernel when the whole step is decode-shaped and the row fits its slices (split
+// operands with precision 1), else one CTA per token row
+LnPick b200rwkv_engine::launch_ln(const LnMixParams& p, const StepShape& sh, cudaStream_t s, Profiler* prof) {
     LnMixParams lp = p;
-    lp.kq_tile = th;
-    if (ln_cluster_ok && MT == 1) {
+    lp.kq_tile = sh.th;
+    if (ln_cluster_ok && sh.MT == 1) {
         launch_cluster = PRE_CLUSTER;
-        if (split_on) launch_k(ln_mix_cluster_kernel<true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, lp, KC_LN, s, prof);
+        if (sh.split) launch_k(ln_mix_cluster_kernel<true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, lp, KC_LN, s, prof);
         else launch_k(ln_mix_cluster_kernel<false>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, lp, KC_LN, s, prof);
-        return {LNK_MIX_CLUSTER, 1, split_on ? 1 : 0};
+        return {LNK_MIX_CLUSTER, 1, sh.split ? 1 : 0};
     }
-    launch_k(ln_mix_kernel, dim3(MT * 16), dim3(LN_THREADS), 0, lp, KC_LN, s, prof);
+    launch_k(ln_mix_kernel, dim3(sh.rows), dim3(LN_THREADS), 0, lp, KC_LN, s, prof);
     return {LNK_MIX, ln_nv(p.C), 0};
 }
 
 // RWKV-6 decode front half (LN1 + token shift + ddlerp LoRA) as one launch of 16 clusters x 8; the caller checked
-// pre6_fits(q.Dm, C) and that the step is decode-shaped (th = 16, or 32 with split operands)
-LnPick b200rwkv_engine::launch_pre6(const Pre6Params& q0, int th, cudaStream_t s, Profiler* prof) {
+// pre6_fits(q.Dm, C) and that the step is decode-shaped (MT == 1)
+LnPick b200rwkv_engine::launch_pre6(const Pre6Params& q0, const StepShape& sh, cudaStream_t s, Profiler* prof) {
     Pre6Params q = q0;
-    q.ln.kq_tile = th;
+    q.ln.kq_tile = sh.th;
     launch_cluster = PRE_CLUSTER;
-    if (split_on) {
+    if (sh.split) {
         if (q.Dm == 32) launch_k(pre6_kernel<2, true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
         else launch_k(pre6_kernel<4, true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
     } else {
         if (q.Dm == 32) launch_k(pre6_kernel<2, false>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
         else launch_k(pre6_kernel<4, false>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
     }
-    return {LNK_PRE6, q.Dm / 16, split_on ? 1 : 0};
+    return {LNK_PRE6, q.Dm / 16, sh.split ? 1 : 0};
 }
 
-// final residual update + ln_out of a step of MT token tiles into the head operand of `th_rows` output rows
-LnPick b200rwkv_engine::launch_ln_out(const LnOutParams& p, int MT, int th_rows, cudaStream_t s, Profiler* prof) {
+// final residual update + ln_out of a step into the head operand, which holds the step's output rows
+LnPick b200rwkv_engine::launch_ln_out(const LnOutParams& p, const StepShape& sh, cudaStream_t s, Profiler* prof) {
     LnOutParams lo = p;
-    lo.kq_tile = th_rows;
-    const bool split = split_on && MT == 1;
-    if (split) launch_k(ln_out_kernel<true>, dim3(MT * 16), dim3(LN_THREADS), 0, lo, KC_LN, s, prof);
-    else launch_k(ln_out_kernel<false>, dim3(MT * 16), dim3(LN_THREADS), 0, lo, KC_LN, s, prof);
-    return {LNK_OUT, ln_nv(p.C), split ? 1 : 0};
+    lo.kq_tile = sh.th_rows;
+    if (sh.split) launch_k(ln_out_kernel<true>, dim3(sh.rows), dim3(LN_THREADS), 0, lo, KC_LN, s, prof);
+    else launch_k(ln_out_kernel<false>, dim3(sh.rows), dim3(LN_THREADS), 0, lo, KC_LN, s, prof);
+    return {LNK_OUT, ln_nv(p.C), sh.split ? 1 : 0};
 }
 
 static inline int mt_bucket(int rows) { return rows <= 16 ? 1 : (rows <= 32 ? 2 : (rows <= 64 ? 4 : 8)); }
+
+// The shape of a step of T tokens and R output rows, for every launch of it.  Split operands only when the whole step is
+// decode-shaped: a precision-1 engine keeps its steps at <= 16 tokens (infer), the head's operand then holds 32 rows too.
+StepShape b200rwkv_engine::step_shape(int T, int R) const {
+    StepShape sh;
+    sh.MT = mt_bucket(T);
+    sh.MTR = R > 0 ? mt_bucket(R) : 0;
+    sh.rows = 16 * sh.MT;
+    sh.split = split_on && sh.MT == 1;
+    sh.th = sh.split ? 32 : sh.rows;
+    sh.th_rows = sh.split ? 32 : 16 * sh.MTR;
+    return sh;
+}
 
 // last logits row of every slot of this step -> keep[slot] (rank 0 gathers the vocabulary shards); see sample.cuh
 void b200rwkv_engine::enqueue_keep(cudaStream_t s, int MTR) {
@@ -1524,15 +1562,15 @@ void b200rwkv_engine::enqueue_keep(cudaStream_t s, int MTR) {
     launch_k(keep_rows_kernel, dim3(MTR * 16, KEEP_CHUNKS), dim3(KEEP_THREADS), 0, kp, KC_OTHER, s, nullptr);
 }
 
-void b200rwkv_engine::run_step(int MT, int MTR) {
-    const int key = MT * 8 + MTR;
+void b200rwkv_engine::run_step(const StepShape& sh) {
+    const int key = sh.MT * 8 + sh.MTR;
     auto it = graphs.find(key);
     if (it == graphs.end()) {
         cudaGraph_t g = nullptr;
         CK(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
         try {
-            enqueue_step(stream, MT, MTR, nullptr);
-            enqueue_keep(stream, MTR);
+            enqueue_step(stream, sh, nullptr);
+            enqueue_keep(stream, sh.MTR);
         } catch (...) {
             cudaStreamEndCapture(stream, &g);
             if (g) cudaGraphDestroy(g);
@@ -1720,7 +1758,7 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         last_T = T;
         CK(cudaMemcpyAsync(d_meta, hm, meta_ints * 4, cudaMemcpyHostToDevice, stream));
         CK(cudaEventRecord(meta_ev[mb], stream));
-        run_step(mt_bucket(T), R > 0 ? mt_bucket(R) : 0);
+        run_step(step_shape(T, R));
         // step rows [T][C] -> the rows of every token of this call, in entry order
         auto gather_rows = [&](float* dst, const float* src) {
             int t0 = 0;
@@ -2052,6 +2090,18 @@ int32_t Group::spmd(const std::function<int32_t(int)>& fn) {
         return B200RWKV_ERR_INVALID;             \
     }                                            \
     return B200RWKV_OK;
+
+// entries that answer a count: the count `body` returns, or the negative status of its failure
+template <typename F>
+static int32_t api_count(F body) {
+    int32_t n = 0;
+    const int32_t st = [&]() -> int32_t {
+        API_BEGIN((b200rwkv_engine*)nullptr)
+        n = body();
+        API_END
+    }();
+    return st < 0 ? st : n;
+}
 
 extern "C" {
 
@@ -2527,7 +2577,7 @@ static int32_t rank_bench_decode(b200rwkv_engine* e, int32_t nslot, const int32_
         marks.resize(steps);
         for (auto& m : marks) CK(cudaEventCreate(&m));
     }
-    const int MT = mt_bucket(nslot);
+    const StepShape sh = e->step_shape(nslot, nslot);
     for (int st = 0; st < nsteps; ++st) {
         if (st == warmup) {
             CK(cudaStreamSynchronize(e->stream));
@@ -2536,7 +2586,7 @@ static int32_t rank_bench_decode(b200rwkv_engine* e, int32_t nslot, const int32_
         }
         if (flush) CK(cudaMemsetAsync(flush, st & 0xff, flush_bytes, e->stream));
         CK(cudaMemcpyAsync(e->d_meta, d_all + (size_t)st * e->meta_ints, e->meta_ints * 4, cudaMemcpyDeviceToDevice, e->stream));
-        e->run_step(MT, MT);
+        e->run_step(sh);
         if (step_ms_out && st >= warmup) CK(cudaEventRecord(marks[st - warmup], e->stream));
     }
     CK(cudaEventRecord(eb, e->stream));
@@ -2570,8 +2620,7 @@ static int32_t rank_profile_step(b200rwkv_engine* e, int32_t nslot, const int32_
     CK(cudaMemcpyAsync(e->d_meta, all.data(), e->meta_ints * 4, cudaMemcpyHostToDevice, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     Profiler prof;
-    const int MT = mt_bucket(nslot);
-    e->enqueue_step(e->stream, MT, MT, &prof);
+    e->enqueue_step(e->stream, e->step_shape(nslot, nslot), &prof);
     CK(cudaStreamSynchronize(e->stream));
     for (int i = 0; i < 4; ++i) { ms[i] = 0.f; launches[i] = 0; }
     for (auto& r : prof.recs) {
@@ -2604,7 +2653,7 @@ static int32_t rank_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int3
     std::vector<int> all;
     build_decode_metas(e, nslot, slot, tokens, 1, all);
     CK(cudaMemcpyAsync(e->d_meta, all.data(), e->meta_ints * 4, cudaMemcpyHostToDevice, e->stream));
-    const int MT = mt_bucket(nslot);
+    const StepShape sh = e->step_shape(nslot, nslot);
     // traced copy of the step graph (the production graphs carry null trace pointers)
     e->trace_capture = true;
     e->step_trace_types.clear();
@@ -2613,7 +2662,7 @@ static int32_t rank_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int3
     cudaGraphExec_t ge = nullptr;
     CK(cudaStreamBeginCapture(e->stream, cudaStreamCaptureModeThreadLocal));
     try {
-        e->enqueue_step(e->stream, MT, MT, nullptr);
+        e->enqueue_step(e->stream, sh, nullptr);
     } catch (...) {
         cudaStreamEndCapture(e->stream, &g);
         if (g) cudaGraphDestroy(g);
@@ -2717,12 +2766,77 @@ int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int3
     API_END
 }
 
+// The step under an operator-level entry (b200rwkv_op_wkv / op_ln / op_gemm).  The constructor checks the step's entries
+// (slot, token count) before any CUDA call; start() makes a temporary engine object with the step's pool size and precision,
+// one metadata block per launch from its fill_meta and the step's shape from its step_shape: what a step of these entries
+// derives.
+struct OpStep {
+    int S, T = 0, R = 0;
+    bool split;
+    std::vector<int> slots, counts;
+    std::unique_ptr<b200rwkv_engine> e;
+    std::vector<int*> metas;                       // device, one per launch; e->d_meta is the first
+    StepShape sh{};
+
+    OpStep(int S_, int nslot, const int32_t* slot, const int32_t* count, int precision) : S(S_), split(precision == 1) {
+        REQUIRE(S >= 1 && S <= 1024, B200RWKV_ERR_INVALID, "S must be 1..1024 (max_batch)");
+        REQUIRE(nslot >= 1 && nslot <= S && slot && count, B200RWKV_ERR_INVALID, "nslot must be 1..S with slot and count");
+        REQUIRE(precision == 0 || precision == 1, B200RWKV_ERR_INVALID, "precision must be 0 or 1");
+        std::vector<char> seen(S, 0);
+        for (int i = 0; i < nslot; ++i) {
+            REQUIRE(slot[i] >= 0 && slot[i] < S, B200RWKV_ERR_STATE, "slot out of range");
+            REQUIRE(!seen[slot[i]], B200RWKV_ERR_INVALID, "duplicate slot in one step");
+            seen[slot[i]] = 1;
+            REQUIRE(count[i] >= 1 && count[i] <= A16_MAX_ROWS - T, B200RWKV_ERR_INVALID, "counts must be >= 1 and sum to <= 128");
+            T += count[i];
+        }
+        REQUIRE(!split || T <= 16, B200RWKV_ERR_UNSUPPORTED, "precision 1 runs decode-shaped steps (T <= 16)");
+        slots.assign(slot, slot + nslot);
+        counts.assign(count, count + nslot);
+    }
+    // tokens: [launches][T] ids, or null for id 0; outmode: fill_meta's, per entry
+    void start(int device, int launches, const uint32_t* tokens, const std::vector<int>& outmode) {
+        CK(cudaSetDevice(device));
+        e.reset(new b200rwkv_engine());
+        e->dev = device;
+        e->S = S;                                  // e->maxT stays A16_MAX_ROWS: the metadata layout of every engine
+        e->split_on = split;
+        CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
+        for (int l = 0; l < launches; ++l) {
+            std::vector<uint32_t> tk(A16_MAX_ROWS, 0);
+            if (tokens) std::copy(tokens + (size_t)l * T, tokens + (size_t)(l + 1) * T, tk.begin());
+            std::vector<const uint32_t*> toks(slots.size());
+            for (size_t i = 0, t0 = 0; i < slots.size(); t0 += counts[i], ++i) toks[i] = tk.data() + t0;
+            std::vector<int> meta(MetaView::ints(e->maxT, S), 0);
+            REQUIRE(e->fill_meta(meta.data(), slots, counts, toks, outmode, &R) == T, B200RWKV_ERR_INVALID, "internal: step metadata");
+            metas.push_back((int*)up(meta.data(), meta.size() * 4));
+        }
+        e->d_meta = metas[0];
+        sh = e->step_shape(T, R);
+    }
+    // the layout start() built the blocks with, whatever the entry sets e->maxT to afterwards
+    MetaView meta(int l) const { return MetaView{metas[l], A16_MAX_ROWS, S}; }
+    void* up(const void* h, size_t bytes) {
+        void* d = e->dalloc(bytes, false);
+        CK(cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice));
+        return d;
+    }
+    // per-token rows as the engine's activation buffers hold them: sh.rows rows, the ones past T filled with NaN so that a read
+    // outside the step shows in the output
+    float* rows_up(const float* h, int cols) {
+        if (!h) return nullptr;
+        float* d = (float*)e->dalloc((size_t)sh.rows * cols * 4, false);
+        CK(cudaMemset(d, 0xFF, (size_t)sh.rows * cols * 4));
+        CK(cudaMemcpy(d, h, (size_t)T * cols * 4, cudaMemcpyHostToDevice));
+        return d;
+    }
+};
+
 // Operator-level entry for the parity tests: ONE WKV launch of a step (recurrence + GroupNorm + bonus + gate) on caller-supplied
-// head vectors and state pool, no model around it.  The step metadata comes from the engine's fill_meta on a temporary engine
-// object, the launch from launch_wkv (kernel per version and output form, grid, shared memory, programmatic dependent launch),
-// the k-major decay slice from wd2_k_major and the d1 operand from the f16 conversion of the projection operands: a step runs
-// exactly this.  The committed fla fixtures (tests/golden/wkv6_fla.npz, wkv7_fla.npz) and the float64 reference of
-// tests/test_gpu_wkv.py reach the CUDA kernels through it.
+// head vectors and state pool, no model around it.  The step comes from OpStep, the launch from launch_wkv (kernel per version
+// and output form, grid, shared memory, programmatic dependent launch), the k-major decay slice from wd2_k_major and the d1
+// operand from the f16 conversion of the projection operands: a step runs exactly this.  The committed fla fixtures
+// (tests/golden/wkv6_fla.npz, wkv7_fla.npz) and the float64 reference of tests/test_gpu_wkv.py reach the CUDA kernels through it.
 int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args) {
     API_BEGIN((b200rwkv_engine*)nullptr)
     REQUIRE(args, B200RWKV_ERR_INVALID, "null arguments");
@@ -2730,20 +2844,7 @@ int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args) {
     const int version = x.version;
     REQUIRE(version == 5 || version == 6 || version == 7, B200RWKV_ERR_UNSUPPORTED, "version must be 5, 6 or 7");
     REQUIRE(x.H >= 1 && x.H <= 128, B200RWKV_ERR_INVALID, "H must be 1..128 (num_emb <= 8192)");
-    REQUIRE(x.S >= 1 && x.S <= 1024, B200RWKV_ERR_INVALID, "S must be 1..1024 (max_batch)");
-    REQUIRE(x.nslot >= 1 && x.nslot <= x.S && x.slot && x.count, B200RWKV_ERR_INVALID, "nslot must be 1..S with slot and count");
-    REQUIRE(x.precision == 0 || x.precision == 1, B200RWKV_ERR_INVALID, "precision must be 0 or 1");
-    std::vector<char> seen(x.S, 0);
-    int T = 0;
-    for (int i = 0; i < x.nslot; ++i) {
-        REQUIRE(x.slot[i] >= 0 && x.slot[i] < x.S, B200RWKV_ERR_STATE, "slot out of range");
-        REQUIRE(!seen[x.slot[i]], B200RWKV_ERR_INVALID, "duplicate slot in one step");
-        seen[x.slot[i]] = 1;
-        REQUIRE(x.count[i] >= 1 && x.count[i] <= A16_MAX_ROWS - T, B200RWKV_ERR_INVALID, "counts must be >= 1 and sum to <= 128");
-        T += x.count[i];
-    }
-    const bool split = x.precision == 1;
-    REQUIRE(!split || T <= 16, B200RWKV_ERR_UNSUPPORTED, "precision 1 runs decode-shaped steps (T <= 16)");
+    OpStep st(x.S, x.nslot, x.slot, x.count, x.precision);
     REQUIRE(x.r && x.k && x.v && x.g && x.lnx_w && x.lnx_b && x.state && x.out, B200RWKV_ERR_INVALID, "null r, k, v, g, ln_x, state or out");
     const bool fold = version == 6 && (x.d1 || x.time_decay_w2 || x.decay_bias);
     if (fold) {
@@ -2757,45 +2858,18 @@ int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args) {
         REQUIRE(x.layer0 || x.nu, B200RWKV_ERR_INVALID, "v7 layers after 0 need nu");
     }
 
-    const int H = x.H, S = x.S, Cc = H * 64;
-    const int MT = mt_bucket(T), rows = 16 * MT;   // what enqueue_step derives from the step's token count
-    const int th = split ? 32 : rows;
-    CK(cudaSetDevice(device));
-    std::unique_ptr<b200rwkv_engine> e(new b200rwkv_engine());
-    e->dev = device;
-    e->S = S;                                      // e->maxT stays A16_MAX_ROWS: the metadata layout of every engine
-    CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
+    const int H = x.H, S = x.S, Cc = H * 64, T = st.T;
+    st.start(device, 1, nullptr, std::vector<int>(x.nslot, 0));
+    const StepShape& sh = st.sh;
     wkv_smem_limits();
 
-    std::vector<int> slots(x.slot, x.slot + x.nslot), counts(x.count, x.count + x.nslot), outmode(x.nslot, 0);
-    std::vector<uint32_t> tok0(A16_MAX_ROWS, 0);
-    std::vector<const uint32_t*> toks(x.nslot, tok0.data());
-    std::vector<int> meta(MetaView::ints(e->maxT, S), 0);
-    int R = 0;
-    REQUIRE(e->fill_meta(meta.data(), slots, counts, toks, outmode, &R) == T, B200RWKV_ERR_INVALID, "internal: step metadata");
-    e->d_meta = (int*)e->dalloc(meta.size() * 4, false);
-    CK(cudaMemcpy(e->d_meta, meta.data(), meta.size() * 4, cudaMemcpyHostToDevice));
-
-    auto up = [&](const void* h, size_t bytes) {
-        void* d = e->dalloc(bytes, false);
-        CK(cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice));
-        return d;
-    };
-    // per-token rows as the engine's activation buffers hold them: `rows` rows, the ones past T filled with NaN so that a read
-    // outside the step shows in the output
-    auto rows_up = [&](const float* h) -> float* {
-        if (!h) return nullptr;
-        float* d = (float*)e->dalloc((size_t)rows * Cc * 4, false);
-        CK(cudaMemset(d, 0xFF, (size_t)rows * Cc * 4));
-        CK(cudaMemcpy(d, h, (size_t)T * Cc * 4, cudaMemcpyHostToDevice));
-        return d;
-    };
-    auto vec_up = [&](const float* h) { return h ? (const float*)up(h, (size_t)Cc * 4) : nullptr; };
+    auto rows_up = [&](const float* h) { return st.rows_up(h, Cc); };
+    auto vec_up = [&](const float* h) { return h ? (const float*)st.up(h, (size_t)Cc * 4) : nullptr; };
     WkvParams p;
     memset(&p, 0, sizeof(p));
-    p.version = version; p.ld = Cc; p.meta = MetaView{e->d_meta, e->maxT, S}; p.H = H;
+    p.version = version; p.ld = Cc; p.meta = st.meta(0); p.H = H;
     const size_t state_bytes = (size_t)S * H * 64 * 64 * 4;
-    p.state = (float*)up(x.state, state_bytes);
+    p.state = (float*)st.up(x.state, state_bytes);
     p.r = rows_up(x.r); p.k = rows_up(x.k); p.v = rows_up(x.v); p.g = rows_up(x.g);
     if (version == 5) p.w_static = vec_up(x.w);
     else if (!fold) p.w = rows_up(x.w);
@@ -2808,38 +2882,34 @@ int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args) {
     }
     if (fold) {
         const std::vector<__half> wt = wd2_k_major(reinterpret_cast<const __half*>(x.time_decay_w2), 0, H, x.Dd);
-        p.wd2t = (const __half*)up(wt.data(), wt.size() * 2);
+        p.wd2t = (const __half*)st.up(wt.data(), wt.size() * 2);
         p.decay_bias = vec_up(x.decay_bias);
         p.Dd = x.Dd;
-        float* d1 = (float*)up(x.d1, (size_t)T * x.Dd * 4);
-        __half* a16 = (__half*)e->dalloc((size_t)cdiv(x.Dd, GEMM_BK) * A16_KB_HALVES * 2, true);
-        a16_from_f32_kernel<<<cdiv(T * x.Dd, 256), 256>>>(d1, T, x.Dd, th, split, a16);
+        float* d1 = (float*)st.up(x.d1, (size_t)T * x.Dd * 4);
+        __half* a16 = (__half*)st.e->dalloc(a16_halves(x.Dd) * 2, true);
+        a16_from_f32_kernel<<<cdiv(T * x.Dd, 256), 256>>>(d1, T, x.Dd, sh.th, sh.split, a16);
         CK(cudaGetLastError());
         p.d1 = a16;
     }
     // the output in the A16 layout of `th` token rows, the caller's contents first
-    const size_t halves = (size_t)cdiv(Cc, GEMM_BK) * A16_KB_HALVES;
-    std::vector<uint16_t> h16(halves, 0);
-    for (int m = 0; m < th; ++m)
-        for (int c = 0; c < Cc; ++c) h16[a16_index(m, c, th)] = x.out[(size_t)m * Cc + c];
-    p.out = (__half*)up(h16.data(), halves * 2);
+    std::vector<uint16_t> h16 = a16_pack(x.out, Cc, Cc, sh.th, 0, Cc);
+    p.out = (__half*)st.up(h16.data(), h16.size() * 2);
     CK(cudaDeviceSynchronize());                   // every upload has landed before the launch
-    e->launch_wkv(p, rows, th, split, e->stream, nullptr);
+    st.e->launch_wkv(p, sh, st.e->stream, nullptr);
     CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(e->stream));
-    CK(cudaMemcpy(h16.data(), p.out, halves * 2, cudaMemcpyDeviceToHost));
-    for (int m = 0; m < th; ++m)
-        for (int c = 0; c < Cc; ++c) x.out[(size_t)m * Cc + c] = h16[a16_index(m, c, th)];
+    CK(cudaStreamSynchronize(st.e->stream));
+    CK(cudaMemcpy(h16.data(), p.out, h16.size() * 2, cudaMemcpyDeviceToHost));
+    a16_unpack(h16, Cc, Cc, sh.th, sh.th, 0, Cc, x.out);
     CK(cudaMemcpy(x.state, p.state, state_bytes, cudaMemcpyDeviceToHost));
     if (version == 7) CK(cudaMemcpy(x.v_first, p.v_first, (size_t)T * Cc * 4, cudaMemcpyDeviceToHost));
     API_END
 }
 
 // Operator-level entry for the parity tests: ONE LN stage of a step (embed + LN0, LN1 / LN2, the RWKV-6 front half or ln_out)
-// on caller-supplied rows and pool, no model.  The step metadata comes from the engine's fill_meta on a temporary engine
-// object, the parameter blocks are the kernels' own, and the launch from launch_embed / launch_ln / launch_pre6 /
-// launch_ln_out (kernel choice, cluster and programmatic-dependent-launch attributes, token rows of the operands): a step runs
-// exactly this.  tests/test_gpu_ln.py holds the LN kernels to a float64 reference through it.
+// on caller-supplied rows and pool, no model.  The step comes from OpStep, the parameter blocks are the kernels' own, and the
+// launch from launch_embed / launch_ln / launch_pre6 / launch_ln_out (kernel choice, cluster and programmatic-dependent-launch
+// attributes, token rows of the operands): a step runs exactly this.  tests/test_gpu_ln.py holds the LN kernels to a float64
+// reference through it.
 int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
     API_BEGIN((b200rwkv_engine*)nullptr)
     REQUIRE(args, B200RWKV_ERR_INVALID, "null arguments");
@@ -2847,21 +2917,9 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
     const int stage = x.stage, C = x.C, S = x.S, NL = x.launches;
     REQUIRE(stage >= 0 && stage <= 3, B200RWKV_ERR_INVALID, "stage must be 0 (embed), 1 (LN), 2 (front half) or 3 (ln_out)");
     REQUIRE(C >= 64 && C <= LN_MAXC && C % 64 == 0, B200RWKV_ERR_INVALID, "C must be a multiple of 64 and <= 8192");
-    REQUIRE(S >= 1 && S <= 1024, B200RWKV_ERR_INVALID, "S must be 1..1024 (max_batch)");
-    REQUIRE(x.nslot >= 1 && x.nslot <= S && x.slot && x.count, B200RWKV_ERR_INVALID, "nslot must be 1..S with slot and count");
-    REQUIRE(x.precision == 0 || x.precision == 1, B200RWKV_ERR_INVALID, "precision must be 0 or 1");
     REQUIRE(NL >= 1 && NL <= 16, B200RWKV_ERR_INVALID, "launches must be 1..16");
-    std::vector<char> seen(S, 0);
-    int T = 0;
-    for (int i = 0; i < x.nslot; ++i) {
-        REQUIRE(x.slot[i] >= 0 && x.slot[i] < S, B200RWKV_ERR_STATE, "slot out of range");
-        REQUIRE(!seen[x.slot[i]], B200RWKV_ERR_INVALID, "duplicate slot in one step");
-        seen[x.slot[i]] = 1;
-        REQUIRE(x.count[i] >= 1 && x.count[i] <= A16_MAX_ROWS - T, B200RWKV_ERR_INVALID, "counts must be >= 1 and sum to <= 128");
-        T += x.count[i];
-    }
-    const bool split = x.precision == 1;
-    REQUIRE(!split || T <= 16, B200RWKV_ERR_UNSUPPORTED, "precision 1 runs decode-shaped steps (T <= 16)");
+    OpStep st(S, x.nslot, x.slot, x.count, x.precision);
+    const int T = st.T;
     if (stage == 0) {
         REQUIRE(x.emb && x.V >= 1 && x.tokens && x.ln_w && x.ln_b && x.x_out, B200RWKV_ERR_INVALID,
                 "embed needs emb, V >= 1, tokens, ln_w, ln_b and x_out");
@@ -2896,87 +2954,46 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
         }
     }
 
-    const int MT = mt_bucket(T), rows = 16 * MT;   // what enqueue_step derives from the step's token count
-    const int th = split ? 32 : rows;
-    CK(cudaSetDevice(device));
-    std::unique_ptr<b200rwkv_engine> e(new b200rwkv_engine());
-    e->dev = device;
-    e->S = S;                                      // e->maxT stays A16_MAX_ROWS: the metadata layout of every engine
-    e->ln_cluster_ok = ln_cluster_fits(C);         // as build() decides them for a model of C channels
-    e->split_on = split;
-    CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
+    st.start(device, NL, x.tokens, outmode);
+    b200rwkv_engine* e = st.e.get();
+    e->ln_cluster_ok = ln_cluster_fits(C);         // as build() decides it for a model of C channels
+    const StepShape& sh = st.sh;
+    const int th = sh.th;
+    const int hrows = std::max(sh.th_rows, 16);    // the caller's head_out has 16 rows even when the step has no output row
 
-    auto up = [&](const void* h, size_t bytes) {
-        void* d = e->dalloc(bytes, false);
-        CK(cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice));
-        return d;
-    };
-    // step metadata of every launch (they differ only in the token ids)
-    std::vector<int> slots(x.slot, x.slot + x.nslot), counts(x.count, x.count + x.nslot);
-    std::vector<int*> metas(NL);
-    int R = 0;
-    for (int l = 0; l < NL; ++l) {
-        std::vector<uint32_t> tk(A16_MAX_ROWS, 0);
-        if (x.tokens) std::copy(x.tokens + (size_t)l * T, x.tokens + (size_t)(l + 1) * T, tk.begin());
-        std::vector<const uint32_t*> toks(x.nslot);
-        for (int i = 0, t0 = 0; i < x.nslot; t0 += counts[i], ++i) toks[i] = tk.data() + t0;
-        std::vector<int> meta(MetaView::ints(e->maxT, S), 0);
-        REQUIRE(e->fill_meta(meta.data(), slots, counts, toks, outmode, &R) == T, B200RWKV_ERR_INVALID, "internal: step metadata");
-        metas[l] = (int*)up(meta.data(), meta.size() * 4);
-    }
-    const int MTR = R > 0 ? mt_bucket(R) : 0;
-    const int th_rows = split ? 32 : 16 * MTR;     // the head operand holds output rows
-    const int hrows = split ? 32 : 16 * std::max(MTR, 1);
-
-    // per-token rows as the engine's activation buffers hold them: `rows` rows, the ones past T filled with NaN so that a read
-    // outside the step shows in the output
-    auto rows_up = [&](const float* h, int cols) -> float* {
-        float* d = (float*)e->dalloc((size_t)rows * cols * 4, false);
-        CK(cudaMemset(d, 0xFF, (size_t)rows * cols * 4));
-        CK(cudaMemcpy(d, h, (size_t)T * cols * 4, cudaMemcpyHostToDevice));
-        return d;
-    };
     auto rows_down = [&](float* h, const float* d) { CK(cudaMemcpy(h, d, (size_t)T * C * 4, cudaMemcpyDeviceToHost)); };
     // A16 operands: `nmat` matrices of K columns with `tr` token rows, exchanged with the caller as [nmat][tr][K]
-    auto a16_stride = [](int K) { return (size_t)cdiv(K, GEMM_BK) * A16_KB_HALVES; };
     auto a16_up = [&](const uint16_t* h, int nmat, int K, int tr) {
-        const size_t st = a16_stride(K);
-        std::vector<uint16_t> b(st * nmat, 0);
-        for (int j = 0; j < nmat; ++j)
-            for (int m = 0; m < tr; ++m)
-                for (int k = 0; k < K; ++k) b[j * st + a16_index(m, k, tr)] = h[((size_t)j * tr + m) * K + k];
-        return (__half*)up(b.data(), b.size() * 2);
+        const std::vector<uint16_t> b = a16_pack(h, nmat * K, K, tr, (size_t)tr * K, K);
+        return (__half*)st.up(b.data(), b.size() * 2);
     };
     auto a16_down = [&](uint16_t* h, const __half* d, int nmat, int K, int tr) {
-        const size_t st = a16_stride(K);
-        std::vector<uint16_t> b(st * nmat);
+        std::vector<uint16_t> b(a16_halves(K) * nmat);
         CK(cudaMemcpy(b.data(), d, b.size() * 2, cudaMemcpyDeviceToHost));
-        for (int j = 0; j < nmat; ++j)
-            for (int m = 0; m < tr; ++m)
-                for (int k = 0; k < K; ++k) h[((size_t)j * tr + m) * K + k] = b[j * st + a16_index(m, k, tr)];
+        a16_unpack(b, nmat * K, K, tr, tr, (size_t)tr * K, K, h);
     };
 
     const size_t TC = (size_t)T * C;
-    const float* ln_w = (const float*)up(x.ln_w, (size_t)C * 4);
-    const float* ln_b = (const float*)up(x.ln_b, (size_t)C * 4);
-    float* cdst = x.commit_dst ? (float*)up(x.commit_dst, (size_t)S * C * 4) : nullptr;
+    const float* ln_w = (const float*)st.up(x.ln_w, (size_t)C * 4);
+    const float* ln_b = (const float*)st.up(x.ln_b, (size_t)C * 4);
+    float* cdst = x.commit_dst ? (float*)st.up(x.commit_dst, (size_t)S * C * 4) : nullptr;
     unsigned* gbar = (unsigned*)e->dalloc(256, true);      // the front half's barrier counters, shared by every launch
     float** hid_tab = nullptr;
     std::vector<float*> hid_rows(NL, nullptr);
     const int gcl = x.n_gate > 0 ? C / x.n_gate : 0;
     auto residual = [&](auto& p, int l) {          // LnMixParams / LnOutParams: x_in + gate (.) sum parts of launch l
-        p.x_in = rows_up(x.x_in + l * TC, C);
+        p.x_in = st.rows_up(x.x_in + l * TC, C);
         p.C = C;
-        p.meta = MetaView{metas[l], e->maxT, S};
+        p.meta = st.meta(l);
         p.n_parts = x.n_parts;
-        for (int q = 0; q < x.n_parts; ++q) p.parts[q] = rows_up(x.parts + ((size_t)l * x.n_parts + q) * TC, C);
+        for (int q = 0; q < x.n_parts; ++q) p.parts[q] = st.rows_up(x.parts + ((size_t)l * x.n_parts + q) * TC, C);
         p.n_gate = x.n_gate;
         p.gate_cl = gcl;
-        for (int q = 0; q < x.n_gate; ++q) p.gates[q] = rows_up(x.gates + ((size_t)l * x.n_gate + q) * T * gcl, gcl);
+        for (int q = 0; q < x.n_gate; ++q) p.gates[q] = st.rows_up(x.gates + ((size_t)l * x.n_gate + q) * T * gcl, gcl);
         p.ln_w = ln_w; p.ln_b = ln_b;
         p.commit_dst = cdst;
-        p.commit_src = x.commit_src ? rows_up(x.commit_src + l * TC, C) : nullptr;
-        if (x.hidden) hid_rows[l] = rows_up(x.hidden + l * TC, C);
+        p.commit_src = x.commit_src ? st.rows_up(x.commit_src + l * TC, C) : nullptr;
+        if (x.hidden) hid_rows[l] = st.rows_up(x.hidden + l * TC, C);
     };
 
     std::vector<EmbedParams> em(NL);
@@ -2984,46 +3001,46 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
     std::vector<Pre6Params> pq(NL);
     std::vector<LnOutParams> lo(NL);
     if (stage == 0) {
-        const __half* emb = (const __half*)up(x.emb, (size_t)x.V * C * 2);
+        const __half* emb = (const __half*)st.up(x.emb, (size_t)x.V * C * 2);
         for (int l = 0; l < NL; ++l) {
             EmbedParams& p = em[l];
             memset(&p, 0, sizeof(p));
-            p.emb = emb; p.C = C; p.V = x.V; p.meta = MetaView{metas[l], e->maxT, S};
+            p.emb = emb; p.C = C; p.V = x.V; p.meta = st.meta(l);
             p.ln_w = ln_w; p.ln_b = ln_b;
-            p.x_out = rows_up(x.x_out + l * TC, C);
+            p.x_out = st.rows_up(x.x_out + l * TC, C);
         }
     } else if (stage == 1 || stage == 2) {
-        const float* shift = (const float*)up(x.shift_state, (size_t)S * C * 4);
-        const float* mu = (const float*)up(x.mu, (size_t)x.n_mix * C * 4);
+        const float* shift = (const float*)st.up(x.shift_state, (size_t)S * C * 4);
+        const float* mu = (const float*)st.up(x.mu, (size_t)x.n_mix * C * 4);
         if (x.hidden) hid_tab = (float**)e->dalloc((size_t)NL * sizeof(float*), true);
         for (int l = 0; l < NL; ++l) {
             LnMixParams& p = lm[l];
             memset(&p, 0, sizeof(p));
             residual(p, l);
-            p.x_out = x.x_out ? rows_up(x.x_out + l * TC, C) : const_cast<float*>(p.x_in);
+            p.x_out = x.x_out ? st.rows_up(x.x_out + l * TC, C) : const_cast<float*>(p.x_in);
             p.shift_state = shift;
             p.n_mix = x.n_mix;
             const __half* mix = a16_up(x.mix_out + (size_t)l * x.n_mix * th * C, x.n_mix, C, th);
-            for (int j = 0; j < x.n_mix; ++j) { p.mu[j] = mu + (size_t)j * C; p.mix_out[j] = const_cast<__half*>(mix) + j * a16_stride(C); }
-            p.xx_out = rows_up(x.xx_out + l * TC, C);
-            p.sx_out = x.sx_out ? rows_up(x.sx_out + l * TC, C) : nullptr;
+            for (int j = 0; j < x.n_mix; ++j) { p.mu[j] = mu + (size_t)j * C; p.mix_out[j] = const_cast<__half*>(mix) + j * a16_halves(C); }
+            p.xx_out = st.rows_up(x.xx_out + l * TC, C);
+            p.sx_out = x.sx_out ? st.rows_up(x.sx_out + l * TC, C) : nullptr;
             p.hid_slot = hid_tab ? hid_tab + l : nullptr;
         }
         if (hid_tab) CK(cudaMemcpy(hid_tab, hid_rows.data(), (size_t)NL * sizeof(float*), cudaMemcpyHostToDevice));
         if (stage == 2) {
             const int Dm = x.Dm;
-            const __half* W1 = (const __half*)up(x.W1, (size_t)5 * Dm * C * 2);
-            const __half* W2 = (const __half*)up(x.W2, (size_t)5 * C * Dm * 2);
-            const float* mu5 = (const float*)up(x.mu5, (size_t)5 * C * 4);
+            const __half* W1 = (const __half*)st.up(x.W1, (size_t)5 * Dm * C * 2);
+            const __half* W2 = (const __half*)st.up(x.W2, (size_t)5 * C * Dm * 2);
+            const float* mu5 = (const float*)st.up(x.mu5, (size_t)5 * C * 4);
             for (int l = 0; l < NL; ++l) {
                 Pre6Params& q = pq[l];
                 memset(&q, 0, sizeof(q));
                 q.ln = lm[l];
                 q.W1 = W1; q.W2 = W2;
                 const __half* o5 = a16_up(x.out5 + (size_t)l * 5 * th * C, 5, C, th);
-                for (int j = 0; j < 5; ++j) { q.mu[j] = mu5 + (size_t)j * C; q.out[j] = const_cast<__half*>(o5) + j * a16_stride(C); }
+                for (int j = 0; j < 5; ++j) { q.mu[j] = mu5 + (size_t)j * C; q.out[j] = const_cast<__half*>(o5) + j * a16_halves(C); }
                 q.lora = const_cast<__half*>(a16_up(x.lora_out + (size_t)l * 5 * th * Dm, 5, Dm, th));
-                q.lora_stride = (int)a16_stride(Dm); q.lora_kq = rup(Dm, GEMM_BK) / 32;
+                q.lora_stride = (int)a16_halves(Dm); q.lora_kq = rup(Dm, GEMM_BK) / 32;
                 q.Dm = Dm;
                 q.gbar = gbar;
             }
@@ -3040,10 +3057,10 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
     CK(cudaDeviceSynchronize());                   // every upload has landed before the launches
     LnPick pick{};
     for (int l = 0; l < NL; ++l) {
-        if (stage == 0) pick = e->launch_embed(em[l], rows, e->stream, nullptr);
-        else if (stage == 1) pick = e->launch_ln(lm[l], MT, th, e->stream, nullptr);
-        else if (stage == 2) pick = e->launch_pre6(pq[l], th, e->stream, nullptr);
-        else pick = e->launch_ln_out(lo[l], MT, th_rows, e->stream, nullptr);
+        if (stage == 0) pick = e->launch_embed(em[l], sh, e->stream, nullptr);
+        else if (stage == 1) pick = e->launch_ln(lm[l], sh, e->stream, nullptr);
+        else if (stage == 2) pick = e->launch_pre6(pq[l], sh, e->stream, nullptr);
+        else pick = e->launch_ln_out(lo[l], sh, e->stream, nullptr);
     }
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(e->stream));
@@ -3094,28 +3111,18 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
                 tag + "f16 outputs are written in chunks of 8 columns: N and grp must be multiples of 8");
         REQUIRE(quant_type == QT_NONE || s.K % GEMM_BK == 0, B200RWKV_ERR_UNSUPPORTED, tag + "quantised matrices need K % 128 == 0");
     }
-    const bool split = precision == 1;
-    const int MT = split ? 2 : mt_bucket(T);       // token tiles of the kernel: split operands are the hi and lo tiles of 16 tokens
-    const int th = 16 * MT;                        // token rows of every operand / output in the A16 layout, rows of `out`
-    const int mt_launch = split ? 1 : MT;          // what the engine's step passes to launch_gemm
-    CK(cudaSetDevice(device));
-    std::unique_ptr<b200rwkv_engine> e(new b200rwkv_engine());
-    e->dev = device;
+    // one entry of T tokens: make_launch points every launch's valid token rows at the step metadata's T
+    const int32_t slot0 = 0;
+    OpStep st(1, 1, &slot0, &T, precision);
+    st.start(device, 1, nullptr, {0});
+    b200rwkv_engine* e = st.e.get();
+    const StepShape& sh = st.sh;
+    const int th = sh.th;                          // token rows of every operand / output in the A16 layout, rows of `out`
     CK(cudaDeviceGetAttribute(&e->num_sms, cudaDevAttrMultiProcessorCount, device));
-    e->maxT = th;                                  // sizes the stream-K workspace (make_launch)
-    CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
+    e->maxT = th;                                  // sizes the stream-K workspace (make_launch); the metadata keeps its layout
     gemm_smem_limits(quant_type);
-    e->d_meta = (int*)e->dalloc(64);               // meta[0] = T: the valid token rows of every launch
-    CK(cudaMemcpy(e->d_meta, &T, 4, cudaMemcpyHostToDevice));
-
-    auto up = [&](const void* h, size_t bytes) {
-        void* d = e->dalloc(bytes, false);
-        CK(cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice));
-        return d;
-    };
     // f16 destination in the A16 layout: `grp` columns per matrix (one matrix of ldo columns without groups)
-    struct Dst { int grp = 0, nmat = 1; size_t stride = 0; };
-    std::vector<Dst> dst(nseg);
+    auto mat_cols = [](const b200rwkv_gemm_seg& s) { return s.grp > 0 ? s.grp : s.ldo; };
     std::vector<StTensor> wt(nseg);
     std::vector<SegDesc> sv(nseg);
     size_t wmax = 0;
@@ -3130,15 +3137,10 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
         SegDesc& d = sv[i];
         d.t = &wt[i]; d.N = s.N; d.K = s.K;
         d.proto.out_mode = s.out_mode; d.proto.act = s.act; d.proto.grp = s.out_mode == OUT_F32 ? 0 : s.grp;
-        d.proto.bias = s.bias ? (const float*)up(s.bias, (size_t)s.N * 4) : nullptr;
-        if (s.out_mode == OUT_LERP_A16) { d.proto.aux2 = (const float*)up(s.lerp_mu, (size_t)s.N * 4); d.proto.ld_aux = s.N; }
+        d.proto.bias = s.bias ? (const float*)st.up(s.bias, (size_t)s.N * 4) : nullptr;
+        if (s.out_mode == OUT_LERP_A16) { d.proto.aux2 = (const float*)st.up(s.lerp_mu, (size_t)s.N * 4); d.proto.ld_aux = s.N; }
         if (s.out_mode != OUT_F32) {
-            Dst& o = dst[i];
-            o.grp = s.grp;
-            const int cols = o.grp > 0 ? o.grp : s.ldo;
-            o.nmat = o.grp > 0 ? cdiv(s.ldo, o.grp) : 1;
-            o.stride = (size_t)cdiv(cols, GEMM_BK) * A16_KB_HALVES;
-            d.proto.grp_stride = (int)o.stride;
+            d.proto.grp_stride = (int)a16_halves(mat_cols(s));
             d.proto.ldo = th;
         } else {
             d.proto.ldo = s.ldo;
@@ -3151,7 +3153,7 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
     g.p.ws = e->gemm_ws;
 
     // the plan as launch_gemm will run it, and the cut of every tile by the kernel's own formula
-    const int G = mt_launch >= 4 ? g.grid_wide : g.grid;
+    const int G = sh.MT >= 4 ? g.grid_wide : g.grid;
     const unsigned TB = (unsigned)g.p.total_blocks;
     int maxc = 0;
     for (int i = 0; i < nseg; ++i) {
@@ -3174,27 +3176,20 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
         for (int i = 0; i < nseg; ++i) {
             const b200rwkv_gemm_seg& s = seg[i];
             GemmSeg& sg = runs[l].p.seg[i];
-            __half* a = (__half*)e->dalloc((size_t)sg.KB * A16_KB_HALVES * 2, true);
+            __half* a = (__half*)e->dalloc(a16_halves(s.K) * 2, true);
             CK(cudaMemcpy(xs.p, s.x + (size_t)l * T * s.K, (size_t)T * s.K * 4, cudaMemcpyHostToDevice));
-            a16_from_f32_kernel<<<(int)std::min<size_t>(((size_t)T * s.K + 255) / 256, (size_t)e->num_sms * 8), 256>>>((const float*)xs.p, T, s.K, th, split, a);
+            a16_from_f32_kernel<<<(int)std::min<size_t>(((size_t)T * s.K + 255) / 256, (size_t)e->num_sms * 8), 256>>>((const float*)xs.p, T, s.K, th, sh.split, a);
             CK(cudaGetLastError());
             CK(cudaDeviceSynchronize());           // xs is refilled by the next upload
             sg.A = a;
             const size_t cells = (size_t)th * s.ldo;
             if (s.out_mode == OUT_F32) {
-                sg.out = up((const float*)s.out + l * cells, cells * 4);
+                sg.out = st.up((const float*)s.out + l * cells, cells * 4);
                 continue;
             }
-            const Dst& o = dst[i];
-            const uint16_t* src = (const uint16_t*)s.out + l * cells;
             std::vector<uint16_t>& h = h16[i];
-            h.assign(o.stride * o.nmat, 0);
-            for (int m = 0; m < th; ++m)
-                for (int n = 0; n < s.ldo; ++n) {
-                    const int gi = o.grp > 0 ? n / o.grp : 0, nn = n - gi * o.grp;
-                    h[gi * o.stride + a16_index(m, nn, th)] = src[(size_t)m * s.ldo + n];
-                }
-            sg.out = up(h.data(), h.size() * 2);
+            h = a16_pack((const uint16_t*)s.out + l * cells, s.ldo, mat_cols(s), th, mat_cols(s), s.ldo);
+            sg.out = st.up(h.data(), h.size() * 2);
             if (s.out_mode == OUT_LERP_A16) {          // all `th` rows exist, as in the engine's activation buffers
                 float* xx = (float*)e->dalloc((size_t)th * s.N * 4, true);
                 float* sx = (float*)e->dalloc((size_t)th * s.N * 4, true);
@@ -3206,7 +3201,7 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
         }
     }
     CK(cudaDeviceSynchronize());                   // every upload has landed before the projection stream starts
-    for (const GemmLaunch& r : runs) e->launch_gemm(r, mt_launch, e->stream, nullptr, split);
+    for (const GemmLaunch& r : runs) e->launch_gemm(r, sh, e->stream, nullptr);
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(e->stream));
     for (int l = 0; l < launches; ++l)
@@ -3217,15 +3212,9 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
                 CK(cudaMemcpy((float*)s.out + l * cells, runs[l].p.seg[i].out, cells * 4, cudaMemcpyDeviceToHost));
                 continue;
             }
-            const Dst& o = dst[i];
             std::vector<uint16_t>& h = h16[i];
             CK(cudaMemcpy(h.data(), runs[l].p.seg[i].out, h.size() * 2, cudaMemcpyDeviceToHost));
-            uint16_t* out = (uint16_t*)s.out + l * cells;
-            for (int m = 0; m < th; ++m)
-                for (int n = 0; n < s.ldo; ++n) {
-                    const int gi = o.grp > 0 ? n / o.grp : 0, nn = n - gi * o.grp;
-                    out[(size_t)m * s.ldo + n] = h[gi * o.stride + a16_index(m, nn, th)];
-                }
+            a16_unpack(h, s.ldo, mat_cols(s), th, th, mat_cols(s), s.ldo, (uint16_t*)s.out + l * cells);
         }
     API_END
 }
@@ -3249,21 +3238,18 @@ int32_t b200rwkv_keep_hidden(b200rwkv_engine* e, int32_t enable) {
 
 // returns the number of rows written (negative status on error)
 int32_t b200rwkv_last_hidden(b200rwkv_engine* e, float* out, size_t cap) {
-    int32_t rows = 0;
-    const int32_t st = [&]() -> int32_t {
-        API_BEGIN(e)
+    return api_count([&]() -> int32_t {
         REQUIRE(e && out, B200RWKV_ERR_INVALID, "null argument");
         std::lock_guard<std::mutex> lk(e->mu);
         CK(cudaSetDevice(e->dev));
         CK(cudaStreamSynchronize(e->stream));
         const bool all = e->hidden_keep && e->d_hidden_all;
-        rows = all ? e->hidden_rows : e->last_T;
+        const int32_t rows = all ? e->hidden_rows : e->last_T;
         const size_t n = (size_t)rows * e->C;
         REQUIRE(n <= cap, B200RWKV_ERR_INVALID, "hidden buffer too small");
         if (n) CK(cudaMemcpy(out, all ? e->d_hidden_all : e->d_hidden, n * 4, cudaMemcpyDeviceToHost));
-        API_END
-    }();
-    return st < 0 ? st : rows;
+        return rows;
+    });
 }
 
 int32_t b200rwkv_keep_hidden_layers(b200rwkv_engine* e, int32_t n, const int32_t* layers) {
@@ -3295,9 +3281,7 @@ int32_t b200rwkv_keep_hidden_layers(b200rwkv_engine* e, int32_t n, const int32_t
 
 // returns the number of rows written (negative status on error)
 int32_t b200rwkv_last_hidden_layer(b200rwkv_engine* e, int32_t layer, float* out, size_t cap) {
-    int32_t rows = 0;
-    const int32_t st = [&]() -> int32_t {
-        API_BEGIN(e)
+    return api_count([&]() -> int32_t {
         REQUIRE(layer >= 0, B200RWKV_ERR_INVALID, "last_hidden_layer: negative layer " + std::to_string(layer));
         REQUIRE(e && out, B200RWKV_ERR_INVALID, "null argument");
         std::lock_guard<std::mutex> lk(e->mu);
@@ -3311,19 +3295,16 @@ int32_t b200rwkv_last_hidden_layer(b200rwkv_engine* e, int32_t layer, float* out
         CK(cudaSetDevice(e->dev));
         CK(cudaStreamSynchronize(e->stream));
         if (n) CK(cudaMemcpy(out, e->hid_all + (size_t)(it - e->hid_last.begin()) * n, n * 4, cudaMemcpyDeviceToHost));
-        rows = (int32_t)e->hid_last_rows;
-        API_END
-    }();
-    return st < 0 ? st : rows;
+        return (int32_t)e->hid_last_rows;
+    });
 }
 
 // Debug aid for the parity tests: copy a named internal activation buffer of the most recent
 // step to the host as f32 row-major [rows, cols]; returns cols (rows = tokens of the last step,
 // capped by `cap`), or a negative status.  Not used on the product path.
 int32_t b200rwkv_debug_read(b200rwkv_engine* e, const char* name, float* out, size_t cap) {
-    if (!e || !name || !out) return B200RWKV_ERR_INVALID;
-    std::string* errp_ = &g_err;
-    try {
+    return api_count([&]() -> int32_t {
+        REQUIRE(e && name && out, B200RWKV_ERR_INVALID, "null argument");
         std::lock_guard<std::mutex> lk(e->mu);
         CK(cudaSetDevice(e->dev));
         CK(cudaStreamSynchronize(e->stream));
@@ -3364,23 +3345,15 @@ int32_t b200rwkv_debug_read(b200rwkv_engine* e, const char* name, float* out, si
         for (const A& a : as)
             if (n == a.n && a.b->p) {
                 REQUIRE((size_t)T * a.cols <= cap, B200RWKV_ERR_INVALID, "debug buffer too small");
-                std::vector<__half> h(a.b->halves_per_matrix);
+                // T rows through the layout of the last captured step (last_th): a cached graph replay keeps last_th, so T may exceed it
+                std::vector<uint16_t> h(a.b->halves_per_matrix), rows((size_t)T * a.cols);
                 CK(cudaMemcpy(h.data(), a.b->p + (size_t)a.mat * a.b->halves_per_matrix, h.size() * 2, cudaMemcpyDeviceToHost));
-                for (int t = 0; t < T; ++t)
-                    for (int c = 0; c < a.cols; ++c) out[(size_t)t * a.cols + c] = __half2float(h[a16_index(t, c, e->last_th)]);
+                a16_unpack(h, a.cols, a.cols, e->last_th, T, 0, a.cols, rows.data());
+                for (size_t i = 0; i < (size_t)T * a.cols; ++i) out[i] = __half2float(__ushort_as_half(rows[i]));
                 return a.cols;
             }
         throw Error(B200RWKV_ERR_INVALID, "unknown debug buffer: " + n);
-    } catch (const Error& ex) {
-        *errp_ = ex.what();
-        return ex.code;
-    } catch (const std::exception& ex) {
-        *errp_ = ex.what();
-        return B200RWKV_ERR_INVALID;
-    } catch (...) {
-        *errp_ = "unknown exception";
-        return B200RWKV_ERR_INVALID;
-    }
+    });
 }
 
 // Profiling aid: the raw stamp rows of the most recent traced replay (b200rwkv_profile_insitu): one row of 512 uint64 per
@@ -3429,12 +3402,13 @@ int32_t b200rwkv_debug_gemm_time(b200rwkv_engine* e, int32_t which, int32_t reps
     const int n = reps * e->L;
     unsigned long long* d_tr = nullptr;
     if (trace_out) { CK(cudaMalloc(&d_tr, (size_t)e->L * 16 * 8)); CK(cudaMemset(d_tr, 0, (size_t)e->L * 16 * 8)); }
-    for (int i = 0; i < e->L; ++i) e->launch_gemm(pick(i), 1, e->stream, nullptr);
+    const StepShape sh = e->step_shape(16, 16);
+    for (int i = 0; i < e->L; ++i) e->launch_gemm(pick(i), sh, e->stream, nullptr);
     CK(cudaEventRecord(a, e->stream));
     for (int i = 0; i < n; ++i) {
         GemmLaunch g = pick(i);
         if (d_tr && i >= n - e->L) g.p.trace = d_tr + (size_t)(i % e->L) * 16;
-        e->launch_gemm(g, 1, e->stream, nullptr);
+        e->launch_gemm(g, sh, e->stream, nullptr);
     }
     CK(cudaEventRecord(b, e->stream));
     CK(cudaStreamSynchronize(e->stream));
