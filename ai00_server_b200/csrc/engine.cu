@@ -1697,6 +1697,11 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
                 sc_rows[sc_used++] = {keep_valid[slot[i]] ? d_keep + (size_t)slot[i] * V : nullptr, tokens[base[i]], (unsigned)score_base[i]};
     }
     launch_score(0, sc_used);          // before the first step replaces the kept rows
+    {       // a NONE entry with tokens moves its slot's state past the kept row and writes no new one
+        std::lock_guard<std::mutex> lk(keep_mu);
+        for (int i = 0; i < nslot; ++i)
+            if (option[i] == B200RWKV_OPTION_NONE && ntok[i] > 0) keep_valid[slot[i]] = 0;
+    }
     if (hidden_keep && total_tok > hidden_cap_rows) {
         if (d_hidden_all) { CK(cudaFree(d_hidden_all)); d_hidden_all = nullptr; hidden_cap_rows = 0; }
         const size_t want = std::max<size_t>(total_tok, 256);
@@ -1920,8 +1925,10 @@ void b200rwkv_engine::sample_topk(int nrows, const int32_t* slots, const int32_t
     REQUIRE(tk_cand_x, B200RWKV_ERR_UNSUPPORTED, "sample_topk: num_vocab > 65536 is not supported");
     REQUIRE(ids_out && probs_out, B200RWKV_ERR_INVALID, "sample_topk: bad argument");
     REQUIRE(top_k >= 1 && top_k <= TOPK_MAX, B200RWKV_ERR_INVALID, "sample_topk: top_k must be in [1, 128]");
+    REQUIRE(top_k <= V, B200RWKV_ERR_INVALID, "sample_topk: top_k exceeds num_vocab");
     check_sample_slots(nrows, slots, "sample_topk");
     check_sample_lists(nrows, pen_off, pen_tok, pen_val, bias_off, bias_tok, bias_val, "sample_topk");
+    CK(cudaSetDevice(dev));
     TopkParams tp;
     memset(&tp, 0, sizeof(tp));
     tp.keep = d_keep; tp.V = V; tp.nseg = cdiv(V, TOPK_SEG);
@@ -2299,6 +2306,10 @@ static int32_t rank_state_load(b200rwkv_engine* e, int32_t slot, const float* in
     CK(cudaMemcpyAsync(e->d_api, in, n * 4, cudaMemcpyHostToDevice, e->stream));
     e->state_xform(slot, true);
     CK(cudaStreamSynchronize(e->stream));
+    {       // a host state carries no logits row: the slot's kept row belonged to the state just replaced
+        std::lock_guard<std::mutex> lk2(e->keep_mu);
+        e->keep_valid[slot] = 0;
+    }
     API_END
 }
 
@@ -2507,7 +2518,6 @@ int32_t b200rwkv_sample_topk(b200rwkv_engine* e, int32_t nrows, const int32_t* s
     API_BEGIN(e)
     REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
     std::lock_guard<std::mutex> lk(e->sm_mu);
-    CK(cudaSetDevice(e->dev));
     e->sample_topk(nrows, slots, penalty_offset, penalty_token, penalty_value, allow_bits, bias_offset, bias_token, bias_value, top_k,
                    ids_out, probs_out);
     API_END

@@ -140,7 +140,10 @@ int32_t b200rwkv_get_info(b200rwkv_engine*, b200rwkv_info* out);
  * ntok[i] rows for FULL, none for NONE; rows_out[i] receives the row count of entry i
  * (== RnnOutputBatch being empty or not, run.rs:1146-1155).  `logits_cap` is in floats.
  * `logits_out` may be NULL: nothing is copied to the host, the last row of every slot stays in HBM for
- * b200rwkv_sample_topk / b200rwkv_sample_probs.  Token ids >= num_vocab are B200RWKV_ERR_INVALID. */
+ * b200rwkv_sample_topk / b200rwkv_sample_probs.  Token ids >= num_vocab are B200RWKV_ERR_INVALID.
+ * The slot's kept row: a LAST entry with tokens, a FULL or a SCORE entry makes the entry's last row the slot's kept row; a
+ * NONE entry with tokens advances the state without a row and drops the kept row (the slot has none until its next LAST /
+ * FULL / SCORE entry or b200rwkv_state_write); an entry with ntok = 0 leaves the kept row as it was. */
 int32_t b200rwkv_infer(b200rwkv_engine*, int32_t nslot, const int32_t* slot, const int32_t* ntok,
                        const uint32_t* tokens, const int32_t* option, float* logits_out,
                        size_t logits_cap, int32_t* rows_out);
@@ -151,8 +154,9 @@ int32_t b200rwkv_infer(b200rwkv_engine*, int32_t nslot, const int32_t* slot, con
  *     bit-identical to the same call with FULL;
  *   - rows_out[i] = 0: no logits row goes to `logits_out`;
  *   - score_out[j] = log softmax(row predicting x_j)[x_j] in f32, computed as (x_t - m) - logf(sum expf(x - m)), m the row
- *     maximum; the row predicting x_j is the row after x_{j-1} for j >= 1, and the slot's kept row for j = 0 (from the
- *     previous infer call, or from b200rwkv_state_write of a snapshot that carries a row; none: NaN);
+ *     maximum; the row predicting x_j is the row after x_{j-1} for j >= 1, and the slot's kept row for j = 0 (the row of the
+ *     slot's current state: from the previous infer call, or from b200rwkv_state_write of a snapshot that carries a row;
+ *     none, as after b200rwkv_state_load or a NONE entry with tokens: NaN);
  *   - argmax_out[j] = id of the largest logit of that row, lowest id on ties (UINT32_MAX if there is no row).
  * score_out / argmax_out hold sum(ntok) over the SCORE entries, in entry order; argmax_out may be NULL.  LAST, FULL, NONE and
  * SCORE entries mix freely in one call.  Every argument is checked before the first CUDA call.  Tensor parallel engines answer
@@ -177,6 +181,8 @@ int32_t b200rwkv_infer_ex(b200rwkv_engine*, const b200rwkv_infer_args* args);
  * (x fastest; run.rs:987): row 0 time-mix shift, rows 1..N WKV, row N+1 channel-mix shift. */
 int32_t b200rwkv_state_shape(b200rwkv_engine*, int64_t shape[4]);
 int32_t b200rwkv_state_init(b200rwkv_engine*, float* out);                          /* State::init  */
+/* State::load drops the slot's kept logits row: a host state carries none.  State::write makes the snapshot's row (or none,
+ * if the snapshot has none) the slot's kept row; State::read takes the kept row into the snapshot. */
 int32_t b200rwkv_state_load(b200rwkv_engine*, int32_t slot, const float* in);        /* State::load  */
 int32_t b200rwkv_state_back(b200rwkv_engine*, int32_t slot, float* out);             /* State::back  */
 int32_t b200rwkv_state_read(b200rwkv_engine*, int32_t slot, uint64_t* snapshot_id);  /* State::read  (device copy) */
@@ -201,7 +207,9 @@ int32_t b200rwkv_cache_stats(b200rwkv_engine*, int64_t* num_snapshots, int64_t* 
 int32_t b200rwkv_read_state(const b200rwkv_info* info, const uint8_t* st, size_t len, float* out);
 
 /* Replaces `web_rwkv::runtime::softmax::softmax(&context, Vec<TensorCpu<f32>>)` —
- * crates/ai00-core/src/run.rs:1179.  in/out: [rows, num_vocab] f32. */
+ * crates/ai00-core/src/run.rs:1179.  in/out: [rows, num_vocab] f32.  out = expf(x - max) * (1 / sum expf(x - max)) per row,
+ * in f32; a -inf entry gives exactly 0.  Every row needs at least one finite entry (a row of only -inf is NaN); NaN inputs
+ * are outside the contract. */
 int32_t b200rwkv_softmax(b200rwkv_engine*, int32_t rows, const float* in, float* out);
 
 /* GPU front half of token sampling (SURVEY.md §8f-1).  Replaces, for samplers that only need the head of the sorted
@@ -210,7 +218,8 @@ int32_t b200rwkv_softmax(b200rwkv_engine*, int32_t rows, const float* in, float*
  * (penalties, sampler/nucleus.rs:61-67), `Formatter::transform` (BNF mask, sampler/bnf.rs:37-40), the bias add
  * (run.rs:679-681), the softmax round trip (run.rs:1164-1190) and the full-vocabulary sort of
  * sampler/nucleus.rs:69-80.  Pass `logits_out = NULL` to b200rwkv_infer: the logits stay in HBM, and this call returns, for
- * each listed slot, the `top_k` most probable tokens of that slot's most recent logits row after
+ * each listed slot, the `top_k` most probable tokens of that slot's kept logits row (the row of its current state, see
+ * b200rwkv_infer; a slot without one, as after b200rwkv_state_load or a NONE entry with tokens, is B200RWKV_ERR_STATE) after
  *     logits[penalty_token[j]] -= penalty_value[j]     j in [penalty_offset[i], penalty_offset[i+1])
  *     logits[t] = -inf  where bit t of allow_bits row i is 0                    (allow_bits may be NULL)
  *     logits[bias_token[j]]    += bias_value[j]        j in [bias_offset[i], bias_offset[i+1])
@@ -218,8 +227,10 @@ int32_t b200rwkv_softmax(b200rwkv_engine*, int32_t rows, const float* in, float*
  * probs = softmax over the whole adjusted row.  Order: logit descending, token id ascending on ties.  ids_out / probs_out:
  * [nrows][top_k].  The draw itself (top_p cut, temperature, RNG, penalty update; nucleus.rs:81-123) stays in the host
  * sampler, now over <= 128 pairs.  Samplers that need the whole distribution (Mirostat, Typical, Nucleus with top_k > 128)
- * use b200rwkv_sample_probs below.  A row whose every token is disallowed yields ids 0 .. top_k-1, each with probability 0.
- * Thread contract: the softmax task's (run.rs:1237). */
+ * use b200rwkv_sample_probs below.  A row whose every token is disallowed yields ids 0 .. top_k-1, each with probability 0;
+ * more generally, after the tokens with a finite adjusted logit come the lowest disallowed ids, in ascending order.
+ * Penalty and bias tokens >= num_vocab are ignored.  top_k outside [1, min(128, num_vocab)] is B200RWKV_ERR_INVALID, checked
+ * before any CUDA call.  Thread contract: the softmax task's (run.rs:1237). */
 int32_t b200rwkv_sample_topk(b200rwkv_engine*, int32_t nrows, const int32_t* slots, const int32_t* penalty_offset,
                              const uint32_t* penalty_token, const float* penalty_value, const uint32_t* allow_bits,
                              const int32_t* bias_offset, const uint32_t* bias_token, const float* bias_value, int32_t top_k,
@@ -227,8 +238,8 @@ int32_t b200rwkv_sample_topk(b200rwkv_engine*, int32_t nrows, const int32_t* slo
 
 /* The whole adjusted distribution on the device, for samplers that read every probability: MirostatSampler
  * (sampler/mirostat.rs:44-90), TypicalSampler (sampler/typical.rs:70-131) and NucleusSampler with top_k > 128.  Writes, for
- * each listed slot's most recent logits row (the row b200rwkv_sample_topk reads), exactly the vector run.rs:673-691 hands to
- * `Sampler::sample`: probs_out[i] = softmax(row adjusted as in b200rwkv_sample_topk), [nrows][num_vocab] f32, the adjustment
+ * each listed slot's kept logits row (the row of its current state, the row b200rwkv_sample_topk reads), exactly the vector
+ * run.rs:673-691 hands to `Sampler::sample`: probs_out[i] = softmax(row adjusted as in b200rwkv_sample_topk), [nrows][num_vocab] f32, the adjustment
  * lists meaning and validated what they do there (allow_bits may be NULL).  The sampler itself stays on the host, unchanged.
  *   - probabilities are expf(x - max) * (1 / sum expf(x - max)) in f32; a disallowed token is exactly 0.  For num_vocab <=
  *     65536 every candidate probability b200rwkv_sample_topk returns for the same row and lists equals probs_out[i][id].
