@@ -18,6 +18,7 @@
 #include <mutex>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "gemm.cuh"
@@ -66,6 +67,80 @@ static std::string watchdog_report() {
     snprintf(buf, sizeof buf, " [device watchdog: code=%u block=%u thread=%u a0=0x%x a1=%u a2=%u]", g_wd_host[0] & 0xFFFFu, g_wd_host[1],
              g_wd_host[2], g_wd_host[3], g_wd_host[4], g_wd_host[5]);
     return buf;
+}
+
+// =========================================================================================
+// owners of CUDA resources: move-only, released when they go out of scope (destructors ignore errors), and usable
+// wherever the raw pointer or handle is
+// =========================================================================================
+// A device (cudaMalloc) or pinned host (cudaMallocHost) block of `bytes` bytes
+template <typename T, bool Pinned = false>
+struct Buf {
+    T* p = nullptr;
+    size_t bytes = 0;
+    Buf() = default;
+    explicit Buf(size_t n) { grow(n, n); }
+    Buf(Buf&& o) noexcept : p(std::exchange(o.p, nullptr)), bytes(std::exchange(o.bytes, (size_t)0)) {}
+    Buf& operator=(Buf&& o) noexcept { std::swap(p, o.p); std::swap(bytes, o.bytes); return *this; }
+    ~Buf() { if (p) Pinned ? cudaFreeHost(p) : cudaFree(p); }
+    operator T*() const { return p; }
+    // Smaller than `need` bytes: free the block, then allocate `alloc` bytes.  Freeing first keeps the peak at the new block;
+    // a failed allocation leaves the owner empty, so the next call retries.
+    void grow(size_t need, size_t alloc) {
+        if (bytes >= need) return;
+        T* old = std::exchange(p, nullptr);
+        bytes = 0;
+        if (old) CK(Pinned ? cudaFreeHost(old) : cudaFree(old));
+        void* q = nullptr;
+        CK(Pinned ? cudaMallocHost(&q, alloc) : cudaMalloc(&q, alloc));
+        p = static_cast<T*>(q);
+        bytes = alloc;
+    }
+};
+template <typename T> using HostBuf = Buf<T, true>;
+
+template <typename H, cudaError_t (*Destroy)(H)>
+struct Handle {
+    H h = nullptr;
+    Handle() = default;
+    explicit Handle(H x) : h(x) {}
+    Handle(Handle&& o) noexcept : h(std::exchange(o.h, nullptr)) {}
+    Handle& operator=(Handle&& o) noexcept { std::swap(h, o.h); return *this; }
+    ~Handle() { if (h) Destroy(h); }
+    operator H() const { return h; }
+};
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+using GraphExec = Handle<cudaGraphExec_t, cudaGraphExecDestroy>;
+
+static Event new_event(unsigned flags = cudaEventDefault) {
+    cudaEvent_t ev = nullptr;
+    CK(cudaEventCreateWithFlags(&ev, flags));
+    return Event(ev);
+}
+static Stream new_stream() {
+    cudaStream_t s = nullptr;
+    CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+    return Stream(s);
+}
+// The work `enqueue` issues on `s`, captured into a graph and instantiated; a throw ends and drops the partial capture.
+template <typename F>
+static GraphExec capture_graph(cudaStream_t s, F&& enqueue) {
+    cudaGraph_t g = nullptr;
+    CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    try {
+        enqueue();
+    } catch (...) {
+        cudaStreamEndCapture(s, &g);
+        if (g) cudaGraphDestroy(g);
+        throw;
+    }
+    CK(cudaStreamEndCapture(s, &g));
+    cudaGraphExec_t ge = nullptr;
+    const cudaError_t instantiated = cudaGraphInstantiate(&ge, g, 0);
+    cudaGraphDestroy(g);
+    CK(instantiated);
+    return GraphExec(ge);
 }
 
 // =========================================================================================
@@ -366,11 +441,11 @@ struct Layer {
 };
 
 struct Profiler {
-    struct Rec { int cls; cudaEvent_t a, b; };
+    struct Rec { int cls; Event a, b; };
     std::vector<Rec> recs;
 };
 
-struct Snapshot { float* buf = nullptr; float* logits = nullptr; size_t bytes = 0; };   // CachedItem {state, output} on the device (run.rs:199-205)
+struct Snapshot { Buf<float> buf, logits; };   // CachedItem {state, output} on the device (run.rs:199-205)
 
 // The LN-stage kernel a launch picked (b200rwkv_ln_args::kernel_out): kernel, its NV (float4 per thread of the per-token
 // kernels) or Dm / 16 (pre6_kernel), and whether it wrote split (hi + lo) operands.
@@ -454,8 +529,8 @@ struct b200rwkv_engine {
     bool connected = false;
     TpBar tpbar;
     unsigned* d_epoch = nullptr;
-    cudaStream_t stream = nullptr, sm_stream = nullptr;
-    std::vector<void*> allocs;
+    Stream stream, sm_stream;
+    std::vector<Buf<void>> allocs;
     size_t weight_bytes_total = 0;
 
     // model
@@ -481,10 +556,9 @@ struct b200rwkv_engine {
 
     // step plumbing
     static constexpr int META_RING = 4;
-    cudaEvent_t meta_ev[META_RING] = {nullptr, nullptr, nullptr, nullptr};
+    Event meta_ev[META_RING];
     bool hidden_keep = false;          // b200rwkv_keep_hidden: accumulate the hidden rows of every token of an infer call
-    float* d_hidden_all = nullptr;
-    size_t hidden_cap_rows = 0;
+    Buf<float> d_hidden_all;
     int hidden_rows = 0;
     // b200rwkv_keep_hidden_layers: the residual stream after chosen layers for every token of an infer call.  LN1 of layer
     // l + 1 writes the rows of layer l into the step buffer d_hid_tab[l] points to (null: not recorded); layer L - 1 comes
@@ -493,40 +567,37 @@ struct b200rwkv_engine {
     std::vector<int> hid_layers;       // recorded layers, in the order the caller gave them
     float** d_hid_tab = nullptr;       // [L]
     float* hid_step = nullptr;         // [HID_MAX_LAYERS][maxT][C], step buffer k belongs to hid_layers[k]
-    float* hid_all = nullptr;          // [hid_layers.size()][tokens of the call][C]
-    size_t hid_all_floats = 0;
+    Buf<float> hid_all;                // [hid_layers.size()][tokens of the call][C]
     std::vector<int> hid_last;         // layers recorded by the most recent infer call (the layout of hid_all)
     size_t hid_last_rows = 0;
     const float* hid_step_src(int k) const { return hid_layers[k] == L - 1 ? d_hidden : hid_step + (size_t)k * maxT * C; }
-    int *d_meta = nullptr, *h_meta = nullptr;
-    int* d_meta_all = nullptr;
+    int* d_meta = nullptr;
+    HostBuf<int> h_meta;
     size_t meta_ints = 0;
-    std::map<int, cudaGraphExec_t> graphs;
-    std::map<int, long long> graph_launches;   // kernels per captured step graph
+    struct StepGraph { GraphExec exec; long long launches; };     // a captured step graph and the kernels it launches
+    std::map<int, StepGraph> graphs;
     long long launch_total = 0;                // kernels launched by this engine's steps since creation
     long long launches_last_step = 0;
     int last_T = 0, last_th = 16;      // tokens / A16 token rows of the most recent step
 
     // softmax
-    float *sm_in = nullptr, *sm_out = nullptr;
-    int sm_rows_cap = 0;
+    Buf<float> sm_in, sm_out;
 
     // sampling front half (sample.cuh): last logits row of every slot, candidate scratch, staging blobs
     float* d_keep = nullptr;                 // [S][V] (rank 0)
     std::vector<char> keep_valid;            // slot has a logits row (guarded by keep_mu)
     std::mutex keep_mu;
-    cudaEvent_t step_done = nullptr;         // recorded on `stream` after every step: the sampling stream waits on it
+    Event step_done;                         // recorded on `stream` after every step: the sampling stream waits on it
     float* tk_cand_x = nullptr; unsigned* tk_cand_id = nullptr; float2* tk_stats = nullptr;
     unsigned* tk_out_id = nullptr; float* tk_out_p = nullptr;
-    uint8_t *tk_dev = nullptr, *tk_host = nullptr;
-    size_t tk_cap = 0;
+    Buf<uint8_t> tk_dev;
+    HostBuf<uint8_t> tk_host;
     // b200rwkv_sample_probs: [nrows][V rounded up to 4] f32 rows | [nrows][segments] float2 statistics; grown on demand
-    uint8_t* sp_dev = nullptr;
-    size_t sp_cap = 0;
+    Buf<uint8_t> sp_dev;
     // scoring (b200rwkv_infer_ex, OPTION_SCORE): [ScoreRow x n | score f32 x n | argmax u32 x n], pinned host and device,
     // n = the call's scored tokens; grown on demand
-    uint8_t *sc_dev = nullptr, *sc_host = nullptr;
-    size_t sc_cap = 0;
+    Buf<uint8_t> sc_dev;
+    HostBuf<uint8_t> sc_host;
     void enqueue_keep(cudaStream_t s, int MTR);
     void check_sample_slots(int nrows, const int32_t* slots, const char* who);
     SampleAdjust stage_sample_args(int nrows, const int32_t* slots, const int32_t* pen_off, const uint32_t* pen_tok,
@@ -548,8 +619,7 @@ struct b200rwkv_engine {
     void blend_loras(const StTensor& t);
 
     // temp upload buffer during build
-    __half* d_tmp = nullptr;
-    size_t d_tmp_bytes = 0;
+    Buf<__half> d_tmp;
     const StTensor* d_tmp_holds = nullptr;
 
     ~b200rwkv_engine();
@@ -604,55 +674,24 @@ struct b200rwkv_engine {
     void state_xform(int slot, bool import, float* snap = nullptr);
 };
 
+// The members release their resources after this body, once the device has finished every queued use of them.
 b200rwkv_engine::~b200rwkv_engine() {
     cudaSetDevice(dev);
     cudaDeviceSynchronize();
-    for (auto& kv : graphs) cudaGraphExecDestroy(kv.second);
-    for (auto& kv : snaps) { cudaFree(kv.second.buf); if (kv.second.logits) cudaFree(kv.second.logits); }
     for (int q = 0; q < 8; ++q)
         if (peer_ipc[q] && peer_base[q]) cudaIpcCloseMemHandle(peer_base[q]);
-    for (void* p : allocs) cudaFree(p);
-    if (d_tmp) cudaFree(d_tmp);          // only still set when build() threw
-    if (sm_in) cudaFree(sm_in);
-    if (sm_out) cudaFree(sm_out);
-    if (h_meta) cudaFreeHost(h_meta);
-    if (tk_dev) cudaFree(tk_dev);
-    if (tk_host) cudaFreeHost(tk_host);
-    if (sp_dev) cudaFree(sp_dev);
-    if (sc_dev) cudaFree(sc_dev);
-    if (sc_host) cudaFreeHost(sc_host);
-    if (step_done) cudaEventDestroy(step_done);
-    for (auto& ev : meta_ev) if (ev) cudaEventDestroy(ev);
-    if (d_hidden_all) cudaFree(d_hidden_all);
-    if (hid_all) cudaFree(hid_all);
-    if (stream) cudaStreamDestroy(stream);
-    if (sm_stream) cudaStreamDestroy(sm_stream);
 }
 
-// scratch device allocation released on every exit path
-struct DevTmp {
-    void* p = nullptr;
-    explicit DevTmp(size_t bytes) {
-        cudaError_t e_ = cudaMalloc(&p, std::max<size_t>(bytes, 16));
-        if (e_ != cudaSuccess) throw Error(B200RWKV_ERR_CUDA, std::string("cudaMalloc (scratch): ") + cudaGetErrorString(e_));
-    }
-    ~DevTmp() { if (p) cudaFree(p); }
-    DevTmp(const DevTmp&) = delete;
-    DevTmp& operator=(const DevTmp&) = delete;
-};
-
 void* b200rwkv_engine::dalloc(size_t bytes, bool zero) {
-    void* p = nullptr;
     bytes = std::max<size_t>(bytes, 16);
-    CK(cudaMalloc(&p, bytes));
-    allocs.push_back(p);
-    if (zero) CK(cudaMemset(p, 0, bytes));
-    return p;
+    allocs.emplace_back(bytes);
+    if (zero) CK(cudaMemset(allocs.back(), 0, bytes));
+    return allocs.back();
 }
 
 const __half* b200rwkv_engine::upload_tmp(const StTensor& t) {
     if (d_tmp_holds != &t) {
-        REQUIRE(t.nbytes <= d_tmp_bytes, B200RWKV_ERR_INVALID, "internal: temp buffer too small");
+        REQUIRE(t.nbytes <= d_tmp.bytes, B200RWKV_ERR_INVALID, "internal: temp buffer too small");
         CK(cudaMemcpy(d_tmp, t.data, t.nbytes, cudaMemcpyHostToDevice));
         d_tmp_holds = &t;
         blend_loras(t);
@@ -701,10 +740,10 @@ void b200rwkv_engine::blend_loras(const StTensor& t) {
                     a->shape[1] >= 1 && a->shape[1] <= 4096,
                 B200RWKV_ERR_INVALID, "LoRA shapes do not match " + t.name + " (expected lora.0 [in, r], lora.1 [out, r])");
         const int r = (int)a->shape[1];
-        DevTmp da(a->nbytes), db(b->nbytes);
-        CK(cudaMemcpy(da.p, a->data, a->nbytes, cudaMemcpyHostToDevice));
-        CK(cudaMemcpy(db.p, b->data, b->nbytes, cudaMemcpyHostToDevice));
-        lora_blend_kernel<<<num_sms * 8, 256>>>(d_tmp, (const __half*)db.p, (const __half*)da.p, out, in, r, lo.alpha);
+        Buf<__half> da(a->nbytes), db(b->nbytes);
+        CK(cudaMemcpy(da, a->data, a->nbytes, cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(db, b->data, b->nbytes, cudaMemcpyHostToDevice));
+        lora_blend_kernel<<<num_sms * 8, 256>>>(d_tmp, db, da, out, in, r, lo.alpha);
         CK(cudaGetLastError());
         CK(cudaDeviceSynchronize());
     }
@@ -714,9 +753,9 @@ float* b200rwkv_engine::vec_f32(const StFile& st, const std::string& name, size_
     const StTensor& t = st.get(name);
     REQUIRE((size_t)t.numel() >= off + count, B200RWKV_ERR_INVALID, "tensor too small: " + name);
     float* d = (float*)dalloc(count * 4, false);
-    DevTmp tmp(count * 2);
-    CK(cudaMemcpy(tmp.p, t.data + off * 2, count * 2, cudaMemcpyHostToDevice));
-    f16_to_f32_kernel<<<cdiv((int)count, 256), 256>>>((const __half*)tmp.p, d, count, scale, bias);
+    Buf<__half> tmp(count * 2);
+    CK(cudaMemcpy(tmp, t.data + off * 2, count * 2, cudaMemcpyHostToDevice));
+    f16_to_f32_kernel<<<cdiv((int)count, 256), 256>>>(tmp, d, count, scale, bias);
     CK(cudaGetLastError());
     CK(cudaDeviceSynchronize());
     return d;
@@ -855,16 +894,16 @@ void b200rwkv_engine::launch_k(void (*kern)(P, X...), dim3 grid, dim3 block, siz
     }
     cfg.attrs = at;
     cfg.numAttrs = na;
-    cudaEvent_t ea = nullptr, eb = nullptr;
+    Event ea, eb;
     if (prof) {
-        CK(cudaEventCreate(&ea));
-        CK(cudaEventCreate(&eb));
+        ea = new_event();
+        eb = new_event();
         CK(cudaEventRecord(ea, s));
     }
     CK(cudaLaunchKernelEx(&cfg, kern, params, extra...));
     if (prof) {
         CK(cudaEventRecord(eb, s));
-        prof->recs.push_back({cls, ea, eb});
+        prof->recs.push_back({cls, std::move(ea), std::move(eb)});
     }
     ++launches_last_step;
 }
@@ -979,8 +1018,8 @@ void b200rwkv_engine::build(const StFile& st) {
     const int ver = info.version;
     const int c0 = rank * Cl, f0 = rank * Fl, v0 = rank * Vl;
 
-    CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&sm_stream, cudaStreamNonBlocking));
+    stream = new_stream();
+    sm_stream = new_stream();
     if (quant_layers > 0 && quant_type != QT_NONE) {
         REQUIRE(quant_type == QT_INT8 || quant_type == QT_NF4, B200RWKV_ERR_UNSUPPORTED, "quant_type must be Int8 or NF4 (SF4 is not implemented)");
         REQUIRE(world == 1, B200RWKV_ERR_UNSUPPORTED, "quantised layers are single-GPU in this version");
@@ -993,14 +1032,15 @@ void b200rwkv_engine::build(const StFile& st) {
     // ---- step metadata ----
     meta_ints = MetaView::ints(maxT, S);
     d_meta = (int*)dalloc(meta_ints * 4);
-    CK(cudaMallocHost(&h_meta, meta_ints * 4 * META_RING));
+    h_meta = HostBuf<int>(meta_ints * 4 * META_RING);
     memset(h_meta, 0, meta_ints * 4 * META_RING);
-    for (auto& ev : meta_ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    for (auto& ev : meta_ev) ev = new_event(cudaEventDisableTiming);
     MetaView mv{d_meta, maxT, S};
 
     // ---- temp upload buffer: largest tensor ----
-    for (auto& kv : st.tensors) d_tmp_bytes = std::max(d_tmp_bytes, kv.second.nbytes);
-    CK(cudaMalloc(&d_tmp, d_tmp_bytes));
+    size_t tmp_bytes = 0;
+    for (auto& kv : st.tensors) tmp_bytes = std::max(tmp_bytes, kv.second.nbytes);
+    d_tmp = Buf<__half>(tmp_bytes);
 
     // ---- state ----
     att_shift = (float*)dalloc((size_t)L * S * C * 4);
@@ -1038,7 +1078,7 @@ void b200rwkv_engine::build(const StFile& st) {
     split_att = S_att; split_ffn = S_ffn;
     d_hidden = (float*)dalloc(TC * 4);
     d_hid_tab = (float**)dalloc((size_t)L * sizeof(float*));
-    CK(cudaEventCreateWithFlags(&step_done, cudaEventDisableTiming));
+    step_done = new_event(cudaEventDisableTiming);
     keep_valid.assign(S, 0);
     if (rank == 0) {
         d_keep = (float*)dalloc((size_t)S * V * 4);
@@ -1248,9 +1288,9 @@ void b200rwkv_engine::build(const StFile& st) {
                 const StTensor& td = st.get(a + "time_decay");
                 REQUIRE(td.numel() == C, B200RWKV_ERR_UNSUPPORTED, "v5 time_decay must be [H, N]");
                 float* d = (float*)dalloc((size_t)Cl * 4, false);
-                DevTmp tmp((size_t)Cl * 2);
-                CK(cudaMemcpy(tmp.p, td.data + (size_t)c0 * 2, (size_t)Cl * 2, cudaMemcpyHostToDevice));
-                decay_table_kernel<<<cdiv(Cl, 256), 256>>>((const __half*)tmp.p, d, Cl);
+                Buf<__half> tmp((size_t)Cl * 2);
+                CK(cudaMemcpy(tmp, td.data + (size_t)c0 * 2, (size_t)Cl * 2, cudaMemcpyHostToDevice));
+                decay_table_kernel<<<cdiv(Cl, 256), 256>>>(tmp, d, Cl);
                 CK(cudaDeviceSynchronize());
                 wk.w_static = d;
             }
@@ -1386,8 +1426,7 @@ void b200rwkv_engine::build(const StFile& st) {
         finalize_tp();
     }
     CK(cudaDeviceSynchronize());
-    CK(cudaFree(d_tmp));
-    d_tmp = nullptr;
+    d_tmp = Buf<__half>();
 }
 
 // -----------------------------------------------------------------------------------------
@@ -1566,25 +1605,14 @@ void b200rwkv_engine::run_step(const StepShape& sh) {
     const int key = sh.MT * 8 + sh.MTR;
     auto it = graphs.find(key);
     if (it == graphs.end()) {
-        cudaGraph_t g = nullptr;
-        CK(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
-        try {
+        GraphExec ge = capture_graph(stream, [&] {
             enqueue_step(stream, sh, nullptr);
             enqueue_keep(stream, sh.MTR);
-        } catch (...) {
-            cudaStreamEndCapture(stream, &g);
-            if (g) cudaGraphDestroy(g);
-            throw;
-        }
-        CK(cudaStreamEndCapture(stream, &g));
-        cudaGraphExec_t ge = nullptr;
-        CK(cudaGraphInstantiate(&ge, g, 0));
-        CK(cudaGraphDestroy(g));
-        it = graphs.emplace(key, ge).first;
-        graph_launches[key] = launches_last_step;
+        });
+        it = graphs.emplace(key, StepGraph{std::move(ge), launches_last_step}).first;
     }
-    CK(cudaGraphLaunch(it->second, stream));
-    launch_total += graph_launches[key];         // kernels of THIS graph, not of whichever was captured last
+    CK(cudaGraphLaunch(it->second.exec, stream));
+    launch_total += it->second.launches;         // kernels of THIS graph, not of whichever was captured last
 }
 
 // fills one step's metadata; returns T
@@ -1671,7 +1699,7 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
     auto launch_score = [&](size_t first, size_t n) {
         if (n == 0) return;
         ScoreParams sp;
-        sp.rows = reinterpret_cast<const ScoreRow*>(sc_dev) + first;
+        sp.rows = reinterpret_cast<const ScoreRow*>(sc_dev.p) + first;
         sp.V = V;
         sp.score = reinterpret_cast<float*>(sc_dev + total_score * sizeof(ScoreRow));
         sp.argmax = reinterpret_cast<unsigned*>(sc_dev + total_score * (sizeof(ScoreRow) + 4));
@@ -1680,17 +1708,10 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         CK(cudaGetLastError());
     };
     if (total_score > 0) {
-        const size_t want = total_score * (sizeof(ScoreRow) + 8);
-        if (want > sc_cap) {
-            if (sc_dev) { CK(cudaFree(sc_dev)); sc_dev = nullptr; }
-            if (sc_host) { CK(cudaFreeHost(sc_host)); sc_host = nullptr; }
-            sc_cap = 0;
-            const size_t bytes = std::max<size_t>(want, 256 * (sizeof(ScoreRow) + 8));
-            CK(cudaMalloc(&sc_dev, bytes));
-            CK(cudaMallocHost(&sc_host, bytes));
-            sc_cap = bytes;
-        }
-        sc_rows = reinterpret_cast<ScoreRow*>(sc_host);
+        const size_t want = total_score * (sizeof(ScoreRow) + 8), bytes = std::max<size_t>(want, 256 * (sizeof(ScoreRow) + 8));
+        sc_dev.grow(want, bytes);
+        sc_host.grow(want, bytes);
+        sc_rows = reinterpret_cast<ScoreRow*>(sc_host.p);
         std::lock_guard<std::mutex> lk(keep_mu);
         for (int i = 0; i < nslot; ++i)
             if (option[i] == B200RWKV_OPTION_SCORE && ntok[i] > 0)
@@ -1702,22 +1723,12 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         for (int i = 0; i < nslot; ++i)
             if (option[i] == B200RWKV_OPTION_NONE && ntok[i] > 0) keep_valid[slot[i]] = 0;
     }
-    if (hidden_keep && total_tok > hidden_cap_rows) {
-        if (d_hidden_all) { CK(cudaFree(d_hidden_all)); d_hidden_all = nullptr; hidden_cap_rows = 0; }
-        const size_t want = std::max<size_t>(total_tok, 256);
-        CK(cudaMalloc(&d_hidden_all, want * C * 4));
-        hidden_cap_rows = want;
-    }
+    if (hidden_keep) d_hidden_all.grow(total_tok * C * 4, std::max<size_t>(total_tok, 256) * C * 4);
     hidden_rows = 0;
     const size_t n_hid = hid_layers.size();
     hid_last.clear();
     hid_last_rows = 0;
-    if (n_hid * total_tok * C > hid_all_floats) {
-        if (hid_all) { CK(cudaFree(hid_all)); hid_all = nullptr; hid_all_floats = 0; }
-        const size_t want = n_hid * std::max<size_t>(total_tok, 256) * C;
-        CK(cudaMalloc(&hid_all, want * 4));
-        hid_all_floats = want;
-    }
+    hid_all.grow(n_hid * total_tok * C * 4, n_hid * std::max<size_t>(total_tok, 256) * C * 4);
     int step_no = 0;
     for (;;) {
         int n_active = 0;
@@ -1892,15 +1903,9 @@ SampleAdjust b200rwkv_engine::stage_sample_args(int nrows, const int32_t* slots,
                  o_pt = al(o_bo + (size_t)(nrows + 1) * 4), o_pv = al(o_pt + (size_t)npen * 4), o_bt = al(o_pv + (size_t)npen * 4),
                  o_bv = al(o_bt + (size_t)nbias * 4), o_al = al(o_bv + (size_t)nbias * 4),
                  total = al(o_al + (allow_bits ? (size_t)nrows * words * 4 : 0));
-    if (total > tk_cap) {
-        if (tk_dev) { CK(cudaFree(tk_dev)); tk_dev = nullptr; }
-        if (tk_host) { CK(cudaFreeHost(tk_host)); tk_host = nullptr; }
-        tk_cap = 0;
-        const size_t want = std::max<size_t>(total * 2, 1 << 20);
-        CK(cudaMalloc(&tk_dev, want));
-        CK(cudaMallocHost(&tk_host, want));
-        tk_cap = want;
-    }
+    const size_t want = std::max<size_t>(total * 2, 1 << 20);
+    tk_dev.grow(total, want);
+    tk_host.grow(total, want);
     std::vector<int32_t> zeros(nrows + 1, 0);
     memcpy(tk_host + o_slot, slots, (size_t)nrows * 4);
     memcpy(tk_host + o_po, pen_off ? pen_off : zeros.data(), (size_t)(nrows + 1) * 4);
@@ -1956,15 +1961,9 @@ void b200rwkv_engine::sample_probs(int nrows, const int32_t* slots, const int32_
     memset(&pp, 0, sizeof(pp));
     pp.keep = d_keep; pp.V = V; pp.nseg = cdiv(V, TOPK_SEG); pp.ld = (V + 3) & ~3;
     const size_t row_bytes = (size_t)nrows * pp.ld * 4, need = row_bytes + (size_t)nrows * pp.nseg * sizeof(float2);
-    if (need > sp_cap) {
-        if (sp_dev) { CK(cudaFree(sp_dev)); sp_dev = nullptr; }
-        sp_cap = 0;
-        const size_t want = std::min(std::max<size_t>(need * 2, 1 << 20), (size_t)S * (pp.ld * 4 + pp.nseg * sizeof(float2)));
-        CK(cudaMalloc(&sp_dev, want));
-        sp_cap = want;
-    }
+    sp_dev.grow(need, std::min(std::max<size_t>(need * 2, 1 << 20), (size_t)S * (pp.ld * 4 + pp.nseg * sizeof(float2))));
     pp.adj = stage_sample_args(nrows, slots, pen_off, pen_tok, pen_val, allow_bits, bias_off, bias_tok, bias_val);
-    pp.out = (float*)sp_dev;
+    pp.out = (float*)sp_dev.p;
     pp.stats = (float2*)(sp_dev + row_bytes);
     probs_stats_kernel<<<dim3(pp.nseg, nrows), TOPK_SEG_THREADS, 0, sm_stream>>>(pp);
     CK(cudaGetLastError());
@@ -2344,13 +2343,8 @@ static void snapshot_copy(b200rwkv_engine* e, int slot, float* buf, bool to_snap
 static Snapshot snapshot_alloc(b200rwkv_engine* e, bool with_logits) {
     Snapshot sn;
     const size_t rec = 2 * (size_t)e->C + (size_t)e->Hl * e->N * e->N;
-    sn.bytes = rec * e->L * 4;
-    CK(cudaMalloc(&sn.buf, sn.bytes));
-    if (with_logits) {
-        cudaError_t ce = cudaMalloc(&sn.logits, (size_t)e->V * 4);
-        if (ce != cudaSuccess) { cudaFree(sn.buf); CK(ce); }
-        sn.bytes += (size_t)e->V * 4;
-    }
+    sn.buf = Buf<float>(rec * e->L * 4);
+    if (with_logits) sn.logits = Buf<float>((size_t)e->V * 4);
     return sn;
 }
 
@@ -2366,19 +2360,13 @@ static int32_t rank_state_read(b200rwkv_engine* e, int32_t slot, uint64_t* snaps
         has_row = e->d_keep && e->keep_valid[slot];
     }
     Snapshot sn = snapshot_alloc(e, has_row);
-    try {
-        snapshot_copy(e, slot, sn.buf, true);
-        // the slot's last logits row travels with the state (CachedItem.output, run.rs:199-205): a cache hit can be sampled
-        // on the device without re-running the last token
-        if (has_row) CK(cudaMemcpyAsync(sn.logits, e->d_keep + (size_t)slot * e->V, (size_t)e->V * 4, cudaMemcpyDeviceToDevice, e->stream));
-        CK(cudaStreamSynchronize(e->stream));
-    } catch (...) {
-        cudaFree(sn.buf);
-        if (sn.logits) cudaFree(sn.logits);
-        throw;
-    }
+    snapshot_copy(e, slot, sn.buf, true);
+    // the slot's last logits row travels with the state (CachedItem.output, run.rs:199-205): a cache hit can be sampled
+    // on the device without re-running the last token
+    if (has_row) CK(cudaMemcpyAsync(sn.logits, e->d_keep + (size_t)slot * e->V, (size_t)e->V * 4, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
     const uint64_t id = e->next_snap++;
-    e->snaps[id] = sn;
+    e->snaps[id] = std::move(sn);
     *snapshot_id = id;
     API_END
 }
@@ -2410,8 +2398,6 @@ static int32_t rank_state_free(b200rwkv_engine* e, uint64_t snapshot_id) {
     auto it = e->snaps.find(snapshot_id);
     REQUIRE(it != e->snaps.end(), B200RWKV_ERR_STATE, "unknown snapshot id");
     CK(cudaSetDevice(e->dev));
-    CK(cudaFree(it->second.buf));
-    if (it->second.logits) CK(cudaFree(it->second.logits));
     e->snaps.erase(it);
     API_END
 }
@@ -2443,19 +2429,13 @@ static int32_t rank_snapshot_load(b200rwkv_engine* e, const float* state_in, con
     std::lock_guard<std::mutex> lk(e->mu);
     CK(cudaSetDevice(e->dev));
     Snapshot sn = snapshot_alloc(e, logits_in != nullptr && e->d_keep != nullptr);
-    try {
-        const size_t n = (size_t)e->L * (e->N + 2) * e->C;
-        CK(cudaMemcpyAsync(e->d_api, state_in, n * 4, cudaMemcpyHostToDevice, e->stream));
-        e->state_xform(0, true, sn.buf);
-        if (sn.logits) CK(cudaMemcpyAsync(sn.logits, logits_in, (size_t)e->V * 4, cudaMemcpyHostToDevice, e->stream));
-        CK(cudaStreamSynchronize(e->stream));
-    } catch (...) {
-        cudaFree(sn.buf);
-        if (sn.logits) cudaFree(sn.logits);
-        throw;
-    }
+    const size_t n = (size_t)e->L * (e->N + 2) * e->C;
+    CK(cudaMemcpyAsync(e->d_api, state_in, n * 4, cudaMemcpyHostToDevice, e->stream));
+    e->state_xform(0, true, sn.buf);
+    if (sn.logits) CK(cudaMemcpyAsync(sn.logits, logits_in, (size_t)e->V * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
     const uint64_t id = e->next_snap++;
-    e->snaps[id] = sn;
+    e->snaps[id] = std::move(sn);
     *snapshot_id = id;
     API_END
 }
@@ -2466,7 +2446,7 @@ int32_t b200rwkv_cache_stats(b200rwkv_engine* e, int64_t* num_snapshots, int64_t
     std::lock_guard<std::mutex> lk(e->mu);
     CK(cudaSetDevice(e->dev));
     int64_t used = 0;
-    for (auto& kv : e->snaps) used += (int64_t)kv.second.bytes;
+    for (auto& kv : e->snaps) used += (int64_t)(kv.second.buf.bytes + kv.second.logits.bytes);
     size_t fr = 0, tot = 0;
     CK(cudaMemGetInfo(&fr, &tot));
     if (num_snapshots) *num_snapshots = (int64_t)e->snaps.size();
@@ -2496,13 +2476,9 @@ int32_t b200rwkv_softmax(b200rwkv_engine* e, int32_t rows, const float* in, floa
     if (rows == 0) return B200RWKV_OK;
     std::lock_guard<std::mutex> lk(e->sm_mu);
     CK(cudaSetDevice(e->dev));
-    if (rows > e->sm_rows_cap) {
-        if (e->sm_in) { CK(cudaFree(e->sm_in)); CK(cudaFree(e->sm_out)); e->sm_in = e->sm_out = nullptr; }
-        CK(cudaMalloc(&e->sm_in, (size_t)rows * e->V * 4));
-        CK(cudaMalloc(&e->sm_out, (size_t)rows * e->V * 4));
-        e->sm_rows_cap = rows;
-    }
     const size_t bytes = (size_t)rows * e->V * 4;
+    e->sm_in.grow(bytes, bytes);
+    e->sm_out.grow(bytes, bytes);
     CK(cudaMemcpyAsync(e->sm_in, in, bytes, cudaMemcpyHostToDevice, e->sm_stream));
     softmax_kernel<<<rows, 1024, 0, e->sm_stream>>>(e->sm_in, e->sm_out, e->V);
     CK(cudaGetLastError());
@@ -2573,20 +2549,15 @@ static int32_t rank_bench_decode(b200rwkv_engine* e, int32_t nslot, const int32_
     std::vector<int> all;
     build_decode_metas(e, nslot, slot, tokens, nsteps, all);
     long long launches_before = 0;
-    int* d_all = nullptr;
-    CK(cudaMalloc(&d_all, all.size() * 4));
+    Buf<int> d_all(all.size() * 4);
     CK(cudaMemcpy(d_all, all.data(), all.size() * 4, cudaMemcpyHostToDevice));
-    void* flush = nullptr;
+    Buf<void> flush;
     const size_t flush_bytes = 256u << 20;
-    if (flush_l2) CK(cudaMalloc(&flush, flush_bytes));
-    cudaEvent_t ea, eb;
-    CK(cudaEventCreate(&ea));
-    CK(cudaEventCreate(&eb));
-    std::vector<cudaEvent_t> marks;            // per-step boundaries (optional): the distribution of the step time
-    if (step_ms_out) {
-        marks.resize(steps);
-        for (auto& m : marks) CK(cudaEventCreate(&m));
-    }
+    if (flush_l2) flush = Buf<void>(flush_bytes);
+    Event ea = new_event(), eb = new_event();
+    std::vector<Event> marks;                  // per-step boundaries (optional): the distribution of the step time
+    if (step_ms_out)
+        for (int i = 0; i < steps; ++i) marks.push_back(new_event());
     const StepShape sh = e->step_shape(nslot, nslot);
     for (int st = 0; st < nsteps; ++st) {
         if (st == warmup) {
@@ -2609,12 +2580,7 @@ static int32_t rank_bench_decode(b200rwkv_engine* e, int32_t nslot, const int32_
     for (int i = 0; i < (int)marks.size(); ++i) {
         CK(cudaEventElapsedTime(step_ms_out + i, i == 0 ? ea : marks[i - 1], marks[i]));
     }
-    for (auto& m : marks) cudaEventDestroy(m);
     if (launches_out) *launches_out = (int64_t)(e->launch_total - launches_before);
-    CK(cudaEventDestroy(ea));
-    CK(cudaEventDestroy(eb));
-    if (flush) CK(cudaFree(flush));
-    CK(cudaFree(d_all));
     API_END
 }
 
@@ -2638,8 +2604,6 @@ static int32_t rank_profile_step(b200rwkv_engine* e, int32_t nslot, const int32_
         CK(cudaEventElapsedTime(&t, r.a, r.b));
         ms[r.cls] += t;
         launches[r.cls] += 1;
-        cudaEventDestroy(r.a);
-        cudaEventDestroy(r.b);
     }
     if (gemm_weight_bytes) *gemm_weight_bytes = (int64_t)e->weight_bytes_total;
     API_END
@@ -2665,24 +2629,13 @@ static int32_t rank_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int3
     CK(cudaMemcpyAsync(e->d_meta, all.data(), e->meta_ints * 4, cudaMemcpyHostToDevice, e->stream));
     const StepShape sh = e->step_shape(nslot, nslot);
     // traced copy of the step graph (the production graphs carry null trace pointers)
-    e->trace_capture = true;
     e->step_trace_types.clear();
     e->step_trace_bytes.clear();
-    cudaGraph_t g = nullptr;
-    cudaGraphExec_t ge = nullptr;
-    CK(cudaStreamBeginCapture(e->stream, cudaStreamCaptureModeThreadLocal));
-    try {
+    const GraphExec ge = capture_graph(e->stream, [&] {
+        e->trace_capture = true;
+        struct Off { bool& f; ~Off() { f = false; } } off{e->trace_capture};     // on every exit
         e->enqueue_step(e->stream, sh, nullptr);
-    } catch (...) {
-        cudaStreamEndCapture(e->stream, &g);
-        if (g) cudaGraphDestroy(g);
-        e->trace_capture = false;
-        throw;
-    }
-    e->trace_capture = false;
-    CK(cudaStreamEndCapture(e->stream, &g));
-    CK(cudaGraphInstantiate(&ge, g, 0));
-    CK(cudaGraphDestroy(g));
+    });
     const int n = (int)e->step_trace_types.size();
     const size_t row = b200rwkv_engine::STEP_TRACE_ROW;
     std::vector<unsigned long long> h((size_t)n * row);
@@ -2713,7 +2666,6 @@ static int32_t rank_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int3
         }
         step_acc += (double)(t1 - t0) * 1e-3;
     }
-    cudaGraphExecDestroy(ge);
     int m = 0;
     for (int i = 0; i < n && m < cap; ++i) {
         if (e_acc[i] <= 0.0) continue;
@@ -2739,18 +2691,19 @@ int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int3
     CK(cudaSetDevice(device));
     const int tiles = cdiv(N, GEMM_BN), KB = K / GEMM_BK;
     const size_t blk = (size_t)q_block_bytes(quant_type), total = (size_t)tiles * KB * blk;
-    DevTmp src((size_t)N * K * 2), dst(total);
-    CK(cudaMemcpy(src.p, w_f16, (size_t)N * K * 2, cudaMemcpyHostToDevice));
+    Buf<__half> src((size_t)N * K * 2);
+    Buf<uint8_t> dst(total);
+    CK(cudaMemcpy(src, w_f16, (size_t)N * K * 2, cudaMemcpyHostToDevice));
     const size_t nwarp = (size_t)tiles * KB * GEMM_BN;
     int nsm = 0;
     CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
     const int grid = (int)std::min<size_t>((nwarp + 7) / 8, (size_t)nsm * 32);
-    if (quant_type == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256>>>((const __half*)src.p, K, 0, 0, N, tiles, KB, (uint8_t*)dst.p);
-    else quantize_weight_kernel<QT_NF4><<<grid, 256>>>((const __half*)src.p, K, 0, 0, N, tiles, KB, (uint8_t*)dst.p);
+    if (quant_type == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256>>>(src, K, 0, 0, N, tiles, KB, dst);
+    else quantize_weight_kernel<QT_NF4><<<grid, 256>>>(src, K, 0, 0, N, tiles, KB, dst);
     CK(cudaGetLastError());
     CK(cudaDeviceSynchronize());
     std::vector<uint8_t> h(total);
-    CK(cudaMemcpy(h.data(), dst.p, total, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(h.data(), dst, total, cudaMemcpyDeviceToHost));
     for (int n = 0; n < N; ++n) {
         const int tile = n / GEMM_BN, r = n % GEMM_BN;
         for (int kb = 0; kb < KB; ++kb) {
@@ -2811,7 +2764,7 @@ struct OpStep {
         e->dev = device;
         e->S = S;                                  // e->maxT stays A16_MAX_ROWS: the metadata layout of every engine
         e->split_on = split;
-        CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
+        e->stream = new_stream();
         for (int l = 0; l < launches; ++l) {
             std::vector<uint32_t> tk(A16_MAX_ROWS, 0);
             if (tokens) std::copy(tokens + (size_t)l * T, tokens + (size_t)(l + 1) * T, tk.begin());
@@ -3156,8 +3109,7 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
             d.proto.ldo = s.ldo;
         }
     }
-    CK(cudaMalloc(&e->d_tmp, wmax));               // make_launch uploads each matrix through the engine's staging buffer
-    e->d_tmp_bytes = wmax;
+    e->d_tmp = Buf<__half>(wmax);                  // make_launch uploads each matrix through the engine's staging buffer
     GemmLaunch g = e->make_launch(sv, grid, quant_type);
     e->gemm_ws = (float*)e->dalloc(e->gemm_ws_floats * 4, false);
     g.p.ws = e->gemm_ws;
@@ -3181,14 +3133,14 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
     // operands and outputs of every launch; the caller's output contents go up first
     std::vector<GemmLaunch> runs(launches, g);
     std::vector<std::vector<uint16_t>> h16(nseg);         // f16 bits of an A16 destination
-    DevTmp xs((size_t)T * std::max_element(seg, seg + nseg, [](const b200rwkv_gemm_seg& a, const b200rwkv_gemm_seg& b) { return a.K < b.K; })->K * 4);
+    Buf<float> xs((size_t)T * std::max_element(seg, seg + nseg, [](const b200rwkv_gemm_seg& a, const b200rwkv_gemm_seg& b) { return a.K < b.K; })->K * 4);
     for (int l = 0; l < launches; ++l) {
         for (int i = 0; i < nseg; ++i) {
             const b200rwkv_gemm_seg& s = seg[i];
             GemmSeg& sg = runs[l].p.seg[i];
             __half* a = (__half*)e->dalloc(a16_halves(s.K) * 2, true);
-            CK(cudaMemcpy(xs.p, s.x + (size_t)l * T * s.K, (size_t)T * s.K * 4, cudaMemcpyHostToDevice));
-            a16_from_f32_kernel<<<(int)std::min<size_t>(((size_t)T * s.K + 255) / 256, (size_t)e->num_sms * 8), 256>>>((const float*)xs.p, T, s.K, th, sh.split, a);
+            CK(cudaMemcpy(xs, s.x + (size_t)l * T * s.K, (size_t)T * s.K * 4, cudaMemcpyHostToDevice));
+            a16_from_f32_kernel<<<(int)std::min<size_t>(((size_t)T * s.K + 255) / 256, (size_t)e->num_sms * 8), 256>>>(xs, T, s.K, th, sh.split, a);
             CK(cudaGetLastError());
             CK(cudaDeviceSynchronize());           // xs is refilled by the next upload
             sg.A = a;
@@ -3406,12 +3358,10 @@ int32_t b200rwkv_debug_gemm_time(b200rwkv_engine* e, int32_t which, int32_t reps
     std::vector<int> m(e->meta_ints, 0);
     m[0] = 16; m[1] = std::min(16, e->S); m[2] = 16;
     CK(cudaMemcpy(e->d_meta, m.data(), e->meta_ints * 4, cudaMemcpyHostToDevice));
-    cudaEvent_t a, b;
-    CK(cudaEventCreate(&a));
-    CK(cudaEventCreate(&b));
+    Event a = new_event(), b = new_event();
     const int n = reps * e->L;
-    unsigned long long* d_tr = nullptr;
-    if (trace_out) { CK(cudaMalloc(&d_tr, (size_t)e->L * 16 * 8)); CK(cudaMemset(d_tr, 0, (size_t)e->L * 16 * 8)); }
+    Buf<unsigned long long> d_tr;
+    if (trace_out) { d_tr = Buf<unsigned long long>((size_t)e->L * 16 * 8); CK(cudaMemset(d_tr, 0, (size_t)e->L * 16 * 8)); }
     const StepShape sh = e->step_shape(16, 16);
     for (int i = 0; i < e->L; ++i) e->launch_gemm(pick(i), sh, e->stream, nullptr);
     CK(cudaEventRecord(a, e->stream));
@@ -3422,7 +3372,7 @@ int32_t b200rwkv_debug_gemm_time(b200rwkv_engine* e, int32_t which, int32_t reps
     }
     CK(cudaEventRecord(b, e->stream));
     CK(cudaStreamSynchronize(e->stream));
-    if (d_tr) { CK(cudaMemcpy(trace_out, d_tr, (size_t)e->L * 16 * 8, cudaMemcpyDeviceToHost)); CK(cudaFree(d_tr)); }
+    if (d_tr) CK(cudaMemcpy(trace_out, d_tr, (size_t)e->L * 16 * 8, cudaMemcpyDeviceToHost));
     float ms = 0.f;
     CK(cudaEventElapsedTime(&ms, a, b));
     *ms_out = ms / n;
