@@ -330,7 +330,9 @@ __global__ void __launch_bounds__(KEEP_THREADS) keep_rows_kernel(const __grid_co
 //   f32 above a logit of about 88; elsewhere the two agree to f32 rounding)
 // Element i of the row always goes to thread (i / 4) % SCORE_THREADS, in the same order, whatever the row's address: the
 // result of a row does not depend on where it sits in d_logits or which rows share the launch.  src == nullptr (a slot with
-// no kept row): NaN and UINT32_MAX.
+// no kept row): NaN and UINT32_MAX.  A NaN anywhere in the row makes the score NaN, as it makes softmax_kernel's row and the
+// reference's exp(x) / sum exp(x) NaN; the argmax skips NaN entries (UINT32_MAX for a row of only NaN).  The NaN flag rides
+// beside the sums and changes none of their arithmetic.
 // ---------------------------------------------------------------------------------------
 struct ScoreRow {
     const float* src;           // [V]
@@ -349,7 +351,9 @@ struct ScoreAcc {
     float m, s;                 // running max, sum expf(x - m)
     float bx;                   // best logit, its lowest id
     unsigned bi;
+    int nan;                    // a NaN was seen (every comparison below is false for one, so the sums skip it)
     __device__ __forceinline__ void add(const float x, const unsigned i) {
+        nan |= x != x;
         if (x > m) { s = s * expf(m - x) + 1.f; m = x; }
         else if (x > -INFINITY) s += expf(x - m);
         if (x > bx || (x == bx && i < bi)) { bx = x; bi = i; }
@@ -359,10 +363,12 @@ struct ScoreAcc {
         if (M > -INFINITY) s = (m > -INFINITY ? s * expf(m - M) : 0.f) + (o.m > -INFINITY ? o.s * expf(o.m - M) : 0.f);
         m = M;
         if (o.bx > bx || (o.bx == bx && o.bi < bi)) { bx = o.bx; bi = o.bi; }
+        nan |= o.nan;
     }
     __device__ __forceinline__ ScoreAcc shfl_xor(const int lane_mask) const {
         return {__shfl_xor_sync(0xffffffffu, m, lane_mask), __shfl_xor_sync(0xffffffffu, s, lane_mask),
-                __shfl_xor_sync(0xffffffffu, bx, lane_mask), __shfl_xor_sync(0xffffffffu, bi, lane_mask)};
+                __shfl_xor_sync(0xffffffffu, bx, lane_mask), __shfl_xor_sync(0xffffffffu, bi, lane_mask),
+                __shfl_xor_sync(0xffffffffu, nan, lane_mask)};
     }
 };
 
@@ -374,7 +380,7 @@ __global__ void __launch_bounds__(SCORE_THREADS) score_rows_kernel(const __grid_
         if (tid == 0) { p.score[rw.dst] = __int_as_float(0x7fc00000); p.argmax[rw.dst] = 0xFFFFFFFFu; }
         return;
     }
-    ScoreAcc a{-INFINITY, 0.f, -INFINITY, 0xFFFFFFFFu};
+    ScoreAcc a{-INFINITY, 0.f, -INFINITY, 0xFFFFFFFFu, 0};
     const int n4 = p.V >> 2;
     const float* s = rw.src;
     if ((reinterpret_cast<uintptr_t>(s) & 15) == 0) {
@@ -394,11 +400,11 @@ __global__ void __launch_bounds__(SCORE_THREADS) score_rows_kernel(const __grid_
     if ((tid & 31) == 0) red[tid >> 5] = a;
     __syncthreads();
     if (tid < 32) {
-        a = (tid < SCORE_THREADS / 32) ? red[tid] : ScoreAcc{-INFINITY, 0.f, -INFINITY, 0xFFFFFFFFu};
+        a = (tid < SCORE_THREADS / 32) ? red[tid] : ScoreAcc{-INFINITY, 0.f, -INFINITY, 0xFFFFFFFFu, 0};
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) a.merge(a.shfl_xor(o));
         if (tid == 0) {
-            p.score[rw.dst] = (__ldcg(s + rw.target) - a.m) - logf(a.s);
+            p.score[rw.dst] = a.nan ? __int_as_float(0x7fc00000) : (__ldcg(s + rw.target) - a.m) - logf(a.s);
             p.argmax[rw.dst] = a.bi;
         }
     }

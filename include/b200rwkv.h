@@ -157,7 +157,10 @@ int32_t b200rwkv_infer(b200rwkv_engine*, int32_t nslot, const int32_t* slot, con
  *     maximum; the row predicting x_j is the row after x_{j-1} for j >= 1, and the slot's kept row for j = 0 (the row of the
  *     slot's current state: from the previous infer call, or from b200rwkv_state_write of a snapshot that carries a row;
  *     none, as after b200rwkv_state_load or a NONE entry with tokens: NaN);
- *   - argmax_out[j] = id of the largest logit of that row, lowest id on ties (UINT32_MAX if there is no row).
+ *   - argmax_out[j] = id of the largest logit of that row, lowest id on ties (UINT32_MAX if there is no row);
+ *   - special values: a NaN anywhere in the row makes score_out[j] NaN, and argmax_out[j] is the lowest id of the largest
+ *     non-NaN logit (UINT32_MAX if every logit is NaN); a -inf target in a row with a finite maximum scores -inf; a row of
+ *     only -inf scores NaN with argmax 0; a target so far below the maximum that x_t - m overflows f32 scores -inf.
  * score_out / argmax_out hold sum(ntok) over the SCORE entries, in entry order; argmax_out may be NULL.  LAST, FULL, NONE and
  * SCORE entries mix freely in one call.  Every argument is checked before the first CUDA call.  Tensor parallel engines answer
  * B200RWKV_ERR_UNSUPPORTED for SCORE entries.  b200rwkv_infer refuses option 3. */

@@ -11,6 +11,9 @@ Error bound of one score (derived in `score_bound`): the kernel computes (x_t - 
   - logf within 1 ulp of log S (<= log V), x_t - m rounded once, the final subtraction rounded once.
 With u = 2^-24:  |err| <= (4 + 5k + k + 8) u + 2u log V + u (|x_t - m| + log V) + u |x_t - m|.  For the vocabularies here
 (V <= 2048, k <= 8) that is below 2^-16 + 2^-22 |x_t - m|, the bound the tests assert and report ratios against.
+tests/test_gpu_score_rows.py derives the bound per row from the kernel's thread map, with the rounding of every expf argument
+counted as well, for every vocabulary (65536 and above included) and for rows built to hit the kernel's edges; at V <= 2048 it
+stays inside this headline.
 """
 import dataclasses
 
