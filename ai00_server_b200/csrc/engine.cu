@@ -400,7 +400,6 @@ static bool state_from_st(const StFile& st, int L, int H, int N, int C, std::vec
 // engine
 // =========================================================================================
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
-static inline int rup(int a, int b) { return cdiv(a, b) * b; }
 
 enum KClass { KC_GEMM = 0, KC_WKV = 1, KC_LN = 2, KC_OTHER = 3 };
 
@@ -423,26 +422,28 @@ struct SegDesc {
 
 struct A16Buf {
     __half* p = nullptr;
-    int kq = 0;                // k32 blocks per m-tile (padded K / 32)
     size_t halves_per_matrix = 0;
 };
 
+// What a step launches for one layer.  Decode-shaped steps (MT == 1) of a layer with a front half run it in place of LN1
+// and the `lora` launches; every step then runs `pre`, WKV, O, LN2 and `ffn`.
 struct Layer {
     LnMixParams ln1, ln2;
-    std::vector<GemmLaunch> pre;    // launches between LN1 and WKV
-    int wd2_index = -1;             // v6: index in `pre` of the decay-LoRA stage-2 launch (skipped when the WKV kernel evaluates it in place)
+    // v6 decode front half (pre6.cuh: LN1 + token shift + ddlerp LoRA in one launch), when the model fits pre6_kernel.  Its
+    // `ln` stays empty: the launch takes LN1's parameters, whose residual partials finalize_tp wires after build.
+    bool has_pre6 = false;
+    Pre6Params pre6{};
+    std::vector<GemmLaunch> lora;   // v6 ddlerp LoRA W1, W2: after LN1 on the steps that do not run the front half
+    std::vector<GemmLaunch> pre;    // launches every step runs between LN1 (or the front half) and WKV
     WkvParams wkv;
     GemmLaunch o;
     std::vector<GemmLaunch> ffn;    // launches after LN2
-    // v6 decode front half as one launch (pre6.cuh): row-major copies of the ddlerp LoRA weights
-    const __half* w1_raw = nullptr;
-    const __half* w2_raw = nullptr;
-    const float* mu5[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
 };
 
 struct Profiler {
     struct Rec { int cls; Event a, b; };
     std::vector<Rec> recs;
+    size_t weight_bytes = 0;        // algorithmic weight bytes of the projection launches enqueued
 };
 
 struct Snapshot { Buf<float> buf, logits; };   // CachedItem {state, output} on the device (run.rs:199-205)
@@ -531,7 +532,6 @@ struct b200rwkv_engine {
     unsigned* d_epoch = nullptr;
     Stream stream, sm_stream;
     std::vector<Buf<void>> allocs;
-    size_t weight_bytes_total = 0;
 
     // model
     __half* emb = nullptr;
@@ -635,10 +635,9 @@ struct b200rwkv_engine {
     template <typename P, typename... X>
     void launch_k(void (*kern)(P, X...), dim3 grid, dim3 block, size_t smem, const P& params, int cls, cudaStream_t s, Profiler* prof,
                   X... extra);
-    bool fold_wd2 = false;
     bool split_on = false;        // precision 1: split (hi + lo f16) projection operands, every step decode-shaped
     bool split_act = false;
-    bool fused_pre_ok = false, ln_cluster_ok = false;     // decode-shaped cluster kernels of pre6.cuh fit the model
+    bool ln_cluster_ok = false;   // the decode-shaped cluster LN kernels of pre6.cuh fit the model
     unsigned* pre_gbar = nullptr;
     int launch_cluster = 0;                       // consumed by the next launch_k
     // profiling aid (b200rwkv_profile_insitu): 8 globaltimer stamps of CTA 0 per launch of the per-op chain
@@ -763,8 +762,7 @@ float* b200rwkv_engine::vec_f32(const StFile& st, const std::string& name, size_
 
 A16Buf b200rwkv_engine::a16_alloc(int K, int nmat) {
     A16Buf b;
-    b.kq = rup(K, GEMM_BK) / 32;             // whole 128-wide k blocks, zero padded
-    b.halves_per_matrix = a16_halves(K);
+    b.halves_per_matrix = a16_halves(K);     // whole 128-wide k blocks, zero padded
     b.p = (__half*)dalloc(b.halves_per_matrix * 2 * nmat, true);
     return b;
 }
@@ -864,7 +862,6 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
     g.p.nrows = d_meta;   // T by default
     g.p.w_lbo = GEMM_W_LBO; g.p.w_sbo = GEMM_W_SBO; g.p.a_lbo = GEMM_A_LBO; g.p.a_sbo = GEMM_A_SBO;
     gemm_ws_floats = std::max(gemm_ws_floats, (size_t)tile * g.p.max_contrib * (size_t)maxT * GEMM_BN);
-    weight_bytes_total += g.weight_bytes;
     return g;
 }
 
@@ -910,10 +907,13 @@ void b200rwkv_engine::launch_k(void (*kern)(P, X...), dim3 grid, dim3 block, siz
 
 void b200rwkv_engine::launch_gemm(const GemmLaunch& g, const StepShape& sh, cudaStream_t s, Profiler* prof, bool head) {
     const int MT = head ? sh.MTR : sh.MT;
+    GemmParams p = g.p;
+    for (int i = 0; i < p.nseg; ++i)
+        if (p.seg[i].out_mode != OUT_F32) p.seg[i].ldo = sh.th;     // A16 outputs feed a projection of this step
     if (g.qtype != QT_NONE) {
         REQUIRE(!sh.split, B200RWKV_ERR_UNSUPPORTED, "internal: quantised projections run with f16 activations");
         const int grid = MT >= 4 ? g.grid_wide : g.grid;
-#define QLAUNCH(MT_, QT_) launch_k(qgemm_kernel<MT_, QT_>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<MT_, QT_>::SMEM_BYTES, g.p, KC_GEMM, s, prof)
+#define QLAUNCH(MT_, QT_) launch_k(qgemm_kernel<MT_, QT_>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<MT_, QT_>::SMEM_BYTES, p, KC_GEMM, s, prof)
         if (g.qtype == QT_INT8) {
             switch (MT) { case 1: QLAUNCH(1, QT_INT8); break; case 2: QLAUNCH(2, QT_INT8); break; case 4: QLAUNCH(4, QT_INT8); break; default: QLAUNCH(8, QT_INT8); break; }
         } else {
@@ -925,12 +925,12 @@ void b200rwkv_engine::launch_gemm(const GemmLaunch& g, const StepShape& sh, cuda
     // RING 2 = one stage less than fits, so the small kernels around a projection can share its SMs (findings r1 §7)
     switch (MT) {
         case 1:
-            if (sh.split) launch_k(gemm_kernel<2, 2, true>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<2, 2>::SMEM_BYTES, g.p, KC_GEMM, s, prof);
-            else launch_k(gemm_kernel<1, 2>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<1, 2>::SMEM_BYTES, g.p, KC_GEMM, s, prof);
+            if (sh.split) launch_k(gemm_kernel<2, 2, true>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<2, 2>::SMEM_BYTES, p, KC_GEMM, s, prof);
+            else launch_k(gemm_kernel<1, 2>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<1, 2>::SMEM_BYTES, p, KC_GEMM, s, prof);
             break;
-        case 2: launch_k(gemm_kernel<2>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<2>::SMEM_BYTES, g.p, KC_GEMM, s, prof); break;
-        case 4: launch_k(gemm_kernel<4>, dim3(g.grid_wide), dim3(GEMM_THREADS), GemmCfg<4>::SMEM_BYTES, g.p, KC_GEMM, s, prof); break;
-        default: launch_k(gemm_kernel<8>, dim3(g.grid_wide), dim3(GEMM_THREADS), GemmCfg<8>::SMEM_BYTES, g.p, KC_GEMM, s, prof); break;
+        case 2: launch_k(gemm_kernel<2>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<2>::SMEM_BYTES, p, KC_GEMM, s, prof); break;
+        case 4: launch_k(gemm_kernel<4>, dim3(g.grid_wide), dim3(GEMM_THREADS), GemmCfg<4>::SMEM_BYTES, p, KC_GEMM, s, prof); break;
+        default: launch_k(gemm_kernel<8>, dim3(g.grid_wide), dim3(GEMM_THREADS), GemmCfg<8>::SMEM_BYTES, p, KC_GEMM, s, prof); break;
     }
 }
 
@@ -1107,16 +1107,17 @@ void b200rwkv_engine::build(const StFile& st) {
         embed.x_out = x_a;
     }
 
+    // step-shape fields (kq_tile, d1_kq, an A16 ldo) stay 0 here: the launch_* functions fill them in per step
     auto base_ln = [&](LnMixParams& p) {
         memset(&p, 0, sizeof(p));
-        p.C = C; p.meta = mv; p.kq_tile = C / 32;
+        p.C = C; p.meta = mv;
     };
     auto f32_seg = [&](const StTensor& t, int n0, int Nn, int k0, int K, const A16Buf& ab, float* out, int ldo, int act,
                        const float* bias, int a_koff = 0, int a_mat = 0) {
         SegDesc d;
         d.t = &t; d.n0 = n0; d.N = Nn; d.k0 = k0; d.K = K;
         REQUIRE(a_koff % GEMM_BK == 0, B200RWKV_ERR_INVALID, "internal: split-K slices start on k-block boundaries");
-        d.proto.A = ab.p + (size_t)a_mat * ab.halves_per_matrix + (size_t)(a_koff / GEMM_BK) * A16_KB_HALVES; d.proto.a_k8 = ab.kq * 4;
+        d.proto.A = ab.p + (size_t)a_mat * ab.halves_per_matrix + (size_t)(a_koff / GEMM_BK) * A16_KB_HALVES;
         d.proto.out_mode = OUT_F32; d.proto.act = act; d.proto.bias = bias; d.proto.out = out; d.proto.ldo = ldo;
         return d;
     };
@@ -1124,8 +1125,8 @@ void b200rwkv_engine::build(const StFile& st) {
                        const float* bias) {
         SegDesc d;
         d.t = &t; d.n0 = n0; d.N = Nn; d.k0 = k0; d.K = K;
-        d.proto.A = ab.p; d.proto.a_k8 = ab.kq * 4;
-        d.proto.out_mode = OUT_A16; d.proto.act = act; d.proto.bias = bias; d.proto.out = dst.p; d.proto.ldo = dst.kq;
+        d.proto.A = ab.p;
+        d.proto.out_mode = OUT_A16; d.proto.act = act; d.proto.bias = bias; d.proto.out = dst.p;
         return d;
     };
 
@@ -1140,15 +1141,12 @@ void b200rwkv_engine::build(const StFile& st) {
         // launch that mixed both kinds (R/K/V/G + decay LoRA, v7 R/K/V + adapters) goes out as two in those layers
         const int lq = (l < quant_layers) ? quant_type : QT_NONE;
 
-        // ---------------- LN1 (+ residual update from the previous layer's channel mix) ----------------
+        // ---------------- LN1 (+ residual update from the previous layer's channel mix, wired by finalize_tp) ----------------
         LnMixParams& n1 = ly.ln1;
         base_ln(n1);
         n1.x_in = (l == 0) ? x_a : x_b;
         n1.x_out = x_a;
         if (l > 0) {
-            n1.n_parts = S_ffn;
-            for (int sp = 0; sp < S_ffn; ++sp) n1.parts[sp] = part_ffn + (size_t)sp * TC;
-            if (ver != 7) { n1.n_gate = 1; n1.gate_cl = Cl; n1.gates[0] = f_rr; }
             n1.commit_dst = ffn_shift + (size_t)(l - 1) * S * C;
             n1.commit_src = xx2;
             n1.hid_slot = d_hid_tab + (l - 1);       // x_out here is the residual stream after layer l - 1
@@ -1165,7 +1163,7 @@ void b200rwkv_engine::build(const StFile& st) {
         wk.r = f_r; wk.k = f_k; wk.v = f_v; wk.g = f_g;
         wk.lnx_w = vec_f32(st, a + "ln_x.weight", c0, Cl);
         wk.lnx_b = vec_f32(st, a + "ln_x.bias", c0, Cl);
-        wk.out = a_out.p; wk.kq_tile = a_out.kq;
+        wk.out = a_out.p;
 
         const StTensor& Wr = st.get(a + "receptance.weight");
         const StTensor& Wk = st.get(a + "key.weight");
@@ -1189,23 +1187,24 @@ void b200rwkv_engine::build(const StFile& st) {
                 d.proto.grp = Dm;
                 d.proto.grp_stride = (int)a_lora[0].halves_per_matrix;
                 sv.push_back(d);
-                ly.pre.push_back(make_launch(sv));
+                ly.lora.push_back(make_launch(sv));
             }
             // W2: [5, C, Dm]; order w,k,v,r,g (SURVEY.md App. A)
+            static const char* names[5] = {"time_mix_w", "time_mix_k", "time_mix_v", "time_mix_r", "time_mix_g"};
+            const float* mu5[5];
+            for (int i = 0; i < 5; ++i) mu5[i] = vec_f32(st, a + names[i], 0, C);
             {
-                static const char* names[5] = {"time_mix_w", "time_mix_k", "time_mix_v", "time_mix_r", "time_mix_g"};
                 std::vector<SegDesc> sv;
                 for (int i = 0; i < 5; ++i) {
                     SegDesc d;
                     d.t = &st.get(a + "time_mix_w2"); d.slice = i; d.n0 = 0; d.N = C; d.k0 = 0; d.K = Dm;
                     d.proto.A = a_lora[0].p + (size_t)i * a_lora[0].halves_per_matrix;
-                    d.proto.a_k8 = a_lora[0].kq * 4;
                     d.proto.out_mode = OUT_LERP_A16; d.proto.act = ACT_NONE;
-                    d.proto.out = a_x[i].p; d.proto.ldo = a_x[i].kq;
-                    d.proto.aux0 = xx1; d.proto.aux1 = sx1; d.proto.aux2 = vec_f32(st, a + names[i], 0, C); d.proto.ld_aux = C;
+                    d.proto.out = a_x[i].p;
+                    d.proto.aux0 = xx1; d.proto.aux1 = sx1; d.proto.aux2 = mu5[i]; d.proto.ld_aux = C;
                     sv.push_back(d);
                 }
-                ly.pre.push_back(make_launch(sv));
+                ly.lora.push_back(make_launch(sv));
             }
             {   // the raw copies below are indexed with these exact shapes
                 const StTensor& w1 = st.get(a + "time_mix_w1");
@@ -1222,10 +1221,14 @@ void b200rwkv_engine::build(const StFile& st) {
                     CK(cudaMemcpy(d, t.data, t.nbytes, cudaMemcpyHostToDevice));
                     return d;
                 };
-                ly.w1_raw = upload_raw(st.get(a + "time_mix_w1"));
-                ly.w2_raw = upload_raw(st.get(a + "time_mix_w2"));
-                for (int i = 0; i < 5; ++i) ly.mu5[i] = ly.pre[1].p.seg[i].aux2;
-                fused_pre_ok = true;
+                Pre6Params& q = ly.pre6;
+                q.W1 = upload_raw(st.get(a + "time_mix_w1"));     // row-major copies of the ddlerp LoRA weights
+                q.W2 = upload_raw(st.get(a + "time_mix_w2"));
+                for (int i = 0; i < 5; ++i) { q.mu[i] = mu5[i]; q.out[i] = a_x[i].p; }
+                q.lora = a_lora[0].p; q.lora_stride = (int)a_lora[0].halves_per_matrix;
+                q.Dm = Dm;
+                q.gbar = pre_gbar;
+                ly.has_pre6 = true;
             }
             // R,K,V,G (column parallel by head) + decay LoRA stage 1 (replicated)
             {
@@ -1247,13 +1250,7 @@ void b200rwkv_engine::build(const StFile& st) {
                 }
             }
             // decay LoRA stage 2: w = exp(-exp(time_decay + Wd2 d))
-            {
-                std::vector<SegDesc> sv;
-                sv.push_back(f32_seg(st.get(a + "time_decay_w2"), c0, Cl, 0, Dd, a_lora[1], f_w, Cl, ACT_EXPNEGEXP,
-                                     vec_f32(st, a + "time_decay", c0, Cl)));
-                ly.wd2_index = (int)ly.pre.size();
-                ly.pre.push_back(make_launch(sv));
-            }
+            const float* time_decay = vec_f32(st, a + "time_decay", c0, Cl);
             if (Dd <= 128 && Dd % 8 == 0) {
                 // k-major copy of this rank's time_decay_w2 rows, one contiguous [Dd][64] slice per head: the WKV
                 // kernels evaluate the decay LoRA stage 2 themselves (one launch / phase less per layer)
@@ -1262,11 +1259,13 @@ void b200rwkv_engine::build(const StFile& st) {
                 __half* dw = (__half*)dalloc(tmp.size() * 2, false);
                 CK(cudaMemcpy(dw, tmp.data(), tmp.size() * 2, cudaMemcpyHostToDevice));
                 wk.wd2t = dw;
-                wk.decay_bias = ly.pre[ly.wd2_index].p.seg[0].bias;
+                wk.decay_bias = time_decay;
                 wk.d1 = a_lora[1].p;
-                wk.d1_kq = a_lora[1].kq;
                 wk.Dd = Dd;
-                fold_wd2 = true;
+            } else {
+                std::vector<SegDesc> sv;
+                sv.push_back(f32_seg(st.get(a + "time_decay_w2"), c0, Cl, 0, Dd, a_lora[1], f_w, Cl, ACT_EXPNEGEXP, time_decay));
+                ly.pre.push_back(make_launch(sv));
             }
             wk.w = f_w;
             wk.u = vec_f32(st, a + "time_first", c0, Cl);
@@ -1353,8 +1352,6 @@ void b200rwkv_engine::build(const StFile& st) {
         LnMixParams& n2 = ly.ln2;
         base_ln(n2);
         n2.x_in = x_a; n2.x_out = x_b;
-        n2.n_parts = S_att;
-        for (int sp = 0; sp < S_att; ++sp) n2.parts[sp] = part_att + (size_t)sp * TC;
         n2.ln_w = vec_f32(st, b + "ln2.weight", 0, C);
         n2.ln_b = vec_f32(st, b + "ln2.bias", 0, C);
         n2.shift_state = ffn_sh;
@@ -1397,12 +1394,9 @@ void b200rwkv_engine::build(const StFile& st) {
     // ---------------- ln_out + head ----------------
     memset(&lnout, 0, sizeof(lnout));
     lnout.x_in = x_b; lnout.C = C; lnout.meta = mv;
-    lnout.n_parts = S_ffn;
-    for (int sp = 0; sp < S_ffn; ++sp) lnout.parts[sp] = part_ffn + (size_t)sp * TC;
-    if (ver != 7) { lnout.n_gate = 1; lnout.gate_cl = Cl; lnout.gates[0] = f_rr; }
     lnout.ln_w = vec_f32(st, "ln_out.weight", 0, C);
     lnout.ln_b = vec_f32(st, "ln_out.bias", 0, C);
-    lnout.head_in = a_head.p; lnout.kq_tile = a_head.kq;
+    lnout.head_in = a_head.p;
     lnout.commit_dst = ffn_shift + (size_t)(L - 1) * S * C;
     lnout.commit_src = xx2;
     lnout.hidden_out = d_hidden;
@@ -1415,6 +1409,7 @@ void b200rwkv_engine::build(const StFile& st) {
 
     gemm_ws = (float*)dalloc(gemm_ws_floats * 4, false);
     for (auto& ly : layers) {
+        for (auto& g : ly.lora) g.p.ws = gemm_ws;
         for (auto& g : ly.pre) g.p.ws = gemm_ws;
         ly.o.p.ws = gemm_ws;
         for (auto& g : ly.ffn) g.p.ws = gemm_ws;
@@ -1471,10 +1466,6 @@ void b200rwkv_engine::finalize_tp() {
 void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler* prof) {
     launches_last_step = 0;
     last_th = sh.th;
-    auto pre_skipped = [&](const Layer& ly, int gi) {
-        if (fold_wd2 && gi == ly.wd2_index) return true;                 // the WKV kernel evaluates the decay LoRA stage 2
-        return fused_pre_ok && sh.MT == 1 && ly.w1_raw && gi < 2;        // the front-half kernel holds both ddlerp LoRA stages
-    };
     auto gemm = [&](const GemmLaunch& g, bool head = false) {
         GemmLaunch g2 = g;
         if (d_step_trace && trace_capture) {
@@ -1482,8 +1473,7 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler
             if ((long long)step_trace_bytes.size() <= launches_last_step) step_trace_bytes.resize(launches_last_step + 1, 0);
             step_trace_bytes[launches_last_step] = (long long)g.weight_bytes;
         }
-        for (int i = 0; i < g2.p.nseg; ++i)
-            if (g2.p.seg[i].out_mode != OUT_F32) g2.p.seg[i].ldo = sh.th;   // A16 outputs feed a projection of this step
+        if (prof) prof->weight_bytes += g.weight_bytes;
         launch_gemm(g2, sh, s, prof, head);
     };
     launch_embed(embed, sh, s, prof);
@@ -1494,24 +1484,16 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler
     };
     for (int l = 0; l < L; ++l) {
         Layer& ly = layers[l];
-        const bool fused = fused_pre_ok && sh.MT == 1 && ly.w1_raw;
-        if (fused) {
-            // LN1 + token shift + ddlerp LoRA (W1, tanh, W2, lerps) in one launch
-            Pre6Params q;
-            memset(&q, 0, sizeof(q));
+        if (ly.has_pre6 && sh.MT == 1) {
+            Pre6Params q = ly.pre6;
             q.ln = ly.ln1;
             q.ln.trace = tr_next(6);
-            q.W1 = ly.w1_raw; q.W2 = ly.w2_raw;
-            for (int j = 0; j < 5; ++j) { q.mu[j] = ly.mu5[j]; q.out[j] = a_x[j].p; }
-            q.lora = a_lora[0].p; q.lora_stride = (int)a_lora[0].halves_per_matrix; q.lora_kq = a_lora[0].kq;
-            q.Dm = info.time_mix_adapter;
-            q.gbar = pre_gbar;
             launch_pre6(q, sh, s, prof);
         } else {
             ln_stage(ly.ln1);
+            for (auto& g : ly.lora) gemm(g);
         }
-        for (int gi = 0; gi < (int)ly.pre.size(); ++gi)
-            if (!pre_skipped(ly, gi)) gemm(ly.pre[gi]);
+        for (auto& g : ly.pre) gemm(g);
         {
             WkvParams wp = ly.wkv;
             wp.trace = tr_next(2);
@@ -2605,7 +2587,7 @@ static int32_t rank_profile_step(b200rwkv_engine* e, int32_t nslot, const int32_
         ms[r.cls] += t;
         launches[r.cls] += 1;
     }
-    if (gemm_weight_bytes) *gemm_weight_bytes = (int64_t)e->weight_bytes_total;
+    if (gemm_weight_bytes) *gemm_weight_bytes = (int64_t)prof.weight_bytes;
     API_END
 }
 
@@ -3003,7 +2985,7 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
                 const __half* o5 = a16_up(x.out5 + (size_t)l * 5 * th * C, 5, C, th);
                 for (int j = 0; j < 5; ++j) { q.mu[j] = mu5 + (size_t)j * C; q.out[j] = const_cast<__half*>(o5) + j * a16_halves(C); }
                 q.lora = const_cast<__half*>(a16_up(x.lora_out + (size_t)l * 5 * th * Dm, 5, Dm, th));
-                q.lora_stride = (int)a16_halves(Dm); q.lora_kq = rup(Dm, GEMM_BK) / 32;
+                q.lora_stride = (int)a16_halves(Dm);
                 q.Dm = Dm;
                 q.gbar = gbar;
             }
@@ -3102,12 +3084,8 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
         d.proto.out_mode = s.out_mode; d.proto.act = s.act; d.proto.grp = s.out_mode == OUT_F32 ? 0 : s.grp;
         d.proto.bias = s.bias ? (const float*)st.up(s.bias, (size_t)s.N * 4) : nullptr;
         if (s.out_mode == OUT_LERP_A16) { d.proto.aux2 = (const float*)st.up(s.lerp_mu, (size_t)s.N * 4); d.proto.ld_aux = s.N; }
-        if (s.out_mode != OUT_F32) {
-            d.proto.grp_stride = (int)a16_halves(mat_cols(s));
-            d.proto.ldo = th;
-        } else {
-            d.proto.ldo = s.ldo;
-        }
+        if (s.out_mode != OUT_F32) d.proto.grp_stride = (int)a16_halves(mat_cols(s));
+        else d.proto.ldo = s.ldo;
     }
     e->d_tmp = Buf<__half>(wmax);                  // make_launch uploads each matrix through the engine's staging buffer
     GemmLaunch g = e->make_launch(sv, grid, quant_type);
@@ -3300,7 +3278,9 @@ int32_t b200rwkv_debug_read(b200rwkv_engine* e, const char* name, float* out, si
         std::vector<A> as;
         for (int i = 0; i < 6; ++i) as.push_back({"a_x" + std::to_string(i), &e->a_x[i], e->C, 0});
         for (int i = 0; i < 5; ++i)
-            for (int m = 0; m < 5; ++m) as.push_back({"a_lora" + std::to_string(i) + "_" + std::to_string(m), &e->a_lora[i], e->a_lora[i].kq * 32, m});
+            for (int m = 0; m < 5; ++m)
+                as.push_back({"a_lora" + std::to_string(i) + "_" + std::to_string(m), &e->a_lora[i],
+                              (int)(e->a_lora[i].halves_per_matrix / A16_KB_HALVES) * GEMM_BK, m});
         as.push_back({"a_out", &e->a_out, e->Cl, 0});
         as.push_back({"a_kk", &e->a_kk, e->Fl, 0});
         as.push_back({"a_head", &e->a_head, e->C, 0});
@@ -3338,8 +3318,9 @@ int32_t b200rwkv_debug_trace(b200rwkv_engine* e, uint64_t* out, size_t cap, int3
 }
 
 // Profiling aid: time one projection launch class in isolation, round-robin over the layers so
-// every launch streams cold weights.  which: 0.. = index into the pre-WKV launches, 10 = output
-// projection, 20/21 = channel-mix launches, 30 = head.  Returns ms per launch and weight bytes.
+// every launch streams cold weights.  which: 0.. = the launches between LN1 and WKV of a step of
+// more than 16 tokens (the ddlerp LoRA launches first), 10 = output projection, 20.. = channel-mix
+// launches, 30 = head; any other index is refused.  Returns ms per launch and weight bytes.
 int32_t b200rwkv_debug_gemm_time(b200rwkv_engine* e, int32_t which, int32_t reps, float* ms_out, int64_t* bytes_out,
                                  uint64_t* trace_out /* [L][8] stamps of CTA 0 for the last round, or null */) {
     API_BEGIN(e)
@@ -3347,12 +3328,13 @@ int32_t b200rwkv_debug_gemm_time(b200rwkv_engine* e, int32_t which, int32_t reps
     std::lock_guard<std::mutex> lk(e->mu);
     CK(cudaSetDevice(e->dev));
     auto pick = [&](int l) -> const GemmLaunch& {
-        Layer& ly = e->layers[l % e->L];
+        const Layer& ly = e->layers[l % e->L];
+        const int nl = (int)ly.lora.size(), np = (int)ly.pre.size(), nf = (int)ly.ffn.size();
         if (which == 30) return e->head;
-        if (which >= 20) { REQUIRE(which - 20 < (int)ly.ffn.size(), B200RWKV_ERR_INVALID, "no such launch"); return ly.ffn[which - 20]; }
         if (which == 10) return ly.o;
-        REQUIRE(which < (int)ly.pre.size(), B200RWKV_ERR_INVALID, "no such launch");
-        return ly.pre[which];
+        if (which >= 20 && which < 20 + nf) return ly.ffn[which - 20];
+        REQUIRE(which >= 0 && which < nl + np, B200RWKV_ERR_INVALID, "no such launch");
+        return which < nl ? ly.lora[which] : ly.pre[which - nl];
     };
     // a valid 16-token meta so row masks are full
     std::vector<int> m(e->meta_ints, 0);

@@ -69,7 +69,7 @@ struct GemmSeg {
     int act;
     const float* bias;    // optional [N], added before the activation
     void* out;
-    int ldo;              // OUT_F32: row stride (floats); A16 modes: k32 blocks per m-tile of the destination
+    int ldo;              // OUT_F32: row stride (floats); A16 modes: token rows of the destination (the step's th)
     int grp;              // OUT_A16: columns per destination matrix (0 = single matrix)
     int grp_stride;       // OUT_A16: halves between destination matrices
     const float* aux0;    // OUT_LERP_A16: xx [T, ld_aux]

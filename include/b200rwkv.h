@@ -274,7 +274,7 @@ int32_t b200rwkv_bench_decode(b200rwkv_engine*, int32_t nslot, const int32_t* sl
 
 /* Per-kernel-class device time of ONE un-graphed decode step, CUDA events around every launch
  * on the engine's stream.  classes: 0 = projection GEMMs, 1 = WKV, 2 = LN/mix/embed, 3 = other.
- * ms[4], launches[4], and algorithmic weight bytes streamed by the GEMM launches. */
+ * ms[4], launches[4], and the algorithmic weight bytes streamed by the step's GEMM launches. */
 int32_t b200rwkv_profile_step(b200rwkv_engine*, int32_t nslot, const int32_t* slot,
                               const uint32_t* tokens, float ms[4], int32_t launches[4],
                               int64_t* gemm_weight_bytes);
@@ -438,7 +438,9 @@ int32_t b200rwkv_debug_read(b200rwkv_engine*, const char* name, float* out, size
  * front-half kernel); types[i] = 0 LN, 2 WKV, 6 front half, 1000000 + weight MiB for a projection launch. */
 int32_t b200rwkv_debug_trace(b200rwkv_engine*, uint64_t* out, size_t cap, int32_t* types, int32_t* nphase);
 
-/* Profiling aid: one projection launch class timed in isolation over all layers. */
+/* Profiling aid: one projection launch class timed in isolation over all layers, as a 16-token step runs it.  which: 0.. =
+ * the launches between LN1 and WKV of a step of more than 16 tokens (the RWKV-6 ddlerp LoRA launches first), 10 = output
+ * projection, 20.. = channel-mix launches, 30 = head; an index with no such launch is B200RWKV_ERR_INVALID. */
 int32_t b200rwkv_debug_gemm_time(b200rwkv_engine*, int32_t which, int32_t reps, float* ms_out, int64_t* bytes_out,
                                  uint64_t* trace_out);
 

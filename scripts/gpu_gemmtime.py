@@ -4,7 +4,7 @@ import numpy as np
 from ai00_server_b200 import capi, runtime, synth
 st = synth.make_st("v6-7b", 0)
 m = runtime.Model(st, max_batch=16, token_chunk_size=64)
-for which, name in [(0, "W1"), (1, "W2"), (2, "RKVG+d1"), (3, "Wd2"), (10, "O"), (20, "ffnKR"), (21, "ffnV"), (30, "head")]:
+for which, name in [(0, "W1"), (1, "W2"), (2, "RKVG+d1"), (10, "O"), (20, "ffnKR"), (21, "ffnV"), (30, "head")]:
     ms = C.c_float(0); nb = C.c_int64(0)
     tr = np.zeros((32, 16), np.uint64)
     capi.check(capi.lib().b200rwkv_debug_gemm_time(m._h, which, 3, C.byref(ms), C.byref(nb), capi.ptr(tr)), m._h)
