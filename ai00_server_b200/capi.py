@@ -18,6 +18,7 @@ OK = 0
 ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA, ERR_STATE = -1, -2, -3, -4
 OPTION_LAST, OPTION_FULL, OPTION_NONE = 0, 1, 2
 OPTION_SCORE = 3                # b200rwkv_infer_ex only: per-token log-probabilities and argmax ids, no logits rows
+POOL_LAST, POOL_MEAN = 0, 1      # b200rwkv_keep_hidden_pooled: the entry's last row / the f32 mean of its rows
 TP_HANDLE_BYTES = 128
 
 
@@ -161,6 +162,8 @@ SYMBOLS = [
     ("b200rwkv_last_hidden", C.c_int32, [_P, _P, C.c_size_t]),
     ("b200rwkv_keep_hidden_layers", C.c_int32, [_P, C.c_int32, _P]),
     ("b200rwkv_last_hidden_layer", C.c_int32, [_P, C.c_int32, _P, C.c_size_t]),
+    ("b200rwkv_keep_hidden_pooled", C.c_int32, [_P, C.c_int32, _P, C.c_int32]),
+    ("b200rwkv_last_hidden_pooled", C.c_int32, [_P, C.c_int32, _P, C.c_size_t, _P]),
     ("b200rwkv_debug_read", C.c_int32, [_P, C.c_char_p, _P, C.c_size_t]),
     ("b200rwkv_debug_trace", C.c_int32, [_P, _P, C.c_size_t, _P, _P]),
     ("b200rwkv_debug_gemm_time", C.c_int32, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_int64), _P]),

@@ -571,6 +571,19 @@ struct b200rwkv_engine {
     std::vector<int> hid_last;         // layers recorded by the most recent infer call (the layout of hid_all)
     size_t hid_last_rows = 0;
     const float* hid_step_src(int k) const { return hid_layers[k] == L - 1 ? d_hidden : hid_step + (size_t)k * maxT * C; }
+    // b200rwkv_keep_hidden_pooled: one row per entry and pooled layer, reduced by hidden_pool_kernel after every step.  A
+    // pooled layer's rows are recorded like a kept layer's: into the kept layer's step buffer where keep_hidden_layers asked
+    // for it too, else into pool_step (so a layer only pooling asked for is never gathered token by token).
+    std::vector<int> pool_layers;      // pooled layers, in the order the caller gave them
+    int pool_mode = B200RWKV_POOL_LAST;
+    float* pool_step = nullptr;        // [POOL_MAX_LAYERS][maxT][C], step buffer k belongs to pool_layers[k]
+    float* pool_rows = nullptr;        // [POOL_MAX_LAYERS][S][C]: row (k, i) belongs to pool_layers[k] and entry i of the call
+    const float* pool_src[POOL_MAX_LAYERS] = {nullptr};     // where a step's rows of pool_layers[k] are (set by upload_hid_tab)
+    Buf<PoolEntry> pool_dev;           // the call's (entry, step) list, one slice per launch; grown on demand
+    HostBuf<PoolEntry> pool_host;
+    std::vector<int> pool_last;        // layers pooled by the most recent infer call
+    std::vector<int32_t> pool_last_ntok;       // its entries' token counts
+    void upload_hid_tab();
     int* d_meta = nullptr;
     HostBuf<int> h_meta;
     size_t meta_ints = 0;
@@ -1597,6 +1610,23 @@ void b200rwkv_engine::run_step(const StepShape& sh) {
     launch_total += it->second.launches;         // kernels of THIS graph, not of whichever was captured last
 }
 
+// The device table of step buffers the LN stages record into: cell l is set for the layers keep_hidden_layers or
+// keep_hidden_pooled asked for (layer L - 1 comes from ln_out_kernel's d_hidden and has no cell).  A layer both asked for
+// is recorded once, into the kept layer's buffer.
+void b200rwkv_engine::upload_hid_tab() {
+    std::vector<float*> tab(L, nullptr);
+    for (size_t k = 0; k < hid_layers.size(); ++k)
+        if (hid_layers[k] < L - 1) tab[hid_layers[k]] = hid_step + k * maxT * C;
+    for (size_t k = 0; k < pool_layers.size(); ++k) {
+        const int l = pool_layers[k];
+        if (l < L - 1 && !tab[l]) tab[l] = pool_step + k * maxT * C;
+        pool_src[k] = l == L - 1 ? d_hidden : tab[l];
+    }
+    // on the engine's stream and complete before returning: the step kernels read the table before griddepcontrol.wait
+    CK(cudaMemcpyAsync(d_hid_tab, tab.data(), tab.size() * sizeof(float*), cudaMemcpyHostToDevice, stream));
+    CK(cudaStreamSynchronize(stream));
+}
+
 // fills one step's metadata; returns T
 int b200rwkv_engine::fill_meta(int* m, const std::vector<int>& slots, const std::vector<int>& counts,
                                const std::vector<const uint32_t*>& toks, const std::vector<int>& outmode, int* R_out) {
@@ -1711,6 +1741,16 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
     hid_last.clear();
     hid_last_rows = 0;
     hid_all.grow(n_hid * total_tok * C * 4, n_hid * std::max<size_t>(total_tok, 256) * C * 4);
+    // pooled rows: every step lists its entries in its own slice of the pinned list (never rewritten within the call); an
+    // entry takes at least one token of every step it is in, so the call's tokens bound the list
+    const size_t n_pool = pool_layers.size();
+    pool_last.clear();
+    size_t pool_used = 0;
+    if (n_pool) {
+        const size_t bytes = std::max<size_t>(total_tok, 256) * sizeof(PoolEntry);
+        pool_dev.grow(total_tok * sizeof(PoolEntry), bytes);
+        pool_host.grow(total_tok * sizeof(PoolEntry), bytes);
+    }
     int step_no = 0;
     for (;;) {
         int n_active = 0;
@@ -1769,6 +1809,26 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         };
         if (hidden_keep) gather_rows(d_hidden_all, d_hidden);       // b200rwkv_last_hidden
         for (size_t k = 0; k < n_hid; ++k) gather_rows(hid_all + k * total_tok * C, hid_step_src((int)k));     // b200rwkv_last_hidden_layer
+        if (n_pool) {        // b200rwkv_last_hidden_pooled: this step's rows into every entry's pooled row
+            PoolEntry* pe = pool_host + pool_used;
+            int t0 = 0;
+            for (size_t j = 0; j < s_entry.size(); ++j) {
+                const int i = s_entry[j];
+                pe[j] = {t0, s_counts[j], i, pos[i], ntok[i]};
+                t0 += s_counts[j];
+            }
+            CK(cudaMemcpyAsync(pool_dev + pool_used, pe, s_entry.size() * sizeof(PoolEntry), cudaMemcpyHostToDevice, stream));
+            PoolParams pp;
+            pp.ent = pool_dev + pool_used;
+            std::copy(pool_src, pool_src + POOL_MAX_LAYERS, pp.src);
+            pp.dst = pool_rows;
+            pp.C = C; pp.dst_rows = S; pp.mode = pool_mode;
+            hidden_pool_kernel<<<dim3((unsigned)s_entry.size(), (unsigned)n_pool, (unsigned)cdiv(C / 4, POOL_THREADS)), POOL_THREADS, 0,
+                                 stream>>>(pp);
+            CK(cudaGetLastError());
+            ++launch_total;
+            pool_used += s_entry.size();
+        }
         if (sc_rows) {       // this step's SCORE rows, scored against each entry's next token
             const size_t first = sc_used;
             int r = 0;
@@ -1840,6 +1900,8 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
     if (hidden_keep) hidden_rows = (int)total_tok;
     hid_last = hid_layers;
     hid_last_rows = total_tok;
+    pool_last = pool_layers;
+    pool_last_ntok.assign(ntok, ntok + nslot);
 }
 
 // GPU sampling front half (sample.cuh).  Runs on the softmax stream under the softmax mutex: the reference samples from the
@@ -3209,14 +3271,60 @@ int32_t b200rwkv_keep_hidden_layers(b200rwkv_engine* e, int32_t n, const int32_t
                 "keep_hidden_layers: layer " + std::to_string(layers[i]) + " is outside [0, " + std::to_string(e->L) + ")");
     CK(cudaSetDevice(e->dev));
     if (n > 0 && !e->hid_step) e->hid_step = (float*)e->dalloc((size_t)b200rwkv_engine::HID_MAX_LAYERS * e->maxT * e->C * 4);
-    std::vector<float*> tab(e->L, nullptr);
-    for (int k = 0; k < n; ++k)
-        if (layers[k] < e->L - 1) tab[layers[k]] = e->hid_step + (size_t)k * e->maxT * e->C;
-    // on the engine's stream and complete before returning: the step kernels read the table before griddepcontrol.wait
-    CK(cudaMemcpyAsync(e->d_hid_tab, tab.data(), tab.size() * sizeof(float*), cudaMemcpyHostToDevice, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
     e->hid_layers.assign(layers, layers + n);
+    e->upload_hid_tab();
     API_END
+}
+
+int32_t b200rwkv_keep_hidden_pooled(b200rwkv_engine* e, int32_t n, const int32_t* layers, int32_t mode) {
+    API_BEGIN(e)
+    REQUIRE(n >= 0 && n <= POOL_MAX_LAYERS, B200RWKV_ERR_INVALID,
+            "keep_hidden_pooled: n must be in [0, " + std::to_string(POOL_MAX_LAYERS) + "]");
+    REQUIRE(n == 0 || layers, B200RWKV_ERR_INVALID, "keep_hidden_pooled: null layers");
+    REQUIRE(mode == B200RWKV_POOL_LAST || mode == B200RWKV_POOL_MEAN, B200RWKV_ERR_INVALID,
+            "keep_hidden_pooled: unknown mode " + std::to_string(mode));
+    for (int i = 0; i < n; ++i) {
+        REQUIRE(layers[i] >= 0, B200RWKV_ERR_INVALID, "keep_hidden_pooled: negative layer " + std::to_string(layers[i]));
+        REQUIRE(std::find(layers, layers + i, layers[i]) == layers + i, B200RWKV_ERR_INVALID,
+                "keep_hidden_pooled: layer " + std::to_string(layers[i]) + " is listed twice");
+    }
+    REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (int i = 0; i < n; ++i)
+        REQUIRE(layers[i] < e->L, B200RWKV_ERR_INVALID,
+                "keep_hidden_pooled: layer " + std::to_string(layers[i]) + " is outside [0, " + std::to_string(e->L) + ")");
+    CK(cudaSetDevice(e->dev));
+    if (n > 0 && !e->pool_step) e->pool_step = (float*)e->dalloc((size_t)POOL_MAX_LAYERS * e->maxT * e->C * 4);
+    if (n > 0 && !e->pool_rows) e->pool_rows = (float*)e->dalloc((size_t)POOL_MAX_LAYERS * e->S * e->C * 4);
+    e->pool_layers.assign(layers, layers + n);
+    e->pool_mode = mode;
+    e->upload_hid_tab();
+    API_END
+}
+
+// returns the number of rows written, one per entry of the call (negative status on error)
+int32_t b200rwkv_last_hidden_pooled(b200rwkv_engine* e, int32_t layer, float* out, size_t cap, int32_t* ntok_out) {
+    return api_count([&]() -> int32_t {
+        REQUIRE(layer >= 0, B200RWKV_ERR_INVALID, "last_hidden_pooled: negative layer " + std::to_string(layer));
+        REQUIRE(e && out, B200RWKV_ERR_INVALID, "null argument");
+        std::lock_guard<std::mutex> lk(e->mu);
+        REQUIRE(layer < e->L, B200RWKV_ERR_INVALID,
+                "last_hidden_pooled: layer " + std::to_string(layer) + " is outside [0, " + std::to_string(e->L) + ")");
+        const auto it = std::find(e->pool_last.begin(), e->pool_last.end(), layer);
+        REQUIRE(it != e->pool_last.end(), B200RWKV_ERR_STATE,
+                "last_hidden_pooled: layer " + std::to_string(layer) + " was not pooled by the most recent infer call");
+        const size_t rows = e->pool_last_ntok.size(), C = (size_t)e->C;
+        REQUIRE(rows * C <= cap, B200RWKV_ERR_INVALID, "last_hidden_pooled: buffer too small");
+        CK(cudaSetDevice(e->dev));
+        CK(cudaStreamSynchronize(e->stream));
+        if (rows)
+            CK(cudaMemcpy(out, e->pool_rows + (size_t)(it - e->pool_last.begin()) * e->S * C, rows * C * 4, cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < rows; ++i) {
+            if (e->pool_last_ntok[i] == 0) std::fill_n(out + i * C, C, 0.f);      // no step held the entry: its row was not written
+            if (ntok_out) ntok_out[i] = e->pool_last_ntok[i];
+        }
+        return (int32_t)rows;
+    });
 }
 
 // returns the number of rows written (negative status on error)

@@ -157,4 +157,52 @@ __global__ void decay_table_kernel(const __half* __restrict__ src, float* __rest
         dst[i] = expf(-expf(__half2float(src[i])));
 }
 
+// ---------------------------------------------------------------------------------------
+// Pooled hidden rows (b200rwkv_keep_hidden_pooled): one [C] f32 row per entry of an infer call and pooled layer, reduced from
+// the [T][C] step buffers the LN stages record the residual stream into, so the embeddings route moves num_emb floats per
+// input to the host instead of every token's row.  One launch after every step of the call: CTA (entry of the step, pooled
+// layer, block of POOL_THREADS float4 columns), one float4 column per thread.
+//   POOL_LAST: dst <- the entry's last row of the step (a later step of the same entry overwrites it).
+//   POOL_MEAN: acc = +0.0 on the entry's first step, else dst; acc = __fadd_rn(acc, row) for the step's rows in token order;
+//              the step that holds the entry's final token of the call stores __fdiv_rn(acc, ntok), the others store acc.
+// A channel's sum is one chain of adds in token order whatever the cut into steps, so the bits do not depend on the cut.
+// The steps of a call run in order on one stream: the running sum needs no atomics.
+// ---------------------------------------------------------------------------------------
+struct PoolEntry {
+    int row0, nrows;            // the entry's rows of this step: [row0, row0 + nrows) of the step buffers
+    int dst;                    // destination row (the entry's index in the call)
+    int pos, ntok;              // tokens of the entry before this step, and in the whole call
+};
+constexpr int POOL_MAX_LAYERS = 8;
+constexpr int POOL_THREADS = 256;
+struct PoolParams {
+    const PoolEntry* ent;       // [gridDim.x]
+    const float* src[POOL_MAX_LAYERS];      // step buffer [T][C] of pooled layer k
+    float* dst;                 // [layers][dst_rows][C]
+    int C, dst_rows, mode;      // mode: B200RWKV_POOL_LAST (0) / B200RWKV_POOL_MEAN (1)
+};
+
+__global__ void __launch_bounds__(POOL_THREADS) hidden_pool_kernel(const __grid_constant__ PoolParams p) {
+    const int ld = p.C / 4, c4 = blockIdx.z * POOL_THREADS + threadIdx.x;
+    if (c4 >= ld) return;
+    const PoolEntry en = p.ent[blockIdx.x];
+    const float4* src = reinterpret_cast<const float4*>(p.src[blockIdx.y]) + (size_t)en.row0 * ld + c4;
+    float4* dst = reinterpret_cast<float4*>(p.dst) + ((size_t)blockIdx.y * p.dst_rows + en.dst) * ld + c4;
+    if (p.mode == 0) {
+        *dst = src[(size_t)(en.nrows - 1) * ld];
+        return;
+    }
+    float4 a = en.pos == 0 ? make_float4(0.f, 0.f, 0.f, 0.f) : *dst;
+#pragma unroll 8
+    for (int t = 0; t < en.nrows; ++t) {
+        const float4 v = src[(size_t)t * ld];
+        a.x = __fadd_rn(a.x, v.x); a.y = __fadd_rn(a.y, v.y); a.z = __fadd_rn(a.z, v.z); a.w = __fadd_rn(a.w, v.w);
+    }
+    if (en.pos + en.nrows == en.ntok) {
+        const float n = (float)en.ntok;
+        a.x = __fdiv_rn(a.x, n); a.y = __fdiv_rn(a.y, n); a.z = __fdiv_rn(a.z, n); a.w = __fdiv_rn(a.w, n);
+    }
+    *dst = a;
+}
+
 }  // namespace b200

@@ -463,6 +463,41 @@ class Model:
         finally:
             self.keep_hidden(layers=[])
 
+    _POOL_MODES = {"last": capi.POOL_LAST, "mean": capi.POOL_MEAN}
+
+    def keep_hidden_pooled(self, layers, mode="last") -> None:
+        """Reduce the residual stream after each listed layer to one row per entry of every following infer call
+        (b200rwkv_keep_hidden_pooled): mode "last" keeps the row of the entry's last token, "mean" the f32 mean of its rows
+        in token order (capi.POOL_LAST / POOL_MEAN are accepted too).  At most 8 distinct layers; layers=[] turns it off.
+        Independent of keep_hidden."""
+        a = np.asarray(layers, np.int32).reshape(-1)
+        capi.check(capi.lib().b200rwkv_keep_hidden_pooled(self._h, a.size, capi.ptr(a) if a.size else None,
+                                                          self._POOL_MODES.get(mode, mode)), self._h)
+
+    def last_hidden_pooled(self, layer: int, max_rows: int | None = None):
+        """The pooled rows of the most recent infer call after `layer`, which that call must have pooled: (rows [n, num_emb]
+        f32 in entry order, token counts [n] int32).  max_rows: an upper bound on the call's entries (default max_batch)."""
+        rows = self.max_batch if max_rows is None else max_rows
+        buf = np.empty((max(rows, 1), self.info["num_emb"]), np.float32)
+        ntok = np.zeros(max(rows, 1), np.int32)
+        r = capi.lib().b200rwkv_last_hidden_pooled(self._h, int(layer), capi.ptr(buf), rows * buf.shape[1], capi.ptr(ntok))
+        capi.check(r, self._h)
+        return buf[:r], ntok[:r]
+
+    def embed_many(self, slots, token_lists, layer: int, mode="last") -> np.ndarray:
+        """The embeddings route for several inputs at once: feed token_lists[i] to slots[i] in one infer call with no logits
+        and return the pooled residual stream after `layer`, [n, num_emb] f32.  Only num_emb floats per input leave the
+        device.  Advances the slots' states; turns pooling off afterwards."""
+        token_lists = [[int(t) for t in toks] for toks in token_lists]
+        if len(token_lists) != len(slots) or not all(token_lists):
+            raise capi.B200Error(capi.ERR_INVALID, "embed_many: one non-empty token list per slot")
+        self.keep_hidden_pooled([layer], mode)
+        try:
+            self.infer_raw(list(slots), [len(t) for t in token_lists], sum(token_lists, []), [capi.OPTION_NONE] * len(slots))
+            return self.last_hidden_pooled(layer, max_rows=len(slots))[0].copy()
+        finally:
+            self.keep_hidden_pooled([])
+
     def debug_read(self, name: str, rows: int = 64) -> np.ndarray:
         buf = np.empty(rows * 65536, np.float32)
         cols = capi.lib().b200rwkv_debug_read(self._h, name.encode(), capi.ptr(buf), buf.size)

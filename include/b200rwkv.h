@@ -428,6 +428,31 @@ int32_t b200rwkv_last_hidden(b200rwkv_engine*, float* out, size_t cap);
 int32_t b200rwkv_keep_hidden_layers(b200rwkv_engine*, int32_t n, const int32_t* layers);
 int32_t b200rwkv_last_hidden_layer(b200rwkv_engine*, int32_t layer, float* out, size_t cap);
 
+/* One pooled hidden row per entry, reduced on the device: what the embeddings route returns (one [num_emb] vector per input)
+ * without storing or copying the rows of every token.  "Layer l" is what it is for b200rwkv_keep_hidden_layers.
+ * b200rwkv_keep_hidden_pooled(e, n, layers, mode) makes every following infer / infer_ex call reduce, for each of the n
+ * listed layers, the rows of each entry to one f32 [num_emb] row; n = 0 turns it off.  At most 8 distinct layers; a layer
+ * outside [0, num_layer), a duplicate, n > 8 or an unknown mode is B200RWKV_ERR_INVALID, checked before the first CUDA call.
+ *   B200RWKV_POOL_LAST: the row of the entry's last token in the call, bit-identical to that row of
+ *     b200rwkv_last_hidden_layer.
+ *   B200RWKV_POOL_MEAN: per channel, the f32 sum of the entry's rows in token order, starting from +0.0 with one
+ *     round-to-nearest f32 addition per token, then one round-to-nearest f32 division by the entry's token count.  The
+ *     order is fixed: the mean is this function of the rows b200rwkv_last_hidden_layer returns for the same call, bit for
+ *     bit, however the call is cut into internal steps (token_chunk_size, other entries sharing the steps).
+ * Entries of every option (LAST, FULL, NONE, SCORE) pool alike, and pooling changes no logits, state, kept row or score.  It
+ * adds one kernel launch per internal step and no per-token copy.  Independent of b200rwkv_keep_hidden and
+ * b200rwkv_keep_hidden_layers: any combination may be on at once and none changes what the others return.
+ * b200rwkv_last_hidden_pooled copies layer `layer`'s rows of the most recent infer call, [nslot][num_emb] f32 in entry order,
+ * and returns nslot; ntok_out (may be NULL, else nslot ints) receives every entry's token count, so a caller whose input was
+ * cut over several infer calls can combine the means itself.  An entry without tokens gives a row of zeros and count 0.
+ * B200RWKV_ERR_STATE if that call did not pool the layer, B200RWKV_ERR_INVALID if `cap` (floats) is too small.
+ * Tensor parallelism: the residual stream is replicated over the ranks; in process rank 0 pools it, and with one process
+ * per GPU every rank's engine can (each reduces its own copy). */
+#define B200RWKV_POOL_LAST 0
+#define B200RWKV_POOL_MEAN 1
+int32_t b200rwkv_keep_hidden_pooled(b200rwkv_engine*, int32_t n, const int32_t* layers, int32_t mode);
+int32_t b200rwkv_last_hidden_pooled(b200rwkv_engine*, int32_t layer, float* out, size_t cap, int32_t* ntok_out);
+
 /* Test aid: copy a named internal activation buffer of the most recent step to the host as f32
  * row-major; returns the column count (negative status on error).  Not on the product path. */
 int32_t b200rwkv_debug_read(b200rwkv_engine*, const char* name, float* out, size_t cap);
