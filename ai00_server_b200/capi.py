@@ -107,6 +107,63 @@ ACT_NONE, ACT_TANH, ACT_SIGMOID, ACT_SILU, ACT_RELU2, ACT_EXPNEGEXP, ACT_V7DECAY
 OUT_F32, OUT_A16, OUT_LERP_A16 = 0, 1, 2
 
 
+class KeepArgs(C.Structure):
+    """b200rwkv_keep_args (include/b200rwkv.h)."""
+    _fields_ = [("S", C.c_int32), ("nslot", C.c_int32), ("slot", C.c_void_p), ("count", C.c_void_p), ("option", C.c_void_p),
+                ("world", C.c_int32), ("Vl", C.c_int32), ("shards", C.c_void_p), ("keep", C.c_void_p)]
+
+
+def op_keep(slots, counts, options, shards, keep, device: int = 0):
+    """The kept-row gather of a step (b200rwkv_op_keep): shards [world, R, Vl] f32, keep [S, world * Vl] f32 updated in place."""
+    sl, cn, op = (np.ascontiguousarray(a, np.int32) for a in (slots, counts, options))
+    assert shards.dtype == np.float32 and shards.flags.c_contiguous and shards.ndim == 3
+    assert keep.dtype == np.float32 and keep.flags.c_contiguous and keep.shape[1] == shards.shape[0] * shards.shape[2]
+    a = KeepArgs(keep.shape[0], len(sl), ptr(sl), ptr(cn), ptr(op), shards.shape[0], shards.shape[2], ptr(shards), ptr(keep))
+    check(lib().b200rwkv_op_keep(device, C.byref(a)))
+
+
+WEIGHT_LORA, WEIGHT_F32, WEIGHT_DECAY, WEIGHT_REPACK = range(4)      # b200rwkv_op_weight kinds
+
+
+class WeightArgs(C.Structure):
+    """b200rwkv_weight_args (include/b200rwkv.h)."""
+    _fields_ = [("src", C.c_void_p), ("n", C.c_int64), ("scale", C.c_float), ("bias", C.c_float), ("dst", C.c_void_p),
+                ("w", C.c_void_p), ("lora_b", C.c_void_p), ("lora_a", C.c_void_p), ("out", C.c_int32), ("in_", C.c_int32),
+                ("r", C.c_int32), ("alpha", C.c_float)] + [
+                (n, C.c_int32) for n in ("rows", "ld", "n0", "k0", "N", "K")] + [("blocks", C.c_void_p)]
+
+
+def op_lora_blend(w16, lora_b, lora_a, alpha: float, device: int = 0):
+    """One LoRA pair blended into w16 [out, in] f16 (b200rwkv_op_weight, WEIGHT_LORA): lora_b [out, r], lora_a [in, r] f16.
+    Returns the blended f16 matrix."""
+    w = np.array(w16, np.float16, copy=True, order="C")
+    b, a = np.ascontiguousarray(lora_b, np.float16), np.ascontiguousarray(lora_a, np.float16)
+    assert b.shape == (w.shape[0], a.shape[1]) and a.shape[0] == w.shape[1]
+    args = WeightArgs(w=ptr(w), lora_b=ptr(b), lora_a=ptr(a), out=w.shape[0], in_=w.shape[1], r=a.shape[1], alpha=alpha)
+    check(lib().b200rwkv_op_weight(device, WEIGHT_LORA, C.byref(args)))
+    return w
+
+
+def op_vector(kind: int, src16, scale: float = 1.0, bias: float = 0.0, device: int = 0):
+    """f32(src) * scale + bias (WEIGHT_F32) or expf(-expf(f32(src))) (WEIGHT_DECAY) of a flat f16 array, as f32."""
+    s = np.ascontiguousarray(src16, np.float16).reshape(-1)
+    out = np.empty(s.size, np.float32)
+    args = WeightArgs(src=ptr(s), n=s.size, scale=scale, bias=bias, dst=ptr(out))
+    check(lib().b200rwkv_op_weight(device, kind, C.byref(args)))
+    return out
+
+
+def op_repack(src16, n0: int, k0: int, N: int, K: int, device: int = 0):
+    """Rows [n0, n0 + N) x columns [k0, k0 + K) of src16 [rows, ld] f16 as the projection kernels' weight blocks (WEIGHT_REPACK):
+    [ceil(N / 128), ceil(K / 128), 16, 16, 8, 8] f16."""
+    s = np.ascontiguousarray(src16, np.float16)
+    tiles, kb = -(-N // 128), -(-K // 128)
+    out = np.empty((tiles, kb, 16, 16, 8, 8), np.float16)
+    args = WeightArgs(src=ptr(s), rows=s.shape[0], ld=s.shape[1], n0=n0, k0=k0, N=N, K=K, blocks=ptr(out))
+    check(lib().b200rwkv_op_weight(device, WEIGHT_REPACK, C.byref(args)))
+    return out
+
+
 class InferArgs(C.Structure):
     """b200rwkv_infer_args (include/b200rwkv.h)."""
     _fields_ = [("struct_bytes", C.c_uint32), ("nslot", C.c_int32), ("slot", C.c_void_p), ("ntok", C.c_void_p),
@@ -157,6 +214,8 @@ SYMBOLS = [
     ("b200rwkv_op_wkv", C.c_int32, [C.c_int32, C.POINTER(WkvArgs)]),
     ("b200rwkv_op_ln", C.c_int32, [C.c_int32, C.POINTER(LnArgs)]),
     ("b200rwkv_op_gemm", C.c_int32, [C.c_int32] * 7 + [C.POINTER(GemmSeg), C.POINTER(C.c_int32 * 4)]),
+    ("b200rwkv_op_keep", C.c_int32, [C.c_int32, C.POINTER(KeepArgs)]),
+    ("b200rwkv_op_weight", C.c_int32, [C.c_int32, C.c_int32, C.POINTER(WeightArgs)]),
     ("b200rwkv_launch_count", C.c_int32, [_P, C.POINTER(C.c_int64)]),
     ("b200rwkv_keep_hidden", C.c_int32, [_P, C.c_int32]),
     ("b200rwkv_last_hidden", C.c_int32, [_P, _P, C.c_size_t]),

@@ -739,6 +739,28 @@ void b200rwkv_engine::check_loras(const StFile& model) const {
     }
 }
 
+// The load-time weight kernels with the launch shapes the build gives them; b200rwkv_op_weight runs these same launches.
+static void launch_lora_blend(int num_sms, __half* W, const __half* B, const __half* At, int out, int in, int r, float alpha) {
+    lora_blend_kernel<<<num_sms * 8, 256>>>(W, B, At, out, in, r, alpha);
+    CK(cudaGetLastError());
+}
+static void launch_f16_to_f32(const __half* src, float* dst, size_t count, float scale, float bias) {
+    f16_to_f32_kernel<<<cdiv((int)count, 256), 256>>>(src, dst, count, scale, bias);
+    CK(cudaGetLastError());
+}
+static void launch_decay_table(const __half* src, float* dst, int n) {
+    decay_table_kernel<<<cdiv(n, 256), 256>>>(src, dst, n);
+    CK(cudaGetLastError());
+}
+// rows [n0, n0 + N) and columns [k0, k0 + K) of src [.][ld] into ceil(N / 128) x ceil(K / 128) stage blocks at dst
+static void launch_repack(int num_sms, const __half* src, int ld, int n0, int k0, int N, int K, uint4* dst) {
+    const int tiles = cdiv(N, GEMM_BN), KB = cdiv(K, GEMM_BK);
+    const size_t nchunk = (size_t)tiles * KB * (GEMM_WBYTES / 16);
+    const int grid = (int)std::min<size_t>((nchunk + 255) / 256, (size_t)num_sms * 16);
+    repack_weight_kernel<<<grid, 256>>>(src, ld, n0, k0, N, K, tiles, KB, dst);
+    CK(cudaGetLastError());
+}
+
 void b200rwkv_engine::blend_loras(const StTensor& t) {
     if (loras.empty() || !ends_with(t.name, ".weight") || t.shape.size() != 2) return;
     const std::string base = t.name.substr(0, t.name.size() - 7);
@@ -755,8 +777,7 @@ void b200rwkv_engine::blend_loras(const StTensor& t) {
         Buf<__half> da(a->nbytes), db(b->nbytes);
         CK(cudaMemcpy(da, a->data, a->nbytes, cudaMemcpyHostToDevice));
         CK(cudaMemcpy(db, b->data, b->nbytes, cudaMemcpyHostToDevice));
-        lora_blend_kernel<<<num_sms * 8, 256>>>(d_tmp, db, da, out, in, r, lo.alpha);
-        CK(cudaGetLastError());
+        launch_lora_blend(num_sms, d_tmp, db, da, out, in, r, lo.alpha);
         CK(cudaDeviceSynchronize());
     }
 }
@@ -767,8 +788,7 @@ float* b200rwkv_engine::vec_f32(const StFile& st, const std::string& name, size_
     float* d = (float*)dalloc(count * 4, false);
     Buf<__half> tmp(count * 2);
     CK(cudaMemcpy(tmp, t.data + off * 2, count * 2, cudaMemcpyHostToDevice));
-    f16_to_f32_kernel<<<cdiv((int)count, 256), 256>>>(tmp, d, count, scale, bias);
-    CK(cudaGetLastError());
+    launch_f16_to_f32(tmp, d, count, scale, bias);
     CK(cudaDeviceSynchronize());
     return d;
 }
@@ -842,11 +862,7 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
             CK(cudaDeviceSynchronize());
             continue;
         }
-        const size_t nchunk = (size_t)sg.tiles * sg.KB * (GEMM_WBYTES / 16);
-        const int grid = (int)std::min<size_t>((nchunk + 255) / 256, (size_t)num_sms * 16);
-        repack_weight_kernel<<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, d.K, sg.tiles, sg.KB,
-                                            reinterpret_cast<uint4*>(W + (size_t)sg.blk_begin * GEMM_WBYTES));
-        CK(cudaGetLastError());
+        launch_repack(num_sms, src, ld, d.n0, d.k0, d.N, d.K, reinterpret_cast<uint4*>(W + (size_t)sg.blk_begin * GEMM_WBYTES));
         CK(cudaDeviceSynchronize());   // d_tmp is reused by the next upload
     }
     g.grid = std::max(1, std::min(num_sms, std::max(tile, cdiv(blk, 4))));
@@ -1302,7 +1318,7 @@ void b200rwkv_engine::build(const StFile& st) {
                 float* d = (float*)dalloc((size_t)Cl * 4, false);
                 Buf<__half> tmp((size_t)Cl * 2);
                 CK(cudaMemcpy(tmp, td.data + (size_t)c0 * 2, (size_t)Cl * 2, cudaMemcpyHostToDevice));
-                decay_table_kernel<<<cdiv(Cl, 256), 256>>>(tmp, d, Cl);
+                launch_decay_table(tmp, d, Cl);
                 CK(cudaDeviceSynchronize());
                 wk.w_static = d;
             }
@@ -3218,6 +3234,95 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
             CK(cudaMemcpy(h.data(), runs[l].p.seg[i].out, h.size() * 2, cudaMemcpyDeviceToHost));
             a16_unpack(h, s.ldo, mat_cols(s), th, th, mat_cols(s), s.ldo, (uint16_t*)s.out + l * cells);
         }
+    API_END
+}
+
+// Operator-level entry for the parity tests: the kept-row gather after a step (keep_rows_kernel) over caller-supplied vocabulary
+// shards, no model.  The step's metadata comes from OpStep, every shard sits in its own allocation as each rank's logits block
+// does, and the launch is enqueue_keep's: what rank 0 of a `world`-rank engine runs after a step of these entries.
+int32_t b200rwkv_op_keep(int32_t device, const b200rwkv_keep_args* args) {
+    API_BEGIN((b200rwkv_engine*)nullptr)
+    REQUIRE(args, B200RWKV_ERR_INVALID, "null arguments");
+    const b200rwkv_keep_args& x = *args;
+    REQUIRE(x.world >= 1 && x.world <= 8, B200RWKV_ERR_INVALID, "world must be 1..8");
+    REQUIRE(x.Vl >= 1 && (int64_t)x.Vl * x.world <= ((int64_t)1 << 22), B200RWKV_ERR_INVALID, "Vl must be >= 1 with world * Vl <= 4194304");
+    OpStep st(x.S, x.nslot, x.slot, x.count, 0);
+    REQUIRE(x.option && x.keep, B200RWKV_ERR_INVALID, "null option or keep");
+    std::vector<int> outmode(x.nslot, 0);
+    int R = 0;
+    for (int i = 0; i < x.nslot; ++i) {
+        REQUIRE(x.option[i] >= B200RWKV_OPTION_LAST && x.option[i] <= B200RWKV_OPTION_NONE, B200RWKV_ERR_INVALID, "bad option");
+        outmode[i] = x.option[i] == B200RWKV_OPTION_FULL ? 2 : (x.option[i] == B200RWKV_OPTION_LAST ? 1 : 0);
+        R += x.option[i] == B200RWKV_OPTION_FULL ? x.count[i] : (x.option[i] == B200RWKV_OPTION_LAST ? 1 : 0);
+    }
+    REQUIRE(R == 0 || x.shards, B200RWKV_ERR_INVALID, "null shards");
+    const int world = x.world, Vl = x.Vl, V = world * Vl;
+    const size_t keep_bytes = (size_t)x.S * V * 4;
+    st.start(device, 1, nullptr, outmode);
+    b200rwkv_engine* e = st.e.get();
+    e->rank = 0; e->world = world; e->Vl = Vl; e->V = V;
+    e->d_keep = (float*)st.up(x.keep, keep_bytes);
+    e->off_logits = 0;
+    for (int q = 0; q < world; ++q) e->peer_base[q] = (uint8_t*)st.up(x.shards + (size_t)q * R * Vl, (size_t)R * Vl * 4);
+    CK(cudaDeviceSynchronize());                   // every upload has landed before the launch
+    e->enqueue_keep(e->stream, st.sh.MTR);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaMemcpy(x.keep, e->d_keep, keep_bytes, cudaMemcpyDeviceToHost));
+    API_END
+}
+
+// Operator-level entry for the parity tests: one load-time weight kernel on caller buffers, launched as the build launches it.
+int32_t b200rwkv_op_weight(int32_t device, int32_t kind, const b200rwkv_weight_args* args) {
+    API_BEGIN((b200rwkv_engine*)nullptr)
+    REQUIRE(args, B200RWKV_ERR_INVALID, "null arguments");
+    REQUIRE(kind >= B200RWKV_WEIGHT_LORA && kind <= B200RWKV_WEIGHT_REPACK, B200RWKV_ERR_INVALID,
+            "kind must be 0 (LoRA blend), 1 (f32 vector), 2 (decay table) or 3 (repack)");
+    const b200rwkv_weight_args& x = *args;
+    if (kind == B200RWKV_WEIGHT_LORA) {
+        REQUIRE(x.w && x.lora_b && x.lora_a, B200RWKV_ERR_INVALID, "the LoRA blend needs w, lora_b and lora_a");
+        REQUIRE(x.out >= 1 && x.in >= 1 && (int64_t)x.out * x.in <= ((int64_t)1 << 31) && x.r >= 1 && x.r <= 4096, B200RWKV_ERR_INVALID,
+                "bad out / in / r (r must be 1..4096)");
+    } else if (kind == B200RWKV_WEIGHT_REPACK) {
+        REQUIRE(x.src && x.blocks, B200RWKV_ERR_INVALID, "the repack needs src and blocks");
+        REQUIRE(x.rows >= 1 && x.ld >= 1 && (int64_t)x.rows * x.ld <= ((int64_t)1 << 31) && x.N >= 1 && x.K >= 1 && x.n0 >= 0 &&
+                    x.k0 >= 0 && (int64_t)x.n0 + x.N <= x.rows && (int64_t)x.k0 + x.K <= x.ld,
+                B200RWKV_ERR_INVALID, "the sub-matrix [n0, n0 + N) x [k0, k0 + K) must lie inside src [rows][ld]");
+    } else {
+        REQUIRE(x.src && x.dst && x.n >= 1 && x.n <= ((int64_t)1 << 30), B200RWKV_ERR_INVALID, "needs src, dst and n in 1..2^30");
+    }
+    CK(cudaSetDevice(device));
+    int nsm = 0;
+    CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
+    if (kind == B200RWKV_WEIGHT_LORA) {
+        const size_t wb = (size_t)x.out * x.in * 2;
+        Buf<__half> w(wb), b((size_t)x.out * x.r * 2), a((size_t)x.in * x.r * 2);
+        CK(cudaMemcpy(w, x.w, wb, cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(b, x.lora_b, (size_t)x.out * x.r * 2, cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(a, x.lora_a, (size_t)x.in * x.r * 2, cudaMemcpyHostToDevice));
+        launch_lora_blend(nsm, w, b, a, x.out, x.in, x.r, x.alpha);
+        CK(cudaDeviceSynchronize());
+        CK(cudaMemcpy(x.w, w, wb, cudaMemcpyDeviceToHost));
+    } else if (kind == B200RWKV_WEIGHT_REPACK) {
+        const size_t sb = (size_t)x.rows * x.ld * 2;
+        const size_t db = (size_t)cdiv(x.N, GEMM_BN) * cdiv(x.K, GEMM_BK) * GEMM_WBYTES;
+        Buf<__half> s(sb);
+        Buf<uint8_t> d(db);
+        CK(cudaMemcpy(s, x.src, sb, cudaMemcpyHostToDevice));
+        CK(cudaMemset(d, 0xFF, db));               // a chunk the kernel leaves unwritten shows as NaN bits
+        launch_repack(nsm, s, x.ld, x.n0, x.k0, x.N, x.K, reinterpret_cast<uint4*>(d.p));
+        CK(cudaDeviceSynchronize());
+        CK(cudaMemcpy(x.blocks, d, db, cudaMemcpyDeviceToHost));
+    } else {
+        const size_t n = (size_t)x.n;
+        Buf<__half> s(n * 2);
+        Buf<float> d(n * 4);
+        CK(cudaMemcpy(s, x.src, n * 2, cudaMemcpyHostToDevice));
+        if (kind == B200RWKV_WEIGHT_F32) launch_f16_to_f32(s, d, n, x.scale, x.bias);
+        else launch_decay_table(s, d, (int)n);
+        CK(cudaDeviceSynchronize());
+        CK(cudaMemcpy(x.dst, d, n * 4, cudaMemcpyDeviceToHost));
+    }
     API_END
 }
 

@@ -404,6 +404,53 @@ typedef struct {
 int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t quant_type, int32_t grid, int32_t launches,
                          int32_t nseg, const b200rwkv_gemm_seg* seg, int32_t* plan_out);
 
+/* Operator-level entry (parity tests): the kept-row gather that ends a step -- the step's metadata and the launch rank 0 of a
+ * `world`-rank engine makes after it -- on caller-supplied vocabulary shards and kept rows, no model.  Entries as in
+ * b200rwkv_op_ln's ln_out stage (nslot entries, count[i] >= 1 tokens for distinct pool slot slot[i], T = sum(count) <= 128,
+ * option[i] OPTION_LAST / FULL / NONE), which give the step R logits rows in entry order.
+ *   shards: [world][R][Vl] f32, rank q's logits rows of vocabulary ids [q Vl, (q + 1) Vl); each goes to the device in its own
+ *     allocation, as every rank's logits block is.  May be NULL when R = 0.
+ *   keep: [S][world * Vl] f32, updated in place.  A slot whose entry has a row for its last token gets that row, gathered from
+ *     every shard in rank order; every other slot's row comes back unchanged.
+ * world 1..8, Vl >= 1, world * Vl <= 4194304. */
+typedef struct {
+    int32_t S, nslot;
+    const int32_t *slot, *count, *option;
+    int32_t world, Vl;
+    const float* shards;
+    float* keep;
+} b200rwkv_keep_args;
+int32_t b200rwkv_op_keep(int32_t device, const b200rwkv_keep_args* args);
+
+/* Operator-level entry (parity tests): one of the kernels that prepare weights at load, on caller buffers, with the launch
+ * shape the model build gives it.  f16 arrays are bit patterns; only the members of the chosen kind are read.
+ *   B200RWKV_WEIGHT_LORA: w [out][in] in / out <- f16(f32(w) + alpha * acc), acc the f32 sum over j < r, in order, of
+ *     lora_b[o][j] * lora_a[i][j]: one LoRA pair as b200rwkv_create_ex blends it (lora_b = `<name>.lora.1` [out, r],
+ *     lora_a = `<name>.lora.0` [in, r]; r 1..4096).
+ *   B200RWKV_WEIGHT_F32: dst[i] = f32(src[i]) * scale + bias, i < n: the model's per-channel vectors.
+ *   B200RWKV_WEIGHT_DECAY: dst[i] = expf(-expf(f32(src[i]))), i < n: the RWKV-5 static decay.
+ *   B200RWKV_WEIGHT_REPACK: rows [n0, n0 + N) and columns [k0, k0 + K) of src [rows][ld] into the projection kernels' weight
+ *     blocks: blocks [ceil(N / 128)][ceil(K / 128)] of [k8 16][row group 16][row 8][8 halves] f16, block (tile, kb) holding
+ *     rows tile * 128 + 8 * group + row and columns kb * 128 + 8 * k8 + e of the sub-matrix, zero outside it.
+ * n 1..2^30. */
+#define B200RWKV_WEIGHT_LORA 0
+#define B200RWKV_WEIGHT_F32 1
+#define B200RWKV_WEIGHT_DECAY 2
+#define B200RWKV_WEIGHT_REPACK 3
+typedef struct {
+    const uint16_t* src;            /* F32, DECAY: [n]; REPACK: [rows][ld] */
+    int64_t n;
+    float scale, bias;
+    float* dst;
+    uint16_t* w;                    /* LORA */
+    const uint16_t *lora_b, *lora_a;
+    int32_t out, in, r;
+    float alpha;
+    int32_t rows, ld, n0, k0, N, K; /* REPACK */
+    uint16_t* blocks;
+} b200rwkv_weight_args;
+int32_t b200rwkv_op_weight(int32_t device, int32_t kind, const b200rwkv_weight_args* args);
+
 /* Kernels launched by this engine's forward steps since creation (graph replays counted by their kernel nodes). */
 int32_t b200rwkv_launch_count(b200rwkv_engine*, int64_t* total);
 

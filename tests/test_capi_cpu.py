@@ -216,17 +216,26 @@ def test_ctypes_structs_match_the_header(tmp_path):
                    '  printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b200rwkv_ln_args), offsetof(b200rwkv_ln_args, slot),\n'
                    '  offsetof(b200rwkv_ln_args, precision), offsetof(b200rwkv_ln_args, x_in), offsetof(b200rwkv_ln_args, parts),\n'
                    '  offsetof(b200rwkv_ln_args, n_mix), offsetof(b200rwkv_ln_args, mix_out), offsetof(b200rwkv_ln_args, Dm),\n'
-                   '  offsetof(b200rwkv_ln_args, V), offsetof(b200rwkv_ln_args, kernel_out)); return 0; }\n')
+                   '  offsetof(b200rwkv_ln_args, V), offsetof(b200rwkv_ln_args, kernel_out));\n'
+                   '  printf("%zu %zu %zu %zu %zu\\n", sizeof(b200rwkv_keep_args), offsetof(b200rwkv_keep_args, slot),\n'
+                   '  offsetof(b200rwkv_keep_args, world), offsetof(b200rwkv_keep_args, shards), offsetof(b200rwkv_keep_args, keep));\n'
+                   '  printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b200rwkv_weight_args), offsetof(b200rwkv_weight_args, n),\n'
+                   '  offsetof(b200rwkv_weight_args, scale), offsetof(b200rwkv_weight_args, dst), offsetof(b200rwkv_weight_args, w),\n'
+                   '  offsetof(b200rwkv_weight_args, out), offsetof(b200rwkv_weight_args, alpha), offsetof(b200rwkv_weight_args, rows),\n'
+                   '  offsetof(b200rwkv_weight_args, blocks)); return 0; }\n')
     exe = tmp_path / "sz"
     subprocess.run([gcc, "-std=c99", "-Wall", "-Werror", "-I", os.path.join(root, "include"), str(src), "-o", str(exe)], check=True)
     got = [int(x) for x in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
-    O, G, W, L = capi.Options, capi.GemmSeg, capi.WkvArgs, capi.LnArgs
+    O, G, W, L, K, WA = capi.Options, capi.GemmSeg, capi.WkvArgs, capi.LnArgs, capi.KeepArgs, capi.WeightArgs
     assert got == [C.sizeof(O), O.devices.offset, O.lora_st.offset, O.quant_layers.offset, C.sizeof(capi.Info),
                    C.sizeof(G), G.act.offset, G.lerp_xx.offset, G.out.offset,
                    C.sizeof(W), W.slot.offset, W.precision.offset, W.r.offset, W.nu.offset, W.layer0.offset, W.v_first.offset,
                    W.Dd.offset, W.out.offset,
                    C.sizeof(L), L.slot.offset, L.precision.offset, L.x_in.offset, L.parts.offset, L.n_mix.offset,
-                   L.mix_out.offset, L.Dm.offset, L.V.offset, L.kernel_out.offset]
+                   L.mix_out.offset, L.Dm.offset, L.V.offset, L.kernel_out.offset,
+                   C.sizeof(K), K.slot.offset, K.world.offset, K.shards.offset, K.keep.offset,
+                   C.sizeof(WA), WA.n.offset, WA.scale.offset, WA.dst.offset, WA.w.offset, WA.out.offset, WA.alpha.offset,
+                   WA.rows.offset, WA.blocks.offset]
 
 
 def test_op_gemm_refuses_bad_arguments_without_a_gpu():
@@ -447,6 +456,114 @@ def test_op_ln_refuses_bad_arguments_without_a_gpu():
         for ok in (args(), args(x_out=None, n_parts=0), args(**six), args(**six, precision=1), args(stage=capi.LN_OUT),
                    args(stage=capi.LN_EMBED), args(counts=(60, 68), n_gate=8, n_parts=8)):
             assert call(ok) == capi.ERR_CUDA
+
+
+def test_op_keep_refuses_bad_arguments_without_a_gpu():
+    """b200rwkv_op_keep checks every argument before its first CUDA call: ERR_INVALID for malformed arguments, ERR_STATE for a
+    slot outside the pool."""
+    S, world, Vl = 4, 2, 5
+    shards = np.zeros((world, 8, Vl), np.float32)
+    keep = np.zeros((S, world * Vl), np.float32)
+    P = capi.ptr
+
+    def args(slots=(1, 3), counts=(2, 3), options=(capi.OPTION_FULL, capi.OPTION_LAST), **kw):
+        sl, cn, op = np.array(slots, np.int32), np.array(counts, np.int32), np.array(options, np.int32)
+        a = capi.KeepArgs(S=S, nslot=len(sl), slot=P(sl), count=P(cn), option=P(op), world=world, Vl=Vl, shards=P(shards),
+                          keep=P(keep))
+        for k, val in kw.items():
+            setattr(a, k, val)
+        a._keep = (sl, cn, op)
+        return a
+
+    def call(a):
+        return capi.lib().b200rwkv_op_keep(0, C.byref(a))
+
+    INV, STA = capi.ERR_INVALID, capi.ERR_STATE
+    cases = {
+        "null arguments": (capi.lib().b200rwkv_op_keep(0, None), INV),
+        "world 0": (call(args(world=0)), INV),
+        "world 9": (call(args(world=9)), INV),
+        "Vl 0": (call(args(Vl=0)), INV),
+        "world * Vl > 2^22": (call(args(world=8, Vl=(1 << 19) + 1)), INV),
+        "S = 0": (call(args(S=0)), INV),
+        "no entry": (call(args(nslot=0)), INV),
+        "null slot ids": (call(args(slot=None)), INV),
+        "null counts": (call(args(count=None)), INV),
+        "slot = S": (call(args(slots=(1, 4))), STA),
+        "negative slot": (call(args(slots=(-1, 3))), STA),
+        "duplicate slot": (call(args(slots=(3, 3))), INV),
+        "count 0": (call(args(counts=(2, 0))), INV),
+        "129 tokens": (call(args(counts=(64, 65))), INV),
+        "null options": (call(args(option=None)), INV),
+        "option 3": (call(args(options=(capi.OPTION_LAST, capi.OPTION_SCORE))), INV),
+        "null keep": (call(args(keep=None)), INV),
+        "null shards with rows": (call(args(shards=None)), INV),
+    }
+    for name, (got, want) in cases.items():
+        assert got == want, name
+    if not _has_gpu():                       # well-formed arguments reach the device, and there is none: no CPU fallback
+        none = (capi.OPTION_NONE, capi.OPTION_NONE)
+        for ok in (args(), args(world=1), args(world=8, Vl=1 << 19), args(options=none, shards=None)):
+            assert call(ok) == capi.ERR_CUDA
+
+
+def test_op_weight_refuses_bad_arguments_without_a_gpu():
+    """b200rwkv_op_weight checks every argument of the chosen kind before its first CUDA call: ERR_INVALID for an unknown kind,
+    a null buffer, an empty or oversized shape, or a sub-matrix outside its source."""
+    w = np.zeros((8, 12), np.float16)
+    lb, la = np.zeros((8, 3), np.float16), np.zeros((12, 3), np.float16)
+    src = np.zeros((20, 30), np.float16)
+    blocks = np.zeros(128 * 128, np.float16)
+    dst = np.zeros(600, np.float32)
+    P = capi.ptr
+    L, F, D, R = capi.WEIGHT_LORA, capi.WEIGHT_F32, capi.WEIGHT_DECAY, capi.WEIGHT_REPACK
+
+    def args(**kw):
+        a = capi.WeightArgs(src=P(src), n=600, scale=1.0, bias=0.0, dst=P(dst), w=P(w), lora_b=P(lb), lora_a=P(la), out=8, in_=12,
+                            r=3, alpha=0.5, rows=20, ld=30, n0=3, k0=5, N=17, K=25, blocks=P(blocks))
+        for k, val in kw.items():
+            setattr(a, k, val)
+        return a
+
+    def call(kind, a):
+        return capi.lib().b200rwkv_op_weight(0, kind, C.byref(a))
+
+    INV = capi.ERR_INVALID
+    cases = {
+        "null arguments": (capi.lib().b200rwkv_op_weight(0, L, None), INV),
+        "kind -1": (call(-1, args()), INV),
+        "kind 4": (call(4, args()), INV),
+        "LoRA, null w": (call(L, args(w=None)), INV),
+        "LoRA, null lora_b": (call(L, args(lora_b=None)), INV),
+        "LoRA, null lora_a": (call(L, args(lora_a=None)), INV),
+        "LoRA, out 0": (call(L, args(out=0)), INV),
+        "LoRA, in 0": (call(L, args(in_=0)), INV),
+        "LoRA, r 0": (call(L, args(r=0)), INV),
+        "LoRA, r 4097": (call(L, args(r=4097)), INV),
+        "LoRA, out * in > 2^31": (call(L, args(out=1 << 16, in_=(1 << 15) + 1)), INV),
+        "f32, null src": (call(F, args(src=None)), INV),
+        "f32, null dst": (call(F, args(dst=None)), INV),
+        "f32, n 0": (call(F, args(n=0)), INV),
+        "decay, n > 2^30": (call(D, args(n=(1 << 30) + 1)), INV),
+        "decay, null dst": (call(D, args(dst=None)), INV),
+        "repack, null src": (call(R, args(src=None)), INV),
+        "repack, null blocks": (call(R, args(blocks=None)), INV),
+        "repack, rows 0": (call(R, args(rows=0)), INV),
+        "repack, ld 0": (call(R, args(ld=0)), INV),
+        "repack, N 0": (call(R, args(N=0)), INV),
+        "repack, K 0": (call(R, args(K=0)), INV),
+        "repack, negative n0": (call(R, args(n0=-1)), INV),
+        "repack, negative k0": (call(R, args(k0=-1)), INV),
+        "repack, rows past the source": (call(R, args(N=18)), INV),
+        "repack, columns past the source": (call(R, args(K=26)), INV),
+    }
+    for name, (got, want) in cases.items():
+        assert got == want, name
+    # a kind reads only its own members
+    if not _has_gpu():                       # well-formed arguments reach the device, and there is none: no CPU fallback
+        for kind, ok in ((L, args(src=None, dst=None, blocks=None)), (F, args(w=None, blocks=None)), (D, args(w=None, n=1)),
+                         (R, args(w=None, dst=None, n0=0, k0=0, N=20, K=30))):
+            assert call(kind, ok) == capi.ERR_CUDA
 
 
 def test_c_host_program_links_and_calls_the_library(tmp_path):
