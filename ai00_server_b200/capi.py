@@ -183,6 +183,8 @@ SYMBOLS = [
     ("b200rwkv_info_from_st", C.c_int32, [_P, C.c_size_t, C.POINTER(Info)]),
     ("b200rwkv_create", C.c_int32, [_P, C.c_size_t, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(_P)]),
     ("b200rwkv_create_ex", C.c_int32, [_P, C.c_size_t, C.POINTER(Options), C.POINTER(_P)]),
+    ("b200rwkv_create_adapters", C.c_int32, [_P, C.c_size_t, C.POINTER(Options), C.c_int32, _P, _P, _P, C.POINTER(_P)]),
+    ("b200rwkv_bind_adapter", C.c_int32, [_P, C.c_int32, _P, _P]),
     ("b200rwkv_create_tp", C.c_int32, [_P, C.c_size_t, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(_P)]),
     ("b200rwkv_tp_export", C.c_int32, [_P, _P]),
     ("b200rwkv_tp_connect", C.c_int32, [_P, _P]),
@@ -216,6 +218,7 @@ SYMBOLS = [
     ("b200rwkv_op_gemm", C.c_int32, [C.c_int32] * 7 + [C.POINTER(GemmSeg), C.POINTER(C.c_int32 * 4)]),
     ("b200rwkv_op_keep", C.c_int32, [C.c_int32, C.POINTER(KeepArgs)]),
     ("b200rwkv_op_weight", C.c_int32, [C.c_int32, C.c_int32, C.POINTER(WeightArgs)]),
+    ("b200rwkv_op_adapter", C.c_int32, [C.c_int32] * 5 + [_P, _P, _P, _P, _P]),
     ("b200rwkv_launch_count", C.c_int32, [_P, C.POINTER(C.c_int64)]),
     ("b200rwkv_keep_hidden", C.c_int32, [_P, C.c_int32]),
     ("b200rwkv_last_hidden", C.c_int32, [_P, _P, C.c_size_t]),
@@ -257,6 +260,22 @@ def check(code: int, engine=None):
 
 def ptr(a: np.ndarray):
     return a.ctypes.data_as(C.c_void_p)
+
+
+def op_adapter(x, lora_a, ids, precision: int = 0, device: int = 0):
+    """One adapter shrink launch (b200rwkv_op_adapter): x [T, K] f16 operand rows (precision 1: [2, T, K], hi then lo),
+    lora_a: list of n `.lora.0` matrices [K, r] f16, ids [T] in 0..n.  Returns the tail blocks [T, n, 128] f16
+    (precision 1: [2, T, n, 128])."""
+    x = np.ascontiguousarray(x, dtype=np.float16)
+    T, K = x.shape[-2], x.shape[-1]
+    mats = [np.ascontiguousarray(a, dtype=np.float16) for a in lora_a]
+    n = len(mats)
+    rank = np.array([a.shape[1] for a in mats], np.int32)
+    ptrs = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in mats])
+    ids = np.ascontiguousarray(ids, dtype=np.int32)
+    tail = np.zeros(((2,) if precision == 1 else ()) + (T, n, 128), np.float16)
+    check(lib().b200rwkv_op_adapter(device, T, K, precision, n, ptr(rank), C.cast(ptrs, C.c_void_p), ptr(ids), ptr(x), ptr(tail)))
+    return tail
 
 
 def info_from_st(st: np.ndarray) -> dict:

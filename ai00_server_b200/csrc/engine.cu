@@ -28,6 +28,7 @@
 #include "misc.cuh"
 #include "mix.cuh"
 #include "wkv.cuh"
+#include "adapter.cuh"
 
 namespace b200 {
 
@@ -403,6 +404,15 @@ static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
 enum KClass { KC_GEMM = 0, KC_WKV = 1, KC_LN = 2, KC_OTHER = 3 };
 
+struct SegDesc {
+    const StTensor* t = nullptr;
+    int64_t slice = -1;        // leading-dim index for 3-D tensors
+    int n0 = 0, N = 0, k0 = 0, K = 0;
+    GemmSeg proto;             // A, out_mode, act, bias, out, ldo, grp, grp_stride, aux*
+    int ad_tail = 0;           // unblended adapters: 128-wide tail k blocks after the segment's own (make_launch)
+    SegDesc() { memset(&proto, 0, sizeof(proto)); }
+};
+
 struct GemmLaunch {
     GemmParams p;
     int grid = 0;
@@ -410,15 +420,11 @@ struct GemmLaunch {
     int total_tiles = 0;
     size_t weight_bytes = 0;   // algorithmic (unpadded) weight bytes streamed (f16, or codes + block parameters)
     int qtype = QT_NONE;       // weight format of every segment of the launch (qgemm.cuh)
+    // the plan's inputs, kept during build only: the adapter plans are made from them (b200rwkv_engine::ad_launch)
+    std::vector<SegDesc> src;
+    int force_grid = 0;
 };
 
-struct SegDesc {
-    const StTensor* t = nullptr;
-    int64_t slice = -1;        // leading-dim index for 3-D tensors
-    int n0 = 0, N = 0, k0 = 0, K = 0;
-    GemmSeg proto;             // A, out_mode, act, bias, out, ldo, grp, grp_stride, aux*
-    SegDesc() { memset(&proto, 0, sizeof(proto)); }
-};
 
 struct A16Buf {
     __half* p = nullptr;
@@ -440,6 +446,15 @@ struct Layer {
     std::vector<GemmLaunch> ffn;    // launches after LN2
 };
 
+// The same layer on steps with a bound adapter: `pre`, `o` and `ffn` as in Layer, with every launch that holds an adapted
+// projection replaced by its W' plan, and one shrink launch in front of each of those launches (nproj 0: none).
+struct AdLayer {
+    std::vector<GemmLaunch> pre;
+    GemmLaunch o;
+    std::vector<GemmLaunch> ffn;
+    AdapterParams s_pre, s_o, s_fk, s_fv;
+};
+
 struct Profiler {
     struct Rec { int cls; Event a, b; };
     std::vector<Rec> recs;
@@ -454,8 +469,9 @@ enum LnKernel { LNK_EMBED = 0, LNK_MIX = 1, LNK_MIX_CLUSTER = 2, LNK_PRE6 = 3, L
 struct LnPick { int kernel, variant, split; };
 // The launch shape of one step (b200rwkv_engine::step_shape): MT token tiles of 16 rows and MTR row tiles of the head (0: no
 // output rows), `rows` = 16 * MT rows of the per-token buffers, and the token rows th / th_rows of the step's A16 operands and
-// of the head's operand.  `split`: the operands hold hi + lo f16 rows (th = th_rows = 32).
-struct StepShape { int MT, MTR, rows, th, th_rows; bool split; };
+// of the head's operand.  `split`: the operands hold hi + lo f16 rows (th = th_rows = 32).  `ad`: a slot of the step is bound
+// to an unblended adapter, so the step runs the adapter plans and their shrink launches.
+struct StepShape { int MT, MTR, rows, th, th_rows; bool split; bool ad = false; };
 
 // The A16 layout (common.cuh) on the host.  a16_halves: halves of one matrix of K columns.  a16_pack / a16_unpack move `ncols`
 // columns of token rows between a caller's dense array and consecutive A16 matrices of K columns and `tr` token rows each (the
@@ -628,6 +644,21 @@ struct b200rwkv_engine {
     // LoRA files blended into the projection weights while they are uploaded (borrowed during build only)
     struct LoraSrc { const StFile* st; float alpha; };
     std::vector<LoraSrc> loras;
+    // unblended adapters (b200rwkv_create_adapters): files borrowed during build only, plans and A matrices kept
+    std::vector<LoraSrc> adapters;
+    int n_adapters = 0;
+    std::vector<AdLayer> ad_layers;
+    GemmLaunch ad_head;
+    AdapterParams s_head;
+    int* d_slot_adapter = nullptr;           // [S] adapter bound to each slot, 0 = the base model
+    std::vector<int> slot_adapter;           // host copy (the infer task's)
+    bool step_bound(const std::vector<int>& slots) const {
+        for (int s : slots)
+            if (n_adapters && s >= 0 && s < S && slot_adapter[s]) return true;
+        return false;
+    }
+    GemmLaunch ad_launch(const GemmLaunch& base, AdapterParams& sp);
+    void enqueue_shrink(const AdapterParams& p, const StepShape& sh, cudaStream_t s, Profiler* prof);
     void check_loras(const StFile& model) const;
     void blend_loras(const StTensor& t);
 
@@ -717,9 +748,9 @@ static bool ends_with(const std::string& s, const std::string& suf) {
 
 // Every `<base>.lora.0/.lora.1` pair of a LoRA file must address a projection matrix this engine blends (the matrices that
 // go through upload_tmp); anything else is refused loudly rather than ignored.
-void b200rwkv_engine::check_loras(const StFile& model) const {
+static void check_lora_files(const StFile& model, const std::vector<b200rwkv_engine::LoraSrc>& files) {
     static const char* ok[] = {".att.receptance", ".att.key", ".att.value", ".att.gate", ".att.output", ".ffn.key", ".ffn.value", ".ffn.receptance"};
-    for (const LoraSrc& lo : loras) {
+    for (const b200rwkv_engine::LoraSrc& lo : files) {
         int pairs = 0;
         for (auto& kv : lo.st->tensors) {
             const std::string& n = kv.first;
@@ -737,6 +768,36 @@ void b200rwkv_engine::check_loras(const StFile& model) const {
         }
         REQUIRE(pairs > 0, B200RWKV_ERR_INVALID, "LoRA file holds no <name>.lora.0 / <name>.lora.1 pairs");
     }
+}
+void b200rwkv_engine::check_loras(const StFile& model) const { check_lora_files(model, loras); }
+
+// Adapter files (b200rwkv_create_adapters), host only: the load-time blend's refusals, then every pair's halves, dtypes and
+// shapes against the model, the rank (one 128-wide k block of W'), and no pair on a matrix of a quantised layer.
+static void check_adapter_files(const StFile& model, const std::vector<b200rwkv_engine::LoraSrc>& files, int quant_layers,
+                                int quant_type) {
+    check_lora_files(model, files);
+    for (const b200rwkv_engine::LoraSrc& lo : files)
+        for (auto& kv : lo.st->tensors) {
+            const std::string& n = kv.first;
+            if (!ends_with(n, ".lora.0") && !ends_with(n, ".lora.1")) continue;
+            const std::string base = n.substr(0, n.size() - 7);
+            const StTensor* a = lo.st->find(base + ".lora.0");
+            const StTensor* b = lo.st->find(base + ".lora.1");
+            REQUIRE(a && b, B200RWKV_ERR_INVALID, "adapter file: " + base + " has only one of .lora.0 / .lora.1");
+            if (n != base + ".lora.0") continue;
+            const StTensor* w = model.find(base + ".weight");
+            REQUIRE(w && w->shape.size() == 2, B200RWKV_ERR_UNSUPPORTED, "adapter on " + base + " is not supported (projection matrices only)");
+            REQUIRE(a->dtype == "F16" && b->dtype == "F16", B200RWKV_ERR_UNSUPPORTED, "adapter tensors must be F16: " + base);
+            REQUIRE(a->shape.size() == 2 && b->shape.size() == 2 && b->shape[0] == w->shape[0] && a->shape[0] == w->shape[1] &&
+                        a->shape[1] == b->shape[1] && a->shape[1] >= 1,
+                    B200RWKV_ERR_INVALID, "adapter shapes do not match " + base + ".weight (expected lora.0 [in, r], lora.1 [out, r])");
+            REQUIRE(a->shape[1] <= AD_MAX_RANK, B200RWKV_ERR_UNSUPPORTED,
+                    "adapter rank " + std::to_string(a->shape[1]) + " on " + base + " is above 128");
+            REQUIRE(a->shape[0] % 8 == 0, B200RWKV_ERR_UNSUPPORTED, "adapter on " + base + ": input width must be a multiple of 8");
+            const int layer = base.compare(0, 7, "blocks.") == 0 ? atoi(base.c_str() + 7) : -1;
+            REQUIRE(quant_type == QT_NONE || layer < 0 || layer >= quant_layers, B200RWKV_ERR_UNSUPPORTED,
+                    "adapter on " + base + ": its layer is quantised (adapters need f16 projection matrices)");
+        }
 }
 
 // The load-time weight kernels with the launch shapes the build gives them; b200rwkv_op_weight runs these same launches.
@@ -814,7 +875,7 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
         // A16 outputs are written as whole 16-byte chunks of 8 rows (gemm.cuh epilogue)
         REQUIRE(sg.out_mode == OUT_F32 || (d.N % 8 == 0 && sg.grp % 8 == 0), B200RWKV_ERR_UNSUPPORTED,
                 "LoRA ranks / hidden size must be multiples of 8");
-        sg.KB = cdiv(d.K, GEMM_BK);
+        sg.KB = cdiv(d.K, GEMM_BK) + d.ad_tail;
         sg.tiles = cdiv(d.N, GEMM_BN);
         sg.N = d.N;
         sg.blk_begin = blk;
@@ -822,7 +883,7 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
         blk += sg.tiles * sg.KB;
         tile += sg.tiles;
         kbmax = std::max(kbmax, sg.KB);
-        if (qtype == QT_NONE) g.weight_bytes += (size_t)d.N * d.K * 2;
+        if (qtype == QT_NONE) g.weight_bytes += (size_t)d.N * (d.K + (size_t)d.ad_tail * GEMM_BK) * 2;
         else {
             // quantisation blocks are runs of 128 (Int8) / 64 (NF4) consecutive inputs of one output row of the FULL matrix
             REQUIRE(d.K % GEMM_BK == 0 && d.k0 % GEMM_BK == 0, B200RWKV_ERR_UNSUPPORTED,
@@ -832,6 +893,8 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
         }
     }
     g.p.nseg = (int)segs.size();
+    g.src = segs;
+    g.force_grid = force_grid;
     g.p.total_blocks = blk;
     g.total_tiles = tile;
     uint8_t* W = (uint8_t*)dalloc((size_t)blk * blk_bytes, false);
@@ -862,7 +925,30 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
             CK(cudaDeviceSynchronize());
             continue;
         }
-        launch_repack(num_sms, src, ld, d.n0, d.k0, d.N, d.K, reinterpret_cast<uint4*>(W + (size_t)sg.blk_begin * GEMM_WBYTES));
+        uint4* dst = reinterpret_cast<uint4*>(W + (size_t)sg.blk_begin * GEMM_WBYTES);
+        if (d.ad_tail) {
+            // W' = [W | a_1 B_1 | ... | a_n B_n]: W's columns padded to whole k blocks, then one zero-padded k block per
+            // adapter holding f16(alpha * lora.1) (zeros for an adapter without a pair here), re-tiled like any matrix
+            const int kbw = cdiv(d.K, GEMM_BK), ke = (kbw + d.ad_tail) * GEMM_BK;
+            Buf<__half> E((size_t)d.N * ke * 2);
+            CK(cudaMemset(E, 0, E.bytes));
+            CK(cudaMemcpy2D(E, (size_t)ke * 2, src + (size_t)d.n0 * ld + d.k0, (size_t)ld * 2, (size_t)d.K * 2, d.N,
+                            cudaMemcpyDeviceToDevice));
+            const std::string base = t.name.substr(0, t.name.size() - 7);
+            for (int a = 0; a < d.ad_tail; ++a) {
+                const StTensor* b = adapters[a].st->find(base + ".lora.1");
+                if (!b) continue;
+                const int r = (int)b->shape[1];
+                std::vector<__half> h((size_t)d.N * r);
+                memcpy(h.data(), b->data + (size_t)d.n0 * r * 2, h.size() * 2);
+                for (__half& v : h) v = __float2half_rn(adapters[a].alpha * __half2float(v));
+                CK(cudaMemcpy2D((__half*)E + (size_t)(kbw + a) * GEMM_BK, (size_t)ke * 2, h.data(), (size_t)r * 2, (size_t)r * 2,
+                                d.N, cudaMemcpyHostToDevice));
+            }
+            launch_repack(num_sms, E, ke, 0, 0, d.N, ke, dst);
+        } else {
+            launch_repack(num_sms, src, ld, d.n0, d.k0, d.N, d.K, dst);
+        }
         CK(cudaDeviceSynchronize());   // d_tmp is reused by the next upload
     }
     g.grid = std::max(1, std::min(num_sms, std::max(tile, cdiv(blk, 4))));
@@ -1120,10 +1206,14 @@ void b200rwkv_engine::build(const StFile& st) {
             tk_out_p = (float*)dalloc((size_t)S * TOPK_MAX * 4);
         }
     }
-    for (int i = 0; i < 6; ++i) a_x[i] = a16_alloc(C);
-    a_out = a16_alloc(Cl);
-    a_kk = a16_alloc(Fl);
-    a_head = a16_alloc(C);
+    // with adapters, every projection operand carries one 128-wide tail block per adapter after its own k blocks
+    auto op_cols = [&](int K) { return n_adapters ? (cdiv(K, GEMM_BK) + n_adapters) * GEMM_BK : K; };
+    for (int i = 0; i < 6; ++i) a_x[i] = a16_alloc(op_cols(C));
+    a_out = a16_alloc(op_cols(Cl));
+    a_kk = a16_alloc(op_cols(Fl));
+    a_head = a16_alloc(op_cols(C));
+    slot_adapter.assign(S, 0);
+    if (n_adapters) d_slot_adapter = (int*)dalloc((size_t)S * 4, true);
 
     // ---- embedding + ln0 ----
     {
@@ -1436,14 +1526,45 @@ void b200rwkv_engine::build(const StFile& st) {
         head.p.nrows = d_meta + 2;    // R
     }
 
-    gemm_ws = (float*)dalloc(gemm_ws_floats * 4, false);
-    for (auto& ly : layers) {
-        for (auto& g : ly.lora) g.p.ws = gemm_ws;
-        for (auto& g : ly.pre) g.p.ws = gemm_ws;
-        ly.o.p.ws = gemm_ws;
-        for (auto& g : ly.ffn) g.p.ws = gemm_ws;
+    // adapter plans: every launch that holds an adapted projection again as W', with a shrink launch in front of it
+    if (n_adapters) {
+        ad_layers.resize(L);
+        auto shrink = [&](AdapterParams& sp, bool on_head) {
+            memset(&sp, 0, sizeof(sp));
+            sp.n = n_adapters; sp.meta = mv; sp.slot_adapter = d_slot_adapter; sp.head = on_head ? 1 : 0;
+        };
+        for (int l = 0; l < L; ++l) {
+            Layer& ly = layers[l];
+            AdLayer& ad = ad_layers[l];
+            shrink(ad.s_pre, false); shrink(ad.s_o, false); shrink(ad.s_fk, false); shrink(ad.s_fv, false);
+            for (auto& g : ly.pre) ad.pre.push_back(ad_launch(g, ad.s_pre));
+            ad.o = ad_launch(ly.o, ad.s_o);
+            REQUIRE(ly.ffn.size() == 2, B200RWKV_ERR_INVALID, "internal: channel mix is two launches");
+            ad.ffn.push_back(ad_launch(ly.ffn[0], ad.s_fk));
+            ad.ffn.push_back(ad_launch(ly.ffn[1], ad.s_fv));
+        }
+        shrink(s_head, true);
+        ad_head = ad_launch(head, s_head);
+        ad_head.p.nrows = d_meta + 2;
     }
-    head.p.ws = gemm_ws;
+    gemm_ws = (float*)dalloc(gemm_ws_floats * 4, false);
+    auto wire = [&](GemmLaunch& g) {
+        g.p.ws = gemm_ws;
+        g.src.clear();          // points into the model file, which is borrowed during build only
+    };
+    for (auto& ly : layers) {
+        for (auto& g : ly.lora) wire(g);
+        for (auto& g : ly.pre) wire(g);
+        wire(ly.o);
+        for (auto& g : ly.ffn) wire(g);
+    }
+    wire(head);
+    for (auto& ad : ad_layers) {
+        for (auto& g : ad.pre) wire(g);
+        wire(ad.o);
+        for (auto& g : ad.ffn) wire(g);
+    }
+    wire(ad_head);
 
     if (world == 1) {
         peer_base[0] = comm_base;
@@ -1489,6 +1610,62 @@ void b200rwkv_engine::finalize_tp() {
     connected = true;
 }
 
+// [r][K] rows of A = lora.0^T ([in, r] on disk) for the shrink kernel: one 16-byte load per 8 k of a row
+static std::vector<uint16_t> adapter_a_rows(const uint8_t* lora0, int K, int r) {
+    // whole groups of 8 rows, zeros past r: the shrink kernel loads the 8 rows of its columns without a bound check
+    std::vector<uint16_t> raw((size_t)K * r), rows((size_t)cdiv(r, 8) * 8 * K, 0);
+    memcpy(raw.data(), lora0, raw.size() * 2);
+    for (int k = 0; k < K; ++k)
+        for (int j = 0; j < r; ++j) rows[(size_t)j * K + k] = raw[(size_t)k * r + j];
+    return rows;
+}
+
+// The W' plan of `base` (one tail k block per adapter on each segment that holds a whole adapted projection, or the last
+// split-K slice of one), with the projection added to the shrink launch `sp`; `base` itself when no adapter touches it.
+GemmLaunch b200rwkv_engine::ad_launch(const GemmLaunch& base, AdapterParams& sp) {
+    std::vector<SegDesc> segs = base.src;
+    bool any = false;
+    for (SegDesc& d : segs) {
+        const StTensor& t = *d.t;
+        if (d.slice >= 0 || !ends_with(t.name, ".weight") || t.shape.size() != 2 || d.k0 + d.K != t.shape[1]) continue;
+        const std::string nm = t.name.substr(0, t.name.size() - 7);
+        AdapterProj pj;
+        memset(&pj, 0, sizeof(pj));
+        pj.K = (int)t.shape[1];
+        for (int a = 0; a < n_adapters; ++a) {
+            const StTensor* la = adapters[a].st->find(nm + ".lora.0");
+            if (!la) continue;
+            pj.r[a] = (int)la->shape[1];
+            const std::vector<uint16_t> rows = adapter_a_rows(la->data, pj.K, pj.r[a]);
+            __half* dA = (__half*)dalloc(rows.size() * 2, false);
+            CK(cudaMemcpy(dA, rows.data(), rows.size() * 2, cudaMemcpyHostToDevice));
+            pj.A[a] = dA;
+        }
+        bool has = false;
+        for (int a = 0; a < n_adapters; ++a) has = has || pj.A[a];
+        if (!has) continue;
+        REQUIRE(base.qtype == QT_NONE && world == 1 && d.k0 % GEMM_BK == 0 && sp.nproj < AD_MAX_PROJ, B200RWKV_ERR_INVALID,
+                "internal: adapter on " + nm + " does not fit its launch");
+        pj.op = const_cast<__half*>(d.proto.A) - (size_t)(d.k0 / GEMM_BK) * A16_KB_HALVES;
+        pj.kb0 = cdiv(pj.K, GEMM_BK);
+        sp.p[sp.nproj++] = pj;
+        d.ad_tail = n_adapters;
+        any = true;
+    }
+    if (!any) return base;
+    return make_launch(segs, base.force_grid, QT_NONE);
+}
+
+// the shrink launch of one step phase: (8 columns, 16 rows, projection) CTAs over the step's token rows, or its output rows
+void b200rwkv_engine::enqueue_shrink(const AdapterParams& p0, const StepShape& sh, cudaStream_t s, Profiler* prof) {
+    if (p0.nproj == 0) return;
+    AdapterParams p = p0;
+    p.th = p.head ? sh.th_rows : sh.th;
+    const dim3 grid = adapter_grid(p.head ? 16 * sh.MTR : sh.rows, p.nproj);
+    if (sh.split) launch_k(adapter_shrink_kernel<true>, grid, dim3(AD_THREADS), 0, p, KC_OTHER, s, prof);
+    else launch_k(adapter_shrink_kernel<false>, grid, dim3(AD_THREADS), 0, p, KC_OTHER, s, prof);
+}
+
 // -----------------------------------------------------------------------------------------
 // one forward step over the tokens described by d_meta
 // -----------------------------------------------------------------------------------------
@@ -1513,6 +1690,7 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler
     };
     for (int l = 0; l < L; ++l) {
         Layer& ly = layers[l];
+        AdLayer* ad = sh.ad ? &ad_layers[l] : nullptr;      // a slot of the step is bound: W' plans and their shrinks
         if (ly.has_pre6 && sh.MT == 1) {
             Pre6Params q = ly.pre6;
             q.ln = ly.ln1;
@@ -1522,20 +1700,34 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler
             ln_stage(ly.ln1);
             for (auto& g : ly.lora) gemm(g);
         }
-        for (auto& g : ly.pre) gemm(g);
+        if (ad) enqueue_shrink(ad->s_pre, sh, s, prof);
+        for (auto& g : ad ? ad->pre : ly.pre) gemm(g);
         {
             WkvParams wp = ly.wkv;
             wp.trace = tr_next(2);
             launch_wkv(wp, sh, s, prof);
         }
-        gemm(ly.o);
+        if (ad) enqueue_shrink(ad->s_o, sh, s, prof);
+        gemm(ad ? ad->o : ly.o);
         if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
         ln_stage(ly.ln2);
-        for (auto& g : ly.ffn) gemm(g);
+        if (ad) {
+            enqueue_shrink(ad->s_fk, sh, s, prof);
+            gemm(ad->ffn[0]);
+            enqueue_shrink(ad->s_fv, sh, s, prof);
+            gemm(ad->ffn[1]);
+        } else {
+            for (auto& g : ly.ffn) gemm(g);
+        }
         if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
     }
     launch_ln_out(lnout, sh, s, prof);
-    if (sh.MTR > 0) gemm(head, true);
+    if (sh.MTR > 0 && sh.ad) {
+        enqueue_shrink(s_head, sh, s, prof);
+        gemm(ad_head, true);
+    } else if (sh.MTR > 0) {
+        gemm(head, true);
+    }
     if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
 }
 
@@ -1613,7 +1805,7 @@ void b200rwkv_engine::enqueue_keep(cudaStream_t s, int MTR) {
 }
 
 void b200rwkv_engine::run_step(const StepShape& sh) {
-    const int key = sh.MT * 8 + sh.MTR;
+    const int key = sh.MT * 8 + sh.MTR + (sh.ad ? 128 : 0);
     auto it = graphs.find(key);
     if (it == graphs.end()) {
         GraphExec ge = capture_graph(stream, [&] {
@@ -1812,7 +2004,9 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         last_T = T;
         CK(cudaMemcpyAsync(d_meta, hm, meta_ints * 4, cudaMemcpyHostToDevice, stream));
         CK(cudaEventRecord(meta_ev[mb], stream));
-        run_step(step_shape(T, R));
+        StepShape sh = step_shape(T, R);
+        sh.ad = step_bound(s_slots);
+        run_step(sh);
         // step rows [T][C] -> the rows of every token of this call, in entry order
         auto gather_rows = [&](float* dst, const float* src) {
             int t0 = 0;
@@ -2183,7 +2377,8 @@ struct LoraArg { const uint8_t* st; size_t len; float alpha; };
 
 static int32_t create_rank(const uint8_t* st, size_t len, int32_t device, int32_t max_batch, int32_t token_chunk_size,
                            int32_t precision, int32_t rank, int32_t world, const std::vector<LoraArg>& lora, b200rwkv_engine** out,
-                           int32_t quant_layers = 0, int32_t quant_type = 0) {
+                           int32_t quant_layers = 0, int32_t quant_type = 0,
+                           const std::vector<b200rwkv_engine::LoraSrc>& adapters = {}) {
     API_BEGIN((b200rwkv_engine*)nullptr)
     REQUIRE(out, B200RWKV_ERR_INVALID, "null out");
     *out = nullptr;
@@ -2220,8 +2415,11 @@ static int32_t create_rank(const uint8_t* st, size_t len, int32_t device, int32_
     REQUIRE(quant_layers >= 0 && quant_type >= 0, B200RWKV_ERR_INVALID, "bad quant_layers / quant_type");
     e->quant_layers = quant_type == QT_NONE ? 0 : quant_layers;
     e->quant_type = quant_layers == 0 ? (int)QT_NONE : quant_type;
+    e->adapters = adapters;
+    e->n_adapters = (int)adapters.size();
     e->build(f);
-    e->loras.clear();            // the LoRA images are only borrowed during the build
+    e->loras.clear();            // the LoRA and adapter images are only borrowed during the build
+    e->adapters.clear();
     *out = e.release();
     API_END
 }
@@ -2618,7 +2816,8 @@ static int32_t rank_bench_decode(b200rwkv_engine* e, int32_t nslot, const int32_
     std::vector<Event> marks;                  // per-step boundaries (optional): the distribution of the step time
     if (step_ms_out)
         for (int i = 0; i < steps; ++i) marks.push_back(new_event());
-    const StepShape sh = e->step_shape(nslot, nslot);
+    StepShape sh = e->step_shape(nslot, nslot);
+    sh.ad = e->step_bound(std::vector<int>(slot, slot + nslot));
     for (int st = 0; st < nsteps; ++st) {
         if (st == warmup) {
             CK(cudaStreamSynchronize(e->stream));
@@ -2656,7 +2855,9 @@ static int32_t rank_profile_step(b200rwkv_engine* e, int32_t nslot, const int32_
     CK(cudaMemcpyAsync(e->d_meta, all.data(), e->meta_ints * 4, cudaMemcpyHostToDevice, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     Profiler prof;
-    e->enqueue_step(e->stream, e->step_shape(nslot, nslot), &prof);
+    StepShape sh = e->step_shape(nslot, nslot);
+    sh.ad = e->step_bound(std::vector<int>(slot, slot + nslot));      // bound slots: the adapter plans and their shrinks
+    e->enqueue_step(e->stream, sh, &prof);
     CK(cudaStreamSynchronize(e->stream));
     for (int i = 0; i < 4; ++i) { ms[i] = 0.f; launches[i] = 0; }
     for (auto& r : prof.recs) {
@@ -2687,7 +2888,8 @@ static int32_t rank_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int3
     std::vector<int> all;
     build_decode_metas(e, nslot, slot, tokens, 1, all);
     CK(cudaMemcpyAsync(e->d_meta, all.data(), e->meta_ints * 4, cudaMemcpyHostToDevice, e->stream));
-    const StepShape sh = e->step_shape(nslot, nslot);
+    StepShape sh = e->step_shape(nslot, nslot);
+    sh.ad = e->step_bound(std::vector<int>(slot, slot + nslot));
     // traced copy of the step graph (the production graphs carry null trace pointers)
     e->step_trace_types.clear();
     e->step_trace_bytes.clear();
@@ -3739,6 +3941,126 @@ int32_t b200rwkv_create_ex(const uint8_t* st, size_t len, const b200rwkv_options
     lead->group = std::move(g);
     *out = lead;
     return B200RWKV_OK;
+}
+
+// b200rwkv_create_ex with unblended adapters: everything about the files is checked on the host before any CUDA call
+int32_t b200rwkv_create_adapters(const uint8_t* st, size_t len, const b200rwkv_options* opt, int32_t n, const uint8_t* const* adapter_st,
+                                 const size_t* adapter_len, const float* adapter_alpha, b200rwkv_engine** out) {
+    API_BEGIN((b200rwkv_engine*)nullptr)
+    REQUIRE(out && opt, B200RWKV_ERR_INVALID, "null argument");
+    *out = nullptr;
+    REQUIRE(opt->struct_bytes == sizeof(b200rwkv_options), B200RWKV_ERR_INVALID, "b200rwkv_options.struct_bytes does not match this library");
+    REQUIRE(n >= 1 && n <= AD_MAX, B200RWKV_ERR_INVALID, "number of adapters must be 1..8");
+    REQUIRE(adapter_st && adapter_len && adapter_alpha, B200RWKV_ERR_INVALID, "null adapter list");
+    REQUIRE(opt->num_devices <= 1, B200RWKV_ERR_UNSUPPORTED, "adapters run on one GPU (no tensor parallelism)");
+    REQUIRE(opt->num_lora >= 0 && opt->num_lora <= B200RWKV_MAX_LORA, B200RWKV_ERR_INVALID, "bad num_lora");
+    REQUIRE(opt->quant_layers >= 0 && opt->quant_type >= 0, B200RWKV_ERR_INVALID, "bad quant_layers / quant_type");
+    StFile model(st, len);
+    std::vector<std::unique_ptr<StFile>> files;
+    std::vector<b200rwkv_engine::LoraSrc> srcs;
+    for (int a = 0; a < n; ++a) {
+        REQUIRE(adapter_st[a] && adapter_len[a] > 8, B200RWKV_ERR_INVALID, "null adapter image");
+        files.emplace_back(new StFile(adapter_st[a], adapter_len[a]));
+        srcs.push_back({files.back().get(), adapter_alpha[a]});
+    }
+    check_adapter_files(model, srcs, opt->quant_layers, opt->quant_type);
+    std::vector<LoraArg> lora;
+    for (int i = 0; i < opt->num_lora; ++i) lora.push_back({opt->lora_st[i], opt->lora_len[i], opt->lora_alpha[i]});
+    const int dev0 = opt->num_devices <= 0 ? 0 : opt->devices[0];
+    return create_rank(st, len, dev0, opt->max_batch, opt->token_chunk_size, opt->precision, 0, 1, lora, out, opt->quant_layers,
+                       opt->quant_type, srcs);
+    API_END
+}
+
+// Binds slots to adapters for the next infer calls (the infer task's call, like infer itself); every argument is checked
+// before the table is touched
+int32_t b200rwkv_bind_adapter(b200rwkv_engine* e, int32_t nslot, const int32_t* slots, const int32_t* adapter) {
+    API_BEGIN(e)
+    REQUIRE(slots && adapter, B200RWKV_ERR_INVALID, "bind_adapter: null list");
+    REQUIRE(nslot >= 1 && nslot <= 1024, B200RWKV_ERR_INVALID, "bind_adapter: nslot must be in [1, max_batch]");
+    for (int i = 0; i < nslot; ++i) {          // what needs no engine first
+        REQUIRE(slots[i] >= 0, B200RWKV_ERR_STATE, "bind_adapter: slot out of range");
+        REQUIRE(adapter[i] >= 0, B200RWKV_ERR_INVALID, "bind_adapter: unknown adapter id " + std::to_string(adapter[i]));
+        for (int j = 0; j < i; ++j) REQUIRE(slots[j] != slots[i], B200RWKV_ERR_INVALID, "bind_adapter: duplicate slot");
+    }
+    REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
+    REQUIRE(nslot <= e->S, B200RWKV_ERR_INVALID, "bind_adapter: nslot must be in [1, max_batch]");
+    for (int i = 0; i < nslot; ++i) {
+        REQUIRE(slots[i] < e->S, B200RWKV_ERR_STATE, "bind_adapter: slot out of range");
+        REQUIRE(adapter[i] <= e->n_adapters, B200RWKV_ERR_INVALID, "bind_adapter: unknown adapter id " + std::to_string(adapter[i]));
+    }
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (int i = 0; i < nslot; ++i) e->slot_adapter[slots[i]] = adapter[i];
+    if (e->n_adapters) {
+        CK(cudaSetDevice(e->dev));
+        CK(cudaMemcpyAsync(e->d_slot_adapter, e->slot_adapter.data(), (size_t)e->S * 4, cudaMemcpyHostToDevice, e->stream));
+        CK(cudaStreamSynchronize(e->stream));      // the step kernels read the table before griddepcontrol.wait
+    }
+    API_END
+}
+
+// One shrink launch on caller rows: x [T][K] f16 (precision 1: hi rows, then lo rows) packed into an A16 operand of K + 128 n
+// columns, adapter b + 1 = lora_a[b] ([K][rank[b]] f16, as on disk), token t bound to ids[t]; tail <- the n tail blocks,
+// [T][n][128] (precision 1: hi blocks, then lo blocks).  Tail cells start as NaN, so every cell the kernel misses shows.
+int32_t b200rwkv_op_adapter(int32_t device, int32_t T, int32_t K, int32_t precision, int32_t n, const int32_t* rank,
+                            const uint16_t* const* lora_a, const int32_t* ids, const uint16_t* x, uint16_t* tail) {
+    API_BEGIN((b200rwkv_engine*)nullptr)
+    REQUIRE(rank && lora_a && ids && x && tail, B200RWKV_ERR_INVALID, "null argument");
+    REQUIRE(precision == 0 || precision == 1, B200RWKV_ERR_INVALID, "precision must be 0 or 1");
+    REQUIRE(T >= 1 && T <= (precision ? 16 : A16_MAX_ROWS), B200RWKV_ERR_INVALID, "T must be 1..128 (1..16 with precision 1)");
+    REQUIRE(K >= 8 && K % 8 == 0 && K <= 65536, B200RWKV_ERR_INVALID, "K must be a multiple of 8 in 8..65536");
+    REQUIRE(n >= 1 && n <= AD_MAX, B200RWKV_ERR_INVALID, "n must be 1..8");
+    for (int b = 0; b < n; ++b)
+        REQUIRE(lora_a[b] && rank[b] >= 1 && rank[b] <= AD_MAX_RANK, B200RWKV_ERR_INVALID, "adapter matrix null or rank outside 1..128");
+    for (int t = 0; t < T; ++t) REQUIRE(ids[t] >= 0 && ids[t] <= n, B200RWKV_ERR_INVALID, "adapter id outside 0..n");
+    int ndev = 0;
+    REQUIRE(cudaGetDeviceCount(&ndev) == cudaSuccess && device >= 0 && device < ndev, B200RWKV_ERR_CUDA, "no such CUDA device");
+    CK(cudaSetDevice(device));
+    const bool split = precision == 1;
+    const int th = split ? 32 : 16 * mt_bucket(T), kb0 = cdiv(K, GEMM_BK);
+    const size_t halves = (size_t)(kb0 + n) * A16_KB_HALVES;
+    std::vector<uint16_t> op(halves, 0);
+    for (int t = 0; t < T; ++t)
+        for (int k = 0; k < K; ++k) {
+            op[a16_index(t, k, th)] = x[(size_t)t * K + k];
+            if (split) op[a16_index(t + 16, k, th)] = x[((size_t)T + t) * K + k];
+        }
+    for (int t = 0; t < (split ? 32 : T); ++t)
+        for (int k = kb0 * GEMM_BK; k < (kb0 + n) * GEMM_BK; ++k) op[a16_index(t, k, th)] = 0x7E00;
+    const int maxS = A16_MAX_ROWS;
+    std::vector<int> meta(MetaView::ints(A16_MAX_ROWS, maxS), 0);
+    MetaView hv{meta.data(), A16_MAX_ROWS, maxS};
+    meta[0] = T; meta[1] = T;
+    for (int t = 0; t < T; ++t) const_cast<int*>(hv.tok_slot())[t] = t;
+    Buf<uint16_t> d_op(halves * 2);
+    Buf<int> d_meta(meta.size() * 4), d_ids((size_t)T * 4);
+    CK(cudaMemcpy(d_op, op.data(), halves * 2, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_meta, meta.data(), meta.size() * 4, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_ids, ids, (size_t)T * 4, cudaMemcpyHostToDevice));
+    std::vector<Buf<uint16_t>> d_a;
+    AdapterParams P;
+    memset(&P, 0, sizeof(P));
+    P.nproj = 1; P.n = n; P.meta = MetaView{d_meta, A16_MAX_ROWS, maxS}; P.slot_adapter = d_ids; P.th = th;
+    P.p[0].op = reinterpret_cast<__half*>((uint16_t*)d_op);
+    P.p[0].K = K; P.p[0].kb0 = kb0;
+    for (int b = 0; b < n; ++b) {
+        const std::vector<uint16_t> rows = adapter_a_rows(reinterpret_cast<const uint8_t*>(lora_a[b]), K, rank[b]);
+        d_a.emplace_back(rows.size() * 2);
+        CK(cudaMemcpy(d_a.back(), rows.data(), rows.size() * 2, cudaMemcpyHostToDevice));
+        P.p[0].A[b] = reinterpret_cast<const __half*>((uint16_t*)d_a.back());
+        P.p[0].r[b] = rank[b];
+    }
+    if (split) adapter_shrink_kernel<true><<<adapter_grid(T, 1), AD_THREADS>>>(P);
+    else adapter_shrink_kernel<false><<<adapter_grid(T, 1), AD_THREADS>>>(P);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(op.data(), d_op, halves * 2, cudaMemcpyDeviceToHost));
+    for (int h = 0; h < (split ? 2 : 1); ++h)
+        for (int t = 0; t < T; ++t)
+            for (int b = 0; b < n; ++b)
+                for (int j = 0; j < AD_MAX_RANK; ++j)
+                    tail[(((size_t)h * T + t) * n + b) * AD_MAX_RANK + j] = op[a16_index(t + 16 * h, (kb0 + b) * GEMM_BK + j, th)];
+    API_END
 }
 
 const char* b200rwkv_last_error(b200rwkv_engine* e) { (void)e; return g_err.c_str(); }

@@ -226,11 +226,13 @@ class Model:
 
     def __init__(self, st: np.ndarray, max_batch: int = 8, token_chunk_size: int = 128, device: int = 0,
                  precision: int = 0, rank: int = 0, world: int = 1, exact: bool = False, devices=None, lora=None,
-                 quant: int = 0, quant_type: int | str = 0):
+                 quant: int = 0, quant_type: int | str = 0, adapters=None):
         """devices: list of CUDA ordinals -> ONE engine object owning all tensor-parallel ranks (b200rwkv_create_ex);
         lora: list of (st_bytes, alpha) blended at load (reference lib.rs:466-485);
         quant / quant_type: the reload request's fields (lib.rs:211-215): the first `quant` layers in "Int8" or "NF4";
-        rank / world: one process per GPU instead (b200rwkv_create_tp + tp.connect)."""
+        rank / world: one process per GPU instead (b200rwkv_create_tp + tp.connect);
+        adapters: list of (st_bytes, alpha) kept unblended, ids 1..n, chosen per slot with bind_adapter
+        (b200rwkv_create_adapters)."""
         if isinstance(quant_type, str):
             kinds = {"none": capi.QUANT_NONE, "int8": capi.QUANT_INT8, "nf4": capi.QUANT_NF4, "sf4": 3}
             if quant_type.lower() not in kinds:
@@ -242,7 +244,7 @@ class Model:
         st = np.ascontiguousarray(st, dtype=np.uint8)
         h = C.c_void_p()
         L = capi.lib()
-        if devices is not None or lora or quantised:
+        if devices is not None or lora or quantised or adapters:
             if world != 1:
                 raise capi.B200Error(capi.ERR_INVALID, "devices / lora / quant go through b200rwkv_create_ex (in-process ranks)")
             opt = capi.Options()
@@ -259,7 +261,16 @@ class Model:
                 opt.lora_st[i], opt.lora_len[i], opt.lora_alpha[i] = img.ctypes.data, img.size, float(alpha)
             opt.num_lora = len(lora or [])
             opt.quant_layers, opt.quant_type = (int(quant), int(quant_type)) if quantised else (0, 0)
-            capi.check(L.b200rwkv_create_ex(capi.ptr(st), st.size, C.byref(opt), C.byref(h)))
+            if adapters:
+                imgs = [np.ascontiguousarray(img, dtype=np.uint8) for img, _ in adapters]
+                n = len(imgs)
+                ptrs = (C.c_void_p * n)(*[img.ctypes.data for img in imgs])
+                lens = (C.c_size_t * n)(*[img.size for img in imgs])
+                alphas = (C.c_float * n)(*[float(a) for _, a in adapters])
+                capi.check(L.b200rwkv_create_adapters(capi.ptr(st), st.size, C.byref(opt), n, C.cast(ptrs, C.c_void_p),
+                                                      C.cast(lens, C.c_void_p), C.cast(alphas, C.c_void_p), C.byref(h)))
+            else:
+                capi.check(L.b200rwkv_create_ex(capi.ptr(st), st.size, C.byref(opt), C.byref(h)))
             self._lora_keep = []
         else:
             capi.check(L.b200rwkv_create_tp(capi.ptr(st), st.size, device, max_batch, token_chunk_size, precision,
@@ -464,6 +475,15 @@ class Model:
             self.keep_hidden(layers=[])
 
     _POOL_MODES = {"last": capi.POOL_LAST, "mean": capi.POOL_MEAN}
+
+    def bind_adapter(self, slots, ids) -> None:
+        """Slot slots[i] runs adapter ids[i] (1..n of the `adapters` list, 0 = the base model) from the next infer call on
+        (b200rwkv_bind_adapter)."""
+        slots = np.ascontiguousarray(slots, dtype=np.int32)
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        if slots.shape != ids.shape:
+            raise capi.B200Error(capi.ERR_INVALID, "bind_adapter: slots and ids differ in length")
+        capi.check(capi.lib().b200rwkv_bind_adapter(self._h, slots.size, capi.ptr(slots), capi.ptr(ids)), self._h)
 
     def keep_hidden_pooled(self, layers, mode="last") -> None:
         """Reduce the residual stream after each listed layer to one row per entry of every following infer call

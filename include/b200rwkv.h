@@ -107,6 +107,34 @@ typedef struct {
                                       /* Quant::SF4 is not implemented: create_ex answers B200RWKV_ERR_UNSUPPORTED */
 int32_t b200rwkv_create_ex(const uint8_t* st, size_t len, const b200rwkv_options* opt, b200rwkv_engine** out);
 
+/* Several LoRA adapters on one resident base model, chosen per slot at run time (the reference can only blend LoRA files at
+ * load and needs a restart to drop one, docs/doc-guide/features.md).
+ * b200rwkv_create_adapters = b200rwkv_create_ex plus n (1..8) adapter files kept unblended on the device, ids 1..n.  Adapter
+ * files have the load-time LoRA format: `<name>.lora.0` [in, r] and `<name>.lora.1` [out, r], F16, pairs only on
+ * att.{receptance,key,value,gate,output}, ffn.{key,value,receptance} and head; full tensors and unknown targets are
+ * B200RWKV_ERR_UNSUPPORTED, a missing half or a shape that does not match the matrix B200RWKV_ERR_INVALID, a rank above 128
+ * B200RWKV_ERR_UNSUPPORTED.  Also B200RWKV_ERR_UNSUPPORTED: more than one device, and a pair on a matrix of a quantised layer
+ * (opt->quant_layers).  All of this is checked before any CUDA call.  Images are borrowed during the call only.  LoRA files in
+ * `opt` are blended into the base first; adapters apply on top of them.
+ * Meaning: for a token whose slot is bound to adapter a, every projection W with a pair in a computes
+ *   act(x W^T + u B'^T + bias),  u = x A^T (A = lora.0^T) rounded like the operand x (f16, or an f16 hi + lo pair with
+ *   precision 1),  B' = f16(alpha_a * lora.1)
+ * -- the unblended form of create_ex with lora = [(file_a, alpha_a)].
+ * b200rwkv_bind_adapter: slot slots[i] runs adapter[i] (0 = the base model) from the next infer call on.  A binding belongs to
+ * the slot, not to its state: state_load / state_write / snapshots and the kept row neither carry nor clear it (a kept row is
+ * what the slot's last LAST / FULL / SCORE entry computed, under the adapter bound then).  Called by the infer task, like
+ * b200rwkv_infer.  Checked before any CUDA call: nslot outside [1, max_batch], a duplicate slot or an adapter id outside
+ * 0..n is B200RWKV_ERR_INVALID, a slot out of range B200RWKV_ERR_STATE.  On engines from the other constructors only id 0
+ * exists.  Slots bound to different adapters and unbound slots mix freely in one call; a step in which no slot is bound runs
+ * exactly the launches (and gives exactly the bits) of a create_ex engine.
+ * Resident memory: every projection launch an adapter touches is held a second time, with one 128-wide k block per adapter
+ * appended (W' = [W | alpha_1 B_1 | ...]), plus each adapter's A matrices; adapters on every projection kind and the head cost
+ * about the projection weights again (7B: +14.7 GB, + 1.5 GB of tail blocks and 0.7 GB of A for 4 adapters of rank 64). */
+int32_t b200rwkv_create_adapters(const uint8_t* st, size_t len, const b200rwkv_options* opt, int32_t n,
+                                 const uint8_t* const* adapter_st, const size_t* adapter_len, const float* adapter_alpha,
+                                 b200rwkv_engine** out);
+int32_t b200rwkv_bind_adapter(b200rwkv_engine*, int32_t nslot, const int32_t* slots, const int32_t* adapter);
+
 /* Tensor-parallel construction, one process per GPU (head / column parallel, SURVEY.md §8e).
  * (The in-process alternative -- one handle, all ranks inside -- is b200rwkv_create_ex above.)
  * Every rank calls create_tp with the same model, then exchanges the opaque handle blobs
@@ -450,6 +478,15 @@ typedef struct {
     uint16_t* blocks;
 } b200rwkv_weight_args;
 int32_t b200rwkv_op_weight(int32_t device, int32_t kind, const b200rwkv_weight_args* args);
+
+/* Test entry of the adapter shrink kernel (csrc/adapter.cuh), one launch as a step runs it.  x: T token rows of K f16 operand
+ * values ([T][K]; precision 1: [2][T][K], the hi rows then the lo rows), T 1..128 (1..16 with precision 1), K a multiple of 8
+ * up to 65536.  lora_a[b]: adapter b + 1's `.lora.0` [K][rank[b]] f16, rank 1..128; ids[t] in 0..n: token t's adapter.
+ * tail: the n 128-wide tail blocks of the operand after the launch, [T][n][128] f16 (precision 1: [2][T][n][128]): block
+ * ids[t] - 1 of row t holds u = x A^T rounded to the operand format in columns < its rank and zeros above it, every other block
+ * zeros.  Arguments are checked before the first CUDA call (B200RWKV_ERR_INVALID). */
+int32_t b200rwkv_op_adapter(int32_t device, int32_t T, int32_t K, int32_t precision, int32_t n, const int32_t* rank,
+                            const uint16_t* const* lora_a, const int32_t* ids, const uint16_t* x, uint16_t* tail);
 
 /* Kernels launched by this engine's forward steps since creation (graph replays counted by their kernel nodes). */
 int32_t b200rwkv_launch_count(b200rwkv_engine*, int64_t* total);
