@@ -200,6 +200,7 @@ SYMBOLS = [
     ("b200rwkv_state_read", C.c_int32, [_P, C.c_int32, C.POINTER(C.c_uint64)]),
     ("b200rwkv_state_write", C.c_int32, [_P, C.c_int32, C.c_uint64]),
     ("b200rwkv_state_free", C.c_int32, [_P, C.c_uint64]),
+    ("b200rwkv_infer_snapshots", C.c_int32, [_P, C.POINTER(InferArgs), C.c_int32, _P, _P, _P]),
     ("b200rwkv_snapshot_back", C.c_int32, [_P, C.c_uint64, _P, _P]),
     ("b200rwkv_snapshot_load", C.c_int32, [_P, _P, _P, C.POINTER(C.c_uint64)]),
     ("b200rwkv_cache_stats", C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),

@@ -16,6 +16,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <set>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -470,8 +471,10 @@ struct LnPick { int kernel, variant, split; };
 // The launch shape of one step (b200rwkv_engine::step_shape): MT token tiles of 16 rows and MTR row tiles of the head (0: no
 // output rows), `rows` = 16 * MT rows of the per-token buffers, and the token rows th / th_rows of the step's A16 operands and
 // of the head's operand.  `split`: the operands hold hi + lo f16 rows (th = th_rows = 32).  `ad`: a slot of the step is bound
-// to an unblended adapter, so the step runs the adapter plans and their shrink launches.
-struct StepShape { int MT, MTR, rows, th, th_rows; bool split; bool ad = false; };
+// to an unblended adapter, so the step runs the adapter plans and their shrink launches.  `snap`: the step holds snapshots
+// (b200rwkv_infer_snapshots), so its LN stages, WKV and ln_out also write them and it ends with the snapshot rows' head
+// launch over MTX row tiles (0: every snapshot token has an output row already) and their copy into the snapshots.
+struct StepShape { int MT, MTR, rows, th, th_rows; bool split; bool ad = false; bool snap = false; int MTX = 0; };
 
 // The A16 layout (common.cuh) on the host.  a16_halves: halves of one matrix of K columns.  a16_pack / a16_unpack move `ncols`
 // columns of token rows between a caller's dense array and consecutive A16 matrices of K columns and `tr` token rows each (the
@@ -561,6 +564,20 @@ struct b200rwkv_engine {
     std::vector<float> init_state;     // API layout, empty => zeros
     std::map<uint64_t, Snapshot> snaps;
     uint64_t next_snap = 1;
+    // b200rwkv_infer_snapshots, set up on first use (snap_setup).  One device block per snapshot step, uploaded like the
+    // step metadata: [snap_meta_bytes] a copy of the step's metadata whose output rows are the snapshot tokens without one
+    // (R, out_tok, tok_outrow: the rows of snap_head) | [maxT] record of each token row or null | [maxT] logits row the
+    // snapshot row comes from | [maxT] the snapshot's row or null.
+    size_t snap_meta_bytes = 0, snap_bytes = 0;
+    Buf<uint8_t> snap_dev;
+    HostBuf<uint8_t> snap_host;      // [META_RING][snap_bytes]
+    A16Buf a_snap_head;
+    Buf<float> snap_logits;          // [maxT][V]: rows of snap_head
+    GemmLaunch snap_head, snap_ad_head;      // head / ad_head over a_snap_head into snap_logits
+    AdapterParams s_snap_head;
+    float* const* snap_rec_dev() const { return reinterpret_cast<float* const*>(snap_dev.p + snap_meta_bytes); }
+    void snap_setup();
+    struct SnapPlan { int n; const int32_t* entry; const int32_t* tok; uint64_t* ids; };
 
     // activations
     float *x_a = nullptr, *x_b = nullptr, *xx1 = nullptr, *sx1 = nullptr, *xx2 = nullptr;
@@ -628,6 +645,7 @@ struct b200rwkv_engine {
     Buf<uint8_t> sc_dev;
     HostBuf<uint8_t> sc_host;
     void enqueue_keep(cudaStream_t s, int MTR);
+    void enqueue_snap_rows(cudaStream_t s, const StepShape& sh);
     void check_sample_slots(int nrows, const int32_t* slots, const char* who);
     SampleAdjust stage_sample_args(int nrows, const int32_t* slots, const int32_t* pen_off, const uint32_t* pen_tok,
                                    const float* pen_val, const uint32_t* allow_bits, const int32_t* bias_off,
@@ -712,8 +730,9 @@ struct b200rwkv_engine {
                   const std::vector<int>& outmode /*0 none,1 last,2 full*/, int* R_out);
     // score == nullptr: b200rwkv_infer, which refuses OPTION_SCORE
     struct ScoreOut { float* score; uint32_t* argmax; };
+    // snap: b200rwkv_infer_snapshots (null or n == 0: none)
     void infer(int nslot, const int32_t* slot, const int32_t* ntok, const uint32_t* tokens, const int32_t* option,
-               float* logits_out, size_t cap, int32_t* rows_out, const ScoreOut* score = nullptr);
+               float* logits_out, size_t cap, int32_t* rows_out, const ScoreOut* score = nullptr, const SnapPlan* snap = nullptr);
     void state_xform(int slot, bool import, float* snap = nullptr);
 };
 
@@ -1058,6 +1077,18 @@ void b200rwkv_engine::launch_wkv(const WkvParams& p, const StepShape& sh, cudaSt
     const int rows = sh.rows;
     const dim3 grid(wp.H, std::min(S, rows));
     const size_t sm_b = wkv_smem_bytes(wp.version, wp.version == 6 && wp.wd2t, wp.Dd, rows, sh.split);
+    auto go = [&](auto kern) { launch_k(kern, grid, dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); };
+    if (sh.snap) {
+        switch (wp.version * 2 + (sh.split ? 1 : 0)) {
+            case 10: go(wkv_kernel<5, false, true>); break;
+            case 11: go(wkv_kernel<5, true, true>); break;
+            case 12: go(wkv_kernel<6, false, true>); break;
+            case 13: go(wkv_kernel<6, true, true>); break;
+            case 14: go(wkv_kernel<7, false, true>); break;
+            default: go(wkv_kernel<7, true, true>); break;
+        }
+        return;
+    }
     switch (wp.version * 2 + (sh.split ? 1 : 0)) {
         case 10: launch_k(wkv_kernel<5>, grid, dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
         case 11: launch_k(wkv_kernel<5, true>, grid, dim3(WKV_SA_THREADS), sm_b, wp, KC_WKV, s, prof, rows); break;
@@ -1105,6 +1136,12 @@ static void wkv_smem_limits() {
     CK(cudaFuncSetAttribute(wkv_kernel<5, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
     CK(cudaFuncSetAttribute(wkv_kernel<6, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
     CK(cudaFuncSetAttribute(wkv_kernel<7, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
+    CK(cudaFuncSetAttribute(wkv_kernel<5, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
+    CK(cudaFuncSetAttribute(wkv_kernel<6, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
+    CK(cudaFuncSetAttribute(wkv_kernel<7, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
+    CK(cudaFuncSetAttribute(wkv_kernel<5, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
+    CK(cudaFuncSetAttribute(wkv_kernel<6, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
+    CK(cudaFuncSetAttribute(wkv_kernel<7, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wkv_smem_max));
 }
 
 // k-major copy of the time_decay_w2 rows c0 .. c0 + 64 Hl - 1 (w2: [C][Dd] f16 as stored), one contiguous [Dd][64] slice per
@@ -1683,21 +1720,28 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler
         launch_gemm(g2, sh, s, prof, head);
     };
     launch_embed(embed, sh, s, prof);
-    auto ln_stage = [&](const LnMixParams& lp0) {
+    // snapshot steps: offsets of one layer's parts in a snapshot record [L][C | Hl*N*N | C]
+    const size_t W = (size_t)Hl * N * N, rec = 2 * (size_t)C + W;
+    float* const* snap_rec = sh.snap ? snap_rec_dev() : nullptr;
+    auto ln_stage = [&](const LnMixParams& lp0, size_t snap_off) {
         LnMixParams lp = lp0;
         lp.trace = tr_next(0);
+        lp.snap_rec = snap_rec; lp.snap_off = snap_off;
         launch_ln(lp, sh, s, prof);
     };
     for (int l = 0; l < L; ++l) {
         Layer& ly = layers[l];
         AdLayer* ad = sh.ad ? &ad_layers[l] : nullptr;      // a slot of the step is bound: W' plans and their shrinks
+        // LN1 of layer l commits the channel-mix shift of layer l - 1 (layer 0's commits nothing), LN2 the time-mix shift
+        const size_t off_ffn_prev = l > 0 ? (size_t)(l - 1) * rec + C + W : 0, off_att = (size_t)l * rec;
         if (ly.has_pre6 && sh.MT == 1) {
             Pre6Params q = ly.pre6;
             q.ln = ly.ln1;
             q.ln.trace = tr_next(6);
+            q.ln.snap_rec = snap_rec; q.ln.snap_off = off_ffn_prev;
             launch_pre6(q, sh, s, prof);
         } else {
-            ln_stage(ly.ln1);
+            ln_stage(ly.ln1, off_ffn_prev);
             for (auto& g : ly.lora) gemm(g);
         }
         if (ad) enqueue_shrink(ad->s_pre, sh, s, prof);
@@ -1705,12 +1749,13 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler
         {
             WkvParams wp = ly.wkv;
             wp.trace = tr_next(2);
+            wp.snap_rec = snap_rec; wp.snap_off = off_att + C;
             launch_wkv(wp, sh, s, prof);
         }
         if (ad) enqueue_shrink(ad->s_o, sh, s, prof);
         gemm(ad ? ad->o : ly.o);
         if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
-        ln_stage(ly.ln2);
+        ln_stage(ly.ln2, off_att);
         if (ad) {
             enqueue_shrink(ad->s_fk, sh, s, prof);
             gemm(ad->ffn[0]);
@@ -1721,12 +1766,31 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler
         }
         if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
     }
-    launch_ln_out(lnout, sh, s, prof);
+    {
+        LnOutParams lo = lnout;
+        if (sh.snap) {
+            lo.snap_rec = snap_rec; lo.snap_off = (size_t)(L - 1) * rec + C + W;
+            if (sh.MTX > 0) {
+                lo.snap_meta = MetaView{reinterpret_cast<const int*>(snap_dev.p), maxT, S};
+                lo.snap_head_in = a_snap_head.p;
+                lo.snap_kq = sh.split ? 32 : 16 * sh.MTX;
+            }
+        }
+        launch_ln_out(lo, sh, s, prof);
+    }
     if (sh.MTR > 0 && sh.ad) {
         enqueue_shrink(s_head, sh, s, prof);
         gemm(ad_head, true);
     } else if (sh.MTR > 0) {
         gemm(head, true);
+    }
+    if (sh.MTX > 0) {        // the snapshot tokens without an output row: a head launch of their own, the main one unchanged
+        StepShape shx = sh;
+        shx.MTR = sh.MTX;
+        shx.th_rows = sh.split ? 32 : 16 * sh.MTX;
+        if (sh.ad) enqueue_shrink(s_snap_head, shx, s, prof);
+        if (prof) prof->weight_bytes += head.weight_bytes;
+        launch_gemm(sh.ad ? snap_ad_head : snap_head, shx, s, prof, true);
     }
     if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
 }
@@ -1804,13 +1868,23 @@ void b200rwkv_engine::enqueue_keep(cudaStream_t s, int MTR) {
     launch_k(keep_rows_kernel, dim3(MTR * 16, KEEP_CHUNKS), dim3(KEEP_THREADS), 0, kp, KC_OTHER, s, nullptr);
 }
 
+// the logits row of every snapshot token of this step -> its snapshot (the tables b200rwkv_engine::infer uploaded)
+void b200rwkv_engine::enqueue_snap_rows(cudaStream_t s, const StepShape& sh) {
+    SnapRowParams sp;
+    sp.src = reinterpret_cast<const float* const*>(snap_rec_dev() + maxT);
+    sp.dst = snap_rec_dev() + 2 * maxT;
+    sp.V = V;
+    launch_k(snap_rows_kernel, dim3(sh.rows, KEEP_CHUNKS), dim3(KEEP_THREADS), 0, sp, KC_OTHER, s, nullptr);
+}
+
 void b200rwkv_engine::run_step(const StepShape& sh) {
-    const int key = sh.MT * 8 + sh.MTR + (sh.ad ? 128 : 0);
+    const int key = sh.MT * 8 + sh.MTR + (sh.ad ? 128 : 0) + (sh.snap ? 256 * (1 + sh.MTX) : 0);
     auto it = graphs.find(key);
     if (it == graphs.end()) {
         GraphExec ge = capture_graph(stream, [&] {
             enqueue_step(stream, sh, nullptr);
             enqueue_keep(stream, sh.MTR);
+            if (sh.snap) enqueue_snap_rows(stream, sh);
         });
         it = graphs.emplace(key, StepGraph{std::move(ge), launches_last_step}).first;
     }
@@ -1833,6 +1907,46 @@ void b200rwkv_engine::upload_hid_tab() {
     // on the engine's stream and complete before returning: the step kernels read the table before griddepcontrol.wait
     CK(cudaMemcpyAsync(d_hid_tab, tab.data(), tab.size() * sizeof(float*), cudaMemcpyHostToDevice, stream));
     CK(cudaStreamSynchronize(stream));
+}
+
+// The snapshot step block and the snapshot rows' head launches (b200rwkv_infer_snapshots), made on first use: the copies of
+// head / ad_head read a_snap_head and write snap_logits, over the snapshot metadata's R rows, with counters of their own.
+void b200rwkv_engine::snap_setup() {
+    if (snap_dev) return;
+    snap_meta_bytes = (meta_ints * 4 + 15) & ~(size_t)15;
+    snap_bytes = snap_meta_bytes + 3 * (size_t)maxT * sizeof(void*);
+    snap_dev = Buf<uint8_t>(snap_bytes);
+    snap_host = HostBuf<uint8_t>(snap_bytes * META_RING);
+    const int K = n_adapters ? (cdiv(C, GEMM_BK) + n_adapters) * GEMM_BK : C;      // a_head's columns
+    a_snap_head = a16_alloc(K);
+    snap_logits = Buf<float>((size_t)maxT * V * 4);
+    const int* smeta = reinterpret_cast<const int*>(snap_dev.p);
+    auto rebase = [&](const GemmLaunch& g) {
+        GemmLaunch x = g;
+        for (int i = 0; i < x.p.nseg; ++i) {
+            x.p.seg[i].A = a_snap_head.p + (x.p.seg[i].A - a_head.p);
+            x.p.seg[i].out = snap_logits.p + ((float*)x.p.seg[i].out - d_logits);
+        }
+        x.p.nrows = smeta + 2;
+        x.p.counters = (unsigned*)dalloc((size_t)x.total_tiles * 4, true);
+        return x;
+    };
+    snap_head = rebase(head);
+    if (n_adapters) {
+        snap_ad_head = rebase(ad_head);
+        s_snap_head = s_head;
+        s_snap_head.meta = MetaView{smeta, maxT, S};
+        for (int k = 0; k < s_snap_head.nproj; ++k) s_snap_head.p[k].op = a_snap_head.p + (s_head.p[k].op - a_head.p);
+    }
+}
+
+// allocate a snapshot record (+ a logits row when this rank keeps them)
+static Snapshot snapshot_alloc(b200rwkv_engine* e, bool with_logits) {
+    Snapshot sn;
+    const size_t rec = 2 * (size_t)e->C + (size_t)e->Hl * e->N * e->N;
+    sn.buf = Buf<float>(rec * e->L * 4);
+    if (with_logits) sn.logits = Buf<float>((size_t)e->V * 4);
+    return sn;
 }
 
 // fills one step's metadata; returns T
@@ -1869,7 +1983,7 @@ int b200rwkv_engine::fill_meta(int* m, const std::vector<int>& slots, const std:
 }
 
 void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok, const uint32_t* tokens, const int32_t* option,
-                            float* logits_out, size_t cap, int32_t* rows_out, const ScoreOut* score) {
+                            float* logits_out, size_t cap, int32_t* rows_out, const ScoreOut* score, const SnapPlan* snap) {
     REQUIRE(nslot >= 0 && (nslot == 0 || (slot && ntok && option)), B200RWKV_ERR_INVALID, "infer: null argument");
     REQUIRE(connected, B200RWKV_ERR_INVALID, "tensor-parallel engine is not connected (b200rwkv_tp_connect)");
     const int max_option = score ? B200RWKV_OPTION_SCORE : B200RWKV_OPTION_NONE;
@@ -1895,6 +2009,51 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         REQUIRE(tokens[i] < (uint32_t)V, B200RWKV_ERR_INVALID, "infer: token id " + std::to_string(tokens[i]) + " is outside the vocabulary");
     const bool want_logits = (rank == 0);          // tensor parallel: rank 0 gathers all vocabulary shards
     REQUIRE(!want_logits || !logits_out || total_rows * (size_t)V <= cap || total_rows == 0, B200RWKV_ERR_INVALID, "infer: logits buffer too small");
+    // snapshots: every check before any CUDA call, then the records (new ones, or reused ids overwritten in place)
+    const int nsnap = snap ? snap->n : 0;
+    // records of ids 0, and rows for reused ids that had none: entered into `snaps` only once the call has run, so a failed
+    // call leaves no id with a row it never wrote
+    std::vector<Snapshot> snap_new;
+    std::vector<std::pair<uint64_t, Buf<float>>> row_new;
+    struct SnapDst { int tok; float* state; float* row; };
+    std::vector<std::vector<SnapDst>> snap_at(nslot);      // per entry: token index, record, logits row
+    if (snap) {
+        REQUIRE(nsnap >= 0, B200RWKV_ERR_INVALID, "infer_snapshots: negative snapshot count");
+        REQUIRE(nsnap == 0 || (snap->entry && snap->tok && snap->ids), B200RWKV_ERR_INVALID, "infer_snapshots: null argument");
+        REQUIRE(nsnap == 0 || world == 1, B200RWKV_ERR_UNSUPPORTED, "infer_snapshots: snapshots are not supported under tensor parallelism");
+        std::set<std::pair<int, int>> at;
+        std::set<uint64_t> reused;
+        for (int k = 0; k < nsnap; ++k) {
+            const int i = snap->entry[k], p = snap->tok[k];
+            REQUIRE(i >= 0 && i < nslot, B200RWKV_ERR_INVALID, "infer_snapshots: entry index out of range");
+            REQUIRE(p >= 1 && p <= ntok[i], B200RWKV_ERR_INVALID, "infer_snapshots: position outside [1, ntok] of its entry");
+            REQUIRE(at.insert({i, p}).second, B200RWKV_ERR_INVALID, "infer_snapshots: duplicate (entry, position)");
+            const uint64_t id = snap->ids[k];
+            if (id == 0) continue;
+            REQUIRE(reused.insert(id).second, B200RWKV_ERR_INVALID, "infer_snapshots: snapshot id listed twice");
+            REQUIRE(snaps.count(id), B200RWKV_ERR_STATE, "infer_snapshots: unknown snapshot id");
+        }
+    }
+    if (nsnap > 0) {
+        snap_setup();
+        for (int k = 0; k < nsnap; ++k) {
+            float *state, *row;
+            if (snap->ids[k] == 0) {
+                snap_new.push_back(snapshot_alloc(this, true));
+                state = snap_new.back().buf;
+                row = snap_new.back().logits;
+            } else {
+                Snapshot& sn = snaps.at(snap->ids[k]);
+                state = sn.buf;
+                row = sn.logits;
+                if (!row) {
+                    row_new.emplace_back(snap->ids[k], Buf<float>((size_t)V * 4));
+                    row = row_new.back().second;
+                }
+            }
+            snap_at[snap->entry[k]].push_back({snap->tok[k] - 1, state, row});
+        }
+    }
     // logits_out == NULL: the rows stay in HBM (b200rwkv_sample_topk reads the last row of every slot from there)
     const bool copy_logits = want_logits && logits_out != nullptr;
     // f32-activation mode runs every step decode-shaped (<= 16 tokens): the split-operand kernels are the 16-token ones
@@ -2003,9 +2162,49 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         const int T = fill_meta(hm, s_slots, s_counts, s_toks, s_out, &R);
         last_T = T;
         CK(cudaMemcpyAsync(d_meta, hm, meta_ints * 4, cudaMemcpyHostToDevice, stream));
+        // snapshots of this step's tokens: their records, and where their logits rows come from
+        int n_step_snap = 0, X = 0;
+        if (nsnap > 0) {
+            uint8_t* hs = snap_host + (size_t)mb * snap_bytes;
+            int* smeta = reinterpret_cast<int*>(hs);
+            float** rec = reinterpret_cast<float**>(hs + snap_meta_bytes);
+            const float** src = const_cast<const float**>(rec + maxT);
+            float** dst = rec + 2 * maxT;
+            memset(hs + snap_meta_bytes, 0, 3 * (size_t)maxT * sizeof(void*));
+            memcpy(smeta, hm, meta_ints * 4);
+            MetaView sv{smeta, maxT, S};
+            int* s_outrow = const_cast<int*>(sv.tok_outrow());
+            int* s_outtok = const_cast<int*>(sv.out_tok());
+            const int* torow = MetaView{hm, maxT, S}.tok_outrow();
+            for (int t = 0; t < T; ++t) s_outrow[t] = -1;
+            int t0 = 0;
+            for (size_t j = 0; j < s_entry.size(); ++j) {
+                const int i = s_entry[j];
+                for (const SnapDst& a : snap_at[i]) {
+                    if (a.tok < pos[i] || a.tok >= pos[i] + s_counts[j]) continue;
+                    const int t = t0 + (a.tok - pos[i]);
+                    rec[t] = a.state;
+                    dst[t] = a.row;
+                    if (torow[t] >= 0) {
+                        src[t] = d_logits + (size_t)torow[t] * V;
+                    } else {
+                        s_outrow[t] = X;
+                        s_outtok[X] = t;
+                        src[t] = snap_logits + (size_t)X * V;
+                        ++X;
+                    }
+                    ++n_step_snap;
+                }
+                t0 += s_counts[j];
+            }
+            smeta[2] = X;
+            if (n_step_snap > 0) CK(cudaMemcpyAsync(snap_dev, hs, snap_bytes, cudaMemcpyHostToDevice, stream));
+        }
         CK(cudaEventRecord(meta_ev[mb], stream));
         StepShape sh = step_shape(T, R);
         sh.ad = step_bound(s_slots);
+        sh.snap = n_step_snap > 0;
+        sh.MTX = X > 0 ? mt_bucket(X) : 0;
         run_step(sh);
         // step rows [T][C] -> the rows of every token of this call, in entry order
         auto gather_rows = [&](float* dst, const float* src) {
@@ -2107,6 +2306,13 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         memcpy(score->score, sc_host + total_score * sizeof(ScoreRow), total_score * 4);
         if (score->argmax) memcpy(score->argmax, sc_host + total_score * (sizeof(ScoreRow) + 4), total_score * 4);
     }
+    for (int k = 0, n = 0; k < nsnap; ++k)        // new snapshots get their ids once the call has run
+        if (snap->ids[k] == 0) {
+            const uint64_t id = next_snap++;
+            snaps[id] = std::move(snap_new[n++]);
+            snap->ids[k] = id;
+        }
+    for (auto& r : row_new) snaps.at(r.first).logits = std::move(r.second);
     if (hidden_keep) hidden_rows = (int)total_tok;
     hid_last = hid_layers;
     hid_last_rows = total_tok;
@@ -2528,12 +2734,12 @@ int32_t b200rwkv_get_info(b200rwkv_engine* e, b200rwkv_info* out) {
 
 static int32_t rank_infer(b200rwkv_engine* e, int32_t nslot, const int32_t* slot, const int32_t* ntok, const uint32_t* tokens,
                        const int32_t* option, float* logits_out, size_t logits_cap, int32_t* rows_out,
-                       const b200rwkv_engine::ScoreOut* score = nullptr) {
+                       const b200rwkv_engine::ScoreOut* score = nullptr, const b200rwkv_engine::SnapPlan* snap = nullptr) {
     API_BEGIN(e)
     REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
     std::lock_guard<std::mutex> lk(e->mu);
     CK(cudaSetDevice(e->dev));
-    e->infer(nslot, slot, ntok, tokens, option, logits_out, logits_cap, rows_out, score);
+    e->infer(nslot, slot, ntok, tokens, option, logits_out, logits_cap, rows_out, score, snap);
     API_END
 }
 
@@ -2597,14 +2803,6 @@ static void snapshot_copy(b200rwkv_engine* e, int slot, float* buf, bool to_snap
     }
 }
 
-// allocate a snapshot record (+ a logits row when this rank keeps them)
-static Snapshot snapshot_alloc(b200rwkv_engine* e, bool with_logits) {
-    Snapshot sn;
-    const size_t rec = 2 * (size_t)e->C + (size_t)e->Hl * e->N * e->N;
-    sn.buf = Buf<float>(rec * e->L * 4);
-    if (with_logits) sn.logits = Buf<float>((size_t)e->V * 4);
-    return sn;
-}
 
 static int32_t rank_state_read(b200rwkv_engine* e, int32_t slot, uint64_t* snapshot_id) {
     API_BEGIN(e)
@@ -3799,6 +3997,17 @@ int32_t b200rwkv_infer_ex(b200rwkv_engine* e, const b200rwkv_infer_args* a) {
     const b200rwkv_engine::ScoreOut sc{a->score_out, a->argmax_out};
     return RANKS(e, rank_infer(er, a->nslot, a->slot, a->ntok, a->tokens, a->option, r_ == 0 ? a->logits_out : nullptr,
                                r_ == 0 ? a->logits_cap : 0, r_ == 0 ? a->rows_out : nullptr, &sc));
+}
+int32_t b200rwkv_infer_snapshots(b200rwkv_engine* e, const b200rwkv_infer_args* a, int32_t nsnap, const int32_t* snap_entry,
+                                 const int32_t* snap_tokens, uint64_t* snap_ids) {
+    const int32_t st = check_infer_args(a);
+    if (st < 0) return st;
+    // both tensor-parallel front ends go through every rank's b200rwkv_engine::infer, which refuses snapshots (nsnap > 0) on a
+    // rank of a world above 1 after infer_ex's own checks; nsnap == 0 runs as infer_ex
+    const b200rwkv_engine::ScoreOut sc{a->score_out, a->argmax_out};
+    const b200rwkv_engine::SnapPlan sp{nsnap, snap_entry, snap_tokens, snap_ids};
+    return RANKS(e, rank_infer(er, a->nslot, a->slot, a->ntok, a->tokens, a->option, r_ == 0 ? a->logits_out : nullptr,
+                               r_ == 0 ? a->logits_cap : 0, r_ == 0 ? a->rows_out : nullptr, &sc, &sp));
 }
 int32_t b200rwkv_state_load(b200rwkv_engine* e, int32_t slot, const float* in) { return RANKS(e, rank_state_load(er, slot, in)); }
 

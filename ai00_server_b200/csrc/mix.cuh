@@ -50,6 +50,10 @@ struct LnMixParams {
     // holds a [T, C] buffer that receives x_out (the residual stream after layer l) or null.  It changes only between
     // host-synchronous infer calls, so kernels read it before griddepcontrol.wait and the step graphs never change.
     float* const* hid_slot;
+    // steps that hold snapshots (b200rwkv_infer_snapshots), else null: [T] snapshot record of each token row or null.  A
+    // stage that commits a shift row also writes commit_src's row of every snapshot token to record + snap_off.
+    float* const* snap_rec;
+    size_t snap_off;
 };
 
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
@@ -229,6 +233,13 @@ __device__ __forceinline__ void ln_mix_row_nv(const LnMixParams& p, const int t,
     }
 }
 
+// a snapshot step's copy of the shift row this stage commits: row t of `src` -> record + off (no-op for a null record)
+__device__ __forceinline__ void snap_commit_row(float* rec, const size_t off, const float* src, const int t, const int C) {
+    if (!rec) return;
+    for (int c = 4 * (int)threadIdx.x; c < C; c += 4 * LN_THREADS)
+        *reinterpret_cast<float4*>(rec + off + c) = ld4(src + (size_t)t * C + c);
+}
+
 __device__ __forceinline__ void ln_mix_row(const LnMixParams& p, const int t, float* red, float* hid, unsigned long long* stamps = nullptr) {
     const int nv = (p.C + 4 * LN_THREADS - 1) / (4 * LN_THREADS);
     if (nv <= 1) ln_mix_row_nv<1>(p, t, red, hid);
@@ -248,6 +259,7 @@ __global__ void __launch_bounds__(LN_THREADS) ln_mix_kernel(const __grid_constan
     const int t = blockIdx.x;
     if (t >= p.meta.T()) return;
     ln_mix_row(p, t, red, hid);
+    if (p.snap_rec && p.commit_dst) snap_commit_row(p.snap_rec[t], p.snap_off, p.commit_src, t, p.C);
     trace_stamp(p.trace, 7);
 }
 
@@ -331,6 +343,14 @@ struct LnOutParams {
     float* commit_dst;
     const float* commit_src;
     float* hidden_out;      // optional [T, C]: updated residual (hidden states of the embeddings route)
+    // steps that hold snapshots (b200rwkv_infer_snapshots), else null: the shift row of every snapshot token goes to its
+    // record (LnMixParams::snap_rec), and the tokens snap_meta gives an output row also go, normalised, into row
+    // snap_meta.tok_outrow()[t] of snap_head_in (snap_kq token rows): the operand of the snapshot rows' own head launch
+    float* const* snap_rec;
+    size_t snap_off;
+    MetaView snap_meta;
+    __half* snap_head_in;
+    int snap_kq;
 };
 
 template <int NV, bool SPLIT = false>
@@ -339,6 +359,7 @@ __device__ __forceinline__ void ln_out_row_nv(const LnOutParams& p, const int t,
     const int slot = p.meta.tok_slot()[t];
     const bool last = p.meta.tok_last()[t] != 0;
     const int row = p.meta.tok_outrow()[t];
+    const int row2 = p.snap_head_in ? p.snap_meta.tok_outrow()[t] : -1;
     if (last && p.commit_dst) {
 #pragma unroll
         for (int j = 0; j < NV; ++j) {
@@ -346,7 +367,7 @@ __device__ __forceinline__ void ln_out_row_nv(const LnOutParams& p, const int t,
             if (c < C) *reinterpret_cast<float4*>(p.commit_dst + (size_t)slot * C + c) = ld4(p.commit_src + (size_t)t * C + c);
         }
     }
-    if (row < 0 && !p.hidden_out) return;
+    if (row < 0 && row2 < 0 && !p.hidden_out) return;
     const ResidualSrc r = make_residual_src(p);
     float4 a[NV], w[NV], b[NV];
     residual_row<NV>(r, t, a);
@@ -358,26 +379,30 @@ __device__ __forceinline__ void ln_out_row_nv(const LnOutParams& p, const int t,
         b[j] = ok ? ld4(p.ln_b + c) : make_float4(0.f, 0.f, 0.f, 0.f);
         if (ok && p.hidden_out) *reinterpret_cast<float4*>(p.hidden_out + (size_t)t * C + c) = a[j];
     }
-    if (row < 0) return;
+    if (row < 0 && row2 < 0) return;
     float mean, rstd;
     row_stats<NV>(C, a, red, mean, rstd);
+    auto put = [&](__half* dst, const int rw, const int kq, const int c, const float4 y) {
+        if (SPLIT) {       // rows of the head operand are output rows (<= 16 in a decode-shaped step); lo halves in tile 1
+            uint2 hi, lo;
+            split_pack_h2(y.x, y.y, hi.x, lo.x);
+            split_pack_h2(y.z, y.w, hi.y, lo.y);
+            *reinterpret_cast<uint2*>(dst + a16_index(rw, c, kq)) = hi;
+            *reinterpret_cast<uint2*>(dst + a16_index(rw + 16, c, kq)) = lo;
+        } else {
+            uint2 o;
+            o.x = pack_h2(y.x, y.y);
+            o.y = pack_h2(y.z, y.w);
+            *reinterpret_cast<uint2*>(dst + a16_index(rw, c, kq)) = o;
+        }
+    };
 #pragma unroll
     for (int j = 0; j < NV; ++j) {
         const int c = 4 * (threadIdx.x + LN_THREADS * j);
         if (c < C) {
             const float4 y = ln_apply(a[j], mean, rstd, w[j], b[j]);
-            if (SPLIT) {       // rows of the head operand are output rows (<= 16 in a decode-shaped step); lo halves in tile 1
-                uint2 hi, lo;
-                split_pack_h2(y.x, y.y, hi.x, lo.x);
-                split_pack_h2(y.z, y.w, hi.y, lo.y);
-                *reinterpret_cast<uint2*>(p.head_in + a16_index(row, c, p.kq_tile)) = hi;
-                *reinterpret_cast<uint2*>(p.head_in + a16_index(row + 16, c, p.kq_tile)) = lo;
-            } else {
-                uint2 o;
-                o.x = pack_h2(y.x, y.y);
-                o.y = pack_h2(y.z, y.w);
-                *reinterpret_cast<uint2*>(p.head_in + a16_index(row, c, p.kq_tile)) = o;
-            }
+            if (row >= 0) put(p.head_in, row, p.kq_tile, c, y);
+            if (row2 >= 0) put(p.snap_head_in, row2, p.snap_kq, c, y);
         }
     }
 }
@@ -399,6 +424,7 @@ __global__ void __launch_bounds__(LN_THREADS) ln_out_kernel(const __grid_constan
     const int t = blockIdx.x;
     if (t >= p.meta.T()) return;
     ln_out_row<SPLIT>(p, t, red);
+    if (p.snap_rec) snap_commit_row(p.snap_rec[t], p.snap_off, p.commit_src, t, p.C);
 }
 
 }  // namespace b200

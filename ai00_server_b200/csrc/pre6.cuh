@@ -153,6 +153,7 @@ struct PreLnStatic {       // operands of phase 1 that no kernel of this step wr
     float4 mu[NMIX];
     int T, slot, prev_t, last;     // step metadata is uploaded before the step's first launch
     float* hid;                    // hidden-row buffer of this stage (LnMixParams::hid_slot) or null
+    float* snap;                   // snapshot record of this token (LnMixParams::snap_rec) or null
 };
 
 template <int NMIX>
@@ -164,6 +165,7 @@ __device__ __forceinline__ PreLnStatic<NMIX> pre_ln_static(const LnMixParams& p,
     st.prev_t = p.meta.tok_prev()[t];
     st.last = p.meta.tok_last()[t];
     st.hid = p.hid_slot ? *p.hid_slot : nullptr;
+    st.snap = (p.snap_rec && p.commit_dst && t < st.T) ? p.snap_rec[t] : nullptr;
     const bool act = 4 * (int)threadIdx.x < Cs;
     const int c = act ? (int)rank * Cs + 4 * (int)threadIdx.x : 0;
     const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -189,7 +191,8 @@ __device__ __forceinline__ void pre_ln_slice(const LnMixParams& p, const int t, 
     float4 pv = z4, cm = z4;
     if (act && prev_t < 0) pv = ld4(p.shift_state + (size_t)slot * C + c);
     const bool commit = act && last && p.commit_dst;
-    if (commit) cm = ld4(p.commit_src + (size_t)t * C + c);
+    const bool snap = act && st.snap;
+    if (commit || snap) cm = ld4(p.commit_src + (size_t)t * C + c);
     float4 a = act ? residual_vec(r, t, c) : z4;
     if (act && (p.x_out != p.x_in || p.n_parts > 0)) *reinterpret_cast<float4*>(p.x_out + (size_t)t * C + c) = a;
     if (act && st.hid) *reinterpret_cast<float4*>(st.hid + (size_t)t * C + c) = a;
@@ -208,6 +211,7 @@ __device__ __forceinline__ void pre_ln_slice(const LnMixParams& p, const int t, 
     *reinterpret_cast<float4*>(p.xx_out + (size_t)t * C + c) = a;
     if (p.sx_out) *reinterpret_cast<float4*>(p.sx_out + (size_t)t * C + c) = sx;
     if (commit) *reinterpret_cast<float4*>(p.commit_dst + (size_t)slot * C + c) = cm;
+    if (snap) *reinterpret_cast<float4*>(st.snap + p.snap_off + c) = cm;
 #pragma unroll
     for (int m = 0; m < NMIX; ++m) {
         if (m < p.n_mix) {

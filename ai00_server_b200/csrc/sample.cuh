@@ -321,6 +321,33 @@ __global__ void __launch_bounds__(KEEP_THREADS) keep_rows_kernel(const __grid_co
     }
 }
 
+// The logits row of every snapshot token of a step -> its snapshot (b200rwkv_infer_snapshots): src[t] is the step's output
+// row of token t, or its row of the snapshot head launch; dst[t] the snapshot's row, or null.  One engine, all V columns.
+struct SnapRowParams {
+    const float* const* src;    // [rows of the step]
+    float* const* dst;
+    int V;
+};
+
+__global__ void __launch_bounds__(KEEP_THREADS) snap_rows_kernel(const __grid_constant__ SnapRowParams p) {
+    pdl_launch_dependents();
+    const int t = blockIdx.x;
+    const float* s = p.src[t];
+    float* d = p.dst[t];
+    pdl_wait();
+    if (!d) return;
+    const int n4 = p.V >> 2;
+    const int i0 = blockIdx.y * KEEP_THREADS + threadIdx.x;
+    const bool al = ((reinterpret_cast<uintptr_t>(s) | reinterpret_cast<uintptr_t>(d)) & 15) == 0;
+    for (int i = i0; i < n4; i += KEEP_CHUNKS * KEEP_THREADS) {
+        const float4 v = al ? __ldcg(reinterpret_cast<const float4*>(s) + i)
+                            : make_float4(__ldcg(s + 4 * i), __ldcg(s + 4 * i + 1), __ldcg(s + 4 * i + 2), __ldcg(s + 4 * i + 3));
+        if (al) reinterpret_cast<float4*>(d)[i] = v;
+        else { d[4 * i] = v.x; d[4 * i + 1] = v.y; d[4 * i + 2] = v.z; d[4 * i + 3] = v.w; }
+    }
+    if (i0 < (p.V & 3)) d[4 * n4 + i0] = __ldcg(s + 4 * n4 + i0);      // scalar tail
+}
+
 // ---------------------------------------------------------------------------------------
 // Scoring (b200rwkv_infer_ex, B200RWKV_OPTION_SCORE): for each listed row, log softmax(row)[target] and the row's argmax
 // (lowest id on ties, the sample_topk order), so a caller that wants the probability of a known continuation -- the

@@ -59,6 +59,10 @@ struct WkvParams {
     int d1_kq;
     int Dd;
     unsigned long long* trace;  // profiling aid (null in production)
+    // snapshot steps (wkv_kernel<..., SNAP>): [T] snapshot record of each token row or null (b200rwkv_infer_snapshots); the
+    // state after that token goes to record + snap_off + head * 64 * 64, in the layout of `state`
+    float* const* snap_rec;
+    size_t snap_off;
 };
 
 struct WkvShared {
@@ -73,7 +77,7 @@ struct WkvShared {
 // r, k, v, g (, w, a, nu for v7) and `pre_stride` floats between arrays (staged runs: gathered in
 // one batch of loads so the per-token loop never waits on L2).
 // KC: key columns per thread (8: 128 threads per head); the thread's patch is m[e][f] = M[4*ig + e][KC*j4 + f].
-template <int VER, int KC = 8, bool SPLIT = false>
+template <int VER, int KC = 8, bool SPLIT = false, bool SNAP = false>
 __device__ __forceinline__ void wkv_slot(const WkvParams& p, const int h, const int t0, const int nt, float (&m)[4][KC],
                                          WkvShared& sm, const float* w_local, const int lt0, const float* pre = nullptr,
                                          const int pre_stride = 0, const float* statics = nullptr) {
@@ -174,6 +178,18 @@ __device__ __forceinline__ void wkv_slot(const WkvParams& p, const int h, const 
                 o[e] = acc;
             }
         }
+        if (SNAP) {         // the state after token t, for a snapshot of it; the registers go on unchanged
+            float* rec = p.snap_rec[t];
+            if (rec) {
+                float* Ms = rec + p.snap_off + (size_t)h * (WKV_N * WKV_N);
+#pragma unroll
+                for (int e = 0; e < 4; ++e)
+#pragma unroll
+                    for (int q = 0; q < KC / 4; ++q)
+                        __stcs(reinterpret_cast<float4*>(Ms + (ig * 4 + e) * WKV_N + j4 * KC + q * 4),
+                               make_float4(m[e][q * 4], m[e][q * 4 + 1], m[e][q * 4 + 2], m[e][q * 4 + 3]));
+            }
+        }
 #pragma unroll
         for (int off = LANES / 2; off > 0; off >>= 1)
 #pragma unroll
@@ -247,7 +263,8 @@ __host__ __device__ inline size_t wkv_smem_bytes(int ver, bool fold, int Dd, int
 }
 
 // SPLIT (opt-in B200RWKV_SPLIT_ACT=1): the decay-LoRA input and the output are split operands (hi + lo f16 pairs).
-template <int VER, bool SPLIT = false>
+// SNAP: a step that holds snapshots also stores the state after every token that carries one (WkvParams::snap_rec).
+template <int VER, bool SPLIT = false, bool SNAP = false>
 __global__ void __launch_bounds__(WKV_SA_THREADS, 7) wkv_kernel(const __grid_constant__ WkvParams p, const int max_tokens) {
     constexpr int KC = WKV_SA_KC, LANES = WKV_N / KC, NT = WKV_SA_THREADS;
     __shared__ WkvShared sm;
@@ -383,7 +400,7 @@ __global__ void __launch_bounds__(WKV_SA_THREADS, 7) wkv_kernel(const __grid_con
                 fold_token(ds + tt * Dd, tt);
             }
         __syncthreads();
-        wkv_slot<VER, KC, SPLIT>(p, h, t0, nt, m, sm, fold ? wl : nullptr, 0, staged ? pre_s : nullptr, WKV_STAGE_TOK * WKV_N, statics);
+        wkv_slot<VER, KC, SPLIT, SNAP>(p, h, t0, nt, m, sm, fold ? wl : nullptr, 0, staged ? pre_s : nullptr, WKV_STAGE_TOK * WKV_N, statics);
     } else {
         // long run of one slot (prefill chunk): token by token, the decay row of one token at a time
         for (int tt = 0; tt < nt; ++tt) {
@@ -394,7 +411,7 @@ __global__ void __launch_bounds__(WKV_SA_THREADS, 7) wkv_kernel(const __grid_con
             __syncthreads();
             fold_token(ds, 0);
             __syncthreads();
-            wkv_slot<VER, KC, SPLIT>(p, h, t0 + tt, 1, m, sm, wl, 0, nullptr, WKV_STAGE_TOK * WKV_N, statics);
+            wkv_slot<VER, KC, SPLIT, SNAP>(p, h, t0 + tt, 1, m, sm, wl, 0, nullptr, WKV_STAGE_TOK * WKV_N, statics);
         }
     }
 #pragma unroll

@@ -356,6 +356,47 @@ class Model:
                 scores.append(None)
         return rows, scores
 
+    def infer_snapshots(self, slots, ntok, tokens, options, at, reuse=None):
+        """b200rwkv_infer_snapshots: infer_ex(slots, ntok, tokens, options), and one snapshot per (entry, position) of `at`:
+        the state of entry's slot after its first `position` tokens of this call, with that token's logits row.  `reuse`:
+        None, or one TensorGpu / id / None per snapshot; a given one is overwritten in place.  Returns (rows, scores,
+        [TensorGpu]) with rows and scores as infer_ex returns them."""
+        V = self.info["num_vocab"]
+        n = len(slots)
+        total = sum(nt if o == capi.OPTION_FULL else (1 if (o == capi.OPTION_LAST and nt > 0) else 0)
+                    for nt, o in zip(ntok, options))
+        nscore = sum(nt for nt, o in zip(ntok, options) if o == capi.OPTION_SCORE)
+        out = np.empty((max(total, 1), V), np.float32)
+        score = np.empty(max(nscore, 1), np.float32)
+        argmax = np.empty(max(nscore, 1), np.uint32)
+        a_slot, a_ntok = np.asarray(slots, np.int32), np.asarray(ntok, np.int32)
+        a_tok, a_opt = np.asarray(tokens, np.uint32), np.asarray(options, np.int32)
+        a_rows = np.zeros(max(n, 1), np.int32)
+        args = capi.InferArgs(C.sizeof(capi.InferArgs), n, capi.ptr(a_slot).value, capi.ptr(a_ntok).value, capi.ptr(a_tok).value,
+                              capi.ptr(a_opt).value, capi.ptr(out).value, out.size, capi.ptr(a_rows).value, capi.ptr(score).value,
+                              capi.ptr(argmax).value)
+        k = len(at)
+        s_entry = np.asarray([e for e, _ in at] or [0], np.int32)
+        s_tok = np.asarray([p for _, p in at] or [0], np.int32)
+        reuse = list(reuse) if reuse is not None else [None] * k
+        if len(reuse) != k:
+            raise ValueError(f"reuse holds {len(reuse)} entries for {k} snapshots")
+        ids = np.asarray([(r.id if isinstance(r, TensorGpu) else int(r or 0)) for r in reuse] or [0], np.uint64)
+        capi.check(capi.lib().b200rwkv_infer_snapshots(self._h, C.byref(args), k, capi.ptr(s_entry), capi.ptr(s_tok),
+                                                        capi.ptr(ids)), self._h)
+        rows, scores, off, soff = [], [], 0, 0
+        for i in range(n):
+            r = int(a_rows[i])
+            rows.append(out[off:off + r])
+            off += r
+            if options[i] == capi.OPTION_SCORE:
+                scores.append((score[soff:soff + ntok[i]], argmax[soff:soff + ntok[i]]))
+                soff += ntok[i]
+            else:
+                scores.append(None)
+        snaps = [r if isinstance(r, TensorGpu) else TensorGpu(self, int(ids[j])) for j, r in enumerate(reuse)]
+        return rows, scores, snaps
+
     def perplexity(self, slot: int, tokens, head: float | None = None) -> float:
         """The reference's `perplexity()` (run.rs:699-755) on one SCORE call, quirks included: without `head` a token 0 is
         fed first (its own score is not used) and the sum is divided by len(tokens) + 1; with `head` (the probability of

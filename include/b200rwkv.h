@@ -220,6 +220,32 @@ int32_t b200rwkv_state_read(b200rwkv_engine*, int32_t slot, uint64_t* snapshot_i
 int32_t b200rwkv_state_write(b200rwkv_engine*, int32_t slot, uint64_t snapshot_id);  /* State::write */
 int32_t b200rwkv_state_free(b200rwkv_engine*, uint64_t snapshot_id);                 /* drop TensorGpu */
 
+/* b200rwkv_infer_ex(args), and also snapshot k of the state of entry snap_entry[k]'s slot after the first snap_tokens[k]
+ * tokens that entry feeds in this call (1 <= snap_tokens[k] <= ntok[entry]): what b200rwkv_state_read would have returned
+ * had the call ended there, for a prefix-cache item at a shared boundary or a rollback after verifying several tokens.
+ *  - A snapshot always carries the logits row of its token (the row predicting the next token), whatever the entry's
+ *    option.  It is bit-identical to that token's logits_out row (FULL), the row its SCORE entry scored against, or, at a
+ *    LAST entry's last token, the slot's kept row.  Other rows come from a head launch of their own.
+ *  - snap_ids[k] is in / out: 0 asks for a new snapshot, whose id is written back; an existing id is overwritten in place,
+ *    state and row, with no new state allocation (an id that had no row gains one).
+ *  - Every other output is bit-identical to the same infer_ex call: logits_out, rows_out, scores, argmax ids, the slots'
+ *    states, kept rows and recorded or pooled hidden rows.  Snapshot rows never reach logits_out or a kept row.  With
+ *    nsnap == 0 the call launches exactly what infer_ex launches.
+ *  - The step packing is infer_ex's.  A step that holds snapshots runs the same launches with their snapshot variants
+ *    (the LN stages, WKV and ln_out also write the snapshot tokens' state), plus 1 row copy launch, plus, when one of its
+ *    snapshot tokens has no output row (mid-run LAST / NONE, or NONE at the end), 1 head launch over those tokens (and 1
+ *    adapter shrink launch in front of it when a slot of the step is bound to an adapter and any adapter of the engine has a
+ *    pair on the head: the shrink the step's main head launch runs as well).  A
+ *    snapshot does not carry an adapter binding, as with state_read.
+ *  - Bytes per snapshot: L * (2C + H * 64 * 64) * 4 of state plus num_vocab * 4 of logits row: 34.6 MB of state at the 7B
+ *    shape, 21.6 MB at 3B / v7-2b9.
+ *  - Refused before any CUDA call, with nothing changed: everything infer_ex refuses; B200RWKV_ERR_INVALID for nsnap < 0,
+ *    NULL arrays with nsnap > 0, an entry index outside [0, nslot), a position outside [1, ntok], a duplicate (entry,
+ *    position) or one nonzero id listed twice; B200RWKV_ERR_STATE for an unknown nonzero id; B200RWKV_ERR_UNSUPPORTED
+ *    for nsnap > 0 under tensor parallelism (either front end; nsnap == 0 runs as infer_ex there too). */
+int32_t b200rwkv_infer_snapshots(b200rwkv_engine*, const b200rwkv_infer_args* args, int32_t nsnap, const int32_t* snap_entry,
+                                 const int32_t* snap_tokens, uint64_t* snap_ids);
+
 /* Device-resident state cache (SURVEY.md §8f-4).  The reference's cache holds `CachedItem { state: TensorCpu, output:
  * TensorCpu }` (crates/ai00-core/src/run.rs:199-205): every check-out / check-in is a State::load / State::back PCIe copy of
  * the whole state (34.6 MB per slot at 7B; run.rs:838, 996, 561).  Here a cached item is a snapshot id: state_read /
