@@ -44,6 +44,13 @@ class Options(C.Structure):
 
 QUANT_NONE, QUANT_INT8, QUANT_NF4 = 0, 1, 2
 
+# B200RWKV_TARGET_*: the kinds of matrix the places of b200rwkv_create_adapter_places can hold pairs on
+TARGET_ATT_R, TARGET_ATT_K, TARGET_ATT_V, TARGET_ATT_G = 1 << 0, 1 << 1, 1 << 2, 1 << 3
+TARGET_ATT_O, TARGET_FFN_K, TARGET_FFN_V, TARGET_FFN_R, TARGET_HEAD = 1 << 4, 1 << 5, 1 << 6, 1 << 7, 1 << 8
+TARGETS = {"att.receptance": TARGET_ATT_R, "att.key": TARGET_ATT_K, "att.value": TARGET_ATT_V, "att.gate": TARGET_ATT_G,
+           "att.output": TARGET_ATT_O, "ffn.key": TARGET_FFN_K, "ffn.value": TARGET_FFN_V, "ffn.receptance": TARGET_FFN_R,
+           "head": TARGET_HEAD}
+
 
 class GemmSeg(C.Structure):
     """b200rwkv_gemm_seg (include/b200rwkv.h)."""
@@ -185,6 +192,9 @@ SYMBOLS = [
     ("b200rwkv_create_ex", C.c_int32, [_P, C.c_size_t, C.POINTER(Options), C.POINTER(_P)]),
     ("b200rwkv_create_adapters", C.c_int32, [_P, C.c_size_t, C.POINTER(Options), C.c_int32, _P, _P, _P, C.POINTER(_P)]),
     ("b200rwkv_bind_adapter", C.c_int32, [_P, C.c_int32, _P, _P]),
+    ("b200rwkv_create_adapter_places", C.c_int32, [_P, C.c_size_t, C.POINTER(Options), C.c_int32, C.c_uint32, C.POINTER(_P)]),
+    ("b200rwkv_load_adapter", C.c_int32, [_P, C.c_int32, _P, C.c_size_t, C.c_float]),
+    ("b200rwkv_unload_adapter", C.c_int32, [_P, C.c_int32]),
     ("b200rwkv_create_tp", C.c_int32, [_P, C.c_size_t, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(_P)]),
     ("b200rwkv_tp_export", C.c_int32, [_P, _P]),
     ("b200rwkv_tp_connect", C.c_int32, [_P, _P]),

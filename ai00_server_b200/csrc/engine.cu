@@ -662,14 +662,38 @@ struct b200rwkv_engine {
     // LoRA files blended into the projection weights while they are uploaded (borrowed during build only)
     struct LoraSrc { const StFile* st; float alpha; };
     std::vector<LoraSrc> loras;
-    // unblended adapters (b200rwkv_create_adapters): files borrowed during build only, plans and A matrices kept
+    // unblended adapters (b200rwkv_create_adapters, b200rwkv_create_adapter_places): files borrowed during build only, plans
+    // and A matrices kept.  n_adapters places, ids 1..n; `ad_targets`: the kinds of matrix a places engine plans (0: the
+    // matrices the files pair)
     std::vector<LoraSrc> adapters;
     int n_adapters = 0;
+    uint32_t ad_targets = 0;
     std::vector<AdLayer> ad_layers;
     GemmLaunch ad_head;
     AdapterParams s_head;
     int* d_slot_adapter = nullptr;           // [S] adapter bound to each slot, 0 = the base model
     std::vector<int> slot_adapter;           // host copy (the infer task's)
+    // What b200rwkv_load_adapter / unload_adapter write, per matrix with a W' plan: its W' segment (`tiles` rows of KB weight
+    // blocks; place b's tail block is block kbw + b - 1 of each row), its entry `proj` of the shrink launch `sp`, and each
+    // place's A rows ([128][K] f16, reserved at creation)
+    struct AdMatrix {
+        std::string name;                    // "blocks.<l>.<kind>" or "head"
+        int N, K;
+        uint8_t* W;
+        int tiles, KB, kbw;
+        AdapterParams* sp;
+        int proj;
+        __half* A[AD_MAX];
+    };
+    std::vector<AdMatrix> ad_mats;
+    std::vector<char> place_full;            // [n_adapters]: the place holds an adapter (bind_adapter refuses an empty one)
+    std::map<std::string, StTensor> model_shapes;     // the model's tensor names and shapes, for load_adapter's file checks
+    uint8_t* ad_stage = nullptr;             // load_adapter's staging: [N][128] f16 tail columns | their repacked blocks
+    size_t ad_stage_cols = 0;                // bytes of the first part
+    void set_place_rank(const AdMatrix& m, int id, int r);
+    void load_place(int id, const StFile& f, float alpha);
+    void unload_place(int id);
+    void drop_adapter_graphs();
     bool step_bound(const std::vector<int>& slots) const {
         for (int s : slots)
             if (n_adapters && s >= 0 && s < S && slot_adapter[s]) return true;
@@ -765,35 +789,67 @@ static bool ends_with(const std::string& s, const std::string& suf) {
     return s.size() >= suf.size() && s.compare(s.size() - suf.size(), suf.size(), suf) == 0;
 }
 
+// The projection kinds a LoRA pair may address; bit i of a B200RWKV_TARGET_* mask is kind i, B200RWKV_TARGET_HEAD the head.
+static const char* const LORA_KINDS[] = {".att.receptance", ".att.key", ".att.value", ".att.gate", ".att.output", ".ffn.key",
+                                         ".ffn.value", ".ffn.receptance"};
+static const uint32_t AD_TARGET_ALL = (1u << 9) - 1;
+static uint32_t ad_target_bit(const std::string& base) {
+    if (base == "head") return B200RWKV_TARGET_HEAD;
+    for (int i = 0; i < 8; ++i)
+        if (ends_with(base, LORA_KINDS[i])) return 1u << i;
+    return 0;
+}
+// the matrix `base` sits in one of the first `quant_layers` layers, which hold quantised projection matrices
+static bool in_quant_layer(const std::string& base, int quant_layers, int quant_type) {
+    const int layer = base.compare(0, 7, "blocks.") == 0 ? atoi(base.c_str() + 7) : -1;
+    return quant_type != QT_NONE && layer >= 0 && layer < quant_layers;
+}
+// Matrices an engine from b200rwkv_create_adapter_places plans a W' for: every 2-D `<base>.weight` of the model of a targeted
+// kind outside the quantised layers.
+static std::vector<std::string> ad_place_matrices(const std::map<std::string, StTensor>& model, uint32_t targets,
+                                                  int quant_layers, int quant_type) {
+    std::vector<std::string> out;
+    for (auto& kv : model) {
+        if (!ends_with(kv.first, ".weight") || kv.second.shape.size() != 2) continue;
+        const std::string base = kv.first.substr(0, kv.first.size() - 7);
+        if ((ad_target_bit(base) & targets) && !in_quant_layer(base, quant_layers, quant_type)) out.push_back(base);
+    }
+    return out;
+}
+static const StTensor* st_find(const std::map<std::string, StTensor>& m, const std::string& name) {
+    auto it = m.find(name);
+    return it == m.end() ? nullptr : &it->second;
+}
+
 // Every `<base>.lora.0/.lora.1` pair of a LoRA file must address a projection matrix this engine blends (the matrices that
-// go through upload_tmp); anything else is refused loudly rather than ignored.
-static void check_lora_files(const StFile& model, const std::vector<b200rwkv_engine::LoraSrc>& files) {
-    static const char* ok[] = {".att.receptance", ".att.key", ".att.value", ".att.gate", ".att.output", ".ffn.key", ".ffn.value", ".ffn.receptance"};
+// go through upload_tmp); anything else is refused loudly rather than ignored.  `model`: the model's tensors (names and shapes
+// are what is read).
+static void check_lora_files(const std::map<std::string, StTensor>& model, const std::vector<b200rwkv_engine::LoraSrc>& files) {
     for (const b200rwkv_engine::LoraSrc& lo : files) {
         int pairs = 0;
         for (auto& kv : lo.st->tensors) {
             const std::string& n = kv.first;
             if (ends_with(n, ".lora.1")) continue;
             if (!ends_with(n, ".lora.0")) {
-                REQUIRE(!model.find(n), B200RWKV_ERR_UNSUPPORTED, "LoRA file carries a full tensor (" + n + "): only low-rank pairs on projection matrices are blended");
+                REQUIRE(!st_find(model, n), B200RWKV_ERR_UNSUPPORTED, "LoRA file carries a full tensor (" + n + "): only low-rank pairs on projection matrices are blended");
                 continue;
             }
             const std::string base = n.substr(0, n.size() - 7);
-            bool good = (base == "head");
-            for (const char* o : ok) good = good || ends_with(base, o);
-            REQUIRE(good && model.find(base + ".weight"), B200RWKV_ERR_UNSUPPORTED, "LoRA on " + base + " is not supported (projection matrices only)");
+            const bool good = ad_target_bit(base) != 0;
+            REQUIRE(good && st_find(model, base + ".weight"), B200RWKV_ERR_UNSUPPORTED, "LoRA on " + base + " is not supported (projection matrices only)");
             REQUIRE(lo.st->find(base + ".lora.1"), B200RWKV_ERR_INVALID, "LoRA file: " + base + ".lora.1 is missing");
             ++pairs;
         }
         REQUIRE(pairs > 0, B200RWKV_ERR_INVALID, "LoRA file holds no <name>.lora.0 / <name>.lora.1 pairs");
     }
 }
-void b200rwkv_engine::check_loras(const StFile& model) const { check_lora_files(model, loras); }
+void b200rwkv_engine::check_loras(const StFile& model) const { check_lora_files(model.tensors, loras); }
 
-// Adapter files (b200rwkv_create_adapters), host only: the load-time blend's refusals, then every pair's halves, dtypes and
-// shapes against the model, the rank (one 128-wide k block of W'), and no pair on a matrix of a quantised layer.
-static void check_adapter_files(const StFile& model, const std::vector<b200rwkv_engine::LoraSrc>& files, int quant_layers,
-                                int quant_type) {
+// Adapter files (b200rwkv_create_adapters, b200rwkv_load_adapter), host only: the load-time blend's refusals, then every
+// pair's halves, dtypes and shapes against the model, the rank (one 128-wide k block of W'), and no pair on a matrix of a
+// quantised layer.
+static void check_adapter_files(const std::map<std::string, StTensor>& model, const std::vector<b200rwkv_engine::LoraSrc>& files,
+                                int quant_layers, int quant_type) {
     check_lora_files(model, files);
     for (const b200rwkv_engine::LoraSrc& lo : files)
         for (auto& kv : lo.st->tensors) {
@@ -804,7 +860,7 @@ static void check_adapter_files(const StFile& model, const std::vector<b200rwkv_
             const StTensor* b = lo.st->find(base + ".lora.1");
             REQUIRE(a && b, B200RWKV_ERR_INVALID, "adapter file: " + base + " has only one of .lora.0 / .lora.1");
             if (n != base + ".lora.0") continue;
-            const StTensor* w = model.find(base + ".weight");
+            const StTensor* w = st_find(model, base + ".weight");
             REQUIRE(w && w->shape.size() == 2, B200RWKV_ERR_UNSUPPORTED, "adapter on " + base + " is not supported (projection matrices only)");
             REQUIRE(a->dtype == "F16" && b->dtype == "F16", B200RWKV_ERR_UNSUPPORTED, "adapter tensors must be F16: " + base);
             REQUIRE(a->shape.size() == 2 && b->shape.size() == 2 && b->shape[0] == w->shape[0] && a->shape[0] == w->shape[1] &&
@@ -813,8 +869,7 @@ static void check_adapter_files(const StFile& model, const std::vector<b200rwkv_
             REQUIRE(a->shape[1] <= AD_MAX_RANK, B200RWKV_ERR_UNSUPPORTED,
                     "adapter rank " + std::to_string(a->shape[1]) + " on " + base + " is above 128");
             REQUIRE(a->shape[0] % 8 == 0, B200RWKV_ERR_UNSUPPORTED, "adapter on " + base + ": input width must be a multiple of 8");
-            const int layer = base.compare(0, 7, "blocks.") == 0 ? atoi(base.c_str() + 7) : -1;
-            REQUIRE(quant_type == QT_NONE || layer < 0 || layer >= quant_layers, B200RWKV_ERR_UNSUPPORTED,
+            REQUIRE(!in_quant_layer(base, quant_layers, quant_type), B200RWKV_ERR_UNSUPPORTED,
                     "adapter on " + base + ": its layer is quantised (adapters need f16 projection matrices)");
         }
 }
@@ -833,11 +888,12 @@ static void launch_decay_table(const __half* src, float* dst, int n) {
     CK(cudaGetLastError());
 }
 // rows [n0, n0 + N) and columns [k0, k0 + K) of src [.][ld] into ceil(N / 128) x ceil(K / 128) stage blocks at dst
-static void launch_repack(int num_sms, const __half* src, int ld, int n0, int k0, int N, int K, uint4* dst) {
+static void launch_repack(int num_sms, const __half* src, int ld, int n0, int k0, int N, int K, uint4* dst,
+                          cudaStream_t s = 0) {
     const int tiles = cdiv(N, GEMM_BN), KB = cdiv(K, GEMM_BK);
     const size_t nchunk = (size_t)tiles * KB * (GEMM_WBYTES / 16);
     const int grid = (int)std::min<size_t>((nchunk + 255) / 256, (size_t)num_sms * 16);
-    repack_weight_kernel<<<grid, 256>>>(src, ld, n0, k0, N, K, tiles, KB, dst);
+    repack_weight_kernel<<<grid, 256, 0, s>>>(src, ld, n0, k0, N, K, tiles, KB, dst);
     CK(cudaGetLastError());
 }
 
@@ -954,7 +1010,7 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
             CK(cudaMemcpy2D(E, (size_t)ke * 2, src + (size_t)d.n0 * ld + d.k0, (size_t)ld * 2, (size_t)d.K * 2, d.N,
                             cudaMemcpyDeviceToDevice));
             const std::string base = t.name.substr(0, t.name.size() - 7);
-            for (int a = 0; a < d.ad_tail; ++a) {
+            for (int a = 0; a < (int)adapters.size(); ++a) {      // adapter places are created empty
                 const StTensor* b = adapters[a].st->find(base + ".lora.1");
                 if (!b) continue;
                 const int r = (int)b->shape[1];
@@ -1583,6 +1639,23 @@ void b200rwkv_engine::build(const StFile& st) {
         shrink(s_head, true);
         ad_head = ad_launch(head, s_head);
         ad_head.p.nrows = d_meta + 2;
+        if (ad_targets)
+            REQUIRE(ad_mats.size() == ad_place_matrices(st.tensors, ad_targets, quant_layers, quant_type).size(),
+                    B200RWKV_ERR_INVALID, "internal: a targeted matrix has no W' plan");
+        // load_adapter's staging, and the model's tensor shapes its file checks read
+        size_t cols = 0, blocks = 0;
+        for (const AdMatrix& m : ad_mats) {
+            cols = std::max(cols, (size_t)m.N * GEMM_BK * 2);
+            blocks = std::max(blocks, (size_t)m.tiles * GEMM_WBYTES);
+        }
+        ad_stage_cols = cols;
+        ad_stage = (uint8_t*)dalloc(cols + blocks, false);
+        for (auto& kv : st.tensors) {
+            StTensor t = kv.second;
+            t.data = nullptr;
+            model_shapes.emplace(kv.first, std::move(t));
+        }
+        place_full.assign(n_adapters, adapters.empty() ? 0 : 1);
     }
     gemm_ws = (float*)dalloc(gemm_ws_floats * 4, false);
     auto wire = [&](GemmLaunch& g) {
@@ -1657,40 +1730,112 @@ static std::vector<uint16_t> adapter_a_rows(const uint8_t* lora0, int K, int r) 
     return rows;
 }
 
-// The W' plan of `base` (one tail k block per adapter on each segment that holds a whole adapted projection, or the last
-// split-K slice of one), with the projection added to the shrink launch `sp`; `base` itself when no adapter touches it.
+// The W' plan of `base` (one tail k block per adapter place on each segment that holds a whole planned projection, or the
+// last split-K slice of one), with the projection added to the shrink launch `sp` and to ad_mats; `base` itself when no
+// projection of it is planned.  Planned: a matrix some adapter file pairs, or on a places engine a targeted one (every
+// place's A rows are reserved at the rank limit, so a later load_adapter allocates nothing).
 GemmLaunch b200rwkv_engine::ad_launch(const GemmLaunch& base, AdapterParams& sp) {
     std::vector<SegDesc> segs = base.src;
-    bool any = false;
-    for (SegDesc& d : segs) {
+    std::vector<AdMatrix> mats;
+    std::vector<int> mat_seg;
+    for (size_t i = 0; i < segs.size(); ++i) {
+        SegDesc& d = segs[i];
         const StTensor& t = *d.t;
         if (d.slice >= 0 || !ends_with(t.name, ".weight") || t.shape.size() != 2 || d.k0 + d.K != t.shape[1]) continue;
         const std::string nm = t.name.substr(0, t.name.size() - 7);
+        bool planned = (ad_target_bit(nm) & ad_targets) && !in_quant_layer(nm, quant_layers, quant_type);
+        for (const LoraSrc& a : adapters) planned = planned || a.st->find(nm + ".lora.0");
+        if (!planned) continue;
+        REQUIRE(base.qtype == QT_NONE && world == 1 && d.k0 % GEMM_BK == 0 && sp.nproj < AD_MAX_PROJ, B200RWKV_ERR_INVALID,
+                "internal: adapter on " + nm + " does not fit its launch");
         AdapterProj pj;
         memset(&pj, 0, sizeof(pj));
         pj.K = (int)t.shape[1];
+        AdMatrix m{nm, d.N, pj.K, nullptr, 0, 0, 0, &sp, sp.nproj, {}};
         for (int a = 0; a < n_adapters; ++a) {
-            const StTensor* la = adapters[a].st->find(nm + ".lora.0");
-            if (!la) continue;
+            m.A[a] = (__half*)dalloc((size_t)AD_MAX_RANK * pj.K * 2, true);
+            pj.A[a] = m.A[a];
+            const StTensor* la = a < (int)adapters.size() ? adapters[a].st->find(nm + ".lora.0") : nullptr;
+            if (!la) continue;          // rank 0: the shrink writes zeros into this place's tail block
             pj.r[a] = (int)la->shape[1];
             const std::vector<uint16_t> rows = adapter_a_rows(la->data, pj.K, pj.r[a]);
-            __half* dA = (__half*)dalloc(rows.size() * 2, false);
-            CK(cudaMemcpy(dA, rows.data(), rows.size() * 2, cudaMemcpyHostToDevice));
-            pj.A[a] = dA;
+            CK(cudaMemcpy(m.A[a], rows.data(), rows.size() * 2, cudaMemcpyHostToDevice));
         }
-        bool has = false;
-        for (int a = 0; a < n_adapters; ++a) has = has || pj.A[a];
-        if (!has) continue;
-        REQUIRE(base.qtype == QT_NONE && world == 1 && d.k0 % GEMM_BK == 0 && sp.nproj < AD_MAX_PROJ, B200RWKV_ERR_INVALID,
-                "internal: adapter on " + nm + " does not fit its launch");
         pj.op = const_cast<__half*>(d.proto.A) - (size_t)(d.k0 / GEMM_BK) * A16_KB_HALVES;
         pj.kb0 = cdiv(pj.K, GEMM_BK);
         sp.p[sp.nproj++] = pj;
         d.ad_tail = n_adapters;
-        any = true;
+        mats.push_back(m);
+        mat_seg.push_back((int)i);
     }
-    if (!any) return base;
-    return make_launch(segs, base.force_grid, QT_NONE);
+    if (mats.empty()) return base;
+    GemmLaunch g = make_launch(segs, base.force_grid, QT_NONE);
+    for (size_t j = 0; j < mats.size(); ++j) {
+        const GemmSeg& sg = g.p.seg[mat_seg[j]];
+        mats[j].W = (uint8_t*)g.p.W + (size_t)sg.blk_begin * GEMM_WBYTES;
+        mats[j].tiles = sg.tiles;
+        mats[j].KB = sg.KB;
+        mats[j].kbw = sg.KB - n_adapters;
+        ad_mats.push_back(mats[j]);
+    }
+    return g;
+}
+
+// Place `id`'s rank on one matrix, in the shrink launch that holds it (and its copy for the snapshot rows' head launch).
+// Ranks are launch parameters: the caller drops the captured adapter step graphs.
+void b200rwkv_engine::set_place_rank(const AdMatrix& m, int id, int r) {
+    m.sp->p[m.proj].r[id - 1] = r;
+    if (m.sp == &s_head && snap_dev) s_snap_head.p[m.proj].r[id - 1] = r;
+}
+
+// The step graphs captured with the adapter plans (key bit 128, snapshot variants included) hold the shrink parameters as
+// they were; unbound steps keep theirs.
+void b200rwkv_engine::drop_adapter_graphs() {
+    for (auto it = graphs.begin(); it != graphs.end();) it = (it->first & 128) ? graphs.erase(it) : std::next(it);
+}
+
+// b200rwkv_load_adapter after its checks: into every planned matrix the file pairs, place `id`'s tail block of W' =
+// f16(alpha lora.1) with zeros past the rank (make_launch's rounding, re-tiled by the load-time repack kernel), its A rows
+// and its rank.  The place is empty, so the other matrices already hold zeros and rank 0.  Everything goes on the engine's
+// stream (steps already enqueued finish with the old contents) and is complete on return.
+void b200rwkv_engine::load_place(int id, const StFile& f, float alpha) {
+    CK(cudaSetDevice(dev));
+    __half* cols = reinterpret_cast<__half*>(ad_stage);
+    uint4* blocks = reinterpret_cast<uint4*>(ad_stage + ad_stage_cols);
+    for (const AdMatrix& m : ad_mats) {
+        const StTensor* la = f.find(m.name + ".lora.0");
+        if (!la) continue;
+        const StTensor* lb = f.find(m.name + ".lora.1");
+        const int r = (int)la->shape[1];
+        const __half* b = reinterpret_cast<const __half*>(lb->data);
+        std::vector<__half> e((size_t)m.N * GEMM_BK, __float2half_rn(0.f));
+        for (int n = 0; n < m.N; ++n)
+            for (int j = 0; j < r; ++j) e[(size_t)n * GEMM_BK + j] = __float2half_rn(alpha * __half2float(b[(size_t)n * r + j]));
+        CK(cudaMemcpyAsync(cols, e.data(), e.size() * 2, cudaMemcpyHostToDevice, stream));
+        launch_repack(num_sms, cols, GEMM_BK, 0, 0, m.N, GEMM_BK, blocks, stream);
+        CK(cudaMemcpy2DAsync(m.W + (size_t)(m.kbw + id - 1) * GEMM_WBYTES, (size_t)m.KB * GEMM_WBYTES, blocks, GEMM_WBYTES,
+                             GEMM_WBYTES, m.tiles, cudaMemcpyDeviceToDevice, stream));
+        const std::vector<uint16_t> rows = adapter_a_rows(la->data, m.K, r);
+        CK(cudaMemcpyAsync(m.A[id - 1], rows.data(), rows.size() * 2, cudaMemcpyHostToDevice, stream));
+        set_place_rank(m, id, r);
+    }
+    CK(cudaStreamSynchronize(stream));
+    place_full[id - 1] = 1;
+    drop_adapter_graphs();
+}
+
+// b200rwkv_unload_adapter after its checks: zeros over place `id`'s tail block of every planned matrix, and rank 0 (the shrink
+// then writes zeros into that tail block of the operand and reads none of the place's A rows).
+void b200rwkv_engine::unload_place(int id) {
+    CK(cudaSetDevice(dev));
+    for (const AdMatrix& m : ad_mats) {
+        CK(cudaMemset2DAsync(m.W + (size_t)(m.kbw + id - 1) * GEMM_WBYTES, (size_t)m.KB * GEMM_WBYTES, 0, GEMM_WBYTES, m.tiles,
+                             stream));
+        set_place_rank(m, id, 0);
+    }
+    CK(cudaStreamSynchronize(stream));
+    place_full[id - 1] = 0;
+    drop_adapter_graphs();
 }
 
 // the shrink launch of one step phase: (8 columns, 16 rows, projection) CTAs over the step's token rows, or its output rows
@@ -2584,7 +2729,8 @@ struct LoraArg { const uint8_t* st; size_t len; float alpha; };
 static int32_t create_rank(const uint8_t* st, size_t len, int32_t device, int32_t max_batch, int32_t token_chunk_size,
                            int32_t precision, int32_t rank, int32_t world, const std::vector<LoraArg>& lora, b200rwkv_engine** out,
                            int32_t quant_layers = 0, int32_t quant_type = 0,
-                           const std::vector<b200rwkv_engine::LoraSrc>& adapters = {}) {
+                           const std::vector<b200rwkv_engine::LoraSrc>& adapters = {}, int32_t places = 0,
+                           uint32_t targets = 0) {
     API_BEGIN((b200rwkv_engine*)nullptr)
     REQUIRE(out, B200RWKV_ERR_INVALID, "null out");
     *out = nullptr;
@@ -2622,7 +2768,8 @@ static int32_t create_rank(const uint8_t* st, size_t len, int32_t device, int32_
     e->quant_layers = quant_type == QT_NONE ? 0 : quant_layers;
     e->quant_type = quant_layers == 0 ? (int)QT_NONE : quant_type;
     e->adapters = adapters;
-    e->n_adapters = (int)adapters.size();
+    e->n_adapters = adapters.empty() ? places : (int)adapters.size();
+    e->ad_targets = targets;
     e->build(f);
     e->loras.clear();            // the LoRA and adapter images are only borrowed during the build
     e->adapters.clear();
@@ -4172,12 +4319,76 @@ int32_t b200rwkv_create_adapters(const uint8_t* st, size_t len, const b200rwkv_o
         files.emplace_back(new StFile(adapter_st[a], adapter_len[a]));
         srcs.push_back({files.back().get(), adapter_alpha[a]});
     }
-    check_adapter_files(model, srcs, opt->quant_layers, opt->quant_type);
+    check_adapter_files(model.tensors, srcs, opt->quant_layers, opt->quant_type);
     std::vector<LoraArg> lora;
     for (int i = 0; i < opt->num_lora; ++i) lora.push_back({opt->lora_st[i], opt->lora_len[i], opt->lora_alpha[i]});
     const int dev0 = opt->num_devices <= 0 ? 0 : opt->devices[0];
     return create_rank(st, len, dev0, opt->max_batch, opt->token_chunk_size, opt->precision, 0, 1, lora, out, opt->quant_layers,
                        opt->quant_type, srcs);
+    API_END
+}
+
+// b200rwkv_create_ex with n empty adapter places, W' plans for every targeted matrix of the f16 layers: checked on the host
+// before any CUDA call
+int32_t b200rwkv_create_adapter_places(const uint8_t* st, size_t len, const b200rwkv_options* opt, int32_t n, uint32_t targets,
+                                       b200rwkv_engine** out) {
+    API_BEGIN((b200rwkv_engine*)nullptr)
+    REQUIRE(out && opt, B200RWKV_ERR_INVALID, "null argument");
+    *out = nullptr;
+    REQUIRE(opt->struct_bytes == sizeof(b200rwkv_options), B200RWKV_ERR_INVALID, "b200rwkv_options.struct_bytes does not match this library");
+    REQUIRE(n >= 1 && n <= AD_MAX, B200RWKV_ERR_INVALID, "number of adapter places must be 1..8");
+    REQUIRE(targets != 0 && (targets & ~AD_TARGET_ALL) == 0, B200RWKV_ERR_INVALID,
+            "adapter targets must be a nonzero set of B200RWKV_TARGET_* bits");
+    REQUIRE(opt->num_devices <= 1, B200RWKV_ERR_UNSUPPORTED, "adapters run on one GPU (no tensor parallelism)");
+    REQUIRE(opt->num_lora >= 0 && opt->num_lora <= B200RWKV_MAX_LORA, B200RWKV_ERR_INVALID, "bad num_lora");
+    REQUIRE(opt->quant_layers >= 0 && opt->quant_type >= 0, B200RWKV_ERR_INVALID, "bad quant_layers / quant_type");
+    StFile model(st, len);
+    REQUIRE(!ad_place_matrices(model.tensors, targets, opt->quant_layers, opt->quant_type).empty(), B200RWKV_ERR_UNSUPPORTED,
+            "adapter targets name no f16 projection matrix of this model");
+    std::vector<LoraArg> lora;
+    for (int i = 0; i < opt->num_lora; ++i) lora.push_back({opt->lora_st[i], opt->lora_len[i], opt->lora_alpha[i]});
+    const int dev0 = opt->num_devices <= 0 ? 0 : opt->devices[0];
+    return create_rank(st, len, dev0, opt->max_batch, opt->token_chunk_size, opt->precision, 0, 1, lora, out, opt->quant_layers,
+                       opt->quant_type, {}, n, targets);
+    API_END
+}
+
+// Fills the empty adapter place `id` (the infer task's call, like bind_adapter); every refusal is decided on the host first
+int32_t b200rwkv_load_adapter(b200rwkv_engine* e, int32_t id, const uint8_t* adapter_st, size_t adapter_len, float alpha) {
+    API_BEGIN(e)
+    REQUIRE(id >= 1, B200RWKV_ERR_INVALID, "load_adapter: id " + std::to_string(id) + " outside 1..n");
+    REQUIRE(adapter_st && adapter_len > 8, B200RWKV_ERR_INVALID, "null adapter image");
+    REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
+    REQUIRE(id <= e->n_adapters, B200RWKV_ERR_INVALID, "load_adapter: id " + std::to_string(id) + " outside 1..n");
+    std::lock_guard<std::mutex> lk(e->mu);
+    REQUIRE(!e->place_full[id - 1], B200RWKV_ERR_STATE,
+            "load_adapter: place " + std::to_string(id) + " holds an adapter (unload it first)");
+    StFile f(adapter_st, adapter_len);
+    check_adapter_files(e->model_shapes, {{&f, alpha}}, e->quant_layers, e->quant_type);
+    for (auto& kv : f.tensors) {
+        if (!ends_with(kv.first, ".lora.0")) continue;
+        const std::string base = kv.first.substr(0, kv.first.size() - 7);
+        bool planned = false;
+        for (const b200rwkv_engine::AdMatrix& m : e->ad_mats) planned = planned || m.name == base;
+        REQUIRE(planned, B200RWKV_ERR_UNSUPPORTED,
+                "adapter on " + base + ": this engine holds no W' plan for it (its kind was not targeted at creation)");
+    }
+    e->load_place(id, f, alpha);
+    API_END
+}
+
+// Empties adapter place `id` (the infer task's call); refused while a slot is bound to it
+int32_t b200rwkv_unload_adapter(b200rwkv_engine* e, int32_t id) {
+    API_BEGIN(e)
+    REQUIRE(id >= 1, B200RWKV_ERR_INVALID, "unload_adapter: id " + std::to_string(id) + " outside 1..n");
+    REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
+    REQUIRE(id <= e->n_adapters, B200RWKV_ERR_INVALID, "unload_adapter: id " + std::to_string(id) + " outside 1..n");
+    std::lock_guard<std::mutex> lk(e->mu);
+    REQUIRE(e->place_full[id - 1], B200RWKV_ERR_STATE, "unload_adapter: place " + std::to_string(id) + " is empty");
+    for (int s = 0; s < e->S; ++s)
+        REQUIRE(e->slot_adapter[s] != id, B200RWKV_ERR_STATE,
+                "unload_adapter: slot " + std::to_string(s) + " is bound to adapter " + std::to_string(id));
+    e->unload_place(id);
     API_END
 }
 
@@ -4199,6 +4410,9 @@ int32_t b200rwkv_bind_adapter(b200rwkv_engine* e, int32_t nslot, const int32_t* 
         REQUIRE(adapter[i] <= e->n_adapters, B200RWKV_ERR_INVALID, "bind_adapter: unknown adapter id " + std::to_string(adapter[i]));
     }
     std::lock_guard<std::mutex> lk(e->mu);
+    for (int i = 0; i < nslot; ++i)
+        REQUIRE(adapter[i] == 0 || e->place_full[adapter[i] - 1], B200RWKV_ERR_STATE,
+                "bind_adapter: adapter place " + std::to_string(adapter[i]) + " is empty");
     for (int i = 0; i < nslot; ++i) e->slot_adapter[slots[i]] = adapter[i];
     if (e->n_adapters) {
         CK(cudaSetDevice(e->dev));

@@ -226,13 +226,17 @@ class Model:
 
     def __init__(self, st: np.ndarray, max_batch: int = 8, token_chunk_size: int = 128, device: int = 0,
                  precision: int = 0, rank: int = 0, world: int = 1, exact: bool = False, devices=None, lora=None,
-                 quant: int = 0, quant_type: int | str = 0, adapters=None):
+                 quant: int = 0, quant_type: int | str = 0, adapters=None, adapter_places: int = 0,
+                 adapter_targets=()):
         """devices: list of CUDA ordinals -> ONE engine object owning all tensor-parallel ranks (b200rwkv_create_ex);
         lora: list of (st_bytes, alpha) blended at load (reference lib.rs:466-485);
         quant / quant_type: the reload request's fields (lib.rs:211-215): the first `quant` layers in "Int8" or "NF4";
         rank / world: one process per GPU instead (b200rwkv_create_tp + tp.connect);
         adapters: list of (st_bytes, alpha) kept unblended, ids 1..n, chosen per slot with bind_adapter
-        (b200rwkv_create_adapters)."""
+        (b200rwkv_create_adapters);
+        adapter_places / adapter_targets: n empty adapter places, filled and emptied with load_adapter / unload_adapter,
+        that hold pairs on the named kinds of matrix ("att.key", ..., "head": the keys of capi.TARGETS)
+        (b200rwkv_create_adapter_places)."""
         if isinstance(quant_type, str):
             kinds = {"none": capi.QUANT_NONE, "int8": capi.QUANT_INT8, "nf4": capi.QUANT_NF4, "sf4": 3}
             if quant_type.lower() not in kinds:
@@ -244,7 +248,9 @@ class Model:
         st = np.ascontiguousarray(st, dtype=np.uint8)
         h = C.c_void_p()
         L = capi.lib()
-        if devices is not None or lora or quantised or adapters:
+        if adapters and adapter_places:
+            raise capi.B200Error(capi.ERR_INVALID, "adapters and adapter_places are two constructors: pass one")
+        if devices is not None or lora or quantised or adapters or adapter_places:
             if world != 1:
                 raise capi.B200Error(capi.ERR_INVALID, "devices / lora / quant go through b200rwkv_create_ex (in-process ranks)")
             opt = capi.Options()
@@ -269,6 +275,15 @@ class Model:
                 alphas = (C.c_float * n)(*[float(a) for _, a in adapters])
                 capi.check(L.b200rwkv_create_adapters(capi.ptr(st), st.size, C.byref(opt), n, C.cast(ptrs, C.c_void_p),
                                                       C.cast(lens, C.c_void_p), C.cast(alphas, C.c_void_p), C.byref(h)))
+            elif adapter_places:
+                unknown = [t for t in adapter_targets if t not in capi.TARGETS]
+                if unknown:
+                    raise capi.B200Error(capi.ERR_INVALID, f"unknown adapter targets {unknown}: use keys of capi.TARGETS")
+                mask = 0
+                for t in adapter_targets:
+                    mask |= capi.TARGETS[t]
+                capi.check(L.b200rwkv_create_adapter_places(capi.ptr(st), st.size, C.byref(opt), int(adapter_places), mask,
+                                                            C.byref(h)))
             else:
                 capi.check(L.b200rwkv_create_ex(capi.ptr(st), st.size, C.byref(opt), C.byref(h)))
             self._lora_keep = []
@@ -525,6 +540,15 @@ class Model:
         if slots.shape != ids.shape:
             raise capi.B200Error(capi.ERR_INVALID, "bind_adapter: slots and ids differ in length")
         capi.check(capi.lib().b200rwkv_bind_adapter(self._h, slots.size, capi.ptr(slots), capi.ptr(ids)), self._h)
+
+    def load_adapter(self, id: int, st, alpha: float) -> None:
+        """Fills the empty adapter place `id` with the adapter file `st` at `alpha` (b200rwkv_load_adapter)."""
+        img = np.ascontiguousarray(st, dtype=np.uint8)
+        capi.check(capi.lib().b200rwkv_load_adapter(self._h, int(id), capi.ptr(img), img.size, float(alpha)), self._h)
+
+    def unload_adapter(self, id: int) -> None:
+        """Empties adapter place `id`; no slot may be bound to it (b200rwkv_unload_adapter)."""
+        capi.check(capi.lib().b200rwkv_unload_adapter(self._h, int(id)), self._h)
 
     def keep_hidden_pooled(self, layers, mode="last") -> None:
         """Reduce the residual stream after each listed layer to one row per entry of every following infer call

@@ -129,11 +129,56 @@ int32_t b200rwkv_create_ex(const uint8_t* st, size_t len, const b200rwkv_options
  * exactly the launches (and gives exactly the bits) of a create_ex engine.
  * Resident memory: every projection launch an adapter touches is held a second time, with one 128-wide k block per adapter
  * appended (W' = [W | alpha_1 B_1 | ...]), plus each adapter's A matrices; adapters on every projection kind and the head cost
- * about the projection weights again (7B: +14.7 GB, + 1.5 GB of tail blocks and 0.7 GB of A for 4 adapters of rank 64). */
+ * about the projection weights again (7B: +14.7 GB, + 1.5 GB of tail blocks and 1.4 GB of A for 4 adapters: A is reserved at
+ * rank 128, so that b200rwkv_unload_adapter / b200rwkv_load_adapter below can replace a file by one of any rank). */
 int32_t b200rwkv_create_adapters(const uint8_t* st, size_t len, const b200rwkv_options* opt, int32_t n,
                                  const uint8_t* const* adapter_st, const size_t* adapter_len, const float* adapter_alpha,
                                  b200rwkv_engine** out);
 int32_t b200rwkv_bind_adapter(b200rwkv_engine*, int32_t nslot, const int32_t* slots, const int32_t* adapter);
+
+/* Adapters that come and go while the engine serves (the reference fixes its LoRA files at load; dropping one means a restart).
+ * b200rwkv_create_adapter_places = b200rwkv_create_ex plus n (1..8) empty adapter places, ids 1..n.  A place can hold an
+ * adapter file with pairs on the `targets` kinds of matrix (B200RWKV_TARGET_* bits) in every layer that is not quantised
+ * (opt->quant_layers), and on the head if targeted; bits for matrices the model does not have (ATT_G, FFN_R on v7) are
+ * skipped.  Refused before any CUDA call: n outside 1..8, targets 0 or an unknown bit, a NULL out / opt or a wrong
+ * struct_bytes are B200RWKV_ERR_INVALID; more than one device, or targets that name no f16 matrix of the model,
+ * B200RWKV_ERR_UNSUPPORTED.
+ * b200rwkv_load_adapter fills the empty place `id` with an adapter file (the format of b200rwkv_create_adapters).  Afterwards
+ * slots bound to `id` compute exactly what they would on an engine made by b200rwkv_create_adapters with that file at that
+ * id, under the same plans.  Refused, with nothing changed and before any CUDA call: id outside 1..n, a NULL image, a missing
+ * half or a shape that does not match its matrix are B200RWKV_ERR_INVALID; a place that holds an adapter B200RWKV_ERR_STATE
+ * (replacing one is an unload, then a load, so a bound slot never changes adapter silently); full tensors, non-F16 pairs, a
+ * rank above 128, a pair on a quantised layer and a pair on a matrix this engine holds no W' plan for are
+ * B200RWKV_ERR_UNSUPPORTED.  The plans: on a places engine every targeted matrix of the f16 layers; on a
+ * b200rwkv_create_adapters engine the matrices its files paired at creation (its n places start full).
+ * b200rwkv_unload_adapter empties place `id`: id outside 1..n is B200RWKV_ERR_INVALID; an empty place, or one a slot is bound
+ * to, B200RWKV_ERR_STATE (the message names the slot).  b200rwkv_bind_adapter to an empty place is B200RWKV_ERR_STATE.
+ * All three are made by the infer task, like bind_adapter.  Their writes go on the engine's stream, so steps already enqueued
+ * finish with the old contents, and are complete when the call returns; the image is only borrowed.  Slots bound to other
+ * places, unbound slots, states, kept rows and snapshots are not touched.  The captured step graphs of bound steps are
+ * dropped and captured again on their next use; unbound steps keep theirs.
+ * Resident memory is reserved at creation (load_adapter allocates none).  Figures computed from shapes, not measured, for the
+ * 7B shape (C = 4096, F = 14336, L = 32, V = 65536) with every kind and the head targeted:
+ *   - W' plans: about the projection bytes again, +14.7 GB;
+ *   - one 128-wide tail column per place on every planned matrix: 128 * (7 C + F) * 2 B * L + 128 * V * 2 B, about
+ *     0.37 GB per place;
+ *   - A rows for rank 128 per place and planned matrix: 128 * (5 C + 2 C + F) * 2 B * L + 128 * C * 2 B, about 0.35 GB
+ *     (0.33 GiB) per place (b200rwkv_create_adapters engines reserve the same, so a place can be reloaded with any rank).
+ * Step cost: a step with a bound slot streams the tail blocks of all n places, full or empty -- the cost of a
+ * b200rwkv_create_adapters engine with n files.  Size n to what is needed. */
+#define B200RWKV_TARGET_ATT_R  (1u << 0)   /* att.receptance */
+#define B200RWKV_TARGET_ATT_K  (1u << 1)   /* att.key */
+#define B200RWKV_TARGET_ATT_V  (1u << 2)   /* att.value */
+#define B200RWKV_TARGET_ATT_G  (1u << 3)   /* att.gate (v5 / v6) */
+#define B200RWKV_TARGET_ATT_O  (1u << 4)   /* att.output */
+#define B200RWKV_TARGET_FFN_K  (1u << 5)   /* ffn.key */
+#define B200RWKV_TARGET_FFN_V  (1u << 6)   /* ffn.value */
+#define B200RWKV_TARGET_FFN_R  (1u << 7)   /* ffn.receptance (v5 / v6) */
+#define B200RWKV_TARGET_HEAD   (1u << 8)
+int32_t b200rwkv_create_adapter_places(const uint8_t* st, size_t len, const b200rwkv_options* opt, int32_t n,
+                                       uint32_t targets, b200rwkv_engine** out);
+int32_t b200rwkv_load_adapter(b200rwkv_engine*, int32_t id, const uint8_t* adapter_st, size_t adapter_len, float alpha);
+int32_t b200rwkv_unload_adapter(b200rwkv_engine*, int32_t id);
 
 /* Tensor-parallel construction, one process per GPU (head / column parallel, SURVEY.md §8e).
  * (The in-process alternative -- one handle, all ranks inside -- is b200rwkv_create_ex above.)
