@@ -65,7 +65,9 @@ class WkvArgs(C.Structure):
                 ("count", C.c_void_p), ("precision", C.c_int32)] + [
                 (n, C.c_void_p) for n in ("r", "k", "v", "g", "w", "u", "lnx_w", "lnx_b", "a", "k_k", "k_a", "r_k", "nu")] + [
                 ("layer0", C.c_int32), ("v_first", C.c_void_p), ("d1", C.c_void_p), ("time_decay_w2", C.c_void_p),
-                ("decay_bias", C.c_void_p), ("Dd", C.c_int32), ("state", C.c_void_p), ("out", C.c_void_p)]
+                ("decay_bias", C.c_void_p), ("Dd", C.c_int32), ("state", C.c_void_p), ("out", C.c_void_p),
+                ("nsnap", C.c_int32), ("snap_tok", C.c_void_p), ("snap_rec", C.c_void_p), ("snap_ld", C.c_int64),
+                ("snap_off", C.c_int64)]
 
 
 class LnArgs(C.Structure):
@@ -79,17 +81,21 @@ class LnArgs(C.Structure):
                 (n, C.c_void_p) for n in ("mu", "commit_src", "commit_dst", "hidden", "x_out", "xx_out", "sx_out", "mix_out")] + [
                 ("Dm", C.c_int32)] + [
                 (n, C.c_void_p) for n in ("W1", "W2", "mu5", "lora_out", "out5", "emb")] + [
-                ("V", C.c_int32), ("tokens", C.c_void_p), ("head_out", C.c_void_p), ("kernel_out", C.c_void_p)]
+                ("V", C.c_int32), ("tokens", C.c_void_p), ("head_out", C.c_void_p), ("kernel_out", C.c_void_p),
+                ("nsnap", C.c_int32), ("snap_tok", C.c_void_p), ("snap_rec", C.c_void_p), ("snap_ld", C.c_int64),
+                ("snap_off", C.c_int64), ("snap_head_out", C.c_void_p)]
 
 
 LN_EMBED, LN_MIX, LN_FRONT6, LN_OUT = range(4)                     # b200rwkv_ln_args.stage
 K_EMBED, K_LN_MIX, K_LN_MIX_CLUSTER, K_PRE6, K_LN_OUT = range(5)   # kernel_out[0]
 
 
-def op_ln(stage: int, channels: int, slots, counts, launches: int = 1, precision: int = 0, option=None, device: int = 0, **arrays):
+def op_ln(stage: int, channels: int, slots, counts, launches: int = 1, precision: int = 0, option=None, device: int = 0,
+          snap_tok=None, snap_off: int = 0, **arrays):
     """One LN stage of a step (b200rwkv_op_ln), `launches` times back to back.  `arrays` holds the struct's array members by
-    name (numpy arrays of the header's element types; absent = NULL); output arrays are updated in place.  Returns
-    kernel_out: (kernel, variant, split)."""
+    name (numpy arrays of the header's element types; absent = NULL); output arrays are updated in place.  Snapshots:
+    snap_tok (token rows) with arrays snap_rec [nsnap, snap_ld] f32 and, for ln_out, snap_head_out [rows_x, C] uint16.
+    Returns kernel_out: (kernel, variant, split)."""
     slots, counts = np.ascontiguousarray(slots, np.int32), np.ascontiguousarray(counts, np.int32)
     keep = [slots, counts]
     a = LnArgs(stage=stage, C=channels, S=int(arrays.pop("S")), nslot=len(slots), slot=ptr(slots), count=ptr(counts),
@@ -99,6 +105,12 @@ def op_ln(stage: int, channels: int, slots, counts, launches: int = 1, precision
         option = np.ascontiguousarray(option, np.int32)
         keep.append(option)
         a.option = ptr(option)
+    if snap_tok is not None:
+        snap_tok = np.ascontiguousarray(snap_tok, np.int32)
+        keep.append(snap_tok)
+        rec = arrays["snap_rec"]
+        assert rec.dtype == np.float32 and rec.ndim == 2 and rec.shape[0] == len(snap_tok)
+        a.nsnap, a.snap_tok, a.snap_ld, a.snap_off = len(snap_tok), ptr(snap_tok), rec.shape[1], snap_off
     for name, arr in arrays.items():
         if arr is None:
             continue
@@ -311,11 +323,12 @@ def op_quantize(quant_type: int, w16, device: int = 0):
 
 def op_wkv_step(version: int, slots, counts, state, out, r, k, v, g, lnx_w, lnx_b, w=None, u=None, a=None, k_k=None, k_a=None,
                 r_k=None, nu=None, layer0: bool = True, v_first=None, d1=None, time_decay_w2=None, decay_bias=None, precision: int = 0,
-                device: int = 0):
+                snap_tok=None, snap_rec=None, snap_off: int = 0, device: int = 0):
     """One WKV launch of a step (b200rwkv_op_wkv) over a pool of S slots: entry i feeds counts[i] tokens to pool slot slots[i].
     state [S, H, 64, 64] f32 (M[value][key]), out [gemm_rows(T, precision), H*64] uint16 f16 bits and v7's v_first [T, H*64]
     f32 are updated in place.  Per-token arrays are [T, H*64] (or [T, H, 64]) f32, per-channel ones [H*64]; d1 [T, Dd] f32 and
-    time_decay_w2 [H*64, Dd] f16 turn on the v6 decay fold."""
+    time_decay_w2 [H*64, Dd] f16 turn on the v6 decay fold.  Snapshots: snap_tok (token rows) and snap_rec [nsnap, snap_ld]
+    f32, updated in place: record k receives the state after token snap_tok[k] from column snap_off on."""
     S, H = state.shape[:2]
     assert state.dtype == np.float32 and state.flags.c_contiguous and state.shape[2:] == (64, 64)
     assert out.dtype == np.uint16 and out.flags.c_contiguous and out.shape == (gemm_rows(sum(counts), precision), H * 64)
@@ -329,6 +342,11 @@ def op_wkv_step(version: int, slots, counts, state, out, r, k, v, g, lnx_w, lnx_
     args = WkvArgs(version, H, S, len(sl), p(sl), p(cn), precision, p(r), p(k), p(v), p(g), p(w), p(u), p(lnx_w), p(lnx_b), p(a),
                    p(k_k), p(k_a), p(r_k), p(nu), int(layer0), p(v_first), p(d1), p(w2), p(decay_bias),
                    0 if d1 is None else d1.shape[1], ptr(state), ptr(out))
+    if snap_tok is not None:
+        st_ = np.ascontiguousarray(snap_tok, np.int32)
+        keep.append(st_)
+        assert snap_rec.dtype == np.float32 and snap_rec.flags.c_contiguous and snap_rec.shape[0] == len(st_)
+        args.nsnap, args.snap_tok, args.snap_rec, args.snap_ld, args.snap_off = len(st_), ptr(st_), ptr(snap_rec), snap_rec.shape[1], snap_off
     check(lib().b200rwkv_op_wkv(device, C.byref(args)))
 
 

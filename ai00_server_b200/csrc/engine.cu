@@ -576,7 +576,14 @@ struct b200rwkv_engine {
     GemmLaunch snap_head, snap_ad_head;      // head / ad_head over a_snap_head into snap_logits
     AdapterParams s_snap_head;
     float* const* snap_rec_dev() const { return reinterpret_cast<float* const*>(snap_dev.p + snap_meta_bytes); }
+    void snap_sizes() {
+        snap_meta_bytes = (meta_ints * 4 + 15) & ~(size_t)15;
+        snap_bytes = snap_meta_bytes + 3 * (size_t)maxT * sizeof(void*);
+    }
     void snap_setup();
+    // one snapshot token of a step: its token row, its record, the snapshot's logits row (null: none)
+    struct SnapTok { int t; float* rec; float* row; };
+    int fill_snap(uint8_t* hs, const int* hm, int T, const std::vector<SnapTok>& tk) const;
     struct SnapPlan { int n; const int32_t* entry; const int32_t* tok; uint64_t* ids; };
 
     // activations
@@ -1918,7 +1925,6 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler
             if (sh.MTX > 0) {
                 lo.snap_meta = MetaView{reinterpret_cast<const int*>(snap_dev.p), maxT, S};
                 lo.snap_head_in = a_snap_head.p;
-                lo.snap_kq = sh.split ? 32 : 16 * sh.MTX;
             }
         }
         launch_ln_out(lo, sh, s, prof);
@@ -1977,10 +1983,12 @@ LnPick b200rwkv_engine::launch_pre6(const Pre6Params& q0, const StepShape& sh, c
     return {LNK_PRE6, q.Dm / 16, sh.split ? 1 : 0};
 }
 
-// final residual update + ln_out of a step into the head operand, which holds the step's output rows
+// final residual update + ln_out of a step into the head operand, which holds the step's output rows (and, on a snapshot
+// step, into the snapshot rows' head operand of sh.MTX token tiles)
 LnPick b200rwkv_engine::launch_ln_out(const LnOutParams& p, const StepShape& sh, cudaStream_t s, Profiler* prof) {
     LnOutParams lo = p;
     lo.kq_tile = sh.th_rows;
+    if (lo.snap_head_in) lo.snap_kq = sh.split ? 32 : 16 * sh.MTX;
     if (sh.split) launch_k(ln_out_kernel<true>, dim3(sh.rows), dim3(LN_THREADS), 0, lo, KC_LN, s, prof);
     else launch_k(ln_out_kernel<false>, dim3(sh.rows), dim3(LN_THREADS), 0, lo, KC_LN, s, prof);
     return {LNK_OUT, ln_nv(p.C), sh.split ? 1 : 0};
@@ -2058,8 +2066,7 @@ void b200rwkv_engine::upload_hid_tab() {
 // head / ad_head read a_snap_head and write snap_logits, over the snapshot metadata's R rows, with counters of their own.
 void b200rwkv_engine::snap_setup() {
     if (snap_dev) return;
-    snap_meta_bytes = (meta_ints * 4 + 15) & ~(size_t)15;
-    snap_bytes = snap_meta_bytes + 3 * (size_t)maxT * sizeof(void*);
+    snap_sizes();
     snap_dev = Buf<uint8_t>(snap_bytes);
     snap_host = HostBuf<uint8_t>(snap_bytes * META_RING);
     const int K = n_adapters ? (cdiv(C, GEMM_BK) + n_adapters) * GEMM_BK : C;      // a_head's columns
@@ -2125,6 +2132,39 @@ int b200rwkv_engine::fill_meta(int* m, const std::vector<int>& slots, const std:
     m[0] = T; m[1] = (int)slots.size(); m[2] = R;
     *R_out = R;
     return T;
+}
+
+// Fills one snapshot step block hs [snap_bytes] from the step's metadata hm (T tokens) and its snapshot tokens: the record of
+// each token row, where its logits row comes from and goes to, and a copy of the metadata whose output rows are the
+// snapshot tokens without one, in the order of `tk`.  Returns X, the number of those rows.
+int b200rwkv_engine::fill_snap(uint8_t* hs, const int* hm, int T, const std::vector<SnapTok>& tk) const {
+    int* smeta = reinterpret_cast<int*>(hs);
+    float** rec = reinterpret_cast<float**>(hs + snap_meta_bytes);
+    const float** src = const_cast<const float**>(rec + maxT);
+    float** dst = rec + 2 * maxT;
+    memset(hs + snap_meta_bytes, 0, 3 * (size_t)maxT * sizeof(void*));
+    memcpy(smeta, hm, meta_ints * 4);
+    MetaView sv{smeta, maxT, S};
+    int* s_outrow = const_cast<int*>(sv.tok_outrow());
+    int* s_outtok = const_cast<int*>(sv.out_tok());
+    const int* torow = MetaView{hm, maxT, S}.tok_outrow();
+    for (int t = 0; t < T; ++t) s_outrow[t] = -1;
+    int X = 0;
+    for (const SnapTok& a : tk) {
+        const int t = a.t;
+        rec[t] = a.rec;
+        dst[t] = a.row;
+        if (torow[t] >= 0) {
+            src[t] = d_logits + (size_t)torow[t] * V;
+        } else {
+            s_outrow[t] = X;
+            s_outtok[X] = t;
+            src[t] = snap_logits + (size_t)X * V;
+            ++X;
+        }
+    }
+    smeta[2] = X;
+    return X;
 }
 
 void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok, const uint32_t* tokens, const int32_t* option,
@@ -2310,40 +2350,20 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         // snapshots of this step's tokens: their records, and where their logits rows come from
         int n_step_snap = 0, X = 0;
         if (nsnap > 0) {
-            uint8_t* hs = snap_host + (size_t)mb * snap_bytes;
-            int* smeta = reinterpret_cast<int*>(hs);
-            float** rec = reinterpret_cast<float**>(hs + snap_meta_bytes);
-            const float** src = const_cast<const float**>(rec + maxT);
-            float** dst = rec + 2 * maxT;
-            memset(hs + snap_meta_bytes, 0, 3 * (size_t)maxT * sizeof(void*));
-            memcpy(smeta, hm, meta_ints * 4);
-            MetaView sv{smeta, maxT, S};
-            int* s_outrow = const_cast<int*>(sv.tok_outrow());
-            int* s_outtok = const_cast<int*>(sv.out_tok());
-            const int* torow = MetaView{hm, maxT, S}.tok_outrow();
-            for (int t = 0; t < T; ++t) s_outrow[t] = -1;
+            std::vector<SnapTok> tk;
             int t0 = 0;
             for (size_t j = 0; j < s_entry.size(); ++j) {
                 const int i = s_entry[j];
-                for (const SnapDst& a : snap_at[i]) {
-                    if (a.tok < pos[i] || a.tok >= pos[i] + s_counts[j]) continue;
-                    const int t = t0 + (a.tok - pos[i]);
-                    rec[t] = a.state;
-                    dst[t] = a.row;
-                    if (torow[t] >= 0) {
-                        src[t] = d_logits + (size_t)torow[t] * V;
-                    } else {
-                        s_outrow[t] = X;
-                        s_outtok[X] = t;
-                        src[t] = snap_logits + (size_t)X * V;
-                        ++X;
-                    }
-                    ++n_step_snap;
-                }
+                for (const SnapDst& a : snap_at[i])
+                    if (a.tok >= pos[i] && a.tok < pos[i] + s_counts[j]) tk.push_back({t0 + (a.tok - pos[i]), a.state, a.row});
                 t0 += s_counts[j];
             }
-            smeta[2] = X;
-            if (n_step_snap > 0) CK(cudaMemcpyAsync(snap_dev, hs, snap_bytes, cudaMemcpyHostToDevice, stream));
+            n_step_snap = (int)tk.size();
+            if (n_step_snap > 0) {
+                uint8_t* hs = snap_host + (size_t)mb * snap_bytes;
+                X = fill_snap(hs, hm, T, tk);
+                CK(cudaMemcpyAsync(snap_dev, hs, snap_bytes, cudaMemcpyHostToDevice, stream));
+            }
         }
         CK(cudaEventRecord(meta_ev[mb], stream));
         StepShape sh = step_shape(T, R);
@@ -3336,6 +3356,23 @@ int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int3
     API_END
 }
 
+// The snapshot arguments of b200rwkv_op_wkv / op_ln, before any CUDA call: distinct token rows of a step of T tokens, and
+// records of snap_ld cells that hold `need` cells from snap_off on.  The kernels store records in float4 vectors, so every
+// record part starts on a 16-byte boundary: snap_off and snap_ld are multiples of 4.
+static void snap_args_ok(int nsnap, const int32_t* tok, const float* rec, int64_t ld, int64_t off, int64_t need, int T) {
+    REQUIRE(nsnap >= 0, B200RWKV_ERR_INVALID, "nsnap must be >= 0");
+    if (nsnap == 0) return;
+    REQUIRE(tok && rec, B200RWKV_ERR_INVALID, "snapshots need snap_tok and snap_rec");
+    REQUIRE(off >= 0 && ld >= need && off <= ld - need, B200RWKV_ERR_INVALID, "snap_ld must be >= snap_off + the recorded part");
+    REQUIRE(off % 4 == 0 && ld % 4 == 0, B200RWKV_ERR_INVALID, "snap_off and snap_ld must be multiples of 4 (float4 stores)");
+    std::vector<char> seen(T, 0);
+    for (int k = 0; k < nsnap; ++k) {
+        REQUIRE(tok[k] >= 0 && tok[k] < T, B200RWKV_ERR_INVALID, "snapshot token outside [0, T)");
+        REQUIRE(!seen[tok[k]], B200RWKV_ERR_INVALID, "snapshot token listed twice");
+        seen[tok[k]] = 1;
+    }
+}
+
 // The step under an operator-level entry (b200rwkv_op_wkv / op_ln / op_gemm).  The constructor checks the step's entries
 // (slot, token count) before any CUDA call; start() makes a temporary engine object with the step's pool size and precision,
 // one metadata block per launch from its fill_meta and the step's shape from its step_shape: what a step of these entries
@@ -3346,7 +3383,10 @@ struct OpStep {
     std::vector<int> slots, counts;
     std::unique_ptr<b200rwkv_engine> e;
     std::vector<int*> metas;                       // device, one per launch; e->d_meta is the first
+    std::vector<int> meta0;                        // host copy of the first
     StepShape sh{};
+    MetaView snap_meta{};                          // snap_start(): the snapshot block's metadata and record table
+    float* const* snap_table = nullptr;
 
     OpStep(int S_, int nslot, const int32_t* slot, const int32_t* count, int precision) : S(S_), split(precision == 1) {
         REQUIRE(S >= 1 && S <= 1024, B200RWKV_ERR_INVALID, "S must be 1..1024 (max_batch)");
@@ -3380,9 +3420,28 @@ struct OpStep {
             std::vector<int> meta(MetaView::ints(e->maxT, S), 0);
             REQUIRE(e->fill_meta(meta.data(), slots, counts, toks, outmode, &R) == T, B200RWKV_ERR_INVALID, "internal: step metadata");
             metas.push_back((int*)up(meta.data(), meta.size() * 4));
+            if (l == 0) meta0 = meta;
         }
         e->d_meta = metas[0];
         sh = e->step_shape(T, R);
+    }
+    // Snapshot tokens tok[k] with records rec + k * ld (the caller checked them with snap_args_ok): the step's snapshot block
+    // from the engine's fill_snap, uploaded, and the step's shape as infer sets it.  Returns the device copy of the records;
+    // the block's record table is snap_table.
+    float* snap_start(int nsnap, const int32_t* tok, const float* rec, int64_t ld) {
+        e->meta_ints = MetaView::ints(e->maxT, S);
+        e->snap_sizes();
+        float* d_rec = (float*)up(rec, (size_t)nsnap * ld * 4);
+        std::vector<b200rwkv_engine::SnapTok> tk;
+        for (int k = 0; k < nsnap; ++k) tk.push_back({tok[k], d_rec + (size_t)k * ld, nullptr});
+        std::vector<uint8_t> hs(e->snap_bytes);
+        const int X = e->fill_snap(hs.data(), meta0.data(), T, tk);
+        uint8_t* d = (uint8_t*)up(hs.data(), hs.size());
+        snap_meta = MetaView{reinterpret_cast<const int*>(d), e->maxT, S};
+        snap_table = reinterpret_cast<float* const*>(d + e->snap_meta_bytes);
+        sh.snap = true;
+        sh.MTX = X > 0 ? mt_bucket(X) : 0;
+        return d_rec;
     }
     // the layout start() built the blocks with, whatever the entry sets e->maxT to afterwards
     MetaView meta(int l) const { return MetaView{metas[l], A16_MAX_ROWS, S}; }
@@ -3428,8 +3487,11 @@ int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args) {
         REQUIRE(x.layer0 || x.nu, B200RWKV_ERR_INVALID, "v7 layers after 0 need nu");
     }
 
+    snap_args_ok(x.nsnap, x.snap_tok, x.snap_rec, x.snap_ld, x.snap_off, (int64_t)x.H * 64 * 64, st.T);
+
     const int H = x.H, S = x.S, Cc = H * 64, T = st.T;
     st.start(device, 1, nullptr, std::vector<int>(x.nslot, 0));
+    float* d_rec = x.nsnap > 0 ? st.snap_start(x.nsnap, x.snap_tok, x.snap_rec, x.snap_ld) : nullptr;
     const StepShape& sh = st.sh;
     wkv_smem_limits();
 
@@ -3438,6 +3500,7 @@ int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args) {
     WkvParams p;
     memset(&p, 0, sizeof(p));
     p.version = version; p.ld = Cc; p.meta = st.meta(0); p.H = H;
+    p.snap_rec = st.snap_table; p.snap_off = (size_t)x.snap_off;
     const size_t state_bytes = (size_t)S * H * 64 * 64 * 4;
     p.state = (float*)st.up(x.state, state_bytes);
     p.r = rows_up(x.r); p.k = rows_up(x.k); p.v = rows_up(x.v); p.g = rows_up(x.g);
@@ -3472,6 +3535,7 @@ int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args) {
     a16_unpack(h16, Cc, Cc, sh.th, sh.th, 0, Cc, x.out);
     CK(cudaMemcpy(x.state, p.state, state_bytes, cudaMemcpyDeviceToHost));
     if (version == 7) CK(cudaMemcpy(x.v_first, p.v_first, (size_t)T * Cc * 4, cudaMemcpyDeviceToHost));
+    if (d_rec) CK(cudaMemcpy(x.snap_rec, d_rec, (size_t)x.nsnap * x.snap_ld * 4, cudaMemcpyDeviceToHost));
     API_END
 }
 
@@ -3523,13 +3587,22 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
             outmode[i] = x.option[i] == B200RWKV_OPTION_FULL ? 2 : (x.option[i] == B200RWKV_OPTION_LAST ? 1 : 0);
         }
     }
+    snap_args_ok(x.nsnap, x.snap_tok, x.snap_rec, x.snap_ld, x.snap_off, C, T);
+    if (x.nsnap > 0) {
+        REQUIRE(stage != 0, B200RWKV_ERR_INVALID, "the embed stage takes no snapshots");
+        REQUIRE(NL == 1, B200RWKV_ERR_INVALID, "snapshots take one launch");
+        // a step's ln_out always commits the last layer's channel-mix shift, and its kernel copies commit_src unchecked
+        REQUIRE(stage != 3 || (x.commit_src && x.snap_head_out), B200RWKV_ERR_INVALID, "ln_out snapshots need the commit and snap_head_out");
+    }
 
     st.start(device, NL, x.tokens, outmode);
+    float* d_rec = x.nsnap > 0 ? st.snap_start(x.nsnap, x.snap_tok, x.snap_rec, x.snap_ld) : nullptr;
     b200rwkv_engine* e = st.e.get();
     e->ln_cluster_ok = ln_cluster_fits(C);         // as build() decides it for a model of C channels
     const StepShape& sh = st.sh;
     const int th = sh.th;
     const int hrows = std::max(sh.th_rows, 16);    // the caller's head_out has 16 rows even when the step has no output row
+    const int xrows = sh.split ? 32 : 16 * sh.MTX;  // snap_head_out
 
     auto rows_down = [&](float* h, const float* d) { CK(cudaMemcpy(h, d, (size_t)T * C * 4, cudaMemcpyDeviceToHost)); };
     // A16 operands: `nmat` matrices of K columns with `tr` token rows, exchanged with the caller as [nmat][tr][K]
@@ -3595,6 +3668,7 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
             p.xx_out = st.rows_up(x.xx_out + l * TC, C);
             p.sx_out = x.sx_out ? st.rows_up(x.sx_out + l * TC, C) : nullptr;
             p.hid_slot = hid_tab ? hid_tab + l : nullptr;
+            p.snap_rec = st.snap_table; p.snap_off = (size_t)x.snap_off;
         }
         if (hid_tab) CK(cudaMemcpy(hid_tab, hid_rows.data(), (size_t)NL * sizeof(float*), cudaMemcpyHostToDevice));
         if (stage == 2) {
@@ -3622,6 +3696,11 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
             residual(p, l);
             p.head_in = const_cast<__half*>(a16_up(x.head_out + (size_t)l * hrows * C, 1, C, hrows));
             p.hidden_out = hid_rows[l];
+            p.snap_rec = st.snap_table; p.snap_off = (size_t)x.snap_off;
+            if (sh.MTX > 0) {
+                p.snap_meta = st.snap_meta;
+                p.snap_head_in = const_cast<__half*>(a16_up(x.snap_head_out, 1, C, xrows));
+            }
         }
     }
     CK(cudaDeviceSynchronize());                   // every upload has landed before the launches
@@ -3637,7 +3716,11 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
     for (int l = 0; l < NL; ++l) {
         if (stage == 0) { rows_down(x.x_out + l * TC, em[l].x_out); continue; }
         if (x.hidden) rows_down(x.hidden + l * TC, hid_rows[l]);
-        if (stage == 3) { a16_down(x.head_out + (size_t)l * hrows * C, lo[l].head_in, 1, C, hrows); continue; }
+        if (stage == 3) {
+            a16_down(x.head_out + (size_t)l * hrows * C, lo[l].head_in, 1, C, hrows);
+            if (lo[l].snap_head_in) a16_down(x.snap_head_out, lo[l].snap_head_in, 1, C, xrows);
+            continue;
+        }
         const LnMixParams& p = lm[l];
         if (x.x_out) rows_down(x.x_out + l * TC, p.x_out);
         else rows_down(x.x_in + l * TC, p.x_in);
@@ -3650,6 +3733,7 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
         }
     }
     if (cdst) CK(cudaMemcpy(x.commit_dst, cdst, (size_t)S * C * 4, cudaMemcpyDeviceToHost));
+    if (d_rec) CK(cudaMemcpy(x.snap_rec, d_rec, (size_t)x.nsnap * x.snap_ld * 4, cudaMemcpyDeviceToHost));
     if (x.kernel_out) { x.kernel_out[0] = pick.kernel; x.kernel_out[1] = pick.variant; x.kernel_out[2] = pick.split; }
     API_END
 }

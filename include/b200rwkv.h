@@ -409,7 +409,11 @@ int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int3
  *   state: in/out [S][H][64][64] in the device orientation M[value][key] (v5/v6: the transpose of S[key][value]).
  *   precision 0: out holds f16 outputs; 1 (T <= 16): split outputs, hi at row t and lo at row t + 16.
  *   out: [rows][C] f16 bits, de-tiled, rows = 16 x token tiles of the step (16 / 32 / 64 / 128 by T; 32 with precision 1).
- *   The caller's contents are uploaded first: cells the kernel does not write come back unchanged. */
+ *   The caller's contents are uploaded first: cells the kernel does not write come back unchanged.
+ *   Snapshots (nsnap 0 / NULL arrays: none), as a step of b200rwkv_infer_snapshots takes them: snap_tok [nsnap] distinct step
+ *   token rows in [0, T); snap_rec [nsnap][snap_ld] f32 in/out, uploaded first, where record k receives the state after token
+ *   snap_tok[k] at snap_rec[k] + snap_off + h * 4096 (the layout of one slot of `state`); snap_ld >= snap_off + H * 4096,
+ *   and snap_off and snap_ld are multiples of 4 (the kernels store records as 16-byte vectors). */
 typedef struct {
     int32_t version, H, S, nslot;
     const int32_t *slot, *count;
@@ -425,6 +429,10 @@ typedef struct {
     int32_t Dd;
     float* state;
     uint16_t* out;
+    int32_t nsnap;
+    const int32_t* snap_tok;
+    float* snap_rec;
+    int64_t snap_ld, snap_off;
 } b200rwkv_wkv_args;
 int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args);
 
@@ -449,7 +457,15 @@ int32_t b200rwkv_op_wkv(int32_t device, const b200rwkv_wkv_args* args);
  *   rows) or 32 with precision 1 (T <= 16), where hi sits at row t and lo at row t + 16.  The caller's contents are uploaded
  *   first: cells the kernel does not write come back unchanged.  kernel_out (may be NULL) receives {kernel, variant, split}:
  *   kernel 0 embed_ln0, 1 ln_mix, 2 ln_mix_cluster, 3 pre6 (variant Dm / 16), 4 ln_out; variant of the other kernels =
- *   float4 per thread (1 / 2 / 4 / 8; always 1 in ln_mix_cluster). */
+ *   float4 per thread (1 / 2 / 4 / 8; always 1 in ln_mix_cluster).
+ *   Snapshots (nsnap 0 / NULL arrays: none; stages 1-3, launches 1), as a step of b200rwkv_infer_snapshots takes them:
+ *   snap_tok [nsnap] distinct step token rows in [0, T); snap_rec [nsnap][snap_ld] f32 in/out, uploaded first, snap_ld >=
+ *   snap_off + C, snap_off and snap_ld multiples of 4 (the kernels store records as 16-byte vectors).  A stage that commits
+ *   (commit_src / commit_dst given; ln_out requires it) copies commit_src row snap_tok[k] to snap_rec[k] + snap_off; without
+ *   a commit the records are left alone.  ln_out also writes LN(a) of every snapshot token that has no head row, the k-th
+ *   such token of snap_tok at row k, into snap_head_out [rows_x][C] f16 bits (required with ln_out snapshots), de-tiled:
+ *   rows_x = 32 with precision 1 (hi at row k, lo at row k + 16), else 16 x mt(X) for X such tokens (mt: 1, 2, 4, 8 token
+ *   tiles for X <= 16 / 32 / 64 / 128; when X = 0 it may have no rows and is not read). */
 typedef struct {
     int32_t stage, C, S, nslot;
     const int32_t *slot, *count;
@@ -476,6 +492,11 @@ typedef struct {
     const uint32_t* tokens;
     uint16_t* head_out;
     int32_t* kernel_out;
+    int32_t nsnap;
+    const int32_t* snap_tok;
+    float* snap_rec;
+    int64_t snap_ld, snap_off;
+    uint16_t* snap_head_out;
 } b200rwkv_ln_args;
 int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args);
 

@@ -213,10 +213,15 @@ def test_ctypes_structs_match_the_header(tmp_path):
                    '  offsetof(b200rwkv_wkv_args, precision), offsetof(b200rwkv_wkv_args, r), offsetof(b200rwkv_wkv_args, nu),\n'
                    '  offsetof(b200rwkv_wkv_args, layer0), offsetof(b200rwkv_wkv_args, v_first), offsetof(b200rwkv_wkv_args, Dd),\n'
                    '  offsetof(b200rwkv_wkv_args, out));\n'
+                   '  printf("%zu %zu %zu %zu %zu\\n", offsetof(b200rwkv_wkv_args, nsnap), offsetof(b200rwkv_wkv_args, snap_tok),\n'
+                   '  offsetof(b200rwkv_wkv_args, snap_rec), offsetof(b200rwkv_wkv_args, snap_ld), offsetof(b200rwkv_wkv_args, snap_off));\n'
                    '  printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b200rwkv_ln_args), offsetof(b200rwkv_ln_args, slot),\n'
                    '  offsetof(b200rwkv_ln_args, precision), offsetof(b200rwkv_ln_args, x_in), offsetof(b200rwkv_ln_args, parts),\n'
                    '  offsetof(b200rwkv_ln_args, n_mix), offsetof(b200rwkv_ln_args, mix_out), offsetof(b200rwkv_ln_args, Dm),\n'
                    '  offsetof(b200rwkv_ln_args, V), offsetof(b200rwkv_ln_args, kernel_out));\n'
+                   '  printf("%zu %zu %zu %zu %zu %zu\\n", offsetof(b200rwkv_ln_args, nsnap), offsetof(b200rwkv_ln_args, snap_tok),\n'
+                   '  offsetof(b200rwkv_ln_args, snap_rec), offsetof(b200rwkv_ln_args, snap_ld), offsetof(b200rwkv_ln_args, snap_off),\n'
+                   '  offsetof(b200rwkv_ln_args, snap_head_out));\n'
                    '  printf("%zu %zu %zu %zu %zu\\n", sizeof(b200rwkv_keep_args), offsetof(b200rwkv_keep_args, slot),\n'
                    '  offsetof(b200rwkv_keep_args, world), offsetof(b200rwkv_keep_args, shards), offsetof(b200rwkv_keep_args, keep));\n'
                    '  printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b200rwkv_weight_args), offsetof(b200rwkv_weight_args, n),\n'
@@ -231,8 +236,11 @@ def test_ctypes_structs_match_the_header(tmp_path):
                    C.sizeof(G), G.act.offset, G.lerp_xx.offset, G.out.offset,
                    C.sizeof(W), W.slot.offset, W.precision.offset, W.r.offset, W.nu.offset, W.layer0.offset, W.v_first.offset,
                    W.Dd.offset, W.out.offset,
+                   W.nsnap.offset, W.snap_tok.offset, W.snap_rec.offset, W.snap_ld.offset, W.snap_off.offset,
                    C.sizeof(L), L.slot.offset, L.precision.offset, L.x_in.offset, L.parts.offset, L.n_mix.offset,
                    L.mix_out.offset, L.Dm.offset, L.V.offset, L.kernel_out.offset,
+                   L.nsnap.offset, L.snap_tok.offset, L.snap_rec.offset, L.snap_ld.offset, L.snap_off.offset,
+                   L.snap_head_out.offset,
                    C.sizeof(K), K.slot.offset, K.world.offset, K.shards.offset, K.keep.offset,
                    C.sizeof(WA), WA.n.offset, WA.scale.offset, WA.dst.offset, WA.w.offset, WA.out.offset, WA.alpha.offset,
                    WA.rows.offset, WA.blocks.offset]
@@ -319,8 +327,25 @@ def test_op_wkv_refuses_bad_arguments_without_a_gpu():
         return capi.lib().b200rwkv_op_wkv(0, C.byref(a))
 
     fold = dict(w=None, d1=P(d1), time_decay_w2=P(w2), decay_bias=P(vec), Dd=Dd)
+    rec = np.zeros((3, 8 + H * 4096), np.float32)
+    snap_toks = {n: np.array(t, np.int32) for n, t in (("ok", (0, 2, 4)), ("T", (0, 5, 1)), ("neg", (-1, 2, 4)), ("twice", (1, 3, 1)))}
+
+    def snap(tok="ok", n=3, ld=8 + H * 4096, off=8, **kw):
+        return {**dict(nsnap=n, snap_tok=P(snap_toks[tok]), snap_rec=P(rec), snap_ld=ld, snap_off=off), **kw}
+
     INV, UNS, STA = capi.ERR_INVALID, capi.ERR_UNSUPPORTED, capi.ERR_STATE
     cases = {
+        "negative nsnap": (call(args(**snap(n=-1))), INV),
+        "snapshots without tokens": (call(args(**snap(snap_tok=None))), INV),
+        "snapshots without records": (call(args(**snap(snap_rec=None))), INV),
+        "snapshot token T": (call(args(**snap("T"))), INV),
+        "negative snapshot token": (call(args(**snap("neg"))), INV),
+        "snapshot token twice": (call(args(**snap("twice"))), INV),
+        "snap_ld < snap_off + H * 4096": (call(args(**snap(ld=4 + H * 4096))), INV),
+        "negative snap_off": (call(args(**snap(off=-1))), INV),
+        "snap_off past the int64 range": (call(args(**snap(off=2 ** 63 - 4))), INV),
+        "snap_off % 4": (call(args(**snap(off=2))), INV),
+        "snap_ld % 4": (call(args(**snap(ld=10 + H * 4096))), INV),
         "null arguments": (capi.lib().b200rwkv_op_wkv(0, None), INV),
         "version 4": (call(args(version=4)), UNS),
         "H = 0": (call(args(H=0)), INV),
@@ -360,7 +385,8 @@ def test_op_wkv_refuses_bad_arguments_without_a_gpu():
     for name, (got, want) in cases.items():
         assert got == want, name
     if not _has_gpu():                       # well-formed arguments reach the device, and there is none: no CPU fallback
-        for ok in (args(), args(**fold), args(version=5), args(version=7, layer0=0), args(counts=(8, 8), precision=1)):
+        for ok in (args(), args(**fold), args(version=5), args(version=7, layer0=0), args(counts=(8, 8), precision=1),
+                   args(**snap()), args(**snap(n=0, snap_tok=None, snap_rec=None))):
             assert call(ok) == capi.ERR_CUDA
 
 
@@ -395,8 +421,30 @@ def test_op_ln_refuses_bad_arguments_without_a_gpu():
         return capi.lib().b200rwkv_op_ln(0, C.byref(a))
 
     six = dict(stage=capi.LN_FRONT6, n_mix=1)
+    rec = np.zeros((3, 8 + Cc), np.float32)
+    snap_toks = {n: np.array(t, np.int32) for n, t in (("ok", (0, 2, 4)), ("T", (0, 5, 1)), ("neg", (-1, 2, 4)), ("twice", (1, 3, 1)))}
+
+    def snap(tok="ok", n=3, ld=8 + Cc, off=8, **kw):
+        return {**dict(nsnap=n, snap_tok=P(snap_toks[tok]), snap_rec=P(rec), snap_ld=ld, snap_off=off, snap_head_out=P(a16)), **kw}
+
     INV, UNS, STA = capi.ERR_INVALID, capi.ERR_UNSUPPORTED, capi.ERR_STATE
     cases = {
+        "negative nsnap": (call(args(**snap(n=-1))), INV),
+        "snapshots without tokens": (call(args(**snap(snap_tok=None))), INV),
+        "snapshots without records": (call(args(**snap(snap_rec=None))), INV),
+        "snapshot token T": (call(args(**snap("T"))), INV),
+        "negative snapshot token": (call(args(**snap("neg"))), INV),
+        "snapshot token twice": (call(args(**snap("twice"))), INV),
+        "snap_ld < snap_off + C": (call(args(**snap(ld=4 + Cc))), INV),
+        "negative snap_off": (call(args(**snap(off=-1))), INV),
+        "snap_off past the int64 range": (call(args(**snap(off=2 ** 63 - 4))), INV),
+        "snap_off % 4": (call(args(**snap(off=2))), INV),
+        "snap_ld % 4": (call(args(**snap(ld=10 + Cc))), INV),
+        "snapshots on the embed stage": (call(args(stage=capi.LN_EMBED, **snap())), INV),
+        "snapshots over two launches": (call(args(launches=2, **snap())), INV),
+        "ln_out snapshots without the commit": (call(args(stage=capi.LN_OUT, commit_src=None, commit_dst=None, **snap())), INV),
+        "ln_out snapshots without snap_head_out": (call(args(stage=capi.LN_OUT, **snap(snap_head_out=None))), INV),
+        "front half snapshots over two launches": (call(args(**six, launches=2, **snap())), INV),
         "null arguments": (capi.lib().b200rwkv_op_ln(0, None), INV),
         "stage 4": (call(args(stage=4)), INV),
         "C = 0": (call(args(C=0)), INV),
@@ -454,7 +502,9 @@ def test_op_ln_refuses_bad_arguments_without_a_gpu():
         assert got == want, name
     if not _has_gpu():                       # well-formed arguments reach the device, and there is none: no CPU fallback
         for ok in (args(), args(x_out=None, n_parts=0), args(**six), args(**six, precision=1), args(stage=capi.LN_OUT),
-                   args(stage=capi.LN_EMBED), args(counts=(60, 68), n_gate=8, n_parts=8)):
+                   args(stage=capi.LN_EMBED), args(counts=(60, 68), n_gate=8, n_parts=8), args(**snap()), args(**six, **snap()),
+                   args(commit_src=None, commit_dst=None, **snap()), args(stage=capi.LN_OUT, **snap()),
+                   args(stage=capi.LN_EMBED, **snap(n=0, snap_tok=None, snap_rec=None))):
             assert call(ok) == capi.ERR_CUDA
 
 

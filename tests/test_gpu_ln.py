@@ -175,8 +175,9 @@ def make_inputs(c: Case, variants):
     return x
 
 
-def run_op(c: Case, x, launches):
-    """One b200rwkv_op_ln call with sentinel-filled outputs; returns the outputs and the kernel report."""
+def run_op(c: Case, x, launches, **snap):
+    """One b200rwkv_op_ln call with sentinel-filled outputs; returns the outputs and the kernel report.  `snap`: op_ln's
+    snapshot arguments."""
     C, S, T, R = c.C, c.pool, c.T, c.rows
     L = launches
     o = dict(commit_dst=sentinel32((S, C)) if c.commit else None)
@@ -204,7 +205,7 @@ def run_op(c: Case, x, launches):
         hr = 32 if c.precision else capi.gemm_rows(max(nr, 1))
         o["head_out"] = np.full((L, hr, C), SENT16, np.uint16)
     kern = capi.op_ln(STAGE[c.stage], C, [s for s, _ in c.entries], [n for _, n in c.entries], launches=L,
-                      precision=c.precision, option=option, **kw, **o)
+                      precision=c.precision, option=option, **kw, **o, **snap)
     o["x_in_after"] = kw.get("x_in")
     return o, kern, option
 

@@ -398,6 +398,7 @@ def test_launches_added_per_snapshot_step(models, ad_model):
     assert launch_delta(m, [0], [100], [NONE], [(0, 10), (0, 40)]) == 4
     assert launch_delta(m, [0], [100], [NONE], [(0, 10), (0, 40), (0, 70), (0, 100)]) == 8
     assert launch_delta(m, [0], [100], [NONE], []) == 0
+    assert launch_delta(m, [0], [100], [NONE], [(0, p) for p in range(1, 101)]) == 8
     ma = ad_model[0]
     assert launch_delta(ma, [0], [20], [NONE], [(0, 9)]) == 3        # slot 0 is bound
     assert launch_delta(ma, [0], [20], [FULL], [(0, 9)]) == 1
@@ -408,3 +409,64 @@ def test_reuse_list_must_match_the_snapshots(models):
     m, _ = models("tiny6", max_batch=2, chunk=32)
     with pytest.raises(ValueError):
         m.infer_snapshots([0], [4], [1, 2, 3, 4], [NONE], [(0, 1), (0, 2)], reuse=[None])
+
+
+# ---- steps with more than 16 snapshot tokens without an output row (the snapshot head launch at 2, 4 and 8 token tiles) ----
+def mtx_pair(m, n, orc=None, slot=0):
+    """Call A: one NONE entry of n tokens with a snapshot at every token, in one step (chunk >= n); call B: the same tokens
+    from the same state as FULL.  Both steps have T = n and mt_bucket(X) == mt_bucket(R), so A's snapshot head launch is B's
+    head launch over other operand and output rows: every snapshot row equals B's logits row bit for bit, and every
+    snapshot state B's snapshot at the same position.  A's other outputs equal infer_ex's; spot positions match the oracle."""
+    V = m.info["num_vocab"]
+    toks = toks_for(n, 500 + n, V)
+    at = [(0, p) for p in range(1, n + 1)]
+    reset(m, [slot])
+    plain, snap_a = run_pair(m, [slot], [n], toks, [NONE], at)
+    assert_same(plain, snap_a)
+    reset(m, [slot])
+    rows_b, _, snaps_b = m.infer_snapshots([slot], [n], toks, [FULL], at)
+    for p, (sa, sb) in enumerate(zip(snap_a[6], snaps_b), 1):
+        st_a, row_a = m.state.snapshot_back(sa, with_logits=True)
+        st_b = m.state.snapshot_back(sb)
+        assert np.array_equal(row_a, rows_b[0][p - 1]), f"position {p}: snapshot row != the FULL logits row"
+        assert np.array_equal(st_a, st_b), f"position {p}: NONE and FULL snapshot states differ"
+    if orc is not None:
+        for p in sorted({1, 16, 17, n // 2, n}):
+            check_snapshot(m, orc, snap_a[6][p - 1], toks, p)
+    for s in list(snap_a[6]) + list(snaps_b):
+        s.free()
+
+
+@pytest.mark.parametrize("n", [17, 40, 100])
+@pytest.mark.parametrize("preset", ["tiny6", "tiny7", "small6"])
+def test_snapshot_head_over_token_tiles(models, preset, n):
+    m, st = models(preset, max_batch=4, chunk=128)
+    mtx_pair(m, n, O.Oracle(O.parse_st(st), "f16"))
+
+
+def test_snapshot_head_over_token_tiles_bound_adapter():
+    """The same on a bound slot of an engine whose adapter touches the head: the snapshot shrink runs over > 16 rows."""
+    st = synth.make_st("tiny6", 0)
+    ad = synth.make_lora_st("tiny6", rank=8, seed=11, targets=("att.key", "att.value", "ffn.key"))
+    m = runtime.Model(st, max_batch=4, token_chunk_size=128, adapters=[(ad, 0.75)])
+    try:
+        m.bind_adapter([1], [1])
+        w = O.parse_st(st)
+        bound = AdapterOracle(w, "f16", (O.parse_st(ad), 0.75))
+        for n in (17, 40, 100):
+            mtx_pair(m, n, bound, slot=1)
+    finally:
+        m.close()
+
+
+def test_snapshot_head_over_token_tiles_7b_layer_shape():
+    """One layer at the 7B shape with the whole 65536-token vocabulary: the production head plan at 4 and 8 token tiles."""
+    shp = dataclasses.replace(synth.PRESETS["v6-7b"], L=1)
+    st = synth.make_st(shp, 0)
+    m = runtime.Model(st, max_batch=1, token_chunk_size=128)
+    try:
+        assert m.info["num_vocab"] == 65536
+        for n in (40, 100):
+            mtx_pair(m, n)
+    finally:
+        m.close()

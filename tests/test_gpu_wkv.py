@@ -247,8 +247,9 @@ def f16_ulp(x):
     return 2.0 ** (e - 10)
 
 
-def launch(c: Case, ch, tok, state, layer=0):
-    """One b200rwkv_op_wkv call with sentinel-filled outputs; state [S, H, 64, 64] and tok["v_first"] are updated in place."""
+def launch(c: Case, ch, tok, state, layer=0, **snap):
+    """One b200rwkv_op_wkv call with sentinel-filled outputs; state [S, H, 64, 64] and tok["v_first"] are updated in place.
+    `snap`: op_wkv_step's snapshot arguments."""
     T = sum(n for _, n in c.entries)
     out = np.full((capi.gemm_rows(T, c.precision), c.H * 64), SENT16, np.uint16)
     kw = {n: x for n, x in tok.items() if n != "v_first"}
@@ -256,7 +257,8 @@ def launch(c: Case, ch, tok, state, layer=0):
     if c.version == 7:
         kw["v_first"] = tok["v_first"]
         kw["layer0"] = layer == 0
-    capi.op_wkv_step(c.version, [s for s, _ in c.entries], [n for _, n in c.entries], state, out, precision=c.precision, **kw)
+    capi.op_wkv_step(c.version, [s for s, _ in c.entries], [n for _, n in c.entries], state, out, precision=c.precision, **kw,
+                     **snap)
     return out
 
 
