@@ -3146,13 +3146,35 @@ void b200rwkv_host_free(void* p) {
     if (p) cudaFreeHost(p);
 }
 
+// The arguments of the decode routes (bench_decode, profile_step, profile_insitu), before any CUDA call, as infer checks its
+// entries: nslot in [1, min(S, maxT)], slots in [0, S) (ERR_STATE) and distinct (two WKV CTAs would read-modify-write one
+// state), token ids below V for all `nsteps` steps.
+static void check_decode_args(const b200rwkv_engine* e, int32_t nslot, const int32_t* slot, const uint32_t* tokens, int nsteps,
+                              const char* what) {
+    const std::string w(what);
+    REQUIRE(nslot >= 1 && nslot <= e->S && nslot <= e->maxT, B200RWKV_ERR_INVALID, w + ": nslot outside [1, max_batch]");
+    std::vector<char> seen(e->S, 0);
+    for (int i = 0; i < nslot; ++i) {
+        REQUIRE(slot[i] >= 0 && slot[i] < e->S, B200RWKV_ERR_STATE, w + ": slot " + std::to_string(slot[i]) + " out of range");
+        REQUIRE(!seen[slot[i]], B200RWKV_ERR_INVALID, w + ": duplicate slot " + std::to_string(slot[i]));
+        seen[slot[i]] = 1;
+    }
+    for (size_t i = 0; i < (size_t)nsteps * nslot; ++i)
+        REQUIRE(tokens[i] < (uint32_t)e->V, B200RWKV_ERR_INVALID, w + ": token id outside the vocabulary");
+}
+
+// A profiling step moves the listed slots' states on without writing their kept rows (it runs no enqueue_keep): drop them,
+// as infer does for a NONE entry with tokens.
+static void drop_kept_rows(b200rwkv_engine* e, int32_t nslot, const int32_t* slot) {
+    std::lock_guard<std::mutex> lk(e->keep_mu);
+    for (int i = 0; i < nslot; ++i) e->keep_valid[slot[i]] = 0;
+}
+
 static void build_decode_metas(b200rwkv_engine* e, int nslot, const int32_t* slot, const uint32_t* tokens, int nsteps,
                                std::vector<int>& all) {
     all.assign((size_t)nsteps * e->meta_ints, 0);
     std::vector<int> s_slots(slot, slot + nslot), s_counts(nslot, 1), s_out(nslot, 1);
     std::vector<const uint32_t*> s_toks(nslot);
-    for (size_t i = 0; i < (size_t)nsteps * nslot; ++i)
-        REQUIRE(tokens[i] < (uint32_t)e->V, B200RWKV_ERR_INVALID, "token id outside the vocabulary");
     for (int st = 0; st < nsteps; ++st) {
         for (int i = 0; i < nslot; ++i) s_toks[i] = tokens + (size_t)st * nslot + i;
         int R = 0;
@@ -3164,11 +3186,11 @@ static int32_t rank_bench_decode(b200rwkv_engine* e, int32_t nslot, const int32_
                               int32_t steps, int32_t flush_l2, float* ms_out, int64_t* launches_out, float* step_ms_out) {
     API_BEGIN(e)
     REQUIRE(e && slot && tokens && ms_out, B200RWKV_ERR_INVALID, "null argument");
-    REQUIRE(nslot >= 1 && nslot <= e->S && nslot <= e->maxT && steps >= 1 && warmup >= 0, B200RWKV_ERR_INVALID, "bad argument");
-    for (int i = 0; i < nslot; ++i) REQUIRE(slot[i] >= 0 && slot[i] < e->S, B200RWKV_ERR_STATE, "slot out of range");
+    REQUIRE(steps >= 1 && warmup >= 0, B200RWKV_ERR_INVALID, "bench_decode: bad step count");
+    const int nsteps = warmup + steps;
+    check_decode_args(e, nslot, slot, tokens, nsteps, "bench_decode");
     std::lock_guard<std::mutex> lk(e->mu);
     CK(cudaSetDevice(e->dev));
-    const int nsteps = warmup + steps;
     std::vector<int> all;
     build_decode_metas(e, nslot, slot, tokens, nsteps, all);
     long long launches_before = 0;
@@ -3212,13 +3234,14 @@ static int32_t rank_profile_step(b200rwkv_engine* e, int32_t nslot, const int32_
                               int32_t launches[4], int64_t* gemm_weight_bytes) {
     API_BEGIN(e)
     REQUIRE(e && slot && tokens && ms && launches, B200RWKV_ERR_INVALID, "null argument");
-    REQUIRE(nslot >= 1 && nslot <= e->S && nslot <= e->maxT, B200RWKV_ERR_INVALID, "bad argument");
+    check_decode_args(e, nslot, slot, tokens, 1, "profile_step");
     std::lock_guard<std::mutex> lk(e->mu);
     CK(cudaSetDevice(e->dev));
     std::vector<int> all;
     build_decode_metas(e, nslot, slot, tokens, 1, all);
     CK(cudaMemcpyAsync(e->d_meta, all.data(), e->meta_ints * 4, cudaMemcpyHostToDevice, e->stream));
     CK(cudaStreamSynchronize(e->stream));
+    drop_kept_rows(e, nslot, slot);
     Profiler prof;
     StepShape sh = e->step_shape(nslot, nslot);
     sh.ad = e->step_bound(std::vector<int>(slot, slot + nslot));      // bound slots: the adapter plans and their shrinks
@@ -3246,13 +3269,14 @@ static int32_t rank_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int3
     API_BEGIN(e)
     REQUIRE(e && slot && tokens && n_out && types && start_us && end_us && bytes && step_us && reps >= 1 && cap >= 1, B200RWKV_ERR_INVALID,
             "bad argument");
-    REQUIRE(nslot >= 1 && nslot <= e->S && nslot <= e->maxT, B200RWKV_ERR_INVALID, "bad argument");
+    check_decode_args(e, nslot, slot, tokens, 1, "profile_insitu");
     std::lock_guard<std::mutex> lk(e->mu);
     CK(cudaSetDevice(e->dev));
     if (!e->d_step_trace) e->d_step_trace = (unsigned long long*)e->dalloc((size_t)b200rwkv_engine::STEP_TRACE_MAX * b200rwkv_engine::STEP_TRACE_ROW * 8, true);
     std::vector<int> all;
     build_decode_metas(e, nslot, slot, tokens, 1, all);
     CK(cudaMemcpyAsync(e->d_meta, all.data(), e->meta_ints * 4, cudaMemcpyHostToDevice, e->stream));
+    drop_kept_rows(e, nslot, slot);
     StepShape sh = e->step_shape(nslot, nslot);
     sh.ad = e->step_bound(std::vector<int>(slot, slot + nslot));
     // traced copy of the step graph (the production graphs carry null trace pointers)

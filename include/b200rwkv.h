@@ -365,7 +365,12 @@ void b200rwkv_host_free(void* p);
 /* Measurement hook used by bench.py for the kernel-resident number: runs `warmup + steps`
  * decode steps (one token per listed slot per step) with token ids staged in HBM beforehand,
  * no host<->device traffic inside the timed region; returns CUDA-event milliseconds for the
- * `steps` timed steps and the number of kernel launches in that region. */
+ * `steps` timed steps and the number of kernel launches in that region.
+ * The steps are real: they compute bit for bit what b200rwkv_infer computes for the same tokens fed one LAST step at a
+ * time, so every listed slot's state advances by warmup + steps tokens and its kept row becomes the last step's row.
+ * Refused before any CUDA call, with nothing changed: nslot outside [1, max_batch], a duplicate slot, a token id >=
+ * num_vocab, steps < 1 or warmup < 0 are B200RWKV_ERR_INVALID; a slot out of range B200RWKV_ERR_STATE.  The two profiling
+ * calls below make the same slot, token and nslot checks. */
 int32_t b200rwkv_bench_decode(b200rwkv_engine*, int32_t nslot, const int32_t* slot,
                               const uint32_t* tokens /* [(warmup+steps) * nslot] */, int32_t warmup,
                               int32_t steps, int32_t flush_l2, float* ms_out, int64_t* launches_out,
@@ -373,7 +378,9 @@ int32_t b200rwkv_bench_decode(b200rwkv_engine*, int32_t nslot, const int32_t* sl
 
 /* Per-kernel-class device time of ONE un-graphed decode step, CUDA events around every launch
  * on the engine's stream.  classes: 0 = projection GEMMs, 1 = WKV, 2 = LN/mix/embed, 3 = other.
- * ms[4], launches[4], and the algorithmic weight bytes streamed by the step's GEMM launches. */
+ * ms[4], launches[4], and the algorithmic weight bytes streamed by the step's GEMM launches.
+ * The step is real and fully serialised (no programmatic dependent launch): every listed slot's state advances by its token,
+ * bit for bit as a b200rwkv_infer step of the same tokens, and the slots are left without a kept row (as after a NONE entry). */
 int32_t b200rwkv_profile_step(b200rwkv_engine*, int32_t nslot, const int32_t* slot,
                               const uint32_t* tokens, float ms[4], int32_t launches[4],
                               int64_t* gemm_weight_bytes);
@@ -382,7 +389,9 @@ int32_t b200rwkv_profile_step(b200rwkv_engine*, int32_t nslot, const int32_t* sl
  * window = [griddepcontrol.wait released, last CTA exit]; consecutive windows cannot overlap, so class sums are <= the step.
  * types[i]: 0 LN / mix, 2 WKV, 6 fused RWKV-6 front half, 1000000 + weight MiB for a projection launch; bytes[i]: algorithmic
  * weight bytes of a projection launch (else 0); start_us / end_us relative to the first stamp of the step, averaged over
- * `reps` replays; step_us = last exit - first entry.  bench.py's `roofline` comes from here. */
+ * `reps` replays; step_us = last exit - first entry.  bench.py's `roofline` comes from here.
+ * The replays are real steps: every listed slot's state advances reps + 1 times by the same token (a warm-up replay, then
+ * `reps`), bit for bit as reps + 1 b200rwkv_infer steps of those tokens, and the slots are left without a kept row. */
 int32_t b200rwkv_profile_insitu(b200rwkv_engine*, int32_t nslot, const int32_t* slot, const uint32_t* tokens, int32_t reps,
                                 int32_t cap, int32_t* n_out, int32_t* types, double* start_us, double* end_us, int64_t* bytes,
                                 double* step_us);

@@ -197,6 +197,15 @@ class Oracle:
                 self._mat_cache[name] = m
         return m
 
+    def keep_all_matrices(self) -> "Oracle":
+        """Convert every matrix to f32 once and keep it, large ones included: at the 7B layer shape the channel-mix
+        matrices are otherwise converted again for every token, which costs far more than the products themselves.
+        Costs 4 bytes per weight of host memory; the results are unchanged."""
+        for name, m in self.w.items():
+            if m.ndim == 2 and name != "emb.weight":
+                self._mat_cache[name] = _f(m)
+        return self
+
     def _mv(self, name, x):
         """y = W @ q(x); W stored [out, in]."""
         return self._mat(name) @ self._q(x)
