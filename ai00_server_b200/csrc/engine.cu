@@ -631,7 +631,8 @@ struct b200rwkv_engine {
     std::map<int, StepGraph> graphs;
     long long launch_total = 0;                // kernels launched by this engine's steps since creation
     long long launches_last_step = 0;
-    int last_T = 0, last_th = 16;      // tokens / A16 token rows of the most recent step
+    int last_T = 0;                    // tokens of the most recent step
+    StepShape last_sh{1, 0, 16, 16, 16, false};     // shape of the most recent step, replays included (debug_read)
 
     // softmax
     Buf<float> sm_in, sm_out;
@@ -1860,7 +1861,7 @@ void b200rwkv_engine::enqueue_shrink(const AdapterParams& p0, const StepShape& s
 // -----------------------------------------------------------------------------------------
 void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler* prof) {
     launches_last_step = 0;
-    last_th = sh.th;
+    last_sh = sh;
     auto gemm = [&](const GemmLaunch& g, bool head = false) {
         GemmLaunch g2 = g;
         if (d_step_trace && trace_capture) {
@@ -2043,6 +2044,7 @@ void b200rwkv_engine::run_step(const StepShape& sh) {
     }
     CK(cudaGraphLaunch(it->second.exec, stream));
     launch_total += it->second.launches;         // kernels of THIS graph, not of whichever was captured last
+    last_sh = sh;                                // a replay of a cached graph runs this shape, whatever was captured last
 }
 
 // The device table of step buffers the LN stages record into: cell l is set for the layers keep_hidden_layers or
@@ -4121,7 +4123,8 @@ int32_t b200rwkv_debug_read(b200rwkv_engine* e, const char* name, float* out, si
         struct F { const char* n; float* p; int cols; };
         const F fs[] = {{"x_a", e->x_a, e->C}, {"x_b", e->x_b, e->C}, {"xx1", e->xx1, e->C}, {"sx1", e->sx1, e->C}, {"xx2", e->xx2, e->C},
                         {"r", e->f_r, e->Cl}, {"k", e->f_k, e->Cl}, {"v", e->f_v, e->Cl}, {"g", e->f_g, e->Cl}, {"w", e->f_w, e->Cl},
-                        {"a", e->f_a, e->Cl}, {"nu", e->f_nu, e->Cl}, {"rr", e->f_rr, e->Cl}, {"part_att", e->part_att, e->C},
+                        {"a", e->f_a, e->Cl}, {"nu", e->f_nu, e->Cl}, {"v_first", e->f_vfirst, e->Cl}, {"rr", e->f_rr, e->Cl},
+                        {"part_att", e->part_att, e->C},
                         {"part_ffn", e->part_ffn, e->C}, {"hidden", e->d_hidden, e->C}};
         for (const F& f : fs)
             if (n == f.n) {
@@ -4152,14 +4155,19 @@ int32_t b200rwkv_debug_read(b200rwkv_engine* e, const char* name, float* out, si
         as.push_back({"a_out", &e->a_out, e->Cl, 0});
         as.push_back({"a_kk", &e->a_kk, e->Fl, 0});
         as.push_back({"a_head", &e->a_head, e->C, 0});
+        // "<buffer>_lo": the lo halves of a split operand (token rows 16..31), after a step that ran split operands
+        const bool lo = n.size() > 3 && n.compare(n.size() - 3, 3, "_lo") == 0;
+        const std::string base = lo ? n.substr(0, n.size() - 3) : n;
         for (const A& a : as)
-            if (n == a.n && a.b->p) {
+            if (base == a.n && a.b->p) {
+                REQUIRE(!lo || e->last_sh.split, B200RWKV_ERR_STATE, "debug_read: the last step did not run split operands, " + n + " has no lo half");
                 REQUIRE((size_t)T * a.cols <= cap, B200RWKV_ERR_INVALID, "debug buffer too small");
-                // T rows through the layout of the last captured step (last_th): a cached graph replay keeps last_th, so T may exceed it
-                std::vector<uint16_t> h(a.b->halves_per_matrix), rows((size_t)T * a.cols);
+                // the head's operand holds the step's output rows (th_rows), every other operand its token rows (th)
+                const int tr = (a.b == &e->a_head) ? e->last_sh.th_rows : e->last_sh.th, r0 = lo ? 16 : 0;
+                std::vector<uint16_t> h(a.b->halves_per_matrix), rows((size_t)(r0 + T) * a.cols);
                 CK(cudaMemcpy(h.data(), a.b->p + (size_t)a.mat * a.b->halves_per_matrix, h.size() * 2, cudaMemcpyDeviceToHost));
-                a16_unpack(h, a.cols, a.cols, e->last_th, T, 0, a.cols, rows.data());
-                for (size_t i = 0; i < (size_t)T * a.cols; ++i) out[i] = __half2float(__ushort_as_half(rows[i]));
+                a16_unpack(h, a.cols, a.cols, tr, r0 + T, 0, a.cols, rows.data());
+                for (size_t i = 0; i < (size_t)T * a.cols; ++i) out[i] = __half2float(__ushort_as_half(rows[(size_t)r0 * a.cols + i]));
                 return a.cols;
             }
         throw Error(B200RWKV_ERR_INVALID, "unknown debug buffer: " + n);

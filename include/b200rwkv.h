@@ -638,8 +638,13 @@ int32_t b200rwkv_last_hidden_layer(b200rwkv_engine*, int32_t layer, float* out, 
 int32_t b200rwkv_keep_hidden_pooled(b200rwkv_engine*, int32_t n, const int32_t* layers, int32_t mode);
 int32_t b200rwkv_last_hidden_pooled(b200rwkv_engine*, int32_t layer, float* out, size_t cap, int32_t* ntok_out);
 
-/* Test aid: copy a named internal activation buffer of the most recent step to the host as f32
- * row-major; returns the column count (negative status on error).  Not on the product path. */
+/* Test aid: copy a named internal activation buffer of the last layer of the most recent step to the host as f32
+ * row-major, one row per token of that step; returns the column count (negative status on error).  Not on the product
+ * path.  f32 buffers: x_a, x_b, xx1, sx1, xx2, r, k, v, g, w, a, nu, v_first (RWKV-7: the value rows layer 0 wrote),
+ * rr, part_att and part_ffn (split-K slices summed in slice order), hidden.  f16 operands: a_x0..a_x5,
+ * a_lora<i>_<m>, a_out, a_kk, and a_head, whose first rows are the step's output rows.  An f16 operand name with the
+ * suffix "_lo" reads the lo halves of split (hi + lo) operands; the plain name reads the hi halves.  "_lo" is refused
+ * with B200RWKV_ERR_STATE when the most recent step did not run split operands. */
 int32_t b200rwkv_debug_read(b200rwkv_engine*, const char* name, float* out, size_t cap);
 
 /* Profiling aid: raw stamp rows of the most recent b200rwkv_profile_insitu replay, one row of 512 uint64 per launch

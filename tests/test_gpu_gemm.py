@@ -137,6 +137,26 @@ def run(name, T, segs, precision=0, quant=capi.QUANT_NONE, grid=0, launches=3, e
     return plan
 
 
+def project64(xf, w, bias, act, eps=EPS, dz=0.0):
+    """float64 act(xf W^T + bias) of operand rows xf [M, K] (the values the kernel multiplies) and its per-element bound
+    before any f16 hand-off: eps sum_k |x_k W_nk| + dz (an error the caller knows its operand carries, already multiplied
+    through |W|) and the bias add, carried through the activation over the interval it spans, plus a few f32 ulps."""
+    N = w.shape[0]
+    xa = np.abs(xf)
+    z = np.empty((xf.shape[0], N))
+    S = np.empty_like(z)
+    for n0 in range(0, N, 8192):                               # the 65536-row head in chunks
+        wc = w[n0:n0 + 8192].astype(np.float64)
+        z[:, n0:n0 + 8192] = xf @ wc.T
+        S[:, n0:n0 + 8192] = xa @ np.abs(wc).T
+    if bias is not None:
+        z += np.asarray(bias, np.float64)
+    e = eps * S + dz + 2.0 ** -22 * np.abs(z)                  # error of the pre-activation value (accumulation, bias add)
+    y = act64(z, act)
+    dev = np.maximum(np.abs(act64(z - e, act) - y), np.abs(act64(z + e, act) - y))
+    return y, dev + 8 * 2.0 ** -24 * np.abs(y) + 1e-30
+
+
 def check(s, d, T, precision, quant, eps, wseed):
     N, K = s["N"], s["K"]
     out, launches = d["out"], d["x"].shape[0]
@@ -144,20 +164,8 @@ def check(s, d, T, precision, quant, eps, wseed):
     a16 = s["out_mode"] != capi.OUT_F32
     w = dequantised(N, K, wseed, s.get("edge", False), quant) if quant else d["w"]
     x = d["x"].astype(np.float64) if split else d["x"].astype(np.float16).astype(np.float64)
-    xf, xa = x.reshape(-1, K), np.abs(x.reshape(-1, K))
-    z = np.empty((xf.shape[0], N))
-    S = np.empty_like(z)
-    for n0 in range(0, N, 8192):                               # the 65536-row head in chunks
-        wc = w[n0:n0 + 8192].astype(np.float64)
-        z[:, n0:n0 + 8192] = xf @ wc.T
-        S[:, n0:n0 + 8192] = xa @ np.abs(wc).T
-    z, S = z.reshape(launches, T, N), S.reshape(launches, T, N)
-    if "bias" in d:
-        z += d["bias"].astype(np.float64)
-    e = eps * S + 2.0 ** -22 * np.abs(z)                       # error of the pre-activation value (accumulation, bias add)
-    y = act64(z, s["act"])
-    dev = np.maximum(np.abs(act64(z - e, s["act"]) - y), np.abs(act64(z + e, s["act"]) - y))
-    bound = dev + 8 * 2.0 ** -24 * np.abs(y) + 1e-30
+    y, bound = project64(x.reshape(-1, K), w, d.get("bias"), s["act"], eps)
+    y, bound = y.reshape(launches, T, N), bound.reshape(launches, T, N)
     if s["out_mode"] == capi.OUT_LERP_A16:
         xx, sx, mu = (d[k].astype(np.float64) for k in ("xx", "sx", "mu"))
         lerp = xx + sx * (mu + y)
