@@ -39,7 +39,7 @@ class Options(C.Structure):
     _fields_ = [("struct_bytes", C.c_uint32), ("max_batch", C.c_int32), ("token_chunk_size", C.c_int32), ("precision", C.c_int32),
                 ("num_devices", C.c_int32), ("devices", C.c_int32 * 8), ("num_lora", C.c_int32),
                 ("lora_st", C.c_void_p * MAX_LORA), ("lora_len", C.c_size_t * MAX_LORA), ("lora_alpha", C.c_float * MAX_LORA),
-                ("quant_layers", C.c_int32), ("quant_type", C.c_int32)]
+                ("quant_layers", C.c_int32), ("quant_type", C.c_int32), ("batch_invariant", C.c_int32)]
 
 
 QUANT_NONE, QUANT_INT8, QUANT_NF4 = 0, 1, 2
@@ -83,24 +83,26 @@ class LnArgs(C.Structure):
                 (n, C.c_void_p) for n in ("W1", "W2", "mu5", "lora_out", "out5", "emb")] + [
                 ("V", C.c_int32), ("tokens", C.c_void_p), ("head_out", C.c_void_p), ("kernel_out", C.c_void_p),
                 ("nsnap", C.c_int32), ("snap_tok", C.c_void_p), ("snap_rec", C.c_void_p), ("snap_ld", C.c_int64),
-                ("snap_off", C.c_int64), ("snap_head_out", C.c_void_p)]
+                ("snap_off", C.c_int64), ("snap_head_out", C.c_void_p), ("batch_invariant", C.c_int32)]
 
 
 LN_EMBED, LN_MIX, LN_FRONT6, LN_OUT = range(4)                     # b200rwkv_ln_args.stage
 K_EMBED, K_LN_MIX, K_LN_MIX_CLUSTER, K_PRE6, K_LN_OUT = range(5)   # kernel_out[0]
+K_LN_MIX_CLUSTER_WIDE, K_PRE6_WIDE = 5, 6                          # the batch-invariant mode's steps of > 16 tokens
 
 
 def op_ln(stage: int, channels: int, slots, counts, launches: int = 1, precision: int = 0, option=None, device: int = 0,
-          snap_tok=None, snap_off: int = 0, **arrays):
+          snap_tok=None, snap_off: int = 0, batch_invariant: bool = False, **arrays):
     """One LN stage of a step (b200rwkv_op_ln), `launches` times back to back.  `arrays` holds the struct's array members by
     name (numpy arrays of the header's element types; absent = NULL); output arrays are updated in place.  Snapshots:
     snap_tok (token rows) with arrays snap_rec [nsnap, snap_ld] f32 and, for ln_out, snap_head_out [rows_x, C] uint16.
-    Returns kernel_out: (kernel, variant, split)."""
+    batch_invariant: the step as a batch-invariant engine runs it.  Returns kernel_out: (kernel, variant, split)."""
     slots, counts = np.ascontiguousarray(slots, np.int32), np.ascontiguousarray(counts, np.int32)
     keep = [slots, counts]
     a = LnArgs(stage=stage, C=channels, S=int(arrays.pop("S")), nslot=len(slots), slot=ptr(slots), count=ptr(counts),
                precision=precision, launches=launches, n_parts=int(arrays.pop("n_parts", 0)), n_gate=int(arrays.pop("n_gate", 0)),
-               n_mix=int(arrays.pop("n_mix", 0)), Dm=int(arrays.pop("Dm", 0)), V=int(arrays.pop("V", 0)))
+               n_mix=int(arrays.pop("n_mix", 0)), Dm=int(arrays.pop("Dm", 0)), V=int(arrays.pop("V", 0)),
+               batch_invariant=int(batch_invariant))
     if option is not None:
         option = np.ascontiguousarray(option, np.int32)
         keep.append(option)

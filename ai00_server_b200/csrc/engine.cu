@@ -466,7 +466,8 @@ struct Snapshot { Buf<float> buf, logits; };   // CachedItem {state, output} on 
 
 // The LN-stage kernel a launch picked (b200rwkv_ln_args::kernel_out): kernel, its NV (float4 per thread of the per-token
 // kernels) or Dm / 16 (pre6_kernel), and whether it wrote split (hi + lo) operands.
-enum LnKernel { LNK_EMBED = 0, LNK_MIX = 1, LNK_MIX_CLUSTER = 2, LNK_PRE6 = 3, LNK_OUT = 4 };
+// LNK_MIX_CLUSTER_WIDE / LNK_PRE6_WIDE: the batch-invariant mode's variants for steps of 17..128 tokens.
+enum LnKernel { LNK_EMBED = 0, LNK_MIX = 1, LNK_MIX_CLUSTER = 2, LNK_PRE6 = 3, LNK_OUT = 4, LNK_MIX_CLUSTER_WIDE = 5, LNK_PRE6_WIDE = 6 };
 struct LnPick { int kernel, variant, split; };
 // The launch shape of one step (b200rwkv_engine::step_shape): MT token tiles of 16 rows and MTR row tiles of the head (0: no
 // output rows), `rows` = 16 * MT rows of the per-token buffers, and the token rows th / th_rows of the step's A16 operands and
@@ -732,6 +733,10 @@ struct b200rwkv_engine {
     bool split_on = false;        // precision 1: split (hi + lo f16) projection operands, every step decode-shaped
     bool split_act = false;
     bool ln_cluster_ok = false;   // the decode-shaped cluster LN kernels of pre6.cuh fit the model
+    // b200rwkv_options.batch_invariant: steps of more than 16 tokens compute every token with the decode step's arithmetic
+    // (DESIGN.md §6, batch-invariant engines): the cluster LN stages and the RWKV-6 front half in their WIDE variants, every
+    // projection on its `grid` plan (the K split of a decode step)
+    bool batch_inv = false;
     unsigned* pre_gbar = nullptr;
     int launch_cluster = 0;                       // consumed by the next launch_k
     // profiling aid (b200rwkv_profile_insitu): 8 globaltimer stamps of CTA 0 per launch of the per-op chain
@@ -1110,7 +1115,7 @@ void b200rwkv_engine::launch_gemm(const GemmLaunch& g, const StepShape& sh, cuda
         if (p.seg[i].out_mode != OUT_F32) p.seg[i].ldo = sh.th;     // A16 outputs feed a projection of this step
     if (g.qtype != QT_NONE) {
         REQUIRE(!sh.split, B200RWKV_ERR_UNSUPPORTED, "internal: quantised projections run with f16 activations");
-        const int grid = MT >= 4 ? g.grid_wide : g.grid;
+        const int grid = MT >= 4 && !batch_inv ? g.grid_wide : g.grid;
 #define QLAUNCH(MT_, QT_) launch_k(qgemm_kernel<MT_, QT_>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<MT_, QT_>::SMEM_BYTES, p, KC_GEMM, s, prof)
         if (g.qtype == QT_INT8) {
             switch (MT) { case 1: QLAUNCH(1, QT_INT8); break; case 2: QLAUNCH(2, QT_INT8); break; case 4: QLAUNCH(4, QT_INT8); break; default: QLAUNCH(8, QT_INT8); break; }
@@ -1121,14 +1126,15 @@ void b200rwkv_engine::launch_gemm(const GemmLaunch& g, const StepShape& sh, cuda
         return;
     }
     // RING 2 = one stage less than fits, so the small kernels around a projection can share its SMs (findings r1 §7)
+    const int gw = batch_inv ? g.grid : g.grid_wide;
     switch (MT) {
         case 1:
             if (sh.split) launch_k(gemm_kernel<2, 2, true>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<2, 2>::SMEM_BYTES, p, KC_GEMM, s, prof);
             else launch_k(gemm_kernel<1, 2>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<1, 2>::SMEM_BYTES, p, KC_GEMM, s, prof);
             break;
         case 2: launch_k(gemm_kernel<2>, dim3(g.grid), dim3(GEMM_THREADS), GemmCfg<2>::SMEM_BYTES, p, KC_GEMM, s, prof); break;
-        case 4: launch_k(gemm_kernel<4>, dim3(g.grid_wide), dim3(GEMM_THREADS), GemmCfg<4>::SMEM_BYTES, p, KC_GEMM, s, prof); break;
-        default: launch_k(gemm_kernel<8>, dim3(g.grid_wide), dim3(GEMM_THREADS), GemmCfg<8>::SMEM_BYTES, p, KC_GEMM, s, prof); break;
+        case 4: launch_k(gemm_kernel<4>, dim3(gw), dim3(GEMM_THREADS), GemmCfg<4>::SMEM_BYTES, p, KC_GEMM, s, prof); break;
+        default: launch_k(gemm_kernel<8>, dim3(gw), dim3(GEMM_THREADS), GemmCfg<8>::SMEM_BYTES, p, KC_GEMM, s, prof); break;
     }
 }
 
@@ -1887,7 +1893,9 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler
         AdLayer* ad = sh.ad ? &ad_layers[l] : nullptr;      // a slot of the step is bound: W' plans and their shrinks
         // LN1 of layer l commits the channel-mix shift of layer l - 1 (layer 0's commits nothing), LN2 the time-mix shift
         const size_t off_ffn_prev = l > 0 ? (size_t)(l - 1) * rec + C + W : 0, off_att = (size_t)l * rec;
-        if (ly.has_pre6 && sh.MT == 1) {
+        if (ly.has_pre6 && (sh.MT == 1 || batch_inv)) {
+            // batch-invariant steps of > 16 tokens: LN1 as its own wide cluster launch, then the front half's phases 2 and 3
+            if (sh.MT > 1) ln_stage(ly.ln1, off_ffn_prev);
             Pre6Params q = ly.pre6;
             q.ln = ly.ln1;
             q.ln.trace = tr_next(6);
@@ -1954,10 +1962,16 @@ LnPick b200rwkv_engine::launch_embed(const EmbedParams& p, const StepShape& sh, 
 }
 
 // LN1 / LN2 of a step: the 16 x 8 cluster kernel when the whole step is decode-shaped and the row fits its slices (split
-// operands with precision 1), else one CTA per token row
+// operands with precision 1), else one CTA per token row.  In the batch-invariant mode a longer step runs the cluster
+// kernel's WIDE variant, one cluster per token row.
 LnPick b200rwkv_engine::launch_ln(const LnMixParams& p, const StepShape& sh, cudaStream_t s, Profiler* prof) {
     LnMixParams lp = p;
     lp.kq_tile = sh.th;
+    if (ln_cluster_ok && sh.MT > 1 && batch_inv) {
+        launch_cluster = PRE_CLUSTER;
+        launch_k(ln_mix_cluster_kernel<false, true>, dim3(PRE_CLUSTER * sh.rows), dim3(PRE_THREADS), 0, lp, KC_LN, s, prof);
+        return {LNK_MIX_CLUSTER_WIDE, 1, 0};
+    }
     if (ln_cluster_ok && sh.MT == 1) {
         launch_cluster = PRE_CLUSTER;
         if (sh.split) launch_k(ln_mix_cluster_kernel<true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, lp, KC_LN, s, prof);
@@ -1969,11 +1983,17 @@ LnPick b200rwkv_engine::launch_ln(const LnMixParams& p, const StepShape& sh, cud
 }
 
 // RWKV-6 decode front half (LN1 + token shift + ddlerp LoRA) as one launch of 16 clusters x 8; the caller checked
-// pre6_fits(q.Dm, C) and that the step is decode-shaped (MT == 1)
+// pre6_fits(q.Dm, C) and that the step is decode-shaped (MT == 1), or, in the batch-invariant mode, launched LN1 of the
+// longer step before it (the WIDE variant runs phases 2 and 3 over its token groups)
 LnPick b200rwkv_engine::launch_pre6(const Pre6Params& q0, const StepShape& sh, cudaStream_t s, Profiler* prof) {
     Pre6Params q = q0;
     q.ln.kq_tile = sh.th;
     launch_cluster = PRE_CLUSTER;
+    if (sh.MT > 1) {
+        if (q.Dm == 32) launch_k(pre6_kernel<2, false, true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
+        else launch_k(pre6_kernel<4, false, true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
+        return {LNK_PRE6_WIDE, q.Dm / 16, 0};
+    }
     if (sh.split) {
         if (q.Dm == 32) launch_k(pre6_kernel<2, true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
         else launch_k(pre6_kernel<4, true>, dim3(PRE_GRID), dim3(PRE_THREADS), 0, q, KC_LN, s, prof);
@@ -2752,7 +2772,7 @@ static int32_t create_rank(const uint8_t* st, size_t len, int32_t device, int32_
                            int32_t precision, int32_t rank, int32_t world, const std::vector<LoraArg>& lora, b200rwkv_engine** out,
                            int32_t quant_layers = 0, int32_t quant_type = 0,
                            const std::vector<b200rwkv_engine::LoraSrc>& adapters = {}, int32_t places = 0,
-                           uint32_t targets = 0) {
+                           uint32_t targets = 0, bool batch_inv = false) {
     API_BEGIN((b200rwkv_engine*)nullptr)
     REQUIRE(out, B200RWKV_ERR_INVALID, "null out");
     *out = nullptr;
@@ -2792,6 +2812,7 @@ static int32_t create_rank(const uint8_t* st, size_t len, int32_t device, int32_
     e->adapters = adapters;
     e->n_adapters = adapters.empty() ? places : (int)adapters.size();
     e->ad_targets = targets;
+    e->batch_inv = batch_inv;
     e->build(f);
     e->loras.clear();            // the LoRA and adapter images are only borrowed during the build
     e->adapters.clear();
@@ -3578,6 +3599,7 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
     REQUIRE(stage >= 0 && stage <= 3, B200RWKV_ERR_INVALID, "stage must be 0 (embed), 1 (LN), 2 (front half) or 3 (ln_out)");
     REQUIRE(C >= 64 && C <= LN_MAXC && C % 64 == 0, B200RWKV_ERR_INVALID, "C must be a multiple of 64 and <= 8192");
     REQUIRE(NL >= 1 && NL <= 16, B200RWKV_ERR_INVALID, "launches must be 1..16");
+    REQUIRE(x.batch_invariant == 0 || x.batch_invariant == 1, B200RWKV_ERR_INVALID, "batch_invariant must be 0 or 1");
     OpStep st(S, x.nslot, x.slot, x.count, x.precision);
     const int T = st.T;
     if (stage == 0) {
@@ -3600,8 +3622,9 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
         REQUIRE(x.x_out || x.n_parts == 0, B200RWKV_ERR_INVALID, "in place (x_out NULL) takes no parts");
     }
     if (stage == 2) {
-        REQUIRE(T <= 16 && pre6_fits(x.Dm, C), B200RWKV_ERR_UNSUPPORTED,
-                "the front half runs decode-shaped steps (T <= 16) with Dm 32 or 64, C % 128 == 0 and C <= 4096");
+        REQUIRE((T <= 16 || x.batch_invariant) && pre6_fits(x.Dm, C), B200RWKV_ERR_UNSUPPORTED,
+                "the front half runs decode-shaped steps (T <= 16; up to 128 with batch_invariant) with Dm 32 or 64, C % 128 == 0 "
+                "and C <= 4096");
         REQUIRE(x.n_mix == 1 && x.sx_out && x.W1 && x.W2 && x.mu5 && x.lora_out && x.out5, B200RWKV_ERR_INVALID,
                 "the front half needs n_mix 1, sx_out, W1, W2, mu5, lora_out and out5");
     }
@@ -3625,6 +3648,7 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
     float* d_rec = x.nsnap > 0 ? st.snap_start(x.nsnap, x.snap_tok, x.snap_rec, x.snap_ld) : nullptr;
     b200rwkv_engine* e = st.e.get();
     e->ln_cluster_ok = ln_cluster_fits(C);         // as build() decides it for a model of C channels
+    e->batch_inv = x.batch_invariant != 0;
     const StepShape& sh = st.sh;
     const int th = sh.th;
     const int hrows = std::max(sh.th_rows, 16);    // the caller's head_out has 16 rows even when the step has no output row
@@ -3734,7 +3758,10 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
     for (int l = 0; l < NL; ++l) {
         if (stage == 0) pick = e->launch_embed(em[l], sh, e->stream, nullptr);
         else if (stage == 1) pick = e->launch_ln(lm[l], sh, e->stream, nullptr);
-        else if (stage == 2) pick = e->launch_pre6(pq[l], sh, e->stream, nullptr);
+        else if (stage == 2) {
+            if (sh.MT > 1) e->launch_ln(pq[l].ln, sh, e->stream, nullptr);     // as enqueue_step runs a longer step's LN1
+            pick = e->launch_pre6(pq[l], sh, e->stream, nullptr);
+        }
         else pick = e->launch_ln_out(lo[l], sh, e->stream, nullptr);
     }
     CK(cudaGetLastError());
@@ -4377,10 +4404,25 @@ int32_t b200rwkv_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int32_t
 // Replaces `ModelBuilder...build_vN()` + `Bundle::new` + `TokioRuntime::new` (lib.rs:484-497) with everything the reference's
 // ReloadRequest carries for this path: devices (one engine object owning all tensor-parallel ranks, SURVEY.md §8b), LoRA files
 // (lib.rs:466-485), precision (lib.rs:493).
+// b200rwkv_options as this library reads it: both sizes the header has had (the one before `batch_invariant` leaves the
+// mode off), every value checked before any CUDA call
+static int32_t read_options(const b200rwkv_options* opt, bool* batch_inv) {
+    if (opt->struct_bytes != sizeof(b200rwkv_options) && opt->struct_bytes != offsetof(b200rwkv_options, batch_invariant)) {
+        g_err = "b200rwkv_options.struct_bytes does not match this library";
+        return B200RWKV_ERR_INVALID;
+    }
+    const int32_t bi = opt->struct_bytes == sizeof(b200rwkv_options) ? opt->batch_invariant : 0;
+    if (bi != 0 && bi != 1) { g_err = "b200rwkv_options.batch_invariant must be 0 or 1"; return B200RWKV_ERR_INVALID; }
+    if (bi && opt->num_devices > 1) { g_err = "the batch-invariant mode runs on one GPU (no tensor parallelism)"; return B200RWKV_ERR_UNSUPPORTED; }
+    *batch_inv = bi != 0;
+    return B200RWKV_OK;
+}
+
 int32_t b200rwkv_create_ex(const uint8_t* st, size_t len, const b200rwkv_options* opt, b200rwkv_engine** out) {
     if (!out || !opt) { g_err = "null argument"; return B200RWKV_ERR_INVALID; }
     *out = nullptr;
-    if (opt->struct_bytes != sizeof(b200rwkv_options)) { g_err = "b200rwkv_options.struct_bytes does not match this library"; return B200RWKV_ERR_INVALID; }
+    bool batch_inv = false;
+    if (const int32_t rc = read_options(opt, &batch_inv)) return rc;
     const int world = opt->num_devices <= 0 ? 1 : opt->num_devices;
     if (!(world == 1 || world == 2 || world == 4 || world == 8)) { g_err = "num_devices must be 1, 2, 4 or 8"; return B200RWKV_ERR_INVALID; }
     if (opt->num_lora < 0 || opt->num_lora > B200RWKV_MAX_LORA) { g_err = "bad num_lora"; return B200RWKV_ERR_INVALID; }
@@ -4388,7 +4430,8 @@ int32_t b200rwkv_create_ex(const uint8_t* st, size_t len, const b200rwkv_options
     for (int i = 0; i < opt->num_lora; ++i) lora.push_back({opt->lora_st[i], opt->lora_len[i], opt->lora_alpha[i]});
     const int dev0 = opt->num_devices <= 0 ? 0 : opt->devices[0];
     if (world == 1)
-        return create_rank(st, len, dev0, opt->max_batch, opt->token_chunk_size, opt->precision, 0, 1, lora, out, opt->quant_layers, opt->quant_type);
+        return create_rank(st, len, dev0, opt->max_batch, opt->token_chunk_size, opt->precision, 0, 1, lora, out, opt->quant_layers, opt->quant_type,
+                           {}, 0, 0, batch_inv);
     if (opt->quant_layers > 0 && opt->quant_type != B200RWKV_QUANT_NONE) { g_err = "quantised layers are single-GPU in this version"; return B200RWKV_ERR_UNSUPPORTED; }
     for (int r = 0; r < world; ++r)
         for (int q = 0; q < r; ++q)
@@ -4421,7 +4464,12 @@ int32_t b200rwkv_create_adapters(const uint8_t* st, size_t len, const b200rwkv_o
     API_BEGIN((b200rwkv_engine*)nullptr)
     REQUIRE(out && opt, B200RWKV_ERR_INVALID, "null argument");
     *out = nullptr;
-    REQUIRE(opt->struct_bytes == sizeof(b200rwkv_options), B200RWKV_ERR_INVALID, "b200rwkv_options.struct_bytes does not match this library");
+    {
+        bool batch_inv = false;
+        if (const int32_t rc = read_options(opt, &batch_inv)) return rc;
+        // a bound step runs W' plans with another K split: an unbound slot's bits would depend on its neighbours' bindings
+        REQUIRE(!batch_inv, B200RWKV_ERR_UNSUPPORTED, "the batch-invariant mode does not run adapters");
+    }
     REQUIRE(n >= 1 && n <= AD_MAX, B200RWKV_ERR_INVALID, "number of adapters must be 1..8");
     REQUIRE(adapter_st && adapter_len && adapter_alpha, B200RWKV_ERR_INVALID, "null adapter list");
     REQUIRE(opt->num_devices <= 1, B200RWKV_ERR_UNSUPPORTED, "adapters run on one GPU (no tensor parallelism)");
@@ -4451,7 +4499,12 @@ int32_t b200rwkv_create_adapter_places(const uint8_t* st, size_t len, const b200
     API_BEGIN((b200rwkv_engine*)nullptr)
     REQUIRE(out && opt, B200RWKV_ERR_INVALID, "null argument");
     *out = nullptr;
-    REQUIRE(opt->struct_bytes == sizeof(b200rwkv_options), B200RWKV_ERR_INVALID, "b200rwkv_options.struct_bytes does not match this library");
+    {
+        bool batch_inv = false;
+        if (const int32_t rc = read_options(opt, &batch_inv)) return rc;
+        // a bound step runs W' plans with another K split: an unbound slot's bits would depend on its neighbours' bindings
+        REQUIRE(!batch_inv, B200RWKV_ERR_UNSUPPORTED, "the batch-invariant mode does not run adapters");
+    }
     REQUIRE(n >= 1 && n <= AD_MAX, B200RWKV_ERR_INVALID, "number of adapter places must be 1..8");
     REQUIRE(targets != 0 && (targets & ~AD_TARGET_ALL) == 0, B200RWKV_ERR_INVALID,
             "adapter targets must be a nonzero set of B200RWKV_TARGET_* bits");

@@ -177,7 +177,9 @@ __device__ __forceinline__ PreLnStatic<NMIX> pre_ln_static(const LnMixParams& p,
 }
 
 // phase 1 for token t, channel slice `rank` (thread owns channels rank*C/8 + 4*tid .. +3)
-template <int NMIX, bool SPLIT = false>
+// WIDE: a step of up to 128 tokens (the batch-invariant mode), whose A16 operands hold p.kq_tile token rows; a token's
+// arithmetic is the decode step's
+template <int NMIX, bool SPLIT = false, bool WIDE = false>
 __device__ __forceinline__ void pre_ln_slice(const LnMixParams& p, const int t, cg::cluster_group& cl, const unsigned rank,
                                              const PreLnStatic<NMIX>& st, float* red, float (*xch)[2 * PRE_CLUSTER]) {
     const int C = p.C, Cs = C / PRE_CLUSTER;
@@ -226,15 +228,18 @@ __device__ __forceinline__ void pre_ln_slice(const LnMixParams& p, const int t, 
                 uint2 o;
                 o.x = pack_h2(a.x + sx.x * mu.x, a.y + sx.y * mu.y);
                 o.y = pack_h2(a.z + sx.z * mu.z, a.w + sx.w * mu.w);
-                *reinterpret_cast<uint2*>(p.mix_out[m] + a16_index(t, c, 16)) = o;
+                *reinterpret_cast<uint2*>(p.mix_out[m] + a16_index(t, c, WIDE ? p.kq_tile : 16)) = o;
             }
         }
     }
 }
 
-// LN stage alone (channel mix of every version, time mix of RWKV-5/7): 16 clusters x 8, no grid barrier
-template <bool SPLIT = false>
+// LN stage alone (channel mix of every version, time mix of RWKV-5/7): 16 clusters x 8, no grid barrier.  WIDE (the
+// batch-invariant mode's steps of 17..128 tokens, never split): one cluster per token row of the step, so every row is
+// reduced in the decode step's order.
+template <bool SPLIT = false, bool WIDE = false>
 __global__ void __launch_bounds__(PRE_THREADS) ln_mix_cluster_kernel(const __grid_constant__ LnMixParams p) {
+    static_assert(!(SPLIT && WIDE), "split operands run decode-shaped steps only");
     __shared__ float red[32];
     __shared__ float xch[2][2 * PRE_CLUSTER];
     cg::cluster_group cl = cg::this_cluster();
@@ -247,14 +252,18 @@ __global__ void __launch_bounds__(PRE_THREADS) ln_mix_cluster_kernel(const __gri
     pdl_wait();
     trace_stamp(p.trace, 1);
     if (t >= st.T) return;                // uniform over the cluster
-    pre_ln_slice<6, SPLIT>(p, t, cl, rank, st, red, xch);
+    pre_ln_slice<6, SPLIT, WIDE>(p, t, cl, rank, st, red, xch);
     cl.sync();                            // no CTA leaves while a peer may still write into its exchange buffers
     trace_stamp(p.trace, 7);
 }
 
-// KD = Dm / 16
-template <int KD, bool SPLIT = false>
+// KD = Dm / 16.  WIDE: phases 2 and 3 of a step of 17..128 tokens (the batch-invariant mode; the wide ln_mix_cluster_kernel
+// launch before it ran phase 1 for every token): the same 16 x 8 grid walks the step's token groups of 16, so each token
+// meets the same W1 / W2 fragments, K slices and reduction order as in a decode step.  Barrier 1 stays to keep the counter
+// protocol of pre_grid_barrier.
+template <int KD, bool SPLIT = false, bool WIDE = false>
 __global__ void __launch_bounds__(PRE_THREADS, 2) pre6_kernel(const __grid_constant__ Pre6Params p) {
+    static_assert(!(SPLIT && WIDE), "split operands run decode-shaped steps only");
     __shared__ float red[32];
     __shared__ float xch[2][2 * PRE_CLUSTER];
     __shared__ __align__(16) float red2[8][PRE_NT2 * 4 * 32];
@@ -264,7 +273,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 2) pre6_kernel(const __grid_const
     const int g = blockIdx.x / PRE_CLUSTER;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, grp = lane >> 2, tig = lane & 3;
     constexpr int Dm = KD * 16;
-    constexpr int TH = SPLIT ? 32 : 16;                         // token rows of the A16 operands of a decode-shaped step
+    const int TH = WIDE ? p.ln.kq_tile : (SPLIT ? 32 : 16);     // token rows of the A16 operands (16 / 32 in a decode-shaped step)
     constexpr int NR = 5 * Dm;                                  // LoRA rows
     constexpr int RG = (NR + PRE_NCLUSTER - 1) / PRE_NCLUSTER;  // rows per cluster (10 / 20)
     static_assert(RG <= PRE_NT2 * 8, "row group does not fit the n-tiles");
@@ -322,17 +331,20 @@ __global__ void __launch_bounds__(PRE_THREADS, 2) pre6_kernel(const __grid_const
     pdl_wait();
     trace_stamp(tr, 1);
     cta_stamp(1);
-    const int T = min(st.T, 16);
+    const int T = WIDE ? st.T : min(st.T, 16);
+    const int ngrp = WIDE ? (T + 15) / 16 : 1;                  // token groups of 16
 
     // ---------------- phase 1: token g ----------------
-    if (g < T) pre_ln_slice<1, SPLIT>(p.ln, g, cl, rank, st, red, xch);
+    if (!WIDE && g < T) pre_ln_slice<1, SPLIT>(p.ln, g, cl, rank, st, red, xch);
     trace_stamp(tr, 2);
     cta_stamp(2);
     pre_grid_barrier(cl, rank, p.gbar, p.gbar + 32, nullptr, 1);
     trace_stamp(tr, 3);
 
     // ---------------- phase 2: tanh(W1 xxx), rows of cluster g, K slice `rank` ----------------
-    {
+    for (int q = 0; q < ngrp; ++q) {
+        if (q > 0) cl.sync();        // every peer has read `part` of the previous group before it is rewritten
+        const int t0 = 16 * q;
         float acc[PRE_NT2][4];
 #pragma unroll
         for (int nt = 0; nt < PRE_NT2; ++nt)
@@ -347,7 +359,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 2) pre6_kernel(const __grid_const
             for (int i = 0; i < PRE_KSW; ++i) {
                 const int kstep = warp + 8 * i;
                 const int k = (int)rank * Cs + kstep * 16;     // a 16-wide k step never straddles a 128-wide k block
-                const uint32_t* src = reinterpret_cast<const uint32_t*>(xa + a16_index(16 * sp + grp, k + tig * 2, TH));
+                const uint32_t* src = reinterpret_cast<const uint32_t*>(xa + a16_index(t0 + 16 * sp + grp, k + tig * 2, TH));
                 const bool ok = kstep < ksteps;
                 af[i][0] = ok ? __ldcg(src) : 0u;                       // (t = grp,     k lo)
                 af[i][1] = ok ? __ldcg(src + 32) : 0u;                  // (t = grp + 8, k lo)   +8 rows = 64 halves
@@ -381,7 +393,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 2) pre6_kernel(const __grid_const
 #pragma unroll
             for (int r = 0; r < PRE_CLUSTER; ++r) s += v[r];
             const int nt = o / 128, e = (o >> 5) & 3, ln = o & 31;
-            const int t = (ln >> 2) + ((e & 2) ? 8 : 0);
+            const int t = t0 + (ln >> 2) + ((e & 2) ? 8 : 0);
             const int nrow = nt * 8 + (ln & 3) * 2 + (e & 1);
             const int n = g * RG + nrow;
             if (t < T && nrow < RG && n < NR) {
@@ -403,7 +415,8 @@ __global__ void __launch_bounds__(PRE_THREADS, 2) pre6_kernel(const __grid_const
 
     trace_stamp(tr, 5);
     // ---------------- phase 3: x_j = xx + sx * (mu_j + W2_j tanh_j) ----------------
-    {
+    for (int q = 0; q < ngrp; ++q) {
+        const int t0 = 16 * q;
         uint32_t af[PRE_TILES3][KD][4];
         float2 xx[PRE_TILES3][2], sx[PRE_TILES3][2];
         float acc3[SPLIT ? PRE_TILES3 : 1][4];
@@ -416,7 +429,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 2) pre6_kernel(const __grid_const
             for (int i = 0; i < PRE_TILES3; ++i) {
                 const bool ok = tj[i] >= 0;
                 const uint32_t* src = reinterpret_cast<const uint32_t*>(p.lora + (size_t)(ok ? tj[i] : 0) * p.lora_stride +
-                                                                        a16_index(16 + grp, tig * 2, TH));
+                                                                        a16_index(t0 + 16 + grp, tig * 2, TH));
 #pragma unroll
                 for (int ks = 0; ks < KD; ++ks) {      // k16 step ks = k8 chunks 2 ks, 2 ks + 1 (TH rows x 8 halves each)
                     af[i][ks][0] = ok ? __ldcg(src + ks * TH * 8) : 0u;
@@ -433,7 +446,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 2) pre6_kernel(const __grid_const
 #pragma unroll
         for (int i = 0; i < PRE_TILES3; ++i) {
             const bool ok = tj[i] >= 0;
-            const uint32_t* src = reinterpret_cast<const uint32_t*>(p.lora + (size_t)(ok ? tj[i] : 0) * p.lora_stride + a16_index(grp, tig * 2, TH));
+            const uint32_t* src = reinterpret_cast<const uint32_t*>(p.lora + (size_t)(ok ? tj[i] : 0) * p.lora_stride + a16_index(t0 + grp, tig * 2, TH));
 #pragma unroll
             for (int ks = 0; ks < KD; ++ks) {
                 af[i][ks][0] = ok ? __ldcg(src + ks * TH * 8) : 0u;                  // chunk 2*ks, t = grp
@@ -443,7 +456,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 2) pre6_kernel(const __grid_const
             }
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int t = grp + 8 * h;
+                const int t = t0 + grp + 8 * h;
                 const size_t at = (size_t)t * C + tc0[i] + tig * 2;
                 const bool okt = ok && t < T;
                 xx[i][h] = okt ? __ldcg(reinterpret_cast<const float2*>(p.ln.xx_out + at)) : make_float2(0.f, 0.f);
@@ -463,7 +476,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 2) pre6_kernel(const __grid_const
             __half* outp = p.out[tj[i]];
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int t = grp + 8 * h;
+                const int t = t0 + grp + 8 * h;
                 if (t >= T) continue;
                 const float y0 = xx[i][h].x + sx[i][h].x * (mu3[i].x + acc[2 * h]);
                 const float y1 = xx[i][h].y + sx[i][h].y * (mu3[i].y + acc[2 * h + 1]);
@@ -477,7 +490,8 @@ __global__ void __launch_bounds__(PRE_THREADS, 2) pre6_kernel(const __grid_const
                 }
             }
         }
-    }    trace_stamp(tr, 7);
+    }
+    trace_stamp(tr, 7);
 }
 
 }  // namespace b200

@@ -100,6 +100,17 @@ typedef struct {
      * projection matrices in a weight-only quantised format; everything else stays f16).  Single GPU, precision 0 only. */
     int32_t quant_layers;
     int32_t quant_type;               /* B200RWKV_QUANT_* */
+    /* 1: batch-invariant engine.  Every per-token result of a slot (logits rows of LAST / FULL / snapshots, SCORE values and
+     * argmax ids, the kept row, the state after every token, recorded and pooled hidden rows) is then a function of the
+     * model, the precision, the slot's starting state and the tokens it has fed only: bit-identical whatever the other
+     * entries of the call are, whatever token_chunk_size is and however the tokens are cut into calls.  The reference is
+     * the decode step (one token per entry, at most 16 entries): steps of more than 16 tokens run each token with its
+     * arithmetic (DESIGN.md §6, batch-invariant engines).  0: off (the default; nothing changes).  Any other value is
+     * B200RWKV_ERR_INVALID; 1 with num_devices > 1, or with b200rwkv_create_adapters / b200rwkv_create_adapter_places, is
+     * B200RWKV_ERR_UNSUPPORTED (all before any CUDA call).  With precision 1 the flag is accepted and changes nothing: those steps are capped at 16
+     * tokens and already decode-shaped.  struct_bytes = offsetof(b200rwkv_options, batch_invariant), the size before this
+     * field, is accepted and means 0. */
+    int32_t batch_invariant;
 } b200rwkv_options;
 #define B200RWKV_QUANT_NONE 0
 #define B200RWKV_QUANT_INT8 1         /* blocks of 128 inputs: f16 (min, max) + 8-bit codes */
@@ -506,6 +517,10 @@ typedef struct {
     float* snap_rec;
     int64_t snap_ld, snap_off;
     uint16_t* snap_head_out;
+    /* 1: the step runs as a batch-invariant engine runs it (b200rwkv_options.batch_invariant); stages 1 and 2 then take T
+     * up to 128 and, above 16 tokens, launch kernel 5 (ln_mix_cluster WIDE, variant 1) / the LN launch plus kernel 6 (pre6
+     * WIDE, variant Dm / 16) when C fits the cluster kernels.  0: as before.  Other values are B200RWKV_ERR_INVALID. */
+    int32_t batch_invariant;
 } b200rwkv_ln_args;
 int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args);
 
