@@ -43,6 +43,7 @@ class Options(C.Structure):
 
 
 QUANT_NONE, QUANT_INT8, QUANT_NF4 = 0, 1, 2
+QUANT_FP8 = 4             # E4M3 codes + one f32 scale per row (3 is the reference's SF4, not implemented)
 
 # B200RWKV_TARGET_*: the kinds of matrix the places of b200rwkv_create_adapter_places can hold pairs on
 TARGET_ATT_R, TARGET_ATT_K, TARGET_ATT_V, TARGET_ATT_G = 1 << 0, 1 << 1, 1 << 2, 1 << 3
@@ -312,9 +313,14 @@ def info_from_st(st: np.ndarray) -> dict:
 
 def op_quantize(quant_type: int, w16, device: int = 0):
     """The load-time quantiser on one [N, K] f16 matrix (b200rwkv_op_quantize).  Int8: (codes u8 [N, K], min f16 [N, K/128],
-    scale f16 [N, K/128]); NF4: (level indices u8 [N, K], absmax f16 [N, K/64])."""
+    scale f16 [N, K/128]); NF4: (level indices u8 [N, K], absmax f16 [N, K/64]); FP8: (E4M3 codes u8 [N, K], scale f32 [N])."""
     w16 = np.ascontiguousarray(w16, np.float16)
     N, K = w16.shape
+    if quant_type == QUANT_FP8:
+        codes = np.empty((N, K), np.uint8)
+        scale = np.empty(N, np.float32)
+        check(lib().b200rwkv_op_quantize(device, quant_type, N, K, ptr(w16), ptr(codes), ptr(scale), None))
+        return codes, scale
     nb = K // (128 if quant_type == QUANT_INT8 else 64)
     codes = np.empty((N, K), np.uint8)
     p0 = np.empty((N, nb), np.float16)

@@ -24,6 +24,7 @@
 
 #include "gemm.cuh"
 #include "qgemm.cuh"
+#include "fp8gemm.cuh"
 #include "pre6.cuh"
 #include "sample.cuh"
 #include "misc.cuh"
@@ -724,7 +725,7 @@ struct b200rwkv_engine {
     float* vec_f32(const StFile& st, const std::string& name, size_t off, size_t count, float scale = 1.f, float bias = 0.f);
     A16Buf a16_alloc(int K, int nmat = 1);
     GemmLaunch make_launch(std::vector<SegDesc>& segs, int force_grid = 0, int qtype = QT_NONE);
-    int quant_layers = 0, quant_type = QT_NONE;     // the first `quant_layers` layers hold Int8 / NF4 projection matrices
+    int quant_layers = 0, quant_type = QT_NONE;     // the first `quant_layers` layers hold Int8 / NF4 / FP8 projection matrices
     int pick_split(int K, int tiles) const;
     void finalize_tp();
     template <typename P, typename... X>
@@ -976,8 +977,9 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
             // quantisation blocks are runs of 128 (Int8) / 64 (NF4) consecutive inputs of one output row of the FULL matrix
             REQUIRE(d.K % GEMM_BK == 0 && d.k0 % GEMM_BK == 0, B200RWKV_ERR_UNSUPPORTED,
                     "quantised projections need input dimensions that are multiples of 128");
-            g.weight_bytes += qtype == QT_INT8 ? (size_t)d.N * d.K + (size_t)d.N * (d.K / 128) * 4
-                                               : (size_t)d.N * d.K / 2 + (size_t)d.N * (d.K / 64) * 2;
+            if (qtype == QT_FP8) g.weight_bytes += (size_t)d.N * d.K + (size_t)d.N * 4;      // codes + one f32 scale per row
+            else g.weight_bytes += qtype == QT_INT8 ? (size_t)d.N * d.K + (size_t)d.N * (d.K / 128) * 4
+                                                    : (size_t)d.N * d.K / 2 + (size_t)d.N * (d.K / 64) * 2;
         }
     }
     g.p.nseg = (int)segs.size();
@@ -985,7 +987,8 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
     g.force_grid = force_grid;
     g.p.total_blocks = blk;
     g.total_tiles = tile;
-    uint8_t* W = (uint8_t*)dalloc((size_t)blk * blk_bytes, false);
+    // FP8: the launch's row scales follow its blocks, FP8_SCALE_BYTES per tile (fp8gemm.cuh)
+    uint8_t* W = (uint8_t*)dalloc((size_t)blk * blk_bytes + (qtype == QT_FP8 ? (size_t)tile * FP8_SCALE_BYTES : 0), false);
     g.p.W = W;
     for (size_t i = 0; i < segs.size(); ++i) {
         SegDesc& d = segs[i];
@@ -1002,6 +1005,15 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
             REQUIRE(t.shape.size() == 2, B200RWKV_ERR_INVALID, "internal: expected 2-D weight");
             ld = (int)t.shape[1];
             REQUIRE(d.n0 + d.N <= t.shape[0] && d.k0 + d.K <= t.shape[1], B200RWKV_ERR_INVALID, "weight shape mismatch");
+        }
+        if (qtype == QT_FP8) {
+            // one warp per row; the scale is the absmax of the whole source row, whichever k slice this segment holds
+            const int grid = std::min(cdiv(sg.tiles * GEMM_BN, 8), num_sms * 32);
+            float* scales = reinterpret_cast<float*>(W + (size_t)blk * blk_bytes) + (size_t)sg.tile_begin * GEMM_BN;
+            quantize_fp8_kernel<<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, sg.KB, W + (size_t)sg.blk_begin * blk_bytes, scales);
+            CK(cudaGetLastError());
+            CK(cudaDeviceSynchronize());
+            continue;
         }
         if (qtype != QT_NONE) {
             const size_t nwarp = (size_t)sg.tiles * sg.KB * GEMM_BN;
@@ -1116,6 +1128,12 @@ void b200rwkv_engine::launch_gemm(const GemmLaunch& g, const StepShape& sh, cuda
     if (g.qtype != QT_NONE) {
         REQUIRE(!sh.split, B200RWKV_ERR_UNSUPPORTED, "internal: quantised projections run with f16 activations");
         const int grid = MT >= 4 && !batch_inv ? g.grid_wide : g.grid;
+#define FLAUNCH(MT_) launch_k(fp8gemm_kernel<MT_>, dim3(grid), dim3(GEMM_THREADS), Fp8GemmCfg<MT_>::SMEM_BYTES, p, KC_GEMM, s, prof)
+        if (g.qtype == QT_FP8) {
+            switch (MT) { case 1: FLAUNCH(1); break; case 2: FLAUNCH(2); break; case 4: FLAUNCH(4); break; default: FLAUNCH(8); break; }
+            return;
+        }
+#undef FLAUNCH
 #define QLAUNCH(MT_, QT_) launch_k(qgemm_kernel<MT_, QT_>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<MT_, QT_>::SMEM_BYTES, p, KC_GEMM, s, prof)
         if (g.qtype == QT_INT8) {
             switch (MT) { case 1: QLAUNCH(1, QT_INT8); break; case 2: QLAUNCH(2, QT_INT8); break; case 4: QLAUNCH(4, QT_INT8); break; default: QLAUNCH(8, QT_INT8); break; }
@@ -1181,7 +1199,7 @@ int b200rwkv_engine::pick_split(int K, int tiles) const {
     return best;
 }
 
-// dynamic shared memory limits of every projection kernel launch_gemm can pick (the quantised ones only for Int8 / NF4 plans)
+// dynamic shared memory limits of every projection kernel launch_gemm can pick (the quantised ones only for quantised plans)
 static void gemm_smem_limits(int qtype) {
     CK(cudaFuncSetAttribute(gemm_kernel<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<1, 2>::SMEM_BYTES));
     CK(cudaFuncSetAttribute(gemm_kernel<2, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<2, 2>::SMEM_BYTES));
@@ -1193,6 +1211,12 @@ static void gemm_smem_limits(int qtype) {
         QATTR(1, QT_INT8); QATTR(2, QT_INT8); QATTR(4, QT_INT8); QATTR(8, QT_INT8);
         QATTR(1, QT_NF4); QATTR(2, QT_NF4); QATTR(4, QT_NF4); QATTR(8, QT_NF4);
 #undef QATTR
+    }
+    if (qtype == QT_FP8) {
+        CK(cudaFuncSetAttribute(fp8gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<1>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(fp8gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<2>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(fp8gemm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<4>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(fp8gemm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<8>::SMEM_BYTES));
     }
 }
 
@@ -1243,7 +1267,8 @@ void b200rwkv_engine::build(const StFile& st) {
     stream = new_stream();
     sm_stream = new_stream();
     if (quant_layers > 0 && quant_type != QT_NONE) {
-        REQUIRE(quant_type == QT_INT8 || quant_type == QT_NF4, B200RWKV_ERR_UNSUPPORTED, "quant_type must be Int8 or NF4 (SF4 is not implemented)");
+        REQUIRE(quant_type == QT_INT8 || quant_type == QT_NF4 || quant_type == QT_FP8, B200RWKV_ERR_UNSUPPORTED,
+                "quant_type must be Int8, NF4 or FP8 (SF4 is not implemented)");
         REQUIRE(world == 1, B200RWKV_ERR_UNSUPPORTED, "quantised layers are single-GPU in this version");
         REQUIRE(precision == 0, B200RWKV_ERR_UNSUPPORTED, "quantised layers run with precision 0 (f16 operands)");
     }
@@ -3354,14 +3379,15 @@ static int32_t rank_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int3
     API_END
 }
 
-// Operator-level entry for the parity tests: the load-time quantiser (qgemm.cuh) on one matrix, un-tiled on the host into plain
-// row-major codes and per-block parameters so that oracle/quant_numpy.py can be compared bit for bit.
+// Operator-level entry for the parity tests: the load-time quantiser (qgemm.cuh, fp8gemm.cuh) on one matrix, un-tiled on the
+// host into plain row-major codes and per-block (per-row for FP8) parameters so that oracle/quant_numpy.py and
+// tests/fp8_oracle.py can be compared bit for bit.
 int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int32_t K, const uint16_t* w_f16, uint8_t* codes,
                              uint16_t* p0, uint16_t* p1) {
     API_BEGIN((b200rwkv_engine*)nullptr)
-    REQUIRE(quant_type == QT_INT8 || quant_type == QT_NF4, B200RWKV_ERR_UNSUPPORTED, "quant_type must be Int8 or NF4");
+    REQUIRE(quant_type == QT_INT8 || quant_type == QT_NF4 || quant_type == QT_FP8, B200RWKV_ERR_UNSUPPORTED, "quant_type must be Int8, NF4 or FP8");
     REQUIRE(N >= 1 && K >= GEMM_BK && K % GEMM_BK == 0 && (size_t)N * K <= ((size_t)1 << 31) && w_f16 && codes && p0, B200RWKV_ERR_INVALID, "bad argument");
-    REQUIRE(quant_type == QT_NF4 || p1, B200RWKV_ERR_INVALID, "Int8 needs p1 (scales)");
+    REQUIRE(quant_type != QT_INT8 || p1, B200RWKV_ERR_INVALID, "Int8 needs p1 (scales)");
     CK(cudaSetDevice(device));
     const int tiles = cdiv(N, GEMM_BN), KB = K / GEMM_BK;
     const size_t blk = (size_t)q_block_bytes(quant_type), total = (size_t)tiles * KB * blk;
@@ -3372,6 +3398,19 @@ int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int3
     int nsm = 0;
     CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
     const int grid = (int)std::min<size_t>((nwarp + 7) / 8, (size_t)nsm * 32);
+    if (quant_type == QT_FP8) {
+        Buf<float> scales((size_t)tiles * FP8_SCALE_BYTES);
+        quantize_fp8_kernel<<<std::min(cdiv(tiles * GEMM_BN, 8), nsm * 32), 256>>>(src, K, 0, 0, N, tiles, KB, dst, scales);
+        CK(cudaGetLastError());
+        CK(cudaDeviceSynchronize());
+        std::vector<uint8_t> h(total);
+        CK(cudaMemcpy(h.data(), dst, total, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(p0, scales, (size_t)N * 4, cudaMemcpyDeviceToHost));
+        for (int n = 0; n < N; ++n)
+            for (int k = 0; k < K; ++k)
+                codes[(size_t)n * K + k] = h[((size_t)(n / GEMM_BN) * KB + k / GEMM_BK) * blk + fp8_code_offset(n % GEMM_BN, k % GEMM_BK)];
+        return B200RWKV_OK;
+    }
     if (quant_type == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256>>>(src, K, 0, 0, N, tiles, KB, dst);
     else quantize_weight_kernel<QT_NF4><<<grid, 256>>>(src, K, 0, 0, N, tiles, KB, dst);
     CK(cudaGetLastError());
@@ -3802,7 +3841,8 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
     REQUIRE(T >= 1 && T <= A16_MAX_ROWS, B200RWKV_ERR_INVALID, "T must be 1..128");
     REQUIRE(precision == 0 || precision == 1, B200RWKV_ERR_INVALID, "precision must be 0 or 1");
     REQUIRE(grid >= 0 && launches >= 1 && launches <= 16, B200RWKV_ERR_INVALID, "grid must be >= 0 and launches 1..16");
-    REQUIRE(quant_type == QT_NONE || quant_type == QT_INT8 || quant_type == QT_NF4, B200RWKV_ERR_UNSUPPORTED, "quant_type must be 0, 1 or 2");
+    REQUIRE(quant_type == QT_NONE || quant_type == QT_INT8 || quant_type == QT_NF4 || quant_type == QT_FP8, B200RWKV_ERR_UNSUPPORTED,
+            "quant_type must be 0, 1, 2 or 4");
     REQUIRE(precision == 0 || (T <= 16 && quant_type == QT_NONE), B200RWKV_ERR_UNSUPPORTED,
             "precision 1 runs decode-shaped steps (T <= 16) over f16 weights");
     for (int i = 0; i < nseg; ++i) {

@@ -25,7 +25,7 @@
 
 namespace b200 {
 
-enum QuantType : int { QT_NONE = 0, QT_INT8 = 1, QT_NF4 = 2 };
+enum QuantType : int { QT_NONE = 0, QT_INT8 = 1, QT_NF4 = 2, QT_FP8 = 4 };   // 3 is the reference's SF4, not implemented; FP8: fp8gemm.cuh
 
 constexpr int Q_PARAM_BYTES = GEMM_BN * 4;                                  // 4 bytes of block parameters per weight row
 constexpr int Q_INT8_BYTES = GEMM_BN * GEMM_BK + Q_PARAM_BYTES;             // 16 896
@@ -36,7 +36,9 @@ constexpr int Q_DQ_THREADS = Q_DQ_WARPS * 32;                               // =
 constexpr int QGEMM_THREADS = GEMM_THREADS + Q_DQ_THREADS;                  // consumer warpgroup + producer + 4 expansion warps
 constexpr int Q_LUT_BYTES = 256 * 32 * 4;                                   // NF4: [code byte 256][lane 32] half2
 
-__host__ __device__ constexpr int q_block_bytes(int qt) { return qt == QT_INT8 ? Q_INT8_BYTES : (qt == QT_NF4 ? Q_NF4_BYTES : GEMM_WBYTES); }
+__host__ __device__ constexpr int q_block_bytes(int qt) {
+    return qt == QT_INT8 ? Q_INT8_BYTES : (qt == QT_NF4 ? Q_NF4_BYTES : (qt == QT_FP8 ? GEMM_BN * GEMM_BK : GEMM_WBYTES));
+}
 
 __constant__ float c_nf4_levels[16] = {
     -1.0f, -0.6961928009986877f, -0.5250730514526367f, -0.39491748809814453f, -0.28444138169288635f, -0.18477343022823334f,

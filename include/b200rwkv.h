@@ -116,6 +116,10 @@ typedef struct {
 #define B200RWKV_QUANT_INT8 1         /* blocks of 128 inputs: f16 (min, max) + 8-bit codes */
 #define B200RWKV_QUANT_NF4 2          /* blocks of 64 inputs: f16 absmax + 4-bit NormalFloat codes */
                                       /* Quant::SF4 is not implemented: create_ex answers B200RWKV_ERR_UNSUPPORTED */
+#define B200RWKV_QUANT_FP8 4          /* beyond the reference's Quant enum: E4M3 codes, one f32 scale max|w| / 448 per output row
+                                       * of the whole matrix; the projection multiplies the codes' exact values with the f16
+                                       * operand in f32 and scales each output.  Same refusals as Int8 / NF4 (one GPU,
+                                       * precision 0, no adapters on its layers); batch-invariant engines run it. */
 int32_t b200rwkv_create_ex(const uint8_t* st, size_t len, const b200rwkv_options* opt, b200rwkv_engine** out);
 
 /* Several LoRA adapters on one resident base model, chosen per slot at run time (the reference can only blend LoRA files at
@@ -408,9 +412,10 @@ int32_t b200rwkv_profile_insitu(b200rwkv_engine*, int32_t nslot, const int32_t* 
                                 double* step_us);
 
 /* Operator-level entry (parity tests): the load-time quantiser on a caller-supplied row-major f16 matrix [N, K] (K % 128 == 0),
- * returned in plain order: codes [N, K] (one byte per element: Int8 code, or NF4 level index 0..15), p0 [N, K/block] (Int8: block
- * minimum, NF4: block absmax), p1 [N, K/block] (Int8: the scale f16((max - min) / 255); NF4: unused, may be NULL).  p0 / p1 are f16
- * bit patterns.  block = 128 (Int8) or 64 (NF4). */
+ * returned in plain order: codes [N, K] (one byte per element: Int8 code, NF4 level index 0..15, or FP8 E4M3 code), p0 [N, K/block]
+ * (Int8: block minimum, NF4: block absmax), p1 [N, K/block] (Int8: the scale f16((max - min) / 255); NF4, FP8: unused, may be
+ * NULL).  p0 / p1 are f16 bit patterns.  block = 128 (Int8) or 64 (NF4).  FP8: p0 receives the N f32 row scales instead
+ * (4 bytes each, 4N bytes in all). */
 int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int32_t K, const uint16_t* w_f16, uint8_t* codes,
                              uint16_t* p0, uint16_t* p1);
 
@@ -524,8 +529,8 @@ typedef struct {
 } b200rwkv_ln_args;
 int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args);
 
-/* Operator-level entry (parity tests): one projection launch -- the engine's planner (stream-K cuts, forced grids, Int8 / NF4
- * quantisation at load) and its projection kernels -- over caller-supplied matrices, no model.  Segment i computes
+/* Operator-level entry (parity tests): one projection launch -- the engine's planner (stream-K cuts, forced grids, Int8 / NF4 /
+ * FP8 quantisation at load; quant_type B200RWKV_QUANT_*, SF4 refused) and its projection kernels -- over caller-supplied matrices, no model.  Segment i computes
  * act(x W^T + bias) with W [N, K] (row-major f16 bits) and x [launches][T][K] f32, rounded to the f16 operand on the device
  * (precision 0) or split into an f16 hi + lo pair (precision 1: T <= 16, f16 weights).  act: 0 none, 1 tanh, 2 sigmoid,
  * 3 silu, 4 relu^2, 5 exp(-exp), 6 v7 decay.  out_mode: 0 f32 rows; 1 f16 (the operand layout of a following projection,
