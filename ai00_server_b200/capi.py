@@ -252,6 +252,8 @@ SYMBOLS = [
     ("b200rwkv_last_hidden_layer", C.c_int32, [_P, C.c_int32, _P, C.c_size_t]),
     ("b200rwkv_keep_hidden_pooled", C.c_int32, [_P, C.c_int32, _P, C.c_int32]),
     ("b200rwkv_last_hidden_pooled", C.c_int32, [_P, C.c_int32, _P, C.c_size_t, _P]),
+    ("b200rwkv_score_top", C.c_int32, [_P, C.c_int32]),
+    ("b200rwkv_last_score_top", C.c_int32, [_P, _P, _P, C.c_size_t]),
     ("b200rwkv_debug_read", C.c_int32, [_P, C.c_char_p, _P, C.c_size_t]),
     ("b200rwkv_debug_trace", C.c_int32, [_P, _P, C.c_size_t, _P, _P]),
     ("b200rwkv_debug_gemm_time", C.c_int32, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_int64), _P]),

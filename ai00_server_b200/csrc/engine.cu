@@ -654,6 +654,15 @@ struct b200rwkv_engine {
     // n = the call's scored tokens; grown on demand
     Buf<uint8_t> sc_dev;
     HostBuf<uint8_t> sc_host;
+    // b200rwkv_score_top: with top_n > 0 both score buffers go on with [ids u32 x n x top_n | logprobs f32 x n x top_n], and
+    // every score launch is followed by the two score_top launches over the same rows, whose candidate lists go to
+    // top_cand_x / top_cand_id ([max(S, maxT)][segments][128]: a launch lists at most one row per SCORE entry or per token
+    // of a step).  top_last_n / top_last_rows: the setting and the scored tokens of the most recent infer call, whose lists
+    // sit in sc_host.
+    int top_n = 0;
+    float* top_cand_x = nullptr; unsigned* top_cand_id = nullptr;
+    int top_last_n = 0;
+    size_t top_last_rows = 0;
     void enqueue_keep(cudaStream_t s, int MTR);
     void enqueue_snap_rows(cudaStream_t s, const StepShape& sh);
     void check_sample_slots(int nrows, const int32_t* slots, const char* who);
@@ -2307,6 +2316,9 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
     for (int i = 0; i < nslot; ++i) score_base[i + 1] = score_base[i] + (option[i] == B200RWKV_OPTION_SCORE ? (size_t)ntok[i] : 0);
     ScoreRow* sc_rows = nullptr;
     size_t sc_used = 0;
+    // b200rwkv_score_top: n best entries of each scored row, after the score fields of sc_dev / sc_host
+    const int tn = top_n;
+    const size_t top_bytes = (size_t)tn * 8;         // per scored token: tn ids, tn logprobs
     auto launch_score = [&](size_t first, size_t n) {
         if (n == 0) return;
         ScoreParams sp;
@@ -2317,9 +2329,27 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         CK(cudaMemcpyAsync(sc_dev + first * sizeof(ScoreRow), sc_rows + first, n * sizeof(ScoreRow), cudaMemcpyHostToDevice, stream));
         score_rows_kernel<<<(unsigned)n, SCORE_THREADS, 0, stream>>>(sp);
         CK(cudaGetLastError());
+        if (tn > 0) {
+            ScoreTopParams tp;
+            tp.rows = sp.rows;
+            tp.V = V;
+            tp.nseg = cdiv(V, TOPK_SEG);
+            tp.top_n = tn;
+            tp.cand_x = top_cand_x;
+            tp.cand_id = top_cand_id;
+            tp.out_id = reinterpret_cast<unsigned*>(sc_dev + total_score * (sizeof(ScoreRow) + 8));
+            tp.out_lp = reinterpret_cast<float*>(sc_dev + total_score * (sizeof(ScoreRow) + 8) + total_score * tn * 4);
+            score_top_segment_kernel<<<dim3(tp.nseg, (unsigned)n), TOPK_SEG_THREADS, 0, stream>>>(tp);
+            CK(cudaGetLastError());
+            score_top_merge_kernel<<<(unsigned)n, TOPK_MERGE_THREADS, 0, stream>>>(tp);
+            CK(cudaGetLastError());
+        }
     };
+    top_last_n = 0;
+    top_last_rows = 0;
     if (total_score > 0) {
-        const size_t want = total_score * (sizeof(ScoreRow) + 8), bytes = std::max<size_t>(want, 256 * (sizeof(ScoreRow) + 8));
+        const size_t row_bytes = sizeof(ScoreRow) + 8 + top_bytes;
+        const size_t want = total_score * row_bytes, bytes = std::max<size_t>(want, 256 * row_bytes);
         sc_dev.grow(want, bytes);
         sc_host.grow(want, bytes);
         sc_rows = reinterpret_cast<ScoreRow*>(sc_host.p);
@@ -2510,9 +2540,9 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
         for (size_t j = 0; j < s_entry.size(); ++j) pos[s_entry[j]] += s_counts[j];
         ++step_no;
     }
-    if (total_score > 0)      // scores and argmax ids of the whole call: one copy
-        CK(cudaMemcpyAsync(sc_host + total_score * sizeof(ScoreRow), sc_dev + total_score * sizeof(ScoreRow), total_score * 8,
-                           cudaMemcpyDeviceToHost, stream));
+    if (total_score > 0)      // scores, argmax ids and any top-n lists of the whole call: one copy
+        CK(cudaMemcpyAsync(sc_host + total_score * sizeof(ScoreRow), sc_dev + total_score * sizeof(ScoreRow),
+                           total_score * (8 + top_bytes), cudaMemcpyDeviceToHost, stream));
     CK(cudaStreamSynchronize(stream));
     if (total_score > 0) {
         memcpy(score->score, sc_host + total_score * sizeof(ScoreRow), total_score * 4);
@@ -2530,6 +2560,8 @@ void b200rwkv_engine::infer(int nslot, const int32_t* slot, const int32_t* ntok,
     hid_last_rows = total_tok;
     pool_last = pool_layers;
     pool_last_ntok.assign(ntok, ntok + nslot);
+    top_last_n = tn;
+    top_last_rows = total_score;
 }
 
 // GPU sampling front half (sample.cuh).  Runs on the softmax stream under the softmax mutex: the reference samples from the
@@ -4129,6 +4161,42 @@ int32_t b200rwkv_keep_hidden_pooled(b200rwkv_engine* e, int32_t n, const int32_t
     e->pool_mode = mode;
     e->upload_hid_tab();
     API_END
+}
+
+int32_t b200rwkv_score_top(b200rwkv_engine* e, int32_t top_n) {
+    API_BEGIN(e)
+    REQUIRE(top_n >= 0 && top_n <= TOPK_MAX, B200RWKV_ERR_INVALID,
+            "score_top: top_n must be in [0, " + std::to_string(TOPK_MAX) + "]");
+    REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
+    std::lock_guard<std::mutex> lk(e->mu);
+    REQUIRE(top_n == 0 || e->world == 1, B200RWKV_ERR_UNSUPPORTED, "score_top: not supported under tensor parallelism");
+    REQUIRE(top_n == 0 || e->V <= TOPK_MAX_SEGS * TOPK_SEG, B200RWKV_ERR_UNSUPPORTED,
+            "score_top: num_vocab > " + std::to_string(TOPK_MAX_SEGS * TOPK_SEG) + " is not supported");
+    CK(cudaSetDevice(e->dev));
+    if (top_n > 0 && !e->top_cand_x) {
+        const size_t n = (size_t)std::max(e->S, e->maxT) * cdiv(e->V, TOPK_SEG) * TOPK_MAX;
+        e->top_cand_x = (float*)e->dalloc(n * 4);
+        e->top_cand_id = (unsigned*)e->dalloc(n * 4);
+    }
+    e->top_n = top_n;
+    API_END
+}
+
+// returns the number of scored tokens of the most recent infer call (negative status on error)
+int32_t b200rwkv_last_score_top(b200rwkv_engine* e, uint32_t* ids_out, float* logprobs_out, size_t cap) {
+    return api_count([&]() -> int32_t {
+        REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
+        std::lock_guard<std::mutex> lk(e->mu);
+        REQUIRE(e->top_last_n > 0, B200RWKV_ERR_STATE, "last_score_top: the most recent infer call ran without score_top");
+        const size_t rows = e->top_last_rows, n = rows * e->top_last_n;
+        if (!ids_out && !logprobs_out) return (int32_t)rows;       // the row count only
+        REQUIRE(ids_out && logprobs_out, B200RWKV_ERR_INVALID, "last_score_top: one output is NULL");
+        REQUIRE(n <= cap, B200RWKV_ERR_INVALID, "last_score_top: buffer too small");
+        const uint8_t* h = e->sc_host + rows * (sizeof(ScoreRow) + 8);
+        memcpy(ids_out, h, n * 4);
+        memcpy(logprobs_out, h + n * 4, n * 4);
+        return (int32_t)rows;
+    });
 }
 
 // returns the number of rows written, one per entry of the call (negative status on error)

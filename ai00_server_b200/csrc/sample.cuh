@@ -109,6 +109,55 @@ __device__ __forceinline__ float2 segment_stats(const float* sx, float* red) {
     return make_float2(mx, s);
 }
 
+// Bitonic sort of one segment in shared memory, best first (cand_before).  All TOPK_SEG_THREADS threads call it; it
+// synchronises before it reads, not after its last stage.
+__device__ __forceinline__ void sort_segment(float* sx, unsigned* sid) {
+    const int tid = threadIdx.x;
+    for (int k = 2; k <= TOPK_SEG; k <<= 1) {
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            __syncthreads();
+#pragma unroll
+            for (int q = 0; q < TOPK_SEG / 2 / TOPK_SEG_THREADS; ++q) {
+                const int t = tid + TOPK_SEG_THREADS * q;            // compare-exchange index 0 .. 1023
+                const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1)); // lower element of the pair
+                const int l = i | j;
+                const bool up = (i & k) == 0;                         // this block sorts best-first
+                const float xa = sx[i], xb = sx[l];
+                const unsigned ia = sid[i], ib = sid[l];
+                const bool a_first = cand_before(xa, ia, xb, ib);
+                if (a_first != up) { sx[i] = xb; sx[l] = xa; sid[i] = ib; sid[l] = ia; }
+            }
+        }
+    }
+}
+
+// Merges the TOPK_MAX_SEGS sorted lists of TOPK_MAX candidates in shared memory into the best TOPK_MAX, in sx[0 .. 127] /
+// sid[0 .. 127], in five rounds: lists a = 2 p s, b = (2 p + 1) s -> a.  All TOPK_MERGE_THREADS threads call it; it
+// synchronises before it reads, not after its last stage.
+__device__ __forceinline__ void merge_lists(float* sx, unsigned* sid) {
+    const int tid = threadIdx.x;
+    for (int s = 1; s < TOPK_MAX_SEGS; s <<= 1) {
+        const int npair = TOPK_MAX_SEGS / (2 * s);
+        __syncthreads();
+        for (int t = tid; t < npair * TOPK_MAX; t += TOPK_MERGE_THREADS) {
+            const int pr = t / TOPK_MAX, i = t % TOPK_MAX;
+            const int a = (2 * pr) * s * TOPK_MAX + i, b = (2 * pr + 1) * s * TOPK_MAX + (TOPK_MAX - 1 - i);
+            if (!cand_before(sx[a], sid[a], sx[b], sid[b])) { sx[a] = sx[b]; sid[a] = sid[b]; }
+        }
+        for (int j = TOPK_MAX / 2; j > 0; j >>= 1) {
+            __syncthreads();
+            for (int t = tid; t < npair * (TOPK_MAX / 2); t += TOPK_MERGE_THREADS) {
+                const int pr = t / (TOPK_MAX / 2), u = t % (TOPK_MAX / 2);
+                const int i = (2 * pr) * s * TOPK_MAX + (((u & ~(j - 1)) << 1) | (u & (j - 1)));
+                const int l = i + j;
+                const float xa = sx[i], xb = sx[l];
+                const unsigned ia = sid[i], ib = sid[l];
+                if (!cand_before(xa, ia, xb, ib)) { sx[i] = xb; sx[l] = xa; sid[i] = ib; sid[l] = ia; }
+            }
+        }
+    }
+}
+
 __global__ void __launch_bounds__(TOPK_SEG_THREADS) topk_segment_kernel(const __grid_constant__ TopkParams p) {
     __shared__ float sx[TOPK_SEG];
     __shared__ unsigned sid[TOPK_SEG];
@@ -126,23 +175,7 @@ __global__ void __launch_bounds__(TOPK_SEG_THREADS) topk_segment_kernel(const __
     // segment statistics of the softmax
     const float2 st = segment_stats(sx, red);
     if (tid == 0) p.stats[(size_t)row * p.nseg + seg] = st;
-    // bitonic sort, best first
-    for (int k = 2; k <= TOPK_SEG; k <<= 1) {
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            __syncthreads();
-#pragma unroll
-            for (int q = 0; q < TOPK_SEG / 2 / TOPK_SEG_THREADS; ++q) {
-                const int t = tid + TOPK_SEG_THREADS * q;            // compare-exchange index 0 .. 1023
-                const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1)); // lower element of the pair
-                const int l = i | j;
-                const bool up = (i & k) == 0;                         // this block sorts best-first
-                const float xa = sx[i], xb = sx[l];
-                const unsigned ia = sid[i], ib = sid[l];
-                const bool a_first = cand_before(xa, ia, xb, ib);
-                if (a_first != up) { sx[i] = xb; sx[l] = xa; sid[i] = ib; sid[l] = ia; }
-            }
-        }
-    }
+    sort_segment(sx, sid);
     __syncthreads();
     if (tid < TOPK_MAX) {
         const size_t o = ((size_t)row * p.nseg + seg) * TOPK_MAX + tid;
@@ -171,27 +204,7 @@ __global__ void __launch_bounds__(TOPK_MERGE_THREADS) topk_merge_kernel(const __
         sc = warp_sum(sc);
         if (tid == 0) { s_m = M; s_inv = 1.0f / sc; }
     }
-    // five merge rounds: lists a = 2 p s, b = (2 p + 1) s -> a
-    for (int s = 1; s < TOPK_MAX_SEGS; s <<= 1) {
-        const int npair = TOPK_MAX_SEGS / (2 * s);
-        __syncthreads();
-        for (int t = tid; t < npair * TOPK_MAX; t += TOPK_MERGE_THREADS) {
-            const int pr = t / TOPK_MAX, i = t % TOPK_MAX;
-            const int a = (2 * pr) * s * TOPK_MAX + i, b = (2 * pr + 1) * s * TOPK_MAX + (TOPK_MAX - 1 - i);
-            if (!cand_before(sx[a], sid[a], sx[b], sid[b])) { sx[a] = sx[b]; sid[a] = sid[b]; }
-        }
-        for (int j = TOPK_MAX / 2; j > 0; j >>= 1) {
-            __syncthreads();
-            for (int t = tid; t < npair * (TOPK_MAX / 2); t += TOPK_MERGE_THREADS) {
-                const int pr = t / (TOPK_MAX / 2), u = t % (TOPK_MAX / 2);
-                const int i = (2 * pr) * s * TOPK_MAX + (((u & ~(j - 1)) << 1) | (u & (j - 1)));
-                const int l = i + j;
-                const float xa = sx[i], xb = sx[l];
-                const unsigned ia = sid[i], ib = sid[l];
-                if (!cand_before(xa, ia, xb, ib)) { sx[i] = xb; sx[l] = xa; sid[i] = ib; sid[l] = ia; }
-            }
-        }
-    }
+    merge_lists(sx, sid);
     __syncthreads();
     if (tid < p.top_k) {
         // same expression as softmax_kernel (misc.cuh): exp(x - max) * (1 / sum)
@@ -399,6 +412,34 @@ struct ScoreAcc {
     }
 };
 
+// score_rows_kernel's pass over a row, in two halves, for score_top_merge_kernel: the same element-to-thread map, additions
+// and combine order, so both kernels find the same (m, s) bit for bit (tests/test_gpu_score_top.py holds them to it).
+// score_row_warp: thread tid < SCORE_THREADS's share of the row, combined over its warp by an xor tree.  score_row_combine:
+// warp 0 combines the SCORE_THREADS / 32 warps' results in the same way.  (score_rows_kernel keeps its own copy of these
+// lines: calling these helpers from it changes its register allocation.)
+__device__ __forceinline__ void score_row_warp(ScoreAcc& a, const float* s, const int V, const int tid) {
+    const int n4 = V >> 2;
+    if ((reinterpret_cast<uintptr_t>(s) & 15) == 0) {
+        const float4* s4 = reinterpret_cast<const float4*>(s);
+        for (int g = tid; g < n4; g += SCORE_THREADS) {
+            const float4 v = __ldcg(s4 + g);
+            a.add(v.x, 4 * g); a.add(v.y, 4 * g + 1); a.add(v.z, 4 * g + 2); a.add(v.w, 4 * g + 3);
+        }
+    } else {
+        for (int g = tid; g < n4; g += SCORE_THREADS)
+            for (int k = 0; k < 4; ++k) a.add(__ldcg(s + 4 * g + k), 4 * g + k);
+    }
+    if (tid < (V & 3)) a.add(__ldcg(s + 4 * n4 + tid), 4 * n4 + tid);      // scalar tail
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a.merge(a.shfl_xor(o));
+}
+
+__device__ __forceinline__ void score_row_combine(ScoreAcc& a, const ScoreAcc* red, const int tid) {
+    a = (tid < SCORE_THREADS / 32) ? red[tid] : ScoreAcc{-INFINITY, 0.f, -INFINITY, 0xFFFFFFFFu, 0};
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a.merge(a.shfl_xor(o));
+}
+
 __global__ void __launch_bounds__(SCORE_THREADS) score_rows_kernel(const __grid_constant__ ScoreParams p) {
     __shared__ ScoreAcc red[SCORE_THREADS / 32];
     const ScoreRow rw = p.rows[blockIdx.x];
@@ -434,6 +475,92 @@ __global__ void __launch_bounds__(SCORE_THREADS) score_rows_kernel(const __grid_
             p.score[rw.dst] = a.nan ? __int_as_float(0x7fc00000) : (__ldcg(s + rw.target) - a.m) - logf(a.s);
             p.argmax[rw.dst] = a.bi;
         }
+    }
+}
+
+// ---------------------------------------------------------------------------------------
+// Top-n of every scored row (b200rwkv_score_top): the n best entries of each row score_rows_kernel scores, logit descending
+// then id ascending (sample_topk's order on an unadjusted row), with logprob = (x - m) - logf(s) from the same (m, s) as the
+// row's score, so the target's entry, when listed, equals its score bit for bit.  The row list, and so the launch shape, is
+// the score launch's.
+//   kernel 1 (grid = segments x rows): load a segment, NaN entries out of the ranking (sorted last, as padding is), bitonic
+//            sort, keep the segment's best 128 -- topk_segment_kernel without adjustment or statistics;
+//   kernel 2 (grid = rows): warps 0 .. 7 run the score pass over the row while the others load the candidate lists, then
+//            topk_merge_kernel's merge, then the first n entries.  Entries past the row's non-NaN ones, and every entry of a
+//            row with src == nullptr: UINT32_MAX and NaN.  A NaN in the row makes every logprob NaN, as it makes the score.
+// ---------------------------------------------------------------------------------------
+struct ScoreTopParams {
+    const ScoreRow* rows;
+    int V, nseg, top_n;
+    float* cand_x;              // [rows of the launch][nseg][128]
+    unsigned* cand_id;
+    unsigned* out_id;           // [scored tokens][top_n]: row b's list at rows[b].dst
+    float* out_lp;
+};
+
+__global__ void __launch_bounds__(TOPK_SEG_THREADS) score_top_segment_kernel(const __grid_constant__ ScoreTopParams p) {
+    __shared__ float sx[TOPK_SEG];
+    __shared__ unsigned sid[TOPK_SEG];
+    const int seg = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
+    const float* src = p.rows[row].src;
+    if (src == nullptr) return;
+    const int seg0 = seg * TOPK_SEG;
+#pragma unroll
+    for (int j = 0; j < TOPK_SEG / TOPK_SEG_THREADS; ++j) {
+        const int li = tid + TOPK_SEG_THREADS * j, i = seg0 + li;
+        const float x = (i < p.V) ? __ldcg(src + i) : -INFINITY;
+        const bool ranked = i < p.V && x == x;
+        sx[li] = ranked ? x : -INFINITY;
+        sid[li] = ranked ? (unsigned)i : 0xFFFFFFFFu;
+    }
+    sort_segment(sx, sid);
+    __syncthreads();
+    if (tid < TOPK_MAX) {
+        const size_t o = ((size_t)row * p.nseg + seg) * TOPK_MAX + tid;
+        p.cand_x[o] = sx[tid];
+        p.cand_id[o] = sid[tid];
+    }
+}
+
+__global__ void __launch_bounds__(TOPK_MERGE_THREADS) score_top_merge_kernel(const __grid_constant__ ScoreTopParams p) {
+    __shared__ float sx[TOPK_MAX_SEGS * TOPK_MAX];
+    __shared__ unsigned sid[TOPK_MAX_SEGS * TOPK_MAX];
+    __shared__ ScoreAcc red[SCORE_THREADS / 32];
+    __shared__ float s_m, s_log;
+    __shared__ int s_nan;
+    const int row = blockIdx.x, tid = threadIdx.x;
+    const ScoreRow rw = p.rows[row];
+    unsigned* oid = p.out_id + (size_t)rw.dst * p.top_n;
+    float* olp = p.out_lp + (size_t)rw.dst * p.top_n;
+    if (rw.src == nullptr) {
+        if (tid < p.top_n) { oid[tid] = 0xFFFFFFFFu; olp[tid] = __int_as_float(0x7fc00000); }
+        return;
+    }
+    if (tid < SCORE_THREADS) {
+        ScoreAcc a{-INFINITY, 0.f, -INFINITY, 0xFFFFFFFFu, 0};
+        score_row_warp(a, rw.src, p.V, tid);
+        if ((tid & 31) == 0) red[tid >> 5] = a;
+    } else {
+        for (int i = tid - SCORE_THREADS; i < TOPK_MAX_SEGS * TOPK_MAX; i += TOPK_MERGE_THREADS - SCORE_THREADS) {
+            const int sg = i / TOPK_MAX;
+            const bool ok = sg < p.nseg;
+            const size_t o = ((size_t)row * p.nseg + sg) * TOPK_MAX + (i % TOPK_MAX);
+            sx[i] = ok ? p.cand_x[o] : -INFINITY;
+            sid[i] = ok ? p.cand_id[o] : 0xFFFFFFFFu;
+        }
+    }
+    __syncthreads();
+    if (tid < 32) {
+        ScoreAcc a;
+        score_row_combine(a, red, tid);
+        if (tid == 0) { s_m = a.m; s_log = logf(a.s); s_nan = a.nan; }
+    }
+    merge_lists(sx, sid);
+    __syncthreads();
+    if (tid < p.top_n) {
+        const unsigned id = sid[tid];
+        oid[tid] = id;
+        olp[tid] = (s_nan || id == 0xFFFFFFFFu) ? __int_as_float(0x7fc00000) : (sx[tid] - s_m) - s_log;
     }
 }
 

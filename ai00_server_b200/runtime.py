@@ -16,6 +16,7 @@ Every method calls straight into libb200rwkv.so; nothing here computes on the CP
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import enum
 from dataclasses import dataclass, field
@@ -295,6 +296,7 @@ class Model:
             capi.check(L.b200rwkv_create_tp(capi.ptr(st), st.size, device, max_batch, token_chunk_size, precision,
                                             rank, world, C.byref(h)))
         self._h = h
+        self._top_n = 0                # b200rwkv_score_top setting
         self.max_batch, self.token_chunk_size = max_batch, token_chunk_size
         self.rank, self.world = rank, world
         info = capi.Info()
@@ -344,10 +346,17 @@ class Model:
         return res
 
     # ---- raw call with scoring: one b200rwkv_infer_ex ----
-    def infer_ex(self, slots, ntok, tokens, options):
+    def infer_ex(self, slots, ntok, tokens, options, top_n: int | None = None):
         """b200rwkv_infer_ex: `options` may also hold capi.OPTION_SCORE.  Returns (rows, scores): rows per entry as infer_raw
         returns them (0 rows for SCORE entries); scores[i] is (log-probabilities f32 [ntok[i]], argmax ids uint32 [ntok[i]])
-        for a SCORE entry, None otherwise.  Token 0 of a SCORE entry is scored from the slot's kept row (NaN if it has none)."""
+        for a SCORE entry, None otherwise.  Token 0 of a SCORE entry is scored from the slot's kept row (NaN if it has none).
+        With `top_n` (1..128) the call runs with score_top(top_n) and returns (rows, scores, tops), tops[i] the entry's
+        (ids uint32 [ntok[i]][top_n], log-probabilities f32 [ntok[i]][top_n]) for a SCORE entry, None otherwise; the engine's
+        own setting is restored afterwards."""
+        if top_n is not None:
+            with self._score_top_as(top_n):
+                rows, scores = self.infer_ex(slots, ntok, tokens, options)
+                return rows, scores, self._split_tops(ntok, options, self.last_score_top())
         V = self.info["num_vocab"]
         n = len(slots)
         total = sum(nt if o == capi.OPTION_FULL else (1 if (o == capi.OPTION_LAST and nt > 0) else 0)
@@ -416,16 +425,63 @@ class Model:
         snaps = [r if isinstance(r, TensorGpu) else TensorGpu(self, int(ids[j])) for j, r in enumerate(reuse)]
         return rows, scores, snaps
 
-    def perplexity(self, slot: int, tokens, head: float | None = None) -> float:
+    # ---- top-n log-probabilities of every scored row (b200rwkv_score_top) ----
+    def score_top(self, n: int) -> None:
+        """Every following infer_ex / infer_snapshots call also reduces each scored row to its n best (id, log-probability)
+        pairs, read with last_score_top(); 0 turns it off."""
+        capi.check(capi.lib().b200rwkv_score_top(self._h, int(n)), self._h)
+        self._top_n = int(n)
+
+    def last_score_top(self):
+        """(ids uint32 [rows][n], log-probabilities f32 [rows][n]) of the most recent infer call, rows = its scored tokens in
+        score order."""
+        rows = capi.check(capi.lib().b200rwkv_last_score_top(self._h, None, None, 0), self._h)
+        ids = np.empty((rows, self._top_n), np.uint32)
+        lp = np.empty((rows, self._top_n), np.float32)
+        capi.check(capi.lib().b200rwkv_last_score_top(self._h, capi.ptr(ids), capi.ptr(lp), ids.size), self._h)
+        return ids, lp
+
+    @contextlib.contextmanager
+    def _score_top_as(self, n):
+        old = self._top_n
+        self.score_top(n)
+        try:
+            yield
+        finally:
+            self.score_top(old)
+
+    @staticmethod
+    def _split_tops(ntok, options, lists):
+        ids, lp = lists
+        tops, off = [], 0
+        for nt, o in zip(ntok, options):
+            if o == capi.OPTION_SCORE:
+                tops.append((ids[off:off + nt], lp[off:off + nt]))
+                off += nt
+            else:
+                tops.append(None)
+        return tops
+
+    def perplexity(self, slot: int, tokens, head: float | None = None, top_n: int | None = None):
         """The reference's `perplexity()` (run.rs:699-755) on one SCORE call, quirks included: without `head` a token 0 is
         fed first (its own score is not used) and the sum is divided by len(tokens) + 1; with `head` (the probability of
         tokens[0] the caller already holds) the first term is ln(head), the kept row's score of tokens[0] is not used, and the
-        divisor is len(tokens).  Run on the slot's current state, which it advances like the reference's Full run does."""
+        divisor is len(tokens).  Run on the slot's current state, which it advances like the reference's Full run does.
+        With `top_n` returns (perplexity, (ids [len(tokens)][top_n], log-probabilities [len(tokens)][top_n])): the best
+        entries of the row each token was scored from (with `head`, token 0's from the slot's kept row)."""
         tokens = [int(t) for t in tokens]
         fed = tokens if head is not None else [0] + tokens
-        _, scores = self.infer_ex([slot], [len(fed)], fed, [capi.OPTION_SCORE])
+        if top_n is None:
+            _, scores = self.infer_ex([slot], [len(fed)], fed, [capi.OPTION_SCORE])
+            return self._perplexity(fed, head, scores[0][0])
+        _, scores, tops = self.infer_ex([slot], [len(fed)], fed, [capi.OPTION_SCORE], top_n=top_n)
+        k = len(fed) - len(tokens)
+        return self._perplexity(fed, head, scores[0][0]), (tops[0][0][k:], tops[0][1][k:])
+
+    @staticmethod
+    def _perplexity(fed, head, score) -> float:
         logp = [np.float32(np.log(np.float32(head)))] if head is not None else []
-        logp += [np.float32(x) for x in scores[0][0][1:len(fed)]]
+        logp += [np.float32(x) for x in score[1:len(fed)]]
         total = np.float32(0.0)
         for x in logp:                         # `.sum()` over f32 in order, as the iterator does
             total = np.float32(total + x)

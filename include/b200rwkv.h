@@ -658,6 +658,28 @@ int32_t b200rwkv_last_hidden_layer(b200rwkv_engine*, int32_t layer, float* out, 
 int32_t b200rwkv_keep_hidden_pooled(b200rwkv_engine*, int32_t n, const int32_t* layers, int32_t mode);
 int32_t b200rwkv_last_hidden_pooled(b200rwkv_engine*, int32_t layer, float* out, size_t cap, int32_t* ntok_out);
 
+/* The n most likely tokens of every scored row, with their log-probabilities, reduced on the device: an OpenAI-style
+ * server's `logprobs` / `top_logprobs` (prompt tokens with `echo`, and generated tokens fed back as SCORE entries) without
+ * copying logits rows to the host.  b200rwkv_score_top(e, n) makes every following infer_ex / infer_snapshots call also
+ * reduce each scored row -- the row score_out[j] comes from, the slot's kept row for j = 0 included -- to its n best
+ * entries; n = 0 (the default) turns it off.
+ *   - Order: logit descending, then id ascending (b200rwkv_sample_topk's order on an unadjusted row), NaN entries left out.
+ *   - logprob = (x_id - m) - logf(S) with the m and S of the row's score, so the target's entry, if listed, is bit-identical
+ *     to score_out[j], and ids[j][0] == argmax_out[j] whenever the row has a finite maximum.
+ *   - Special values follow score_out: a row with a NaN gives NaN logprobs (its ids are still ranked over the non-NaN
+ *     entries); -inf entries come after the finite ones by ascending id; slots past the row's non-NaN entries, and every
+ *     slot of a token with no row, are UINT32_MAX / NaN.
+ *   - Two kernel launches after each score launch while n > 0; nothing else changes, and n = 0 launches exactly what an
+ *     engine that never set it launches.  The lists reach the host with the scores, in the call's one copy.
+ * n outside [0, 128] is B200RWKV_ERR_INVALID; n > 0 on a tensor-parallel engine or with num_vocab > 65536 is
+ * B200RWKV_ERR_UNSUPPORTED, all before any CUDA call.
+ * b200rwkv_last_score_top copies the most recent infer call's lists, ids_out and logprobs_out [sum of ntok over SCORE
+ * entries][n] in score_out's order (`cap` entries each), and returns that row count: B200RWKV_ERR_STATE if that call ran
+ * with the setting off, B200RWKV_ERR_INVALID if `cap` is too small or only one output is NULL.  With both NULL it copies
+ * nothing and returns the row count. */
+int32_t b200rwkv_score_top(b200rwkv_engine*, int32_t top_n);
+int32_t b200rwkv_last_score_top(b200rwkv_engine*, uint32_t* ids_out, float* logprobs_out, size_t cap);
+
 /* Test aid: copy a named internal activation buffer of the last layer of the most recent step to the host as f32
  * row-major, one row per token of that step; returns the column count (negative status on error).  Not on the product
  * path.  f32 buffers: x_a, x_b, xx1, sx1, xx2, r, k, v, g, w, a, nu, v_first (RWKV-7: the value rows layer 0 wrote),
