@@ -44,6 +44,7 @@ class Options(C.Structure):
 
 QUANT_NONE, QUANT_INT8, QUANT_NF4 = 0, 1, 2
 QUANT_FP8 = 4             # E4M3 codes + one f32 scale per row (3 is the reference's SF4, not implemented)
+QUANT_INT4 = 6            # 4-bit codes + f16 (scale, min) per 128 inputs of a row (5 is unassigned)
 
 # B200RWKV_TARGET_*: the kinds of matrix the places of b200rwkv_create_adapter_places can hold pairs on
 TARGET_ATT_R, TARGET_ATT_K, TARGET_ATT_V, TARGET_ATT_G = 1 << 0, 1 << 1, 1 << 2, 1 << 3
@@ -315,7 +316,8 @@ def info_from_st(st: np.ndarray) -> dict:
 
 def op_quantize(quant_type: int, w16, device: int = 0):
     """The load-time quantiser on one [N, K] f16 matrix (b200rwkv_op_quantize).  Int8: (codes u8 [N, K], min f16 [N, K/128],
-    scale f16 [N, K/128]); NF4: (level indices u8 [N, K], absmax f16 [N, K/64]); FP8: (E4M3 codes u8 [N, K], scale f32 [N])."""
+    scale f16 [N, K/128]); NF4: (level indices u8 [N, K], absmax f16 [N, K/64]); FP8: (E4M3 codes u8 [N, K], scale f32 [N]);
+    Int4: (codes u8 0..15 [N, K], min f16 [N, K/128], scale f16 [N, K/128])."""
     w16 = np.ascontiguousarray(w16, np.float16)
     N, K = w16.shape
     if quant_type == QUANT_FP8:
@@ -323,12 +325,13 @@ def op_quantize(quant_type: int, w16, device: int = 0):
         scale = np.empty(N, np.float32)
         check(lib().b200rwkv_op_quantize(device, quant_type, N, K, ptr(w16), ptr(codes), ptr(scale), None))
         return codes, scale
-    nb = K // (128 if quant_type == QUANT_INT8 else 64)
+    affine = quant_type in (QUANT_INT8, QUANT_INT4)          # (codes, min, scale) per 128-input block
+    nb = K // (128 if affine else 64)
     codes = np.empty((N, K), np.uint8)
     p0 = np.empty((N, nb), np.float16)
     p1 = np.empty((N, nb), np.float16)
-    check(lib().b200rwkv_op_quantize(device, quant_type, N, K, ptr(w16), ptr(codes), ptr(p0), ptr(p1) if quant_type == QUANT_INT8 else None))
-    return (codes, p0, p1) if quant_type == QUANT_INT8 else (codes, p0)
+    check(lib().b200rwkv_op_quantize(device, quant_type, N, K, ptr(w16), ptr(codes), ptr(p0), ptr(p1) if affine else None))
+    return (codes, p0, p1) if affine else (codes, p0)
 
 
 def op_wkv_step(version: int, slots, counts, state, out, r, k, v, g, lnx_w, lnx_b, w=None, u=None, a=None, k_k=None, k_a=None,

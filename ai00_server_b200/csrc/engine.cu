@@ -25,6 +25,7 @@
 #include "gemm.cuh"
 #include "qgemm.cuh"
 #include "fp8gemm.cuh"
+#include "int4gemm.cuh"
 #include "pre6.cuh"
 #include "sample.cuh"
 #include "misc.cuh"
@@ -734,7 +735,7 @@ struct b200rwkv_engine {
     float* vec_f32(const StFile& st, const std::string& name, size_t off, size_t count, float scale = 1.f, float bias = 0.f);
     A16Buf a16_alloc(int K, int nmat = 1);
     GemmLaunch make_launch(std::vector<SegDesc>& segs, int force_grid = 0, int qtype = QT_NONE);
-    int quant_layers = 0, quant_type = QT_NONE;     // the first `quant_layers` layers hold Int8 / NF4 / FP8 projection matrices
+    int quant_layers = 0, quant_type = QT_NONE;     // the first `quant_layers` layers hold Int8 / NF4 / FP8 / Int4 projection matrices
     int pick_split(int K, int tiles) const;
     void finalize_tp();
     template <typename P, typename... X>
@@ -983,10 +984,11 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
         kbmax = std::max(kbmax, sg.KB);
         if (qtype == QT_NONE) g.weight_bytes += (size_t)d.N * (d.K + (size_t)d.ad_tail * GEMM_BK) * 2;
         else {
-            // quantisation blocks are runs of 128 (Int8) / 64 (NF4) consecutive inputs of one output row of the FULL matrix
+            // quantisation blocks are runs of 128 (Int8, Int4) / 64 (NF4) consecutive inputs of one output row of the FULL matrix
             REQUIRE(d.K % GEMM_BK == 0 && d.k0 % GEMM_BK == 0, B200RWKV_ERR_UNSUPPORTED,
                     "quantised projections need input dimensions that are multiples of 128");
             if (qtype == QT_FP8) g.weight_bytes += (size_t)d.N * d.K + (size_t)d.N * 4;      // codes + one f32 scale per row
+            else if (qtype == QT_INT4) g.weight_bytes += (size_t)d.N * d.K / 2 + (size_t)d.N * (d.K / 128) * 4;
             else g.weight_bytes += qtype == QT_INT8 ? (size_t)d.N * d.K + (size_t)d.N * (d.K / 128) * 4
                                                     : (size_t)d.N * d.K / 2 + (size_t)d.N * (d.K / 64) * 2;
         }
@@ -1029,6 +1031,7 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
             const int grid = (int)std::min<size_t>((nwarp + 7) / 8, (size_t)num_sms * 32);
             uint8_t* dstq = W + (size_t)sg.blk_begin * blk_bytes;
             if (qtype == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, sg.KB, dstq);
+            else if (qtype == QT_INT4) quantize_int4_kernel<<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, sg.KB, dstq);
             else quantize_weight_kernel<QT_NF4><<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, sg.KB, dstq);
             CK(cudaGetLastError());
             CK(cudaDeviceSynchronize());
@@ -1143,6 +1146,12 @@ void b200rwkv_engine::launch_gemm(const GemmLaunch& g, const StepShape& sh, cuda
             return;
         }
 #undef FLAUNCH
+#define ILAUNCH(MT_) launch_k(int4gemm_kernel<MT_>, dim3(grid), dim3(GEMM_THREADS), Int4GemmCfg<MT_>::SMEM_BYTES, p, KC_GEMM, s, prof)
+        if (g.qtype == QT_INT4) {
+            switch (MT) { case 1: ILAUNCH(1); break; case 2: ILAUNCH(2); break; case 4: ILAUNCH(4); break; default: ILAUNCH(8); break; }
+            return;
+        }
+#undef ILAUNCH
 #define QLAUNCH(MT_, QT_) launch_k(qgemm_kernel<MT_, QT_>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<MT_, QT_>::SMEM_BYTES, p, KC_GEMM, s, prof)
         if (g.qtype == QT_INT8) {
             switch (MT) { case 1: QLAUNCH(1, QT_INT8); break; case 2: QLAUNCH(2, QT_INT8); break; case 4: QLAUNCH(4, QT_INT8); break; default: QLAUNCH(8, QT_INT8); break; }
@@ -1227,6 +1236,12 @@ static void gemm_smem_limits(int qtype) {
         CK(cudaFuncSetAttribute(fp8gemm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<4>::SMEM_BYTES));
         CK(cudaFuncSetAttribute(fp8gemm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<8>::SMEM_BYTES));
     }
+    if (qtype == QT_INT4) {
+        CK(cudaFuncSetAttribute(int4gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Int4GemmCfg<1>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(int4gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Int4GemmCfg<2>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(int4gemm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, Int4GemmCfg<4>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(int4gemm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, Int4GemmCfg<8>::SMEM_BYTES));
+    }
 }
 
 // dynamic shared memory limit of every WKV kernel launch_wkv can pick: prefill steps of up to 128 tokens, the decay-LoRA slice
@@ -1276,8 +1291,8 @@ void b200rwkv_engine::build(const StFile& st) {
     stream = new_stream();
     sm_stream = new_stream();
     if (quant_layers > 0 && quant_type != QT_NONE) {
-        REQUIRE(quant_type == QT_INT8 || quant_type == QT_NF4 || quant_type == QT_FP8, B200RWKV_ERR_UNSUPPORTED,
-                "quant_type must be Int8, NF4 or FP8 (SF4 is not implemented)");
+        REQUIRE(quant_type == QT_INT8 || quant_type == QT_NF4 || quant_type == QT_FP8 || quant_type == QT_INT4, B200RWKV_ERR_UNSUPPORTED,
+                "quant_type must be Int8, NF4, FP8 or Int4 (SF4 is not implemented)");
         REQUIRE(world == 1, B200RWKV_ERR_UNSUPPORTED, "quantised layers are single-GPU in this version");
         REQUIRE(precision == 0, B200RWKV_ERR_UNSUPPORTED, "quantised layers run with precision 0 (f16 operands)");
     }
@@ -3411,15 +3426,16 @@ static int32_t rank_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int3
     API_END
 }
 
-// Operator-level entry for the parity tests: the load-time quantiser (qgemm.cuh, fp8gemm.cuh) on one matrix, un-tiled on the
-// host into plain row-major codes and per-block (per-row for FP8) parameters so that oracle/quant_numpy.py and
-// tests/fp8_oracle.py can be compared bit for bit.
+// Operator-level entry for the parity tests: the load-time quantiser (qgemm.cuh, fp8gemm.cuh, int4gemm.cuh) on one matrix,
+// un-tiled on the host into plain row-major codes and per-block (per-row for FP8) parameters so that oracle/quant_numpy.py,
+// tests/fp8_oracle.py and tests/int4_oracle.py can be compared bit for bit.
 int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int32_t K, const uint16_t* w_f16, uint8_t* codes,
                              uint16_t* p0, uint16_t* p1) {
     API_BEGIN((b200rwkv_engine*)nullptr)
-    REQUIRE(quant_type == QT_INT8 || quant_type == QT_NF4 || quant_type == QT_FP8, B200RWKV_ERR_UNSUPPORTED, "quant_type must be Int8, NF4 or FP8");
+    REQUIRE(quant_type == QT_INT8 || quant_type == QT_NF4 || quant_type == QT_FP8 || quant_type == QT_INT4, B200RWKV_ERR_UNSUPPORTED,
+            "quant_type must be Int8, NF4, FP8 or Int4");
     REQUIRE(N >= 1 && K >= GEMM_BK && K % GEMM_BK == 0 && (size_t)N * K <= ((size_t)1 << 31) && w_f16 && codes && p0, B200RWKV_ERR_INVALID, "bad argument");
-    REQUIRE(quant_type != QT_INT8 || p1, B200RWKV_ERR_INVALID, "Int8 needs p1 (scales)");
+    REQUIRE((quant_type != QT_INT8 && quant_type != QT_INT4) || p1, B200RWKV_ERR_INVALID, "Int8 / Int4 need p1 (scales)");
     CK(cudaSetDevice(device));
     const int tiles = cdiv(N, GEMM_BN), KB = K / GEMM_BK;
     const size_t blk = (size_t)q_block_bytes(quant_type), total = (size_t)tiles * KB * blk;
@@ -3444,6 +3460,7 @@ int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int3
         return B200RWKV_OK;
     }
     if (quant_type == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256>>>(src, K, 0, 0, N, tiles, KB, dst);
+    else if (quant_type == QT_INT4) quantize_int4_kernel<<<grid, 256>>>(src, K, 0, 0, N, tiles, KB, dst);
     else quantize_weight_kernel<QT_NF4><<<grid, 256>>>(src, K, 0, 0, N, tiles, KB, dst);
     CK(cudaGetLastError());
     CK(cudaDeviceSynchronize());
@@ -3457,6 +3474,15 @@ int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int3
                 for (int k = 0; k < GEMM_BK; ++k) codes[(size_t)n * K + kb * GEMM_BK + k] = b[(size_t)((k >> 4) * GEMM_BN + r) * 16 + (k & 15)];
                 uint16_t pr[2];
                 memcpy(pr, b + GEMM_BN * GEMM_BK + r * 4, 4);
+                p1[(size_t)n * KB + kb] = pr[0];      // scale
+                p0[(size_t)n * KB + kb] = pr[1];      // min
+            } else if (quant_type == QT_INT4) {
+                for (int k = 0; k < GEMM_BK; ++k) {
+                    const int nib = int4_nibble(r, k);
+                    codes[(size_t)n * K + kb * GEMM_BK + k] = (b[nib >> 1] >> (4 * (nib & 1))) & 15;
+                }
+                uint16_t pr[2];
+                memcpy(pr, b + int4_param_offset(r), 4);
                 p1[(size_t)n * KB + kb] = pr[0];      // scale
                 p0[(size_t)n * KB + kb] = pr[1];      // min
             } else {
@@ -3873,8 +3899,8 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
     REQUIRE(T >= 1 && T <= A16_MAX_ROWS, B200RWKV_ERR_INVALID, "T must be 1..128");
     REQUIRE(precision == 0 || precision == 1, B200RWKV_ERR_INVALID, "precision must be 0 or 1");
     REQUIRE(grid >= 0 && launches >= 1 && launches <= 16, B200RWKV_ERR_INVALID, "grid must be >= 0 and launches 1..16");
-    REQUIRE(quant_type == QT_NONE || quant_type == QT_INT8 || quant_type == QT_NF4 || quant_type == QT_FP8, B200RWKV_ERR_UNSUPPORTED,
-            "quant_type must be 0, 1, 2 or 4");
+    REQUIRE(quant_type == QT_NONE || quant_type == QT_INT8 || quant_type == QT_NF4 || quant_type == QT_FP8 || quant_type == QT_INT4,
+            B200RWKV_ERR_UNSUPPORTED, "quant_type must be 0, 1, 2, 4 or 6");
     REQUIRE(precision == 0 || (T <= 16 && quant_type == QT_NONE), B200RWKV_ERR_UNSUPPORTED,
             "precision 1 runs decode-shaped steps (T <= 16) over f16 weights");
     for (int i = 0; i < nseg; ++i) {

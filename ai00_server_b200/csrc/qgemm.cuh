@@ -25,7 +25,8 @@
 
 namespace b200 {
 
-enum QuantType : int { QT_NONE = 0, QT_INT8 = 1, QT_NF4 = 2, QT_FP8 = 4 };   // 3 is the reference's SF4, not implemented; FP8: fp8gemm.cuh
+// 3 is the reference's SF4, not implemented (5 is unassigned); FP8: fp8gemm.cuh, Int4: int4gemm.cuh
+enum QuantType : int { QT_NONE = 0, QT_INT8 = 1, QT_NF4 = 2, QT_FP8 = 4, QT_INT4 = 6 };
 
 constexpr int Q_PARAM_BYTES = GEMM_BN * 4;                                  // 4 bytes of block parameters per weight row
 constexpr int Q_INT8_BYTES = GEMM_BN * GEMM_BK + Q_PARAM_BYTES;             // 16 896
@@ -37,7 +38,9 @@ constexpr int QGEMM_THREADS = GEMM_THREADS + Q_DQ_THREADS;                  // c
 constexpr int Q_LUT_BYTES = 256 * 32 * 4;                                   // NF4: [code byte 256][lane 32] half2
 
 __host__ __device__ constexpr int q_block_bytes(int qt) {
-    return qt == QT_INT8 ? Q_INT8_BYTES : (qt == QT_NF4 ? Q_NF4_BYTES : (qt == QT_FP8 ? GEMM_BN * GEMM_BK : GEMM_WBYTES));
+    return qt == QT_INT8 ? Q_INT8_BYTES
+         : qt == QT_NF4 || qt == QT_INT4 ? Q_NF4_BYTES            // Int4: 8 KB of codes + (scale, min) per row, as NF4's size
+         : qt == QT_FP8 ? GEMM_BN * GEMM_BK : GEMM_WBYTES;
 }
 
 __constant__ float c_nf4_levels[16] = {

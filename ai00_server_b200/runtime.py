@@ -232,7 +232,8 @@ class Model:
         """devices: list of CUDA ordinals -> ONE engine object owning all tensor-parallel ranks (b200rwkv_create_ex);
         lora: list of (st_bytes, alpha) blended at load (reference lib.rs:466-485);
         quant / quant_type: the reload request's fields (lib.rs:211-215): the first `quant` layers in "Int8" or "NF4",
-        or in "FP8" (E4M3 codes with one scale per row; this project's own format);
+        or in "FP8" (E4M3 codes with one scale per row) or "Int4" (4-bit codes with (scale, min) per 128 inputs), this
+        project's own formats;
         rank / world: one process per GPU instead (b200rwkv_create_tp + tp.connect);
         adapters: list of (st_bytes, alpha) kept unblended, ids 1..n, chosen per slot with bind_adapter
         (b200rwkv_create_adapters);
@@ -242,9 +243,10 @@ class Model:
         batch_invariant: every token's results are the bits a decode step gives it, whatever else shares its calls
         (b200rwkv_options.batch_invariant)."""
         if isinstance(quant_type, str):
-            kinds = {"none": capi.QUANT_NONE, "int8": capi.QUANT_INT8, "nf4": capi.QUANT_NF4, "sf4": 3, "fp8": capi.QUANT_FP8}
+            kinds = {"none": capi.QUANT_NONE, "int8": capi.QUANT_INT8, "nf4": capi.QUANT_NF4, "sf4": 3, "fp8": capi.QUANT_FP8,
+                     "int4": capi.QUANT_INT4}
             if quant_type.lower() not in kinds:
-                raise capi.B200Error(capi.ERR_INVALID, "quant_type must be None, Int8, NF4, SF4 or FP8")
+                raise capi.B200Error(capi.ERR_INVALID, "quant_type must be None, Int8, NF4, SF4, FP8 or Int4")
             quant_type = kinds[quant_type.lower()]
         quantised = quant > 0 and quant_type != capi.QUANT_NONE
         if exact:

@@ -99,7 +99,7 @@ typedef struct {
     /* `quant` / `quant_type` of the reload request (lib.rs:211-215, 465: the first `quant_layers` layers keep their eight
      * projection matrices in a weight-only quantised format; everything else stays f16).  Single GPU, precision 0 only. */
     int32_t quant_layers;
-    int32_t quant_type;               /* B200RWKV_QUANT_* */
+    int32_t quant_type;               /* B200RWKV_QUANT_*: NONE, INT8, NF4, FP8 or INT4 (3 = SF4 and 5 are refused) */
     /* 1: batch-invariant engine.  Every per-token result of a slot (logits rows of LAST / FULL / snapshots, SCORE values and
      * argmax ids, the kept row, the state after every token, recorded and pooled hidden rows) is then a function of the
      * model, the precision, the slot's starting state and the tokens it has fed only: bit-identical whatever the other
@@ -120,6 +120,12 @@ typedef struct {
                                        * of the whole matrix; the projection multiplies the codes' exact values with the f16
                                        * operand in f32 and scales each output.  Same refusals as Int8 / NF4 (one GPU,
                                        * precision 0, no adapters on its layers); batch-invariant engines run it. */
+#define B200RWKV_QUANT_INT4 6         /* beyond the reference's Quant enum: Int8's scheme at 4 bits.  Blocks of 128 inputs of one
+                                       * output row keep scale = f16((max - min) / 15), min = f16(min) and 4-bit codes
+                                       * q = floor(15 (w - min) / (max - min) + 0.5); the projection multiplies
+                                       * fma_f16(q, scale, min) (one rounding) with the f16 operand in f32.  Same refusals as
+                                       * Int8 / NF4 (one GPU, precision 0, no adapters on its layers); batch-invariant engines
+                                       * run it. */
 int32_t b200rwkv_create_ex(const uint8_t* st, size_t len, const b200rwkv_options* opt, b200rwkv_engine** out);
 
 /* Several LoRA adapters on one resident base model, chosen per slot at run time (the reference can only blend LoRA files at
@@ -412,10 +418,10 @@ int32_t b200rwkv_profile_insitu(b200rwkv_engine*, int32_t nslot, const int32_t* 
                                 double* step_us);
 
 /* Operator-level entry (parity tests): the load-time quantiser on a caller-supplied row-major f16 matrix [N, K] (K % 128 == 0),
- * returned in plain order: codes [N, K] (one byte per element: Int8 code, NF4 level index 0..15, or FP8 E4M3 code), p0 [N, K/block]
- * (Int8: block minimum, NF4: block absmax), p1 [N, K/block] (Int8: the scale f16((max - min) / 255); NF4, FP8: unused, may be
- * NULL).  p0 / p1 are f16 bit patterns.  block = 128 (Int8) or 64 (NF4).  FP8: p0 receives the N f32 row scales instead
- * (4 bytes each, 4N bytes in all). */
+ * returned in plain order: codes [N, K] (one byte per element: Int8 code, NF4 level index 0..15, FP8 E4M3 code, or Int4 code
+ * 0..15), p0 [N, K/block] (Int8, Int4: block minimum, NF4: block absmax), p1 [N, K/block] (Int8: the scale f16((max - min) / 255),
+ * Int4: the scale f16((max - min) / 15); NF4, FP8: unused, may be NULL).  p0 / p1 are f16 bit patterns.  block = 128 (Int8,
+ * Int4) or 64 (NF4).  FP8: p0 receives the N f32 row scales instead (4 bytes each, 4N bytes in all). */
 int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int32_t K, const uint16_t* w_f16, uint8_t* codes,
                              uint16_t* p0, uint16_t* p1);
 
@@ -530,7 +536,7 @@ typedef struct {
 int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args);
 
 /* Operator-level entry (parity tests): one projection launch -- the engine's planner (stream-K cuts, forced grids, Int8 / NF4 /
- * FP8 quantisation at load; quant_type B200RWKV_QUANT_*, SF4 refused) and its projection kernels -- over caller-supplied matrices, no model.  Segment i computes
+ * FP8 / Int4 quantisation at load; quant_type B200RWKV_QUANT_*, SF4 refused) and its projection kernels -- over caller-supplied matrices, no model.  Segment i computes
  * act(x W^T + bias) with W [N, K] (row-major f16 bits) and x [launches][T][K] f32, rounded to the f16 operand on the device
  * (precision 0) or split into an f16 hi + lo pair (precision 1: T <= 16, f16 weights).  act: 0 none, 1 tanh, 2 sigmoid,
  * 3 silu, 4 relu^2, 5 exp(-exp), 6 v7 decay.  out_mode: 0 f32 rows; 1 f16 (the operand layout of a following projection,

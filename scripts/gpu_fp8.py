@@ -1,4 +1,4 @@
-"""What FP8 (E4M3) weight-only layers buy on the GPU, against f16, Int8 and NF4 layers (every layer quantised).
+"""What FP8 (E4M3) and Int4 weight-only layers buy on the GPU, against f16, Int8 and NF4 layers (every layer quantised).
 
     python scripts/gpu_fp8.py [--runs 3] [--json out.json]
 
@@ -23,7 +23,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ai00_server_b200 import capi, runtime, synth  # noqa: E402
 
-ARMS = {"fp16": None, "int8": "Int8", "nf4": "NF4", "fp8": "FP8"}
+ARMS = {"fp16": None, "int8": "Int8", "nf4": "NF4", "fp8": "FP8", "int4": "Int4"}
 
 
 def stats(xs):
