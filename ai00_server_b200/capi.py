@@ -39,7 +39,8 @@ class Options(C.Structure):
     _fields_ = [("struct_bytes", C.c_uint32), ("max_batch", C.c_int32), ("token_chunk_size", C.c_int32), ("precision", C.c_int32),
                 ("num_devices", C.c_int32), ("devices", C.c_int32 * 8), ("num_lora", C.c_int32),
                 ("lora_st", C.c_void_p * MAX_LORA), ("lora_len", C.c_size_t * MAX_LORA), ("lora_alpha", C.c_float * MAX_LORA),
-                ("quant_layers", C.c_int32), ("quant_type", C.c_int32), ("batch_invariant", C.c_int32)]
+                ("quant_layers", C.c_int32), ("quant_type", C.c_int32), ("batch_invariant", C.c_int32),
+                ("quant_adapters", C.c_int32)]
 
 
 QUANT_NONE, QUANT_INT8, QUANT_NF4 = 0, 1, 2
@@ -243,6 +244,7 @@ SYMBOLS = [
     ("b200rwkv_op_wkv", C.c_int32, [C.c_int32, C.POINTER(WkvArgs)]),
     ("b200rwkv_op_ln", C.c_int32, [C.c_int32, C.POINTER(LnArgs)]),
     ("b200rwkv_op_gemm", C.c_int32, [C.c_int32] * 7 + [C.POINTER(GemmSeg), C.POINTER(C.c_int32 * 4)]),
+    ("b200rwkv_op_gemm_tail", C.c_int32, [C.c_int32] * 5 + [C.POINTER(GemmSeg), _P, _P, C.POINTER(C.c_int32 * 4)]),
     ("b200rwkv_op_keep", C.c_int32, [C.c_int32, C.POINTER(KeepArgs)]),
     ("b200rwkv_op_weight", C.c_int32, [C.c_int32, C.c_int32, C.POINTER(WeightArgs)]),
     ("b200rwkv_op_adapter", C.c_int32, [C.c_int32] * 5 + [_P, _P, _P, _P, _P]),
@@ -405,4 +407,25 @@ def op_gemm(T: int, segs: list[dict], precision: int = 0, quant_type: int = QUAN
                          d.get("grp", 0), p(xx), p(sx), p(mu), out.shape[2], ptr(out))
     plan = (C.c_int32 * 4)()
     check(lib().b200rwkv_op_gemm(device, T, precision, quant_type, grid, launches, len(segs), arr, C.byref(plan)))
+    return tuple(plan)
+
+
+def op_gemm_tail(T: int, seg: dict, e: np.ndarray, u: np.ndarray, quant_type: int = QUANT_NONE, grid: int = 0, device: int = 0):
+    """One W' launch of an adapter plan (b200rwkv_op_gemm_tail): `seg` as one op_gemm segment with launches = 1 (x [1, T, K],
+    out [1, gemm_rows(T), ldo]), plus n = e.shape[1] / 128 tail blocks with contents e [N, 128 n] f16 and the operand's tail
+    u [T, 128 n] f16.  Returns the plan as op_gemm does."""
+    w = np.ascontiguousarray(seg["w"], np.float16)
+    x = np.ascontiguousarray(seg["x"], np.float32)
+    bias = None if seg.get("bias") is None else np.ascontiguousarray(seg["bias"], np.float32)
+    out = seg["out"]
+    e = np.ascontiguousarray(e, np.float16)
+    u = np.ascontiguousarray(u, np.float16)
+    n = e.shape[1] // 128
+    assert out.flags.c_contiguous and out.dtype == (np.float32 if seg.get("out_mode", OUT_F32) == OUT_F32 else np.uint16)
+    assert x.shape == (1, T, w.shape[1]) and out.shape[:2] == (1, gemm_rows(T))
+    assert e.shape == (w.shape[0], 128 * n) and u.shape == (T, 128 * n)
+    s = GemmSeg(w.shape[0], w.shape[1], ptr(w), ptr(x), None if bias is None else ptr(bias), seg.get("act", ACT_NONE),
+                seg.get("out_mode", OUT_F32), seg.get("grp", 0), None, None, None, out.shape[2], ptr(out))
+    plan = (C.c_int32 * 4)()
+    check(lib().b200rwkv_op_gemm_tail(device, T, quant_type, grid, n, C.byref(s), ptr(e), ptr(u), C.byref(plan)))
     return tuple(plan)

@@ -167,6 +167,7 @@ class StFile {
 public:
     std::map<std::string, StTensor> tensors;
 
+    StFile() {}           // tensors filled by the caller (b200rwkv_op_gemm_tail's tail columns)
     StFile(const uint8_t* buf, size_t len) {
         REQUIRE(buf && len >= 8, B200RWKV_ERR_INVALID, "safetensors: buffer too small");
         uint64_t hlen = 0;
@@ -736,6 +737,11 @@ struct b200rwkv_engine {
     A16Buf a16_alloc(int K, int nmat = 1);
     GemmLaunch make_launch(std::vector<SegDesc>& segs, int force_grid = 0, int qtype = QT_NONE);
     int quant_layers = 0, quant_type = QT_NONE;     // the first `quant_layers` layers hold Int8 / NF4 / FP8 / Int4 projection matrices
+    // b200rwkv_options.quant_adapters: adapters may pair matrices of the quantised layers (quantised W' plans: the base plan's
+    // code blocks and f16 tail blocks, GemmParams::tails)
+    bool quant_adapters = false;
+    // quant_layers as the adapter checks see it: no layer refuses adapters with quant_adapters
+    int ad_quant_layers() const { return quant_adapters ? 0 : quant_layers; }
     int pick_split(int K, int tiles) const;
     void finalize_tp();
     template <typename P, typename... X>
@@ -829,7 +835,7 @@ static bool in_quant_layer(const std::string& base, int quant_layers, int quant_
     return quant_type != QT_NONE && layer >= 0 && layer < quant_layers;
 }
 // Matrices an engine from b200rwkv_create_adapter_places plans a W' for: every 2-D `<base>.weight` of the model of a targeted
-// kind outside the quantised layers.
+// kind outside the first `quant_layers` layers (0 with quant_adapters).
 static std::vector<std::string> ad_place_matrices(const std::map<std::string, StTensor>& model, uint32_t targets,
                                                   int quant_layers, int quant_type) {
     std::vector<std::string> out;
@@ -870,8 +876,8 @@ static void check_lora_files(const std::map<std::string, StTensor>& model, const
 void b200rwkv_engine::check_loras(const StFile& model) const { check_lora_files(model.tensors, loras); }
 
 // Adapter files (b200rwkv_create_adapters, b200rwkv_load_adapter), host only: the load-time blend's refusals, then every
-// pair's halves, dtypes and shapes against the model, the rank (one 128-wide k block of W'), and no pair on a matrix of a
-// quantised layer.
+// pair's halves, dtypes and shapes against the model, the rank (one 128-wide k block of W'), and no pair on a matrix of one
+// of the first `quant_layers` layers (0 with quant_adapters: every layer takes adapters).
 static void check_adapter_files(const std::map<std::string, StTensor>& model, const std::vector<b200rwkv_engine::LoraSrc>& files,
                                 int quant_layers, int quant_type) {
     check_lora_files(model, files);
@@ -967,6 +973,7 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
     g.qtype = qtype;
     const size_t blk_bytes = (size_t)q_block_bytes(qtype);
     int blk = 0, tile = 0, kbmax = 0;
+    int qblk = 0, tblk = 0;        // quantised plans: code blocks and f16 tail blocks so far (GemmParams::tails)
     for (size_t i = 0; i < segs.size(); ++i) {
         SegDesc& d = segs[i];
         GemmSeg& sg = g.p.seg[i];
@@ -982,8 +989,14 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
         blk += sg.tiles * sg.KB;
         tile += sg.tiles;
         kbmax = std::max(kbmax, sg.KB);
+        g.p.kbq[i] = sg.KB - d.ad_tail;
+        g.p.qblk[i] = qblk;
+        g.p.tblk[i] = tblk;
+        qblk += sg.tiles * g.p.kbq[i];
+        tblk += sg.tiles * d.ad_tail;
         if (qtype == QT_NONE) g.weight_bytes += (size_t)d.N * (d.K + (size_t)d.ad_tail * GEMM_BK) * 2;
         else {
+            g.weight_bytes += (size_t)d.N * d.ad_tail * GEMM_BK * 2;
             // quantisation blocks are runs of 128 (Int8, Int4) / 64 (NF4) consecutive inputs of one output row of the FULL matrix
             REQUIRE(d.K % GEMM_BK == 0 && d.k0 % GEMM_BK == 0, B200RWKV_ERR_UNSUPPORTED,
                     "quantised projections need input dimensions that are multiples of 128");
@@ -998,14 +1011,44 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
     g.force_grid = force_grid;
     g.p.total_blocks = blk;
     g.total_tiles = tile;
-    // FP8: the launch's row scales follow its blocks, FP8_SCALE_BYTES per tile (fp8gemm.cuh)
-    uint8_t* W = (uint8_t*)dalloc((size_t)blk * blk_bytes + (qtype == QT_FP8 ? (size_t)tile * FP8_SCALE_BYTES : 0), false);
+    // FP8: the launch's row scales follow its code blocks, FP8_SCALE_BYTES per tile (fp8gemm.cuh).  A quantised plan with
+    // adapter tails keeps them apart from its code blocks (GemmParams::tails); an f16 plan holds them among its blocks.
+    const int wblk = qtype == QT_NONE ? blk : qblk;
+    uint8_t* W = (uint8_t*)dalloc((size_t)wblk * blk_bytes + (qtype == QT_FP8 ? (size_t)tile * FP8_SCALE_BYTES : 0), false);
     g.p.W = W;
+    if (qtype == QT_FP8) g.p.scales = reinterpret_cast<const float*>(W + (size_t)wblk * blk_bytes);
+    if (qtype != QT_NONE && tblk) g.p.tails = (const uint8_t*)dalloc((size_t)tblk * GEMM_WBYTES, false);
+    // W' = [W | a_1 B_1 | ... | a_n B_n]: columns col0 + 128 a of E [N][ld] hold f16(alpha * lora.1) of every adapter file
+    // with a pair on `t` (E starts zeroed: zeros past the rank, and for an adapter without a pair here)
+    auto put_tails = [&](__half* E, int ld, int col0, const StTensor& t, const SegDesc& d) {
+        const std::string base = t.name.substr(0, t.name.size() - 7);
+        for (int a = 0; a < (int)adapters.size(); ++a) {      // adapter places are created empty
+            const StTensor* b = adapters[a].st->find(base + ".lora.1");
+            if (!b) continue;
+            const int r = (int)b->shape[1];
+            std::vector<__half> h((size_t)d.N * r);
+            memcpy(h.data(), b->data + (size_t)d.n0 * r * 2, h.size() * 2);
+            for (__half& v : h) v = __float2half_rn(adapters[a].alpha * __half2float(v));
+            CK(cudaMemcpy2D(E + col0 + (size_t)a * GEMM_BK, (size_t)ld * 2, h.data(), (size_t)r * 2, (size_t)r * 2, d.N,
+                            cudaMemcpyHostToDevice));
+        }
+    };
     for (size_t i = 0; i < segs.size(); ++i) {
         SegDesc& d = segs[i];
         const GemmSeg& sg = g.p.seg[i];
         const StTensor& t = *d.t;
         const __half* src = upload_tmp(t);
+        const int kbq = g.p.kbq[i];
+        uint8_t* const wq = W + (size_t)g.p.qblk[i] * blk_bytes;     // the segment's code blocks
+        if (qtype != QT_NONE && d.ad_tail) {
+            // the tail blocks alone, [tile][ad_tail], re-tiled as the f16 plan's
+            const int ke = d.ad_tail * GEMM_BK;
+            Buf<__half> E((size_t)d.N * ke * 2);
+            CK(cudaMemset(E, 0, E.bytes));
+            put_tails(E, ke, 0, t, d);
+            launch_repack(num_sms, E, ke, 0, 0, d.N, ke, reinterpret_cast<uint4*>(const_cast<uint8_t*>(g.p.tails) + (size_t)g.p.tblk[i] * GEMM_WBYTES));
+            CK(cudaDeviceSynchronize());
+        }
         int ld;
         if (d.slice >= 0) {
             REQUIRE(t.shape.size() == 3, B200RWKV_ERR_INVALID, "internal: slice of non-3D tensor");
@@ -1020,43 +1063,31 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
         if (qtype == QT_FP8) {
             // one warp per row; the scale is the absmax of the whole source row, whichever k slice this segment holds
             const int grid = std::min(cdiv(sg.tiles * GEMM_BN, 8), num_sms * 32);
-            float* scales = reinterpret_cast<float*>(W + (size_t)blk * blk_bytes) + (size_t)sg.tile_begin * GEMM_BN;
-            quantize_fp8_kernel<<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, sg.KB, W + (size_t)sg.blk_begin * blk_bytes, scales);
+            float* scales = const_cast<float*>(g.p.scales) + (size_t)sg.tile_begin * GEMM_BN;
+            quantize_fp8_kernel<<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, kbq, wq, scales);
             CK(cudaGetLastError());
             CK(cudaDeviceSynchronize());
             continue;
         }
         if (qtype != QT_NONE) {
-            const size_t nwarp = (size_t)sg.tiles * sg.KB * GEMM_BN;
+            const size_t nwarp = (size_t)sg.tiles * kbq * GEMM_BN;
             const int grid = (int)std::min<size_t>((nwarp + 7) / 8, (size_t)num_sms * 32);
-            uint8_t* dstq = W + (size_t)sg.blk_begin * blk_bytes;
-            if (qtype == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, sg.KB, dstq);
-            else if (qtype == QT_INT4) quantize_int4_kernel<<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, sg.KB, dstq);
-            else quantize_weight_kernel<QT_NF4><<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, sg.KB, dstq);
+            if (qtype == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, kbq, wq);
+            else if (qtype == QT_INT4) quantize_int4_kernel<<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, kbq, wq);
+            else quantize_weight_kernel<QT_NF4><<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, kbq, wq);
             CK(cudaGetLastError());
             CK(cudaDeviceSynchronize());
             continue;
         }
         uint4* dst = reinterpret_cast<uint4*>(W + (size_t)sg.blk_begin * GEMM_WBYTES);
         if (d.ad_tail) {
-            // W' = [W | a_1 B_1 | ... | a_n B_n]: W's columns padded to whole k blocks, then one zero-padded k block per
-            // adapter holding f16(alpha * lora.1) (zeros for an adapter without a pair here), re-tiled like any matrix
+            // W's columns padded to whole k blocks, then the tail blocks, re-tiled like any matrix
             const int kbw = cdiv(d.K, GEMM_BK), ke = (kbw + d.ad_tail) * GEMM_BK;
             Buf<__half> E((size_t)d.N * ke * 2);
             CK(cudaMemset(E, 0, E.bytes));
             CK(cudaMemcpy2D(E, (size_t)ke * 2, src + (size_t)d.n0 * ld + d.k0, (size_t)ld * 2, (size_t)d.K * 2, d.N,
                             cudaMemcpyDeviceToDevice));
-            const std::string base = t.name.substr(0, t.name.size() - 7);
-            for (int a = 0; a < (int)adapters.size(); ++a) {      // adapter places are created empty
-                const StTensor* b = adapters[a].st->find(base + ".lora.1");
-                if (!b) continue;
-                const int r = (int)b->shape[1];
-                std::vector<__half> h((size_t)d.N * r);
-                memcpy(h.data(), b->data + (size_t)d.n0 * r * 2, h.size() * 2);
-                for (__half& v : h) v = __float2half_rn(adapters[a].alpha * __half2float(v));
-                CK(cudaMemcpy2D((__half*)E + (size_t)(kbw + a) * GEMM_BK, (size_t)ke * 2, h.data(), (size_t)r * 2, (size_t)r * 2,
-                                d.N, cudaMemcpyHostToDevice));
-            }
+            put_tails(E, ke, kbw * GEMM_BK, t, d);
             launch_repack(num_sms, E, ke, 0, 0, d.N, ke, dst);
         } else {
             launch_repack(num_sms, src, ld, d.n0, d.k0, d.N, d.K, dst);
@@ -1140,19 +1171,27 @@ void b200rwkv_engine::launch_gemm(const GemmLaunch& g, const StepShape& sh, cuda
     if (g.qtype != QT_NONE) {
         REQUIRE(!sh.split, B200RWKV_ERR_UNSUPPORTED, "internal: quantised projections run with f16 activations");
         const int grid = MT >= 4 && !batch_inv ? g.grid_wide : g.grid;
-#define FLAUNCH(MT_) launch_k(fp8gemm_kernel<MT_>, dim3(grid), dim3(GEMM_THREADS), Fp8GemmCfg<MT_>::SMEM_BYTES, p, KC_GEMM, s, prof)
+        // W' plans (adapter tails) run the tail instantiations
+        const bool tails = p.tails != nullptr;
+#define FLAUNCH(MT_)                                                                                                                \
+    (tails ? launch_k(fp8gemm_tail_kernel<MT_>, dim3(grid), dim3(GEMM_THREADS), Fp8GemmCfg<MT_, true>::SMEM_BYTES, p, KC_GEMM, s, prof) \
+           : launch_k(fp8gemm_kernel<MT_>, dim3(grid), dim3(GEMM_THREADS), Fp8GemmCfg<MT_>::SMEM_BYTES, p, KC_GEMM, s, prof))
         if (g.qtype == QT_FP8) {
             switch (MT) { case 1: FLAUNCH(1); break; case 2: FLAUNCH(2); break; case 4: FLAUNCH(4); break; default: FLAUNCH(8); break; }
             return;
         }
 #undef FLAUNCH
-#define ILAUNCH(MT_) launch_k(int4gemm_kernel<MT_>, dim3(grid), dim3(GEMM_THREADS), Int4GemmCfg<MT_>::SMEM_BYTES, p, KC_GEMM, s, prof)
+#define ILAUNCH(MT_)                                                                                                                  \
+    (tails ? launch_k(int4gemm_tail_kernel<MT_>, dim3(grid), dim3(GEMM_THREADS), Int4GemmCfg<MT_, true>::SMEM_BYTES, p, KC_GEMM, s, prof) \
+           : launch_k(int4gemm_kernel<MT_>, dim3(grid), dim3(GEMM_THREADS), Int4GemmCfg<MT_>::SMEM_BYTES, p, KC_GEMM, s, prof))
         if (g.qtype == QT_INT4) {
             switch (MT) { case 1: ILAUNCH(1); break; case 2: ILAUNCH(2); break; case 4: ILAUNCH(4); break; default: ILAUNCH(8); break; }
             return;
         }
 #undef ILAUNCH
-#define QLAUNCH(MT_, QT_) launch_k(qgemm_kernel<MT_, QT_>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<MT_, QT_>::SMEM_BYTES, p, KC_GEMM, s, prof)
+#define QLAUNCH(MT_, QT_)                                                                                                                  \
+    (tails ? launch_k(qgemm_tail_kernel<MT_, QT_>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<MT_, QT_>::SMEM_BYTES, p, KC_GEMM, s, prof) \
+           : launch_k(qgemm_kernel<MT_, QT_>, dim3(grid), dim3(QGEMM_THREADS), QGemmCfg<MT_, QT_>::SMEM_BYTES, p, KC_GEMM, s, prof))
         if (g.qtype == QT_INT8) {
             switch (MT) { case 1: QLAUNCH(1, QT_INT8); break; case 2: QLAUNCH(2, QT_INT8); break; case 4: QLAUNCH(4, QT_INT8); break; default: QLAUNCH(8, QT_INT8); break; }
         } else {
@@ -1225,7 +1264,9 @@ static void gemm_smem_limits(int qtype) {
     CK(cudaFuncSetAttribute(gemm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<4>::SMEM_BYTES));
     CK(cudaFuncSetAttribute(gemm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<8>::SMEM_BYTES));
     if (qtype == QT_INT8 || qtype == QT_NF4) {
-#define QATTR(MT_, QT_) CK(cudaFuncSetAttribute(qgemm_kernel<MT_, QT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, QGemmCfg<MT_, QT_>::SMEM_BYTES))
+#define QATTR(MT_, QT_)                                                                                                   \
+    CK(cudaFuncSetAttribute(qgemm_kernel<MT_, QT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, QGemmCfg<MT_, QT_>::SMEM_BYTES)); \
+    CK(cudaFuncSetAttribute(qgemm_tail_kernel<MT_, QT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, QGemmCfg<MT_, QT_>::SMEM_BYTES))
         QATTR(1, QT_INT8); QATTR(2, QT_INT8); QATTR(4, QT_INT8); QATTR(8, QT_INT8);
         QATTR(1, QT_NF4); QATTR(2, QT_NF4); QATTR(4, QT_NF4); QATTR(8, QT_NF4);
 #undef QATTR
@@ -1235,12 +1276,20 @@ static void gemm_smem_limits(int qtype) {
         CK(cudaFuncSetAttribute(fp8gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<2>::SMEM_BYTES));
         CK(cudaFuncSetAttribute(fp8gemm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<4>::SMEM_BYTES));
         CK(cudaFuncSetAttribute(fp8gemm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<8>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(fp8gemm_tail_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<1, true>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(fp8gemm_tail_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<2, true>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(fp8gemm_tail_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<4, true>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(fp8gemm_tail_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, Fp8GemmCfg<8, true>::SMEM_BYTES));
     }
     if (qtype == QT_INT4) {
         CK(cudaFuncSetAttribute(int4gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Int4GemmCfg<1>::SMEM_BYTES));
         CK(cudaFuncSetAttribute(int4gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Int4GemmCfg<2>::SMEM_BYTES));
         CK(cudaFuncSetAttribute(int4gemm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, Int4GemmCfg<4>::SMEM_BYTES));
         CK(cudaFuncSetAttribute(int4gemm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, Int4GemmCfg<8>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(int4gemm_tail_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Int4GemmCfg<1, true>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(int4gemm_tail_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Int4GemmCfg<2, true>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(int4gemm_tail_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, Int4GemmCfg<4, true>::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(int4gemm_tail_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, Int4GemmCfg<8, true>::SMEM_BYTES));
     }
 }
 
@@ -1703,7 +1752,7 @@ void b200rwkv_engine::build(const StFile& st) {
         ad_head = ad_launch(head, s_head);
         ad_head.p.nrows = d_meta + 2;
         if (ad_targets)
-            REQUIRE(ad_mats.size() == ad_place_matrices(st.tensors, ad_targets, quant_layers, quant_type).size(),
+            REQUIRE(ad_mats.size() == ad_place_matrices(st.tensors, ad_targets, ad_quant_layers(), quant_type).size(),
                     B200RWKV_ERR_INVALID, "internal: a targeted matrix has no W' plan");
         // load_adapter's staging, and the model's tensor shapes its file checks read
         size_t cols = 0, blocks = 0;
@@ -1806,10 +1855,10 @@ GemmLaunch b200rwkv_engine::ad_launch(const GemmLaunch& base, AdapterParams& sp)
         const StTensor& t = *d.t;
         if (d.slice >= 0 || !ends_with(t.name, ".weight") || t.shape.size() != 2 || d.k0 + d.K != t.shape[1]) continue;
         const std::string nm = t.name.substr(0, t.name.size() - 7);
-        bool planned = (ad_target_bit(nm) & ad_targets) && !in_quant_layer(nm, quant_layers, quant_type);
+        bool planned = (ad_target_bit(nm) & ad_targets) && !in_quant_layer(nm, ad_quant_layers(), quant_type);
         for (const LoraSrc& a : adapters) planned = planned || a.st->find(nm + ".lora.0");
         if (!planned) continue;
-        REQUIRE(base.qtype == QT_NONE && world == 1 && d.k0 % GEMM_BK == 0 && sp.nproj < AD_MAX_PROJ, B200RWKV_ERR_INVALID,
+        REQUIRE((base.qtype == QT_NONE || quant_adapters) && world == 1 && d.k0 % GEMM_BK == 0 && sp.nproj < AD_MAX_PROJ, B200RWKV_ERR_INVALID,
                 "internal: adapter on " + nm + " does not fit its launch");
         AdapterProj pj;
         memset(&pj, 0, sizeof(pj));
@@ -1832,13 +1881,20 @@ GemmLaunch b200rwkv_engine::ad_launch(const GemmLaunch& base, AdapterParams& sp)
         mat_seg.push_back((int)i);
     }
     if (mats.empty()) return base;
-    GemmLaunch g = make_launch(segs, base.force_grid, QT_NONE);
+    // quantised: the codes are quantised from the same rows as the base plan's, so they are its codes
+    GemmLaunch g = make_launch(segs, base.force_grid, base.qtype);
     for (size_t j = 0; j < mats.size(); ++j) {
         const GemmSeg& sg = g.p.seg[mat_seg[j]];
-        mats[j].W = (uint8_t*)g.p.W + (size_t)sg.blk_begin * GEMM_WBYTES;
         mats[j].tiles = sg.tiles;
-        mats[j].KB = sg.KB;
-        mats[j].kbw = sg.KB - n_adapters;
+        if (g.qtype == QT_NONE) {
+            mats[j].W = (uint8_t*)g.p.W + (size_t)sg.blk_begin * GEMM_WBYTES;
+            mats[j].KB = sg.KB;
+            mats[j].kbw = sg.KB - n_adapters;
+        } else {                        // the tail blocks alone: [tile][place]
+            mats[j].W = const_cast<uint8_t*>(g.p.tails) + (size_t)g.p.tblk[mat_seg[j]] * GEMM_WBYTES;
+            mats[j].KB = n_adapters;
+            mats[j].kbw = 0;
+        }
         ad_mats.push_back(mats[j]);
     }
     return g;
@@ -2844,7 +2900,7 @@ static int32_t create_rank(const uint8_t* st, size_t len, int32_t device, int32_
                            int32_t precision, int32_t rank, int32_t world, const std::vector<LoraArg>& lora, b200rwkv_engine** out,
                            int32_t quant_layers = 0, int32_t quant_type = 0,
                            const std::vector<b200rwkv_engine::LoraSrc>& adapters = {}, int32_t places = 0,
-                           uint32_t targets = 0, bool batch_inv = false) {
+                           uint32_t targets = 0, bool batch_inv = false, bool quant_adapters = false) {
     API_BEGIN((b200rwkv_engine*)nullptr)
     REQUIRE(out, B200RWKV_ERR_INVALID, "null out");
     *out = nullptr;
@@ -2885,6 +2941,7 @@ static int32_t create_rank(const uint8_t* st, size_t len, int32_t device, int32_
     e->n_adapters = adapters.empty() ? places : (int)adapters.size();
     e->ad_targets = targets;
     e->batch_inv = batch_inv;
+    e->quant_adapters = quant_adapters;
     e->build(f);
     e->loras.clear();            // the LoRA and adapter images are only borrowed during the build
     e->adapters.clear();
@@ -3892,8 +3949,12 @@ int32_t b200rwkv_op_ln(int32_t device, const b200rwkv_ln_args* args) {
 // stream-K cuts, workspace slots, repacking or quantisation) over caller-supplied matrices, launched by launch_gemm (kernel
 // per token-tile count, ring size, split operands, programmatic dependent launch) `launches` times back to back, as the
 // engine reuses a plan step after step.  A temporary engine object carries just what those two need.
-int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t quant_type, int32_t grid, int32_t launches,
-                         int32_t nseg, const b200rwkv_gemm_seg* seg, int32_t* plan_out) {
+// ntail > 0 (b200rwkv_op_gemm_tail): segment 0 is a W' plan with ntail adapter tail blocks, built through make_launch's own
+// tail path from one stand-in adapter file per block (lora.1 = that block's columns, alpha 1), and its operand's tail blocks
+// hold tail_u as the shrink kernel would have written them.
+static int32_t op_gemm_run(int32_t device, int32_t T, int32_t precision, int32_t quant_type, int32_t grid, int32_t launches,
+                           int32_t nseg, const b200rwkv_gemm_seg* seg, int32_t* plan_out, int32_t ntail = 0,
+                           const uint16_t* tail_e = nullptr, const uint16_t* tail_u = nullptr) {
     API_BEGIN((b200rwkv_engine*)nullptr)
     REQUIRE(seg && nseg >= 1 && nseg <= GEMM_MAX_SEG, B200RWKV_ERR_INVALID, "nseg must be 1..8");
     REQUIRE(T >= 1 && T <= A16_MAX_ROWS, B200RWKV_ERR_INVALID, "T must be 1..128");
@@ -3933,7 +3994,7 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
     size_t wmax = 0;
     for (int i = 0; i < nseg; ++i) {
         const b200rwkv_gemm_seg& s = seg[i];
-        wt[i].name = "op_gemm." + std::to_string(i);
+        wt[i].name = "op_gemm." + std::to_string(i) + ".weight";
         wt[i].dtype = "F16";
         wt[i].shape = {s.N, s.K};
         wt[i].data = reinterpret_cast<const uint8_t*>(s.w);
@@ -3947,6 +4008,22 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
         if (s.out_mode != OUT_F32) d.proto.grp_stride = (int)a16_halves(mat_cols(s));
         else d.proto.ldo = s.ldo;
     }
+    std::vector<StFile> tail_files(ntail);
+    std::vector<std::vector<uint16_t>> tail_cols(ntail);
+    for (int a = 0; a < ntail; ++a) {
+        const int N = seg[0].N;
+        tail_cols[a].resize((size_t)N * GEMM_BK);
+        for (int n = 0; n < N; ++n)
+            memcpy(&tail_cols[a][(size_t)n * GEMM_BK], tail_e + ((size_t)n * ntail + a) * GEMM_BK, GEMM_BK * 2);
+        StTensor& t = tail_files[a].tensors["op_gemm.0.lora.1"];
+        t.name = "op_gemm.0.lora.1";
+        t.dtype = "F16";
+        t.shape = {N, GEMM_BK};
+        t.data = reinterpret_cast<const uint8_t*>(tail_cols[a].data());
+        t.nbytes = tail_cols[a].size() * 2;
+        e->adapters.push_back({&tail_files[a], 1.f});
+    }
+    sv[0].ad_tail = ntail;
     e->d_tmp = Buf<__half>(wmax);                  // make_launch uploads each matrix through the engine's staging buffer
     GemmLaunch g = e->make_launch(sv, grid, quant_type);
     e->gemm_ws = (float*)e->dalloc(e->gemm_ws_floats * 4, false);
@@ -3976,11 +4053,18 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
         for (int i = 0; i < nseg; ++i) {
             const b200rwkv_gemm_seg& s = seg[i];
             GemmSeg& sg = runs[l].p.seg[i];
-            __half* a = (__half*)e->dalloc(a16_halves(s.K) * 2, true);
+            const int nt = i == 0 ? ntail : 0;
+            __half* a = (__half*)e->dalloc((a16_halves(s.K) + (size_t)nt * A16_KB_HALVES) * 2, true);
             CK(cudaMemcpy(xs, s.x + (size_t)l * T * s.K, (size_t)T * s.K * 4, cudaMemcpyHostToDevice));
             a16_from_f32_kernel<<<(int)std::min<size_t>(((size_t)T * s.K + 255) / 256, (size_t)e->num_sms * 8), 256>>>(xs, T, s.K, th, sh.split, a);
             CK(cudaGetLastError());
             CK(cudaDeviceSynchronize());           // xs is refilled by the next upload
+            if (nt) {                              // the operand's tail blocks after its own k blocks, as the shrink writes them
+                std::vector<uint16_t> u((size_t)nt * A16_KB_HALVES, 0);
+                for (int t = 0; t < T; ++t)
+                    for (int k = 0; k < nt * GEMM_BK; ++k) u[a16_index(t, k, th)] = tail_u[(size_t)t * nt * GEMM_BK + k];
+                CK(cudaMemcpy(a + a16_halves(s.K), u.data(), u.size() * 2, cudaMemcpyHostToDevice));
+            }
             sg.A = a;
             const size_t cells = (size_t)th * s.ldo;
             if (s.out_mode == OUT_F32) {
@@ -4016,6 +4100,21 @@ int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t q
             CK(cudaMemcpy(h.data(), runs[l].p.seg[i].out, h.size() * 2, cudaMemcpyDeviceToHost));
             a16_unpack(h, s.ldo, mat_cols(s), th, th, mat_cols(s), s.ldo, (uint16_t*)s.out + l * cells);
         }
+    API_END
+}
+
+int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t quant_type, int32_t grid, int32_t launches,
+                         int32_t nseg, const b200rwkv_gemm_seg* seg, int32_t* plan_out) {
+    return op_gemm_run(device, T, precision, quant_type, grid, launches, nseg, seg, plan_out);
+}
+
+// Operator-level entry for the parity tests: one W' launch (b200rwkv_op_gemm's planner and launcher, adapter tails)
+int32_t b200rwkv_op_gemm_tail(int32_t device, int32_t T, int32_t quant_type, int32_t grid, int32_t n, const b200rwkv_gemm_seg* seg,
+                              const uint16_t* tail_e, const uint16_t* tail_u, int32_t* plan_out) {
+    API_BEGIN((b200rwkv_engine*)nullptr)
+    REQUIRE(n >= 1 && n <= AD_MAX, B200RWKV_ERR_INVALID, "n must be 1..8");
+    REQUIRE(seg && tail_e && tail_u, B200RWKV_ERR_INVALID, "null segment or tail");
+    return op_gemm_run(device, T, 0, quant_type, grid, 1, 1, seg, plan_out, n, tail_e, tail_u);
     API_END
 }
 
@@ -4538,17 +4637,22 @@ int32_t b200rwkv_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int32_t
 // Replaces `ModelBuilder...build_vN()` + `Bundle::new` + `TokioRuntime::new` (lib.rs:484-497) with everything the reference's
 // ReloadRequest carries for this path: devices (one engine object owning all tensor-parallel ranks, SURVEY.md §8b), LoRA files
 // (lib.rs:466-485), precision (lib.rs:493).
-// b200rwkv_options as this library reads it: both sizes the header has had (the one before `batch_invariant` leaves the
-// mode off), every value checked before any CUDA call
-static int32_t read_options(const b200rwkv_options* opt, bool* batch_inv) {
+// b200rwkv_options as this library reads it: both sizes the header has had (the one before `batch_invariant` leaves both
+// flags off; `quant_adapters` fills the tail padding of the current size), every value checked before any CUDA call
+static int32_t read_options(const b200rwkv_options* opt, bool* batch_inv, bool* quant_adapters = nullptr) {
     if (opt->struct_bytes != sizeof(b200rwkv_options) && opt->struct_bytes != offsetof(b200rwkv_options, batch_invariant)) {
         g_err = "b200rwkv_options.struct_bytes does not match this library";
         return B200RWKV_ERR_INVALID;
     }
-    const int32_t bi = opt->struct_bytes == sizeof(b200rwkv_options) ? opt->batch_invariant : 0;
+    const bool full = opt->struct_bytes == sizeof(b200rwkv_options);
+    const int32_t bi = full ? opt->batch_invariant : 0;
+    const int32_t qa = full ? opt->quant_adapters : 0;
     if (bi != 0 && bi != 1) { g_err = "b200rwkv_options.batch_invariant must be 0 or 1"; return B200RWKV_ERR_INVALID; }
+    if (qa != 0 && qa != 1) { g_err = "b200rwkv_options.quant_adapters must be 0 or 1"; return B200RWKV_ERR_INVALID; }
     if (bi && opt->num_devices > 1) { g_err = "the batch-invariant mode runs on one GPU (no tensor parallelism)"; return B200RWKV_ERR_UNSUPPORTED; }
+    if (qa && opt->num_devices > 1) { g_err = "adapters on quantised layers run on one GPU (no tensor parallelism)"; return B200RWKV_ERR_UNSUPPORTED; }
     *batch_inv = bi != 0;
+    if (quant_adapters) *quant_adapters = qa != 0;
     return B200RWKV_OK;
 }
 
@@ -4598,12 +4702,14 @@ int32_t b200rwkv_create_adapters(const uint8_t* st, size_t len, const b200rwkv_o
     API_BEGIN((b200rwkv_engine*)nullptr)
     REQUIRE(out && opt, B200RWKV_ERR_INVALID, "null argument");
     *out = nullptr;
+    bool quant_adapters = false;
     {
         bool batch_inv = false;
-        if (const int32_t rc = read_options(opt, &batch_inv)) return rc;
+        if (const int32_t rc = read_options(opt, &batch_inv, &quant_adapters)) return rc;
         // a bound step runs W' plans with another K split: an unbound slot's bits would depend on its neighbours' bindings
         REQUIRE(!batch_inv, B200RWKV_ERR_UNSUPPORTED, "the batch-invariant mode does not run adapters");
     }
+    const int refused_layers = quant_adapters ? 0 : opt->quant_layers;     // layers whose matrices adapters may not pair
     REQUIRE(n >= 1 && n <= AD_MAX, B200RWKV_ERR_INVALID, "number of adapters must be 1..8");
     REQUIRE(adapter_st && adapter_len && adapter_alpha, B200RWKV_ERR_INVALID, "null adapter list");
     REQUIRE(opt->num_devices <= 1, B200RWKV_ERR_UNSUPPORTED, "adapters run on one GPU (no tensor parallelism)");
@@ -4617,12 +4723,12 @@ int32_t b200rwkv_create_adapters(const uint8_t* st, size_t len, const b200rwkv_o
         files.emplace_back(new StFile(adapter_st[a], adapter_len[a]));
         srcs.push_back({files.back().get(), adapter_alpha[a]});
     }
-    check_adapter_files(model.tensors, srcs, opt->quant_layers, opt->quant_type);
+    check_adapter_files(model.tensors, srcs, refused_layers, opt->quant_type);
     std::vector<LoraArg> lora;
     for (int i = 0; i < opt->num_lora; ++i) lora.push_back({opt->lora_st[i], opt->lora_len[i], opt->lora_alpha[i]});
     const int dev0 = opt->num_devices <= 0 ? 0 : opt->devices[0];
     return create_rank(st, len, dev0, opt->max_batch, opt->token_chunk_size, opt->precision, 0, 1, lora, out, opt->quant_layers,
-                       opt->quant_type, srcs);
+                       opt->quant_type, srcs, 0, 0, false, quant_adapters);
     API_END
 }
 
@@ -4633,9 +4739,10 @@ int32_t b200rwkv_create_adapter_places(const uint8_t* st, size_t len, const b200
     API_BEGIN((b200rwkv_engine*)nullptr)
     REQUIRE(out && opt, B200RWKV_ERR_INVALID, "null argument");
     *out = nullptr;
+    bool quant_adapters = false;
     {
         bool batch_inv = false;
-        if (const int32_t rc = read_options(opt, &batch_inv)) return rc;
+        if (const int32_t rc = read_options(opt, &batch_inv, &quant_adapters)) return rc;
         // a bound step runs W' plans with another K split: an unbound slot's bits would depend on its neighbours' bindings
         REQUIRE(!batch_inv, B200RWKV_ERR_UNSUPPORTED, "the batch-invariant mode does not run adapters");
     }
@@ -4646,13 +4753,13 @@ int32_t b200rwkv_create_adapter_places(const uint8_t* st, size_t len, const b200
     REQUIRE(opt->num_lora >= 0 && opt->num_lora <= B200RWKV_MAX_LORA, B200RWKV_ERR_INVALID, "bad num_lora");
     REQUIRE(opt->quant_layers >= 0 && opt->quant_type >= 0, B200RWKV_ERR_INVALID, "bad quant_layers / quant_type");
     StFile model(st, len);
-    REQUIRE(!ad_place_matrices(model.tensors, targets, opt->quant_layers, opt->quant_type).empty(), B200RWKV_ERR_UNSUPPORTED,
-            "adapter targets name no f16 projection matrix of this model");
+    REQUIRE(!ad_place_matrices(model.tensors, targets, quant_adapters ? 0 : opt->quant_layers, opt->quant_type).empty(),
+            B200RWKV_ERR_UNSUPPORTED, "adapter targets name no f16 projection matrix of this model");
     std::vector<LoraArg> lora;
     for (int i = 0; i < opt->num_lora; ++i) lora.push_back({opt->lora_st[i], opt->lora_len[i], opt->lora_alpha[i]});
     const int dev0 = opt->num_devices <= 0 ? 0 : opt->devices[0];
     return create_rank(st, len, dev0, opt->max_batch, opt->token_chunk_size, opt->precision, 0, 1, lora, out, opt->quant_layers,
-                       opt->quant_type, {}, n, targets);
+                       opt->quant_type, {}, n, targets, false, quant_adapters);
     API_END
 }
 
@@ -4667,7 +4774,7 @@ int32_t b200rwkv_load_adapter(b200rwkv_engine* e, int32_t id, const uint8_t* ada
     REQUIRE(!e->place_full[id - 1], B200RWKV_ERR_STATE,
             "load_adapter: place " + std::to_string(id) + " holds an adapter (unload it first)");
     StFile f(adapter_st, adapter_len);
-    check_adapter_files(e->model_shapes, {{&f, alpha}}, e->quant_layers, e->quant_type);
+    check_adapter_files(e->model_shapes, {{&f, alpha}}, e->ad_quant_layers(), e->quant_type);
     for (auto& kv : f.tensors) {
         if (!ends_with(kv.first, ".lora.0")) continue;
         const std::string base = kv.first.substr(0, kv.first.size() - 7);

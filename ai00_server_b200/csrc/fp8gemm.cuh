@@ -33,9 +33,11 @@ constexpr int FP8_WBYTES = GEMM_BN * GEMM_BK;              // 16 KB of codes per
 constexpr int FP8_SCALE_BYTES = GEMM_BN * 4;               // f32 row scales of one tile
 constexpr float FP8_E4M3_MAX = 448.f;
 
-template <int MT>
+// TAILS (fp8gemm_tail_kernel, W' plans): a ring slot holds a whole f16 tail block before the token operand
+template <int MT, bool TAILS = false>
 struct Fp8GemmCfg {
-    static constexpr int STAGE_BYTES = FP8_WBYTES + MT * GEMM_ABYTES;
+    static constexpr int SLOT_W = TAILS ? GEMM_WBYTES : FP8_WBYTES;
+    static constexpr int STAGE_BYTES = SLOT_W + MT * GEMM_ABYTES;
     static constexpr int NFIT = GEMM_SMEM_BUDGET / STAGE_BYTES;
     static constexpr int NSTAGE = NFIT > 12 ? 12 : NFIT;
     static constexpr int BAR_BYTES = 2 * NSTAGE * 8 + 16;
@@ -103,6 +105,25 @@ struct WgmmaRs<128> {
             : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
     }
 };
+
+// W' plans: the MMAs of one f16 tail block of a ring slot (weights at st, token operand at ast) with the shared-memory A
+// descriptors of gemm.cuh, leaving them as the one group in flight (the previous block's MMAs have retired on return)
+template <int MT>
+__device__ __forceinline__ void tail_block_mma(float (&acc)[2][8 * MT], const uint32_t st, const uint32_t ast) {
+    constexpr uint32_t a_lbo = 16 * MT * 16;
+    wgmma_fence_operand(acc[0]);
+    wgmma_fence_operand(acc[1]);
+    wgmma_fence();
+#pragma unroll
+    for (int k16 = 0; k16 < GEMM_BK / 16; ++k16) {
+        const uint64_t bdesc = gmma_desc(ast + k16 * 2 * a_lbo, a_lbo, GEMM_A_SBO);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+            wgmma_f16<16 * MT>(acc[h], gmma_desc(st + h * 8 * GEMM_W_SBO + k16 * 2 * GEMM_W_LBO, GEMM_W_LBO, GEMM_W_SBO), bdesc);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+}
 
 // ---------------------------------------------------------------------------------------
 // kernel: warps 0-3 consumer warpgroup (conversion + MMA + gemm.cuh epilogue), warp 4 TMA producer
@@ -245,6 +266,131 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) fp8gemm_kernel(const __grid_c
     if (tid == 0 && tr) tr[7] = globaltimer_ns();
     if (tid == 0 && p.trace) p.trace[8 + 3 * cta + 2] = globaltimer_ns();
 }
+
+// W' plans (adapters on quantised layers): code blocks, then f16 tail blocks (GemmParams::tails) with gemm.cuh's shared-memory
+// MMAs.  Stream-K partials are summed linearly, so each CTA scales the code part of its accumulator by the row scales before
+// its first tail block (or at its end) and adds its tail part unscaled: s_n x W^T + u e^T whichever blocks a CTA holds.
+template <int MT>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) fp8gemm_tail_kernel(const __grid_constant__ GemmParams p) {
+    using Cfg = Fp8GemmCfg<MT, true>;
+    constexpr int NSTAGE = Cfg::NSTAGE, STAGE_BYTES = Cfg::STAGE_BYTES, KG = Cfg::KG;
+    extern __shared__ __align__(128) uint8_t smem[];
+    __shared__ int s_last;
+    __shared__ __align__(16) float s_x[GEMM_XPOSE_FLOATS];
+    const uint32_t ring_base = smem_u32(smem);
+    const uint32_t full_bar = ring_base + NSTAGE * STAGE_BYTES;
+    const uint32_t empty_bar = full_bar + NSTAGE * 8;
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const long long TB = p.total_blocks;
+    const int G = gridDim.x, cta = blockIdx.x;
+    const int b0 = (int)((long long)cta * TB / G);
+    const int b1 = (int)((long long)(cta + 1) * TB / G);
+    unsigned long long* const tr = (p.trace && cta == 0) ? p.trace : nullptr;
+
+    if (tid == 0) {
+        if (tr) tr[0] = globaltimer_ns();
+        for (int s = 0; s < NSTAGE; ++s) {
+            mbar_init(full_bar + s * 8, 1);
+            mbar_init(empty_bar + s * 8, GEMM_EPI_WARPS);
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+    pdl_launch_dependents();
+
+    if (warp == GEMM_EPI_WARPS) {
+        // ===================== producer =====================
+        if (lane == 0) tail_producer<MT, NSTAGE, STAGE_BYTES, Cfg::SLOT_W, FP8_WBYTES, true>(p, b0, b1, ring_base, full_bar, empty_bar, tr);
+    } else {
+        // ===================== consumer warpgroup: conversion + MMA + epilogue =====================
+        pdl_wait();
+        constexpr uint32_t a_lbo = 16 * MT * 16;
+        RingPos rp{0, 0u};
+        SegWalk w;
+        w.init(p, b0, b1);
+        while (!w.done()) {
+            const int nblk = w.nblk();
+            const int nq = max(0, min(nblk, p.kbq[w.seg] - w.kb));     // code blocks first, then f16 tail blocks
+            float acc[2][8 * MT];
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int i = 0; i < 8 * MT; ++i) acc[h][i] = 0.f;
+            // the code part of the accumulator times its rows' scales (fragment rows as in gemm_acc_to_rows), before any
+            // tail block adds to it and before the partial or the epilogue
+            auto scale_codes = [&]() {
+                const float* sc = p.scales + (size_t)(p.seg[w.seg].tile_begin + w.tile_local) * GEMM_BN + 16 * warp + (lane >> 2);
+                const float s[2][2] = {{sc[0], sc[8]}, {sc[64], sc[72]}};
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int i = 0; i < 8 * MT; ++i) acc[h][i] = __fmul_rn(acc[h][i], s[h][(i >> 1) & 1]);
+            };
+            uint32_t a[2][KG][2][4];                   // [register buffer][k16 step of the group][weight half][fragment register]
+            int prev_stage = -1;
+            for (int i = 0; i < nblk; ++i) {
+                mbar_wait(full_bar + rp.stage * 8, rp.phase, 12);
+                const uint32_t st = ring_base + rp.stage * STAGE_BYTES;
+                const uint32_t ast = st + Cfg::SLOT_W;
+                if (i >= nq) {
+                    if (i == nq && nq > 0) {
+                        wgmma_wait<0>();
+                        wgmma_fence_operand(acc[0]);
+                        wgmma_fence_operand(acc[1]);
+                        scale_codes();
+                    }
+                    tail_block_mma<MT>(acc, st, ast);
+                } else {
+#pragma unroll
+                    for (int g = 0; g < GEMM_BK / 16 / KG; ++g) {
+                        uint32_t(&ab)[KG][2][4] = a[g & 1];     // the group that last read this buffer has retired
+#pragma unroll
+                        for (int s = 0; s < KG; ++s) {
+                            const uint4 c = lds128(st + (uint32_t)(((g * KG + s) * GEMM_EPI_THREADS + tid) * 16));
+                            e4m3x4_to_f16(c.x, ab[s][0][0], ab[s][0][1]);
+                            e4m3x4_to_f16(c.y, ab[s][0][2], ab[s][0][3]);
+                            e4m3x4_to_f16(c.z, ab[s][1][0], ab[s][1][1]);
+                            e4m3x4_to_f16(c.w, ab[s][1][2], ab[s][1][3]);
+                        }
+                        wgmma_fence_operand(acc[0]);
+                        wgmma_fence_operand(acc[1]);
+                        wgmma_fence();                       // the conversions' register writes before the MMAs that read them
+#pragma unroll
+                        for (int s = 0; s < KG; ++s) {
+                            const uint64_t bdesc = gmma_desc(ast + (g * KG + s) * 2 * a_lbo, a_lbo, GEMM_A_SBO);
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) WgmmaRs<16 * MT>::mma(acc[h], ab[s][h], bdesc);
+                        }
+                        wgmma_commit();
+                        wgmma_wait<1>();                     // the previous group retired: its register buffer may be rewritten
+                    }
+                }
+                // every MMA of the previous block has retired: its ring slot goes back
+                if (prev_stage >= 0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(empty_bar + prev_stage * 8);
+                }
+                prev_stage = rp.stage;
+                rp.advance<NSTAGE>(1);
+            }
+            wgmma_wait<0>();
+            wgmma_fence_operand(acc[0]);
+            wgmma_fence_operand(acc[1]);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar + prev_stage * 8);
+            if (nq == nblk) scale_codes();
+            float v[MT][16];
+            gemm_acc_to_rows<MT>(acc, v, s_x);
+            gemm_epilogue_tile<MT, false>(p, w, cta, G, v, *p.nrows, &s_last, reinterpret_cast<__half*>(s_x));
+            w.next();
+        }
+    }
+    __syncthreads();
+    if (tid == 0 && tr) tr[7] = globaltimer_ns();
+    if (tid == 0 && p.trace) p.trace[8 + 3 * cta + 2] = globaltimer_ns();
+}
+
 
 // ---------------------------------------------------------------------------------------
 // Quantiser (load time).  One warp per weight row of the launch's `tiles` tiles: the absmax over the whole source row (ld

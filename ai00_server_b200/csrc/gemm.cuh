@@ -89,6 +89,12 @@ struct GemmParams {
     uint32_t w_lbo, w_sbo, a_lbo, a_sbo;   // wgmma descriptor strides (bytes)
     unsigned long long* trace;             // profiling aid: 8 globaltimer stamps of CTA 0 (null in production)
     GemmSeg seg[GEMM_MAX_SEG];
+    // Quantised W' plans (adapter tails, read by the *gemm_tail_kernel instantiations only): each tile of segment s is kbq[s]
+    // code blocks, then KB - kbq[s] f16 tail blocks (GEMM_WBYTES each, repack_weight_kernel's layout).  Its code blocks are
+    // blocks qblk[s].. of W, its tail blocks blocks tblk[s].. of `tails`, both tile-major.
+    const uint8_t* tails;
+    const float* scales;                   // FP8: the row scales [global tile][128] behind the code blocks
+    int kbq[GEMM_MAX_SEG], qblk[GEMM_MAX_SEG], tblk[GEMM_MAX_SEG];
 };
 
 // HALF: ring sized to half an SM's shared memory, so the NEXT projection launch (programmatic

@@ -34,9 +34,11 @@ constexpr int INT4_WBYTES = GEMM_BN * GEMM_BK / 2;                   // 8 KB of 
 constexpr int INT4_BLOCK_BYTES = INT4_WBYTES + Q_PARAM_BYTES;        // 8 704: codes + (scale, min) of its 128 rows
 static_assert(INT4_BLOCK_BYTES == Q_NF4_BYTES, "q_block_bytes(QT_INT4)");
 
-template <int MT>
+// TAILS (int4gemm_tail_kernel, W' plans): a ring slot holds a whole f16 tail block before the token operand
+template <int MT, bool TAILS = false>
 struct Int4GemmCfg {
-    static constexpr int STAGE_BYTES = INT4_BLOCK_BYTES + MT * GEMM_ABYTES;
+    static constexpr int SLOT_W = TAILS ? GEMM_WBYTES : INT4_BLOCK_BYTES;
+    static constexpr int STAGE_BYTES = SLOT_W + MT * GEMM_ABYTES;
     static constexpr int NFIT = GEMM_SMEM_BUDGET / STAGE_BYTES;
     static constexpr int NSTAGE = NFIT > 12 ? 12 : NFIT;
     static constexpr int BAR_BYTES = 2 * NSTAGE * 8 + 16;
@@ -225,6 +227,122 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) int4gemm_kernel(const __grid_
     if (tid == 0 && tr) tr[7] = globaltimer_ns();
     if (tid == 0 && p.trace) p.trace[8 + 3 * cta + 2] = globaltimer_ns();
 }
+
+// W' plans (adapters on quantised layers): code blocks, then f16 tail blocks (GemmParams::tails) with gemm.cuh's shared-memory
+// MMAs (fp8gemm.cuh tail_block_mma)
+template <int MT>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) int4gemm_tail_kernel(const __grid_constant__ GemmParams p) {
+    using Cfg = Int4GemmCfg<MT, true>;
+    constexpr int NSTAGE = Cfg::NSTAGE, STAGE_BYTES = Cfg::STAGE_BYTES, KG = Cfg::KG;
+    extern __shared__ __align__(128) uint8_t smem[];
+    __shared__ int s_last;
+    __shared__ __align__(16) float s_x[GEMM_XPOSE_FLOATS];
+    const uint32_t ring_base = smem_u32(smem);
+    const uint32_t full_bar = ring_base + NSTAGE * STAGE_BYTES;
+    const uint32_t empty_bar = full_bar + NSTAGE * 8;
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const long long TB = p.total_blocks;
+    const int G = gridDim.x, cta = blockIdx.x;
+    const int b0 = (int)((long long)cta * TB / G);
+    const int b1 = (int)((long long)(cta + 1) * TB / G);
+    unsigned long long* const tr = (p.trace && cta == 0) ? p.trace : nullptr;
+
+    if (tid == 0) {
+        if (tr) tr[0] = globaltimer_ns();
+        for (int s = 0; s < NSTAGE; ++s) {
+            mbar_init(full_bar + s * 8, 1);
+            mbar_init(empty_bar + s * 8, GEMM_EPI_WARPS);
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+    pdl_launch_dependents();
+
+    if (warp == GEMM_EPI_WARPS) {
+        // ===================== producer =====================
+        if (lane == 0) tail_producer<MT, NSTAGE, STAGE_BYTES, Cfg::SLOT_W, INT4_BLOCK_BYTES, true>(p, b0, b1, ring_base, full_bar, empty_bar, tr);
+    } else {
+        // ===================== consumer warpgroup: conversion + MMA + epilogue =====================
+        pdl_wait();
+        constexpr uint32_t a_lbo = 16 * MT * 16;
+        RingPos rp{0, 0u};
+        SegWalk w;
+        w.init(p, b0, b1);
+        while (!w.done()) {
+            const int nblk = w.nblk();
+            const int nq = max(0, min(nblk, p.kbq[w.seg] - w.kb));     // code blocks first, then f16 tail blocks
+            float acc[2][8 * MT];
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int i = 0; i < 8 * MT; ++i) acc[h][i] = 0.f;
+            uint32_t a[2][KG][2][4];                   // [register buffer][k16 step of the group][weight half][fragment register]
+            int prev_stage = -1;
+            for (int i = 0; i < nblk; ++i) {
+                mbar_wait(full_bar + rp.stage * 8, rp.phase, 12);
+                const uint32_t st = ring_base + rp.stage * STAGE_BYTES;
+                const uint32_t ast = st + Cfg::SLOT_W;
+                if (i >= nq) {
+                    tail_block_mma<MT>(acc, st, ast);
+                } else {
+                    // {scale, min} of rows g, g + 8 (half 0) and 64 + g, 72 + g (half 1) of this thread's fragments
+                    const uint4 pr = lds128(st + INT4_WBYTES + (uint32_t)(tid >> 2) * 16);
+                    const uint32_t prw[4] = {pr.x, pr.y, pr.z, pr.w};
+                    __half2 s2[4], m2[4];
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        s2[j] = u32_as_h2(prmt(prw[j], 0u, 0x1010u));
+                        m2[j] = u32_as_h2(prmt(prw[j], 0u, 0x3232u));
+                    }
+#pragma unroll
+                    for (int g = 0; g < GEMM_BK / 16 / KG; ++g) {
+                        uint32_t(&ab)[KG][2][4] = a[g & 1];     // the group that last read this buffer has retired
+#pragma unroll
+                        for (int s = 0; s < KG; s += 2) {
+                            const uint4 c = lds128(st + (uint32_t)((((g * KG + s) >> 1) * GEMM_EPI_THREADS + tid) * 16));
+                            int4x8_to_f16(c.x, s2[0], m2[0], s2[1], m2[1], ab[s][0]);
+                            int4x8_to_f16(c.y, s2[2], m2[2], s2[3], m2[3], ab[s][1]);
+                            int4x8_to_f16(c.z, s2[0], m2[0], s2[1], m2[1], ab[s + 1][0]);
+                            int4x8_to_f16(c.w, s2[2], m2[2], s2[3], m2[3], ab[s + 1][1]);
+                        }
+                        wgmma_fence_operand(acc[0]);
+                        wgmma_fence_operand(acc[1]);
+                        wgmma_fence();                       // the conversions' register writes before the MMAs that read them
+#pragma unroll
+                        for (int s = 0; s < KG; ++s) {
+                            const uint64_t bdesc = gmma_desc(ast + (g * KG + s) * 2 * a_lbo, a_lbo, GEMM_A_SBO);
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) WgmmaRs<16 * MT>::mma(acc[h], ab[s][h], bdesc);
+                        }
+                        wgmma_commit();
+                        wgmma_wait<1>();                     // the previous group retired: its register buffer may be rewritten
+                    }
+                }
+                // every MMA of the previous block has retired: its ring slot goes back
+                if (prev_stage >= 0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(empty_bar + prev_stage * 8);
+                }
+                prev_stage = rp.stage;
+                rp.advance<NSTAGE>(1);
+            }
+            wgmma_wait<0>();
+            wgmma_fence_operand(acc[0]);
+            wgmma_fence_operand(acc[1]);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar + prev_stage * 8);
+            float v[MT][16];
+            gemm_acc_to_rows<MT>(acc, v, s_x);
+            gemm_epilogue_tile<MT, false>(p, w, cta, G, v, *p.nrows, &s_last, reinterpret_cast<__half*>(s_x));
+            w.next();
+        }
+    }
+    __syncthreads();
+    if (tid == 0 && tr) tr[7] = globaltimer_ns();
+    if (tid == 0 && p.trace) p.trace[8 + 3 * cta + 2] = globaltimer_ns();
+}
+
 
 // ---------------------------------------------------------------------------------------
 // Quantiser (load time).  One warp per (weight row, 128-wide k block) of rows [n0, n0+N), columns [k0, k0+128 KB) of a

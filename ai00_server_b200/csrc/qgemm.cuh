@@ -88,6 +88,72 @@ __device__ __forceinline__ uint32_t int8_pair(const uint32_t w, const uint32_t s
 }
 
 // ---------------------------------------------------------------------------------------
+// Quantised W' plans (adapters on quantised layers): the launch's linear stage blocks walked one at a time, and the producer
+// lane of the tail kernels.  A tile's f16 tail blocks follow its code blocks in the block sequence, so the stream-K cuts,
+// SegWalk and the epilogue are unchanged; only where a block's weights live differs (GemmParams::tails).
+// ---------------------------------------------------------------------------------------
+struct TailPos {
+    int seg, tile, kb;
+    __device__ __forceinline__ void init(const GemmParams& p, const int b) {
+        seg = gemm_find_seg(p, b);
+        const GemmSeg& sg = p.seg[seg];
+        tile = (b - sg.blk_begin) / sg.KB;
+        kb = b - sg.blk_begin - tile * sg.KB;
+    }
+    __device__ __forceinline__ void next(const GemmParams& p) {
+        if (++kb < p.seg[seg].KB) return;
+        kb = 0;
+        if (++tile < p.seg[seg].tiles) return;
+        tile = 0;
+        if (seg + 1 < p.nseg) ++seg;
+    }
+    __device__ __forceinline__ bool tail(const GemmParams& p) const { return kb >= p.kbq[seg]; }
+    __device__ __forceinline__ const uint8_t* tail_src(const GemmParams& p) const {
+        const int q = p.kbq[seg];
+        return p.tails + ((size_t)p.tblk[seg] + (size_t)tile * (p.seg[seg].KB - q) + (kb - q)) * GEMM_WBYTES;
+    }
+    // code block of QB bytes
+    __device__ __forceinline__ const uint8_t* code_src(const GemmParams& p, const int QB) const {
+        return p.W + ((size_t)p.qblk[seg] + (size_t)tile * p.kbq[seg] + kb) * QB;
+    }
+};
+
+// The producer lane of gemm.cuh for W' plans: code blocks of QB bytes and, with TAIL_IN_RING, the 32 KB tail blocks go to the
+// ring slot (SLOT_W bytes), the token operand after them; without it a tail block's slot receives the token operand only.
+template <int MT, int NSTAGE, int STAGE_BYTES, int SLOT_W, int QB, bool TAIL_IN_RING>
+__device__ __forceinline__ void tail_producer(const GemmParams& p, const int b0, const int b1, const uint32_t ring_base,
+                                              const uint32_t full_bar, const uint32_t empty_bar, unsigned long long* tr) {
+    static_assert(!TAIL_IN_RING || SLOT_W >= GEMM_WBYTES, "a tail block fits its ring slot");
+    const uint64_t pol_w = l2_policy_evict_first();
+    const uint64_t pol_a = l2_policy_evict_last();
+    auto weights = [&](const TailPos& q, const uint32_t st, const uint32_t fb) {
+        const bool tail = q.tail(p);
+        const int wb = tail ? (TAIL_IN_RING ? GEMM_WBYTES : 0) : QB;
+        mbar_expect_tx(fb, wb + MT * GEMM_ABYTES);
+        if (wb) bulk_g2s_hint(st, tail ? q.tail_src(p) : q.code_src(p, QB), wb, fb, pol_w);
+    };
+    TailPos pos;
+    pos.init(p, b0);
+    TailPos pre = pos;
+    const int npre = min(b1 - b0, NSTAGE);
+    for (int i = 0; i < npre; ++i, pre.next(p)) weights(pre, ring_base + i * STAGE_BYTES, full_bar + i * 8);    // before the wait, as gemm.cuh
+    pdl_wait();
+    if (tr) tr[2] = globaltimer_ns();
+    int stage = 0;
+    uint32_t ephase = 1;
+    for (int b = b0, it = 0; b < b1; ++b, ++it, pos.next(p)) {
+        const uint32_t st = ring_base + stage * STAGE_BYTES;
+        const uint32_t fb = full_bar + stage * 8;
+        if (it >= NSTAGE) {
+            mbar_wait(empty_bar + stage * 8, ephase, 14);
+            weights(pos, st, fb);
+        }
+        bulk_g2s_hint(st + SLOT_W, p.seg[pos.seg].A + (size_t)pos.kb * A16_KB_HALVES, MT * GEMM_ABYTES, fb, pol_a);
+        if (++stage == NSTAGE) { stage = 0; ephase ^= 1; }
+    }
+}
+
+// ---------------------------------------------------------------------------------------
 // expansion role: 128 threads, thread r = weight row r of every stage block, into the canonical layout of gemm.cuh
 // ---------------------------------------------------------------------------------------
 template <int QT>
@@ -291,6 +357,151 @@ __global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_kernel(const __grid_co
     if (tid == 0 && tr) tr[7] = globaltimer_ns();
     if (tid == 0 && p.trace) p.trace[8 + 3 * cta + 2] = globaltimer_ns();
 }
+
+// W' plans (adapters on quantised layers): qgemm_kernel over code blocks and f16 tail blocks (GemmParams::tails).  A tail
+// block's ring slot holds only its token operand; the expansion warps copy the tail block from global memory into the
+// hand-off buffer instead of expanding codes, and the consumer reads it as any other.  The ring keeps the base kernel's size.
+template <int MT, int QT>
+__global__ void __launch_bounds__(QGEMM_THREADS, 1) qgemm_tail_kernel(const __grid_constant__ GemmParams p) {
+    using Cfg = QGemmCfg<MT, QT>;
+    constexpr int NBUF = Cfg::NBUF;
+    constexpr int NSTAGE = Cfg::NSTAGE, STAGE_BYTES = Cfg::STAGE_BYTES, RAW_W = Cfg::RAW_W;
+    extern __shared__ __align__(128) uint8_t smem[];
+    __shared__ int s_last;
+    __shared__ __align__(16) float s_x[GEMM_XPOSE_FLOATS];
+    const uint32_t smem_base = smem_u32(smem);
+    const uint32_t dq_base = smem_base;
+    const uint32_t lut_base = dq_base + Cfg::DQ_BYTES;
+    const uint32_t ring_base = lut_base + Cfg::LUT;
+    const uint32_t full_bar = ring_base + NSTAGE * STAGE_BYTES;
+    const uint32_t empty_bar = full_bar + NSTAGE * 8;
+    const uint32_t dfull_bar = empty_bar + NSTAGE * 8;
+    const uint32_t dfree_bar = dfull_bar + NBUF * 8;
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const long long TB = p.total_blocks;
+    const int G = gridDim.x, cta = blockIdx.x;
+    const int b0 = (int)((long long)cta * TB / G);
+    const int b1 = (int)((long long)(cta + 1) * TB / G);
+    unsigned long long* const tr = (p.trace && cta == 0) ? p.trace : nullptr;
+    constexpr int EXP_WARP0 = GEMM_THREADS / 32;
+
+    if (tid == 0) {
+        if (tr) tr[0] = globaltimer_ns();
+        for (int s = 0; s < NSTAGE; ++s) {
+            mbar_init(full_bar + s * 8, 1);
+            mbar_init(empty_bar + s * 8, GEMM_EPI_WARPS);
+        }
+        for (int s = 0; s < NBUF; ++s) {
+            mbar_init(dfull_bar + s * 8, Q_DQ_WARPS);          // one arrival per expansion warp
+            mbar_init(dfree_bar + s * 8, GEMM_EPI_WARPS);
+        }
+        mbar_fence_init();
+    }
+    if (QT == QT_NF4 && warp >= EXP_WARP0) {
+        // level-pair table, one copy per lane: entry (byte, lane) = {level[byte & 15], level[byte >> 4]}
+        const int t = tid - GEMM_THREADS;
+        for (int i = t; i < 256 * 32; i += Q_DQ_THREADS) {
+            const int byte = i >> 5;
+            const __half2 e = __halves2half2(__float2half_rn(c_nf4_levels[byte & 15]), __float2half_rn(c_nf4_levels[byte >> 4]));
+            *reinterpret_cast<__half2*>(smem + (lut_base - smem_base) + (size_t)i * 4) = e;
+        }
+    }
+    __syncthreads();
+    pdl_launch_dependents();
+
+    if (warp == GEMM_EPI_WARPS) {
+        // ===================== producer =====================
+        if (lane == 0) tail_producer<MT, NSTAGE, STAGE_BYTES, RAW_W, RAW_W, false>(p, b0, b1, ring_base, full_bar, empty_bar, tr);
+    } else if (warp >= EXP_WARP0) {
+        // ===================== expansion: 4 warps =====================
+        const int r = tid - GEMM_THREADS;
+        RingPos rp{0, 0u};
+        TailPos pos;
+        pos.init(p, b0);
+        for (int b = b0, it = 0; b < b1; ++b, ++it) {
+            const int d = it % NBUF;
+            const int u = it / NBUF;
+            mbar_wait(full_bar + rp.stage * 8, rp.phase, 16);
+            if (u > 0) mbar_wait(dfree_bar + d * 8, (unsigned)(u - 1) & 1u, 17);          // the MMAs that read this buffer retired
+            if (pos.tail(p)) {
+                // 2048 16-byte chunks, already in the buffer's layout: 4 loads in flight per thread at a time (more spill at MT = 8)
+                const uint4* src = reinterpret_cast<const uint4*>(pos.tail_src(p));
+#pragma unroll
+                for (int j0 = 0; j0 < GEMM_WBYTES / 16 / Q_DQ_THREADS; j0 += 4) {
+                    uint4 v[4];
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) v[j] = __ldg(src + (j0 + j) * Q_DQ_THREADS + r);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) sts128(dq_base + d * GEMM_WBYTES + (uint32_t)((j0 + j) * Q_DQ_THREADS + r) * 16, v[j]);
+                }
+            } else {
+                q_expand_block<QT>(ring_base + rp.stage * STAGE_BYTES, dq_base + d * GEMM_WBYTES, lut_base, r, lane);
+            }
+            fence_proxy_async();                     // generic-proxy stores -> visible to the tensor core's async-proxy reads
+            __syncwarp();                            // the other lanes' (fenced) stores happen before lane 0's release
+            if (lane == 0) mbar_arrive(dfull_bar + d * 8);
+            rp.advance<NSTAGE>(1);
+            pos.next(p);
+        }
+    } else {
+        // ===================== consumer warpgroup: MMA + epilogue =====================
+        pdl_wait();
+        constexpr uint32_t a_lbo = 16 * MT * 16;
+        RingPos rp{0, 0u};
+        int it = 0;
+        SegWalk w;
+        w.init(p, b0, b1);
+        while (!w.done()) {
+            const int nblk = w.nblk();
+            float acc[2][8 * MT];
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int i = 0; i < 8 * MT; ++i) acc[h][i] = 0.f;
+            int prev_stage = -1, prev_d = -1;
+            for (int i = 0; i < nblk; ++i, ++it) {
+                const int d = it % NBUF;
+                mbar_wait(full_bar + rp.stage * 8, rp.phase, 12);                     // token operand landed
+                mbar_wait(dfull_bar + d * 8, (unsigned)(it / NBUF) & 1u, 15);         // weights expanded
+                const uint32_t wst = dq_base + d * GEMM_WBYTES;
+                const uint32_t ast = ring_base + rp.stage * STAGE_BYTES + RAW_W;
+                wgmma_fence_operand(acc[0]);
+                wgmma_fence_operand(acc[1]);
+                wgmma_fence();
+#pragma unroll
+                for (int k16 = 0; k16 < GEMM_BK / 16; ++k16) {
+                    const uint64_t bdesc = gmma_desc(ast + k16 * 2 * a_lbo, a_lbo, GEMM_A_SBO);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                        wgmma_f16<16 * MT>(acc[h], gmma_desc(wst + h * 8 * GEMM_W_SBO + k16 * 2 * GEMM_W_LBO, GEMM_W_LBO, GEMM_W_SBO), bdesc);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                     // the previous block's MMAs retired: its ring slot and buffer go back
+                if (prev_stage >= 0) {
+                    __syncwarp();
+                    if (lane == 0) { mbar_arrive(empty_bar + prev_stage * 8); mbar_arrive(dfree_bar + prev_d * 8); }
+                }
+                prev_stage = rp.stage;
+                prev_d = d;
+                rp.advance<NSTAGE>(1);
+            }
+            wgmma_wait<0>();
+            wgmma_fence_operand(acc[0]);
+            wgmma_fence_operand(acc[1]);
+            __syncwarp();
+            if (lane == 0) { mbar_arrive(empty_bar + prev_stage * 8); mbar_arrive(dfree_bar + prev_d * 8); }
+            float v[MT][16];
+            gemm_acc_to_rows<MT>(acc, v, s_x);
+            gemm_epilogue_tile<MT, false>(p, w, cta, G, v, *p.nrows, &s_last, reinterpret_cast<__half*>(s_x));
+            w.next();
+        }
+    }
+    __syncthreads();
+    if (tid == 0 && tr) tr[7] = globaltimer_ns();
+    if (tid == 0 && p.trace) p.trace[8 + 3 * cta + 2] = globaltimer_ns();
+}
+
 
 // ---------------------------------------------------------------------------------------
 // Quantisers (load time).  One warp per (weight row, 128-wide k block): lane l holds elements 4l .. 4l+3.

@@ -228,7 +228,7 @@ class Model:
     def __init__(self, st: np.ndarray, max_batch: int = 8, token_chunk_size: int = 128, device: int = 0,
                  precision: int = 0, rank: int = 0, world: int = 1, exact: bool = False, devices=None, lora=None,
                  quant: int = 0, quant_type: int | str = 0, adapters=None, adapter_places: int = 0,
-                 adapter_targets=(), batch_invariant: bool = False):
+                 adapter_targets=(), batch_invariant: bool = False, quant_adapters: bool = False):
         """devices: list of CUDA ordinals -> ONE engine object owning all tensor-parallel ranks (b200rwkv_create_ex);
         lora: list of (st_bytes, alpha) blended at load (reference lib.rs:466-485);
         quant / quant_type: the reload request's fields (lib.rs:211-215): the first `quant` layers in "Int8" or "NF4",
@@ -241,7 +241,9 @@ class Model:
         that hold pairs on the named kinds of matrix ("att.key", ..., "head": the keys of capi.TARGETS)
         (b200rwkv_create_adapter_places);
         batch_invariant: every token's results are the bits a decode step gives it, whatever else shares its calls
-        (b200rwkv_options.batch_invariant)."""
+        (b200rwkv_options.batch_invariant);
+        quant_adapters: adapters and adapter places may pair matrices of the quantised layers
+        (b200rwkv_options.quant_adapters)."""
         if isinstance(quant_type, str):
             kinds = {"none": capi.QUANT_NONE, "int8": capi.QUANT_INT8, "nf4": capi.QUANT_NF4, "sf4": 3, "fp8": capi.QUANT_FP8,
                      "int4": capi.QUANT_INT4}
@@ -256,7 +258,7 @@ class Model:
         L = capi.lib()
         if adapters and adapter_places:
             raise capi.B200Error(capi.ERR_INVALID, "adapters and adapter_places are two constructors: pass one")
-        if devices is not None or lora or quantised or adapters or adapter_places or batch_invariant:
+        if devices is not None or lora or quantised or adapters or adapter_places or batch_invariant or quant_adapters:
             if world != 1:
                 raise capi.B200Error(capi.ERR_INVALID, "devices / lora / quant go through b200rwkv_create_ex (in-process ranks)")
             opt = capi.Options()
@@ -274,6 +276,7 @@ class Model:
             opt.num_lora = len(lora or [])
             opt.quant_layers, opt.quant_type = (int(quant), int(quant_type)) if quantised else (0, 0)
             opt.batch_invariant = int(bool(batch_invariant))
+            opt.quant_adapters = int(bool(quant_adapters))
             if adapters:
                 imgs = [np.ascontiguousarray(img, dtype=np.uint8) for img, _ in adapters]
                 n = len(imgs)

@@ -111,6 +111,17 @@ typedef struct {
      * tokens and already decode-shaped.  struct_bytes = offsetof(b200rwkv_options, batch_invariant), the size before this
      * field, is accepted and means 0. */
     int32_t batch_invariant;
+    /* 1: adapters (b200rwkv_create_adapters, b200rwkv_create_adapter_places, b200rwkv_load_adapter) may pair matrices of the
+     * quantised layers, and a places engine's `targets` also plan the targeted kinds there.  For a token bound to adapter a,
+     * such a projection computes  act(x Wq^T + f16(alpha_a B_a) r(x A_a^T) + bias)  with Wq the format's dequantised matrix
+     * (B200RWKV_QUANT_*); the adapter term is not scaled by an FP8 row scale, and the adapter matrices are never quantised.
+     * Resident memory: the quantised W' plans hold the layer's codes a second time, plus one f16 128-wide tail block per place.
+     * 0: off (the default; such pairs are B200RWKV_ERR_UNSUPPORTED).  Any other value is B200RWKV_ERR_INVALID; 1 with
+     * num_devices > 1 is B200RWKV_ERR_UNSUPPORTED (both before any CUDA call).  With b200rwkv_create_ex, or with
+     * quant_layers 0, the flag is accepted and changes nothing.  The field fills the struct's tail padding, so sizeof is
+     * unchanged and a caller who zeroed the struct reads 0; struct_bytes = offsetof(b200rwkv_options, batch_invariant) means 0
+     * too. */
+    int32_t quant_adapters;
 } b200rwkv_options;
 #define B200RWKV_QUANT_NONE 0
 #define B200RWKV_QUANT_INT8 1         /* blocks of 128 inputs: f16 (min, max) + 8-bit codes */
@@ -119,13 +130,14 @@ typedef struct {
 #define B200RWKV_QUANT_FP8 4          /* beyond the reference's Quant enum: E4M3 codes, one f32 scale max|w| / 448 per output row
                                        * of the whole matrix; the projection multiplies the codes' exact values with the f16
                                        * operand in f32 and scales each output.  Same refusals as Int8 / NF4 (one GPU,
-                                       * precision 0, no adapters on its layers); batch-invariant engines run it. */
+                                       * precision 0, no adapters on its layers unless quant_adapters); batch-invariant
+                                       * engines run it. */
 #define B200RWKV_QUANT_INT4 6         /* beyond the reference's Quant enum: Int8's scheme at 4 bits.  Blocks of 128 inputs of one
                                        * output row keep scale = f16((max - min) / 15), min = f16(min) and 4-bit codes
                                        * q = floor(15 (w - min) / (max - min) + 0.5); the projection multiplies
                                        * fma_f16(q, scale, min) (one rounding) with the f16 operand in f32.  Same refusals as
-                                       * Int8 / NF4 (one GPU, precision 0, no adapters on its layers); batch-invariant engines
-                                       * run it. */
+                                       * Int8 / NF4 (one GPU, precision 0, no adapters on its layers unless quant_adapters);
+                                       * batch-invariant engines run it. */
 int32_t b200rwkv_create_ex(const uint8_t* st, size_t len, const b200rwkv_options* opt, b200rwkv_engine** out);
 
 /* Several LoRA adapters on one resident base model, chosen per slot at run time (the reference can only blend LoRA files at
@@ -135,7 +147,7 @@ int32_t b200rwkv_create_ex(const uint8_t* st, size_t len, const b200rwkv_options
  * att.{receptance,key,value,gate,output}, ffn.{key,value,receptance} and head; full tensors and unknown targets are
  * B200RWKV_ERR_UNSUPPORTED, a missing half or a shape that does not match the matrix B200RWKV_ERR_INVALID, a rank above 128
  * B200RWKV_ERR_UNSUPPORTED.  Also B200RWKV_ERR_UNSUPPORTED: more than one device, and a pair on a matrix of a quantised layer
- * (opt->quant_layers).  All of this is checked before any CUDA call.  Images are borrowed during the call only.  LoRA files in
+ * (opt->quant_layers) unless opt->quant_adapters.  All of this is checked before any CUDA call.  Images are borrowed during the call only.  LoRA files in
  * `opt` are blended into the base first; adapters apply on top of them.
  * Meaning: for a token whose slot is bound to adapter a, every projection W with a pair in a computes
  *   act(x W^T + u B'^T + bias),  u = x A^T (A = lora.0^T) rounded like the operand x (f16, or an f16 hi + lo pair with
@@ -160,7 +172,7 @@ int32_t b200rwkv_bind_adapter(b200rwkv_engine*, int32_t nslot, const int32_t* sl
 /* Adapters that come and go while the engine serves (the reference fixes its LoRA files at load; dropping one means a restart).
  * b200rwkv_create_adapter_places = b200rwkv_create_ex plus n (1..8) empty adapter places, ids 1..n.  A place can hold an
  * adapter file with pairs on the `targets` kinds of matrix (B200RWKV_TARGET_* bits) in every layer that is not quantised
- * (opt->quant_layers), and on the head if targeted; bits for matrices the model does not have (ATT_G, FFN_R on v7) are
+ * (opt->quant_layers; every layer with opt->quant_adapters), and on the head if targeted; bits for matrices the model does not have (ATT_G, FFN_R on v7) are
  * skipped.  Refused before any CUDA call: n outside 1..8, targets 0 or an unknown bit, a NULL out / opt or a wrong
  * struct_bytes are B200RWKV_ERR_INVALID; more than one device, or targets that name no f16 matrix of the model,
  * B200RWKV_ERR_UNSUPPORTED.
@@ -169,7 +181,7 @@ int32_t b200rwkv_bind_adapter(b200rwkv_engine*, int32_t nslot, const int32_t* sl
  * id, under the same plans.  Refused, with nothing changed and before any CUDA call: id outside 1..n, a NULL image, a missing
  * half or a shape that does not match its matrix are B200RWKV_ERR_INVALID; a place that holds an adapter B200RWKV_ERR_STATE
  * (replacing one is an unload, then a load, so a bound slot never changes adapter silently); full tensors, non-F16 pairs, a
- * rank above 128, a pair on a quantised layer and a pair on a matrix this engine holds no W' plan for are
+ * rank above 128, a pair on a quantised layer (unless quant_adapters) and a pair on a matrix this engine holds no W' plan for are
  * B200RWKV_ERR_UNSUPPORTED.  The plans: on a places engine every targeted matrix of the f16 layers; on a
  * b200rwkv_create_adapters engine the matrices its files paired at creation (its n places start full).
  * b200rwkv_unload_adapter empties place `id`: id outside 1..n is B200RWKV_ERR_INVALID; an empty place, or one a slot is bound
@@ -558,6 +570,15 @@ typedef struct {
 } b200rwkv_gemm_seg;
 int32_t b200rwkv_op_gemm(int32_t device, int32_t T, int32_t precision, int32_t quant_type, int32_t grid, int32_t launches,
                          int32_t nseg, const b200rwkv_gemm_seg* seg, int32_t* plan_out);
+
+/* Operator-level entry (parity tests): one W' launch of an adapter plan, as b200rwkv_op_gemm runs one segment (precision 0,
+ * one launch) with n (1..8) 128-wide adapter tail k blocks after the segment's own: out = act(x W^T + u e^T + bias) with
+ * e [N][128 n] f16 the tail blocks' contents (the engine's f16(alpha B) columns) and u [T][128 n] f16 the operand's tail
+ * (what the adapter shrink writes).  quant_type B200RWKV_QUANT_*: NONE is the f16 W' plan; INT8 / NF4 / FP8 / INT4 quantise W
+ * as b200rwkv_op_gemm does and keep the tail blocks f16 (FP8's row scales apply to x W^T only).  The tail blocks are built by
+ * the engine's own W' planner. */
+int32_t b200rwkv_op_gemm_tail(int32_t device, int32_t T, int32_t quant_type, int32_t grid, int32_t n, const b200rwkv_gemm_seg* seg,
+                              const uint16_t* tail_e, const uint16_t* tail_u, int32_t* plan_out);
 
 /* Operator-level entry (parity tests): the kept-row gather that ends a step -- the step's metadata and the launch rank 0 of a
  * `world`-rank engine makes after it -- on caller-supplied vocabulary shards and kept rows, no model.  Entries as in
