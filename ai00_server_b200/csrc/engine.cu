@@ -4415,20 +4415,34 @@ int32_t b200rwkv_debug_read(b200rwkv_engine* e, const char* name, float* out, si
         as.push_back({"a_out", &e->a_out, e->Cl, 0});
         as.push_back({"a_kk", &e->a_kk, e->Fl, 0});
         as.push_back({"a_head", &e->a_head, e->C, 0});
-        // "<buffer>_lo": the lo halves of a split operand (token rows 16..31), after a step that ran split operands
-        const bool lo = n.size() > 3 && n.compare(n.size() - 3, 3, "_lo") == 0;
-        const std::string base = lo ? n.substr(0, n.size() - 3) : n;
+        // "<buffer>_lo": the lo halves of a split operand (token rows 16..31), after a step that ran split operands;
+        // "<buffer>_tail" (and "_tail_lo"): the n_adapters 128-wide adapter tail blocks of a projection operand, which start
+        // at its own columns rounded up to whole k blocks
+        auto strip = [](std::string& s, const char* suf) {
+            const size_t k = strlen(suf);
+            const bool has = s.size() > k && s.compare(s.size() - k, k, suf) == 0;
+            if (has) s.resize(s.size() - k);
+            return has;
+        };
+        std::string base = n;
+        const bool lo = strip(base, "_lo");
+        const bool tail = strip(base, "_tail");
         for (const A& a : as)
             if (base == a.n && a.b->p) {
+                REQUIRE(!tail || (e->n_adapters && base.rfind("a_lora", 0) != 0), B200RWKV_ERR_STATE,
+                        "debug_read: " + base + " has no adapter tail blocks (an engine with adapters, a projection operand)");
                 REQUIRE(!lo || e->last_sh.split, B200RWKV_ERR_STATE, "debug_read: the last step did not run split operands, " + n + " has no lo half");
-                REQUIRE((size_t)T * a.cols <= cap, B200RWKV_ERR_INVALID, "debug buffer too small");
+                const int k0 = tail ? cdiv(a.cols, GEMM_BK) * GEMM_BK : 0, cols = tail ? e->n_adapters * GEMM_BK : a.cols;
+                REQUIRE((size_t)T * cols <= cap, B200RWKV_ERR_INVALID, "debug buffer too small");
                 // the head's operand holds the step's output rows (th_rows), every other operand its token rows (th)
                 const int tr = (a.b == &e->a_head) ? e->last_sh.th_rows : e->last_sh.th, r0 = lo ? 16 : 0;
-                std::vector<uint16_t> h(a.b->halves_per_matrix), rows((size_t)(r0 + T) * a.cols);
+                std::vector<uint16_t> h(a.b->halves_per_matrix);
                 CK(cudaMemcpy(h.data(), a.b->p + (size_t)a.mat * a.b->halves_per_matrix, h.size() * 2, cudaMemcpyDeviceToHost));
-                a16_unpack(h, a.cols, a.cols, tr, r0 + T, 0, a.cols, rows.data());
-                for (size_t i = 0; i < (size_t)T * a.cols; ++i) out[i] = __half2float(__ushort_as_half(rows[(size_t)r0 * a.cols + i]));
-                return a.cols;
+                // a16_index does not depend on the operand's width: column k0 + k is the unpack's column k shifted
+                for (int m = 0; m < T; ++m)
+                    for (int k = 0; k < cols; ++k)
+                        out[(size_t)m * cols + k] = __half2float(__ushort_as_half(h[a16_index(r0 + m, k0 + k, tr)]));
+                return cols;
             }
         throw Error(B200RWKV_ERR_INVALID, "unknown debug buffer: " + n);
     });

@@ -713,7 +713,11 @@ int32_t b200rwkv_last_score_top(b200rwkv_engine*, uint32_t* ids_out, float* logp
  * rr, part_att and part_ffn (split-K slices summed in slice order), hidden.  f16 operands: a_x0..a_x5,
  * a_lora<i>_<m>, a_out, a_kk, and a_head, whose first rows are the step's output rows.  An f16 operand name with the
  * suffix "_lo" reads the lo halves of split (hi + lo) operands; the plain name reads the hi halves.  "_lo" is refused
- * with B200RWKV_ERR_STATE when the most recent step did not run split operands. */
+ * with B200RWKV_ERR_STATE when the most recent step did not run split operands.  On an engine with unblended adapters,
+ * the suffix "_tail" on a_x0..a_x5, a_out, a_kk or a_head reads the operand's n_adapters x 128 adapter tail columns (the
+ * shrink's u = x A^T of each row in its adapter's block, zeros elsewhere), which start at the operand's own columns
+ * rounded up to whole 128-column blocks; "_tail_lo" reads their lo halves under the "_lo" rule.  "_tail" is refused with
+ * B200RWKV_ERR_STATE on an engine without adapters. */
 int32_t b200rwkv_debug_read(b200rwkv_engine*, const char* name, float* out, size_t cap);
 
 /* Profiling aid: raw stamp rows of the most recent b200rwkv_profile_insitu replay, one row of 512 uint64 per launch

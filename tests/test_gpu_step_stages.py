@@ -52,6 +52,8 @@ from ai00_server_b200 import capi, runtime, synth
 from oracle import quant_numpy as Q
 from oracle import rwkv_numpy as O
 
+import fp8_oracle as F8
+import int4_oracle as I4
 import test_gpu_gemm as G
 import test_gpu_ln as LN
 import test_gpu_wkv as W
@@ -204,16 +206,22 @@ def mix_ref(xx, sx, mu, dsx=0.0):
     return y, np.abs(mu) * dsx + 2 * EPS * (np.abs(sx * mu) + np.abs(y))
 
 
+def operand_rounding(y, dy, split):
+    """A value y (error bound dy) the kernel stored as an operand that could not be read back: the value as the kernel must
+    have rounded it, and the error e_k it may still carry (with split operands the pair's error, else one f16 ulp only where
+    y lies within dy of an f16 rounding boundary)."""
+    if split:
+        return y, dy + 2.0 ** -22 * np.abs(y) + 2.0 ** -25
+    c = lambda v: np.clip(v, -LN.F16_MAX, LN.F16_MAX).astype(np.float16).astype(np.float64)
+    amb = c(y - dy) != c(y + dy)                     # within its bound of an f16 rounding boundary
+    return c(y), np.where(amb, LN.f16_ulp(y), 0.0)
+
+
 def recomputed_operand(y, dy, split, Wm):
     """An operand that was overwritten before it could be read back: its value as the kernel must have rounded it, and
     the projection error that the rounding ambiguity can add, sum_k |W_nk| e_k."""
-    if split:
-        e = dy + 2.0 ** -22 * np.abs(y) + 2.0 ** -25
-        return y, e @ np.abs(Wm.astype(np.float64)).T
-    c = lambda v: np.clip(v, -LN.F16_MAX, LN.F16_MAX).astype(np.float16).astype(np.float64)
-    amb = c(y - dy) != c(y + dy)                     # within its bound of an f16 rounding boundary
-    e = np.where(amb, LN.f16_ulp(y), 0.0)
-    return c(y), (e @ np.abs(Wm.astype(np.float64)).T if amb.any() else 0.0)
+    x, e = operand_rounding(y, dy, split)
+    return x, (e @ np.abs(Wm.astype(np.float64)).T if e.any() else 0.0)
 
 
 class Stages:
@@ -230,6 +238,9 @@ class Stages:
             self.slot_of += [s] * n
         self.first, self.last, self.slot_of = np.array(self.first), np.array(self.last), np.array(self.slot_of)
         self.T = len(self.slot_of)
+        self.out_rows = None           # the tokens with logits rows, once ln_out is checked
+        self.recomputed = {}           # projection weight -> (value, bound) of its recomputed operand (recomputed_op)
+        self.tail_sum = {}             # projection weight -> sum |x_k W_nk| over columns beyond its own (Stages.residual)
 
     def mat(self, name):
         return self.w[name]
@@ -243,7 +254,14 @@ class Stages:
         before = self.st0[self.slot_of, self.l, state_row].astype(np.float64)
         return np.where(self.first[:, None], before, np.roll(own, 1, 0))
 
-    def proj(self, stage, x, wname, act, got, bias=None, a16=None, dz=0.0, wm=None):
+    def recomputed_op(self, y, dy, wname):
+        """recomputed_operand for the projection `wname`, whose operand the channel mix overwrote."""
+        self.recomputed[wname] = (y, dy)
+        return recomputed_operand(y, dy, self.split, self.mat(wname))
+
+    def proj(self, stage, x, wname, act, got, bias=None, a16=None, dz=0.0, wm=None, operand=None):
+        """One projection against float64; `operand`: the A16 buffer the engine multiplies (a projection an adapter can
+        extend, test_gpu_step_stages_ext.py)."""
         Wm = self.mat(wname) if wm is None else wm
         y, b = G.project64(x, Wm, bias, act, G.EPS, dz)
         if a16 is None:
@@ -286,7 +304,7 @@ class Stages:
         def static_mix(stage, i, mu, overwritten=False, wname=None):
             y, dy = mix_ref(xx1, sx1, mu, dsx1)
             if overwritten:
-                ops[i] = recomputed_operand(y, dy, split, self.mat(wname))
+                ops[i] = self.recomputed_op(y, dy, wname)
             else:
                 bits, val = self.op(f"a_x{i}", C)
                 g, want, bound = LN.f16_got(bits, y, dy, split, T)
@@ -313,7 +331,7 @@ class Stages:
                 y = xx1 + sx1 * (mu + yl)
                 dy = np.abs(sx1) * dyl + 2.0 ** -22 * (np.abs(xx1) + np.abs(sx1) * (np.abs(mu) + np.abs(yl)))
                 if j <= 1:             # the decay-LoRA input and the k mix: overwritten by the channel-mix LN
-                    ops[j] = recomputed_operand(y, dy, split, self.mat(a + ("time_decay_w1" if j == 0 else "key.weight")))
+                    ops[j] = self.recomputed_op(y, dy, a + ("time_decay_w1" if j == 0 else "key.weight"))
                 else:
                     bits, val = self.op(f"a_x{j}", C)
                     g, want, bound = LN.f16_got(bits, y, dy, split, T)
@@ -333,7 +351,8 @@ class Stages:
         for n, i in rk.items():
             rows[n] = rd.f32(n)
             x, dz = ops[i]
-            self.proj(f"att {wn[n]} (a_x{i})", x, a + wn[n] + ".weight", capi.ACT_SILU if n == "g" else capi.ACT_NONE, rows[n], dz=dz)
+            self.proj(f"att {wn[n]} (a_x{i})", x, a + wn[n] + ".weight", capi.ACT_SILU if n == "g" else capi.ACT_NONE, rows[n], dz=dz,
+                      operand=f"a_x{i}")
         Dd = s.Dd
         wk = W.Case(version=ver, entries=tuple((sl, n) for sl, n, _, _ in self.entries), H=H, precision=self.cfg.precision)
         ch = dict(lnx_w=np.float32(self.vec(a + "ln_x.weight")), lnx_b=np.float32(self.vec(a + "ln_x.bias")))
@@ -393,10 +412,9 @@ class Stages:
             ck("WKV state", self.wkv_state(self.st1, sl), M, E + EPS * np.abs(M) + 1e-30)
         # ---- output projection, LN2 ----
         part_att = rd.f32("part_att")
-        Wo = self.mat(a + "output.weight")
-        self.proj("output projection (slices summed)", a_out, a + "output.weight", capi.ACT_NONE, part_att)
+        self.proj("output projection (slices summed)", a_out, a + "output.weight", capi.ACT_NONE, part_att, operand="a_out")
         x_b = rd.f32("x_b")
-        want, bound = self.residual(x_a, part_att, None, a_out, Wo, G.pick_split(C, -(-C // 128)))
+        want, bound = self.residual(x_a, part_att, None, a_out, a + "output.weight", G.pick_split(C, -(-C // 128)))
         ck("LN2 x_b = x_a + att", x_b, want, bound)
         xx2 = rd.f32("xx2")
         y, dy = LN.ln_ref(x_b, self.vec(b + "ln2.weight"), self.vec(b + "ln2.bias"), C, cluster)
@@ -419,16 +437,15 @@ class Stages:
         # ---- channel mix ----
         F = s.F
         bits, kk = self.op("a_kk", F)
-        self.proj("ffn key (relu^2)", fops[0], f + "key.weight", capi.ACT_RELU2, None, a16=bits)
+        self.proj("ffn key (relu^2)", fops[0], f + "key.weight", capi.ACT_RELU2, None, a16=bits, operand="a_x0")
         rr = None
         if ver != 7:
             rr = rd.f32("rr")
-            self.proj("ffn receptance (sigmoid)", fops[1], f + "receptance.weight", capi.ACT_SIGMOID, rr)
+            self.proj("ffn receptance (sigmoid)", fops[1], f + "receptance.weight", capi.ACT_SIGMOID, rr, operand="a_x1")
         part_ffn = rd.f32("part_ffn")
-        Wv = self.mat(f + "value.weight")
-        self.proj("ffn value (slices summed)", kk, f + "value.weight", capi.ACT_NONE, part_ffn)
+        self.proj("ffn value (slices summed)", kk, f + "value.weight", capi.ACT_NONE, part_ffn, operand="a_kk")
         hidden = rd.f32("hidden")
-        hid_want, hid_bound = self.residual(x_b, part_ffn, rr, kk, Wv, G.pick_split(F, -(-C // 128)))
+        hid_want, hid_bound = self.residual(x_b, part_ffn, rr, kk, f + "value.weight", G.pick_split(F, -(-C // 128)))
         ck("ln_out hidden = x_b + ffn", hidden, hid_want, hid_bound)
         # ---- ln_out, head, logits ----
         outrow = []
@@ -436,13 +453,13 @@ class Stages:
             outrow += [o == FULL or (o == LAST and j == n - 1) for j in range(n)]
         toks = np.nonzero(outrow)[0]
         R = len(toks)
+        self.out_rows = toks
         if R:
             y, dy = LN.ln_ref(hidden[toks], self.vec("ln_out.weight"), self.vec("ln_out.bias"), C, False)
             bits, head_in = rd.a16("a_head", C, R)
             g, want, bound = LN.f16_got(bits, y, dy, split, R)
             ck("ln_out a_head", g, want, bound)
-            yl, bl = G.project64(head_in, self.mat("head.weight"), None, capi.ACT_NONE, G.EPS)
-            ck("head logits", self.logits, yl, bl)
+            self.proj("head logits", head_in, "head.weight", capi.ACT_NONE, self.logits, operand="a_head")
         # ---- commits ----
         last = np.nonzero(self.last)[0]
         slots = self.slot_of[last]
@@ -450,13 +467,14 @@ class Stages:
         ck.exact("commit ffn shift = xx2 of the last token", self.st1[slots, l, N + 1], xx2[last])
         return x_a, hidden, 2 * hid_bound
 
-    def residual(self, x, part, gate, op, Wm, nsplit):
+    def residual(self, x, part, gate, op, wname, nsplit):
         """x + gate (.) part, with part the split-K slices summed (by the kernel, and by debug_read in slice order): the
-        bound of test_gpu_ln.residual_ref with sum |slice| <= sum_k |op_k W_nk|, plus the f32 sum of the slices."""
+        bound of test_gpu_ln.residual_ref with sum |slice| <= sum_k |op_k W_nk| (over the operand's own columns and any
+        tail columns the projection multiplied), plus the f32 sum of the slices."""
         c = types.SimpleNamespace(n_parts=1, n_gate=1 if gate is not None else 0)
         xs = dict(x_in=[x], parts=[part[None]], gates=[gate[None]] if gate is not None else None)
         y, dy = LN.residual_ref(c, xs, 0)
-        sa = np.abs(op) @ np.abs(Wm.astype(np.float64)).T
+        sa = np.abs(op) @ np.abs(self.mat(wname).astype(np.float64)).T + self.tail_sum.get(wname, 0.0)
         g = np.abs(gate) if gate is not None else 1.0
         return y, dy + 2 * EPS * (nsplit + 2) * g * sa + 1e-300
 
@@ -467,47 +485,72 @@ class Stages:
 
 
 def weights_of(st, cfg: Config):
+    """The model's weights as the engine multiplies them: the first QUANT_LAYERS layers' projection matrices dequantised by
+    the format's engine contract (FP8: f32(s_n value(q)); Int4: fma_f16(q, scale, min))."""
     w = dict(O.parse_st(st))
     if cfg.quant:
-        qt = Q.QUANT_INT8 if cfg.quant == "Int8" else Q.QUANT_NF4
-        w = Q.quantize_model(w, QUANT_LAYERS, qt)
+        qt = {"Int8": Q.QUANT_INT8, "NF4": Q.QUANT_NF4, "FP8": F8.QUANT_FP8, "Int4": I4.QUANT_INT4}[cfg.quant]
+        w = (I4 if qt == I4.QUANT_INT4 else F8).quantize_model(w, QUANT_LAYERS, qt)
     return {k: (v if k == "emb.weight" else np.asarray(v, np.float32)) for k, v in w.items()}
 
 
+class Runner:
+    """The prefix images of one config and the plan's calls on each, every call but the warm-up checked stage by stage.
+    test_gpu_step_stages_ext.py extends the engine (`model_kw`), binds slots before each call (`before`) and checks with
+    its own `stages`."""
+    stages = Stages
+
+    def __init__(self, name, cfg: Config):
+        self.name, self.cfg = name, cfg
+
+    def plan(self):
+        return step_plan(self.cfg)
+
+    def model_kw(self, shp):
+        return dict(quant=QUANT_LAYERS, quant_type=self.cfg.quant) if self.cfg.quant else {}
+
+    def before(self, m, tag, sg=None):
+        """Before the call `tag` (sg None), and before its checks (sg: the call's Stages)."""
+
+    def run(self):
+        cfg = self.cfg
+        s = cfg.shape
+        plan = self.plan()
+        prev = {}                      # step tag -> (hidden, bound) of the previous prefix image
+        v0 = {}                        # step tag -> layer 0's v rows (v7)
+        for l in range(s.L):
+            shp = dataclasses.replace(s, L=l + 1)
+            st = synth.make_st(shp, 0)
+            wts = weights_of(st, cfg)
+            m = runtime.Model(st, max_batch=cfg.batch, token_chunk_size=128, exact=cfg.precision == 1, **self.model_kw(shp))
+            try:
+                cur = {}
+                for tag, entries in plan:
+                    slots = [e[0] for e in entries]
+                    self.before(m, tag)
+                    st0 = np.stack([m.state.back(b) for b in range(cfg.batch)])
+                    out = m.infer_raw(slots, [e[1] for e in entries], sum((e[3] for e in entries), []), [e[2] for e in entries])
+                    st1 = np.stack([m.state.back(b) for b in range(cfg.batch)])
+                    T = sum(e[1] for e in entries)
+                    if tag == "warmup":
+                        continue
+                    ck = Checker(f"{self.name} layer {l} {tag} T={T}")
+                    sg = self.stages(cfg, wts, l, entries, Reader(m, T, cfg.precision == 1, ck), ck, st0, st1)
+                    sg.logits = np.concatenate([r for r in out if len(r)]) if any(len(r) for r in out) else None
+                    sg.v_first0 = v0.get(tag)
+                    self.before(m, tag, sg)
+                    _, hidden, hb = sg.run(prev.get(tag))
+                    cur[tag] = (hidden, hb)
+                    if l == 0 and s.version == 7:
+                        v0[tag] = sg.v_first
+                    ck.done()
+                prev = cur
+            finally:
+                m.close()
+
+
 def run_config(name):
-    cfg = CONFIGS[name]
-    s = cfg.shape
-    plan = step_plan(cfg)
-    prev = {}                      # step tag -> (hidden, bound) of the previous prefix image
-    v0 = {}                        # step tag -> layer 0's v rows (v7)
-    for l in range(s.L):
-        shp = dataclasses.replace(s, L=l + 1)
-        st = synth.make_st(shp, 0)
-        wts = weights_of(st, cfg)
-        kw = dict(quant=QUANT_LAYERS, quant_type=cfg.quant) if cfg.quant else {}
-        m = runtime.Model(st, max_batch=cfg.batch, token_chunk_size=128, exact=cfg.precision == 1, **kw)
-        try:
-            cur = {}
-            for tag, entries in plan:
-                slots = [e[0] for e in entries]
-                st0 = np.stack([m.state.back(b) for b in range(cfg.batch)])
-                out = m.infer_raw(slots, [e[1] for e in entries], sum((e[3] for e in entries), []), [e[2] for e in entries])
-                st1 = np.stack([m.state.back(b) for b in range(cfg.batch)])
-                T = sum(e[1] for e in entries)
-                if tag == "warmup":
-                    continue
-                ck = Checker(f"{name} layer {l} {tag} T={T}")
-                sg = Stages(cfg, wts, l, entries, Reader(m, T, cfg.precision == 1, ck), ck, st0, st1)
-                sg.logits = np.concatenate([r for r in out if len(r)]) if any(len(r) for r in out) else None
-                sg.v_first0 = v0.get(tag)
-                _, hidden, hb = sg.run(prev.get(tag))
-                cur[tag] = (hidden, hb)
-                if l == 0 and s.version == 7:
-                    v0[tag] = sg.v_first
-                ck.done()
-            prev = cur
-        finally:
-            m.close()
+    Runner(name, CONFIGS[name]).run()
 
 
 @pytest.mark.parametrize("name", list(CONFIGS))
