@@ -55,6 +55,15 @@ TARGETS = {"att.receptance": TARGET_ATT_R, "att.key": TARGET_ATT_K, "att.value":
            "head": TARGET_HEAD}
 
 
+# b200rwkv_weight_src.dtype: tensors handed to b200rwkv_update_weights_device
+DTYPE_F16, DTYPE_BF16, DTYPE_F32 = 0, 1, 2
+
+
+class WeightSrc(C.Structure):
+    """b200rwkv_weight_src (include/b200rwkv.h): one model tensor on the engine's device, dense."""
+    _fields_ = [("name", C.c_char_p), ("dtype", C.c_int32), ("data", C.c_void_p)]
+
+
 class GemmSeg(C.Structure):
     """b200rwkv_gemm_seg (include/b200rwkv.h)."""
     _fields_ = [("N", C.c_int32), ("K", C.c_int32), ("w", C.c_void_p), ("x", C.c_void_p), ("bias", C.c_void_p),
@@ -212,6 +221,8 @@ SYMBOLS = [
     ("b200rwkv_create_adapter_places", C.c_int32, [_P, C.c_size_t, C.POINTER(Options), C.c_int32, C.c_uint32, C.POINTER(_P)]),
     ("b200rwkv_load_adapter", C.c_int32, [_P, C.c_int32, _P, C.c_size_t, C.c_float]),
     ("b200rwkv_unload_adapter", C.c_int32, [_P, C.c_int32]),
+    ("b200rwkv_update_weights", C.c_int32, [_P, _P, C.c_size_t]),
+    ("b200rwkv_update_weights_device", C.c_int32, [_P, C.c_int32, C.POINTER(WeightSrc)]),
     ("b200rwkv_create_tp", C.c_int32, [_P, C.c_size_t, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(_P)]),
     ("b200rwkv_tp_export", C.c_int32, [_P, _P]),
     ("b200rwkv_tp_connect", C.c_int32, [_P, _P]),

@@ -166,6 +166,7 @@ struct StTensor {
 class StFile {
 public:
     std::map<std::string, StTensor> tensors;
+    bool duplicate = false;     // the header names a tensor twice (`tensors` holds the first)
 
     StFile() {}           // tensors filled by the caller (b200rwkv_op_gemm_tail's tail columns)
     StFile(const uint8_t* buf, size_t len) {
@@ -231,7 +232,7 @@ public:
                 REQUIRE(ne <= ((uint64_t)1 << 44) && ne * esz == (uint64_t)t.nbytes, B200RWKV_ERR_INVALID,
                         "safetensors: byte length of " + key + " does not match dtype x shape");
                 t.name = key;
-                tensors.emplace(std::move(key), std::move(t));
+                if (!tensors.emplace(std::move(key), std::move(t)).second) duplicate = true;
             }
             ws();
             if (peek() == ',') { ++i_; continue; }
@@ -385,6 +386,12 @@ static float st_elem_f32(const StTensor& t, size_t i) {
 // `blocks.{l}.att.time_state` [H, N, N] (transposed by the converter, convert_safetensors.py:101, crates/converter/src/main.rs:20)
 // -> the host state tensor [L][N+2][C]: row 1+i, column h*N+j <- time_state[h][i][j]; shift rows zero.
 // Returns false (and leaves `out` empty) when the file carries no time_state.
+static void time_state_rows(const StTensor& ts, int l, int H, int N, int C, std::vector<float>& out) {
+    for (int h = 0; h < H; ++h)
+        for (int i = 0; i < N; ++i)
+            for (int j = 0; j < N; ++j)
+                out[((size_t)l * (N + 2) + 1 + i) * C + h * N + j] = st_elem_f32(ts, ((size_t)h * N + i) * N + j);
+}
 static bool state_from_st(const StFile& st, int L, int H, int N, int C, std::vector<float>& out) {
     if (!st.find("blocks.0.att.time_state")) return false;
     out.assign((size_t)L * (N + 2) * C, 0.f);
@@ -393,10 +400,8 @@ static bool state_from_st(const StFile& st, int L, int H, int N, int C, std::vec
         const StTensor* ts = st.find(name);
         REQUIRE(ts, B200RWKV_ERR_INVALID, "missing tensor: " + name);
         REQUIRE(ts->numel() == (int64_t)H * N * N, B200RWKV_ERR_INVALID, "time_state must be [num_head, head_size, head_size]: " + name);
-        for (int h = 0; h < H; ++h)
-            for (int i = 0; i < N; ++i)
-                for (int j = 0; j < N; ++j)
-                    out[((size_t)l * (N + 2) + 1 + i) * C + h * N + j] = st_elem_f32(*ts, ((size_t)h * N + i) * N + j);
+        (void)st_elem_f32(*ts, 0);          // the dtype: F16, F32 or BF16
+        time_state_rows(*ts, l, H, N, C, out);
     }
     return true;
 }
@@ -415,6 +420,27 @@ struct SegDesc {
     GemmSeg proto;             // A, out_mode, act, bias, out, ldo, grp, grp_stride, aux*
     int ad_tail = 0;           // unblended adapters: 128-wide tail k blocks after the segment's own (make_launch)
     SegDesc() { memset(&proto, 0, sizeof(proto)); }
+};
+
+// One weight fill of the build: the tensor it reads (the key of b200rwkv_engine::fills), what it makes of it and where that
+// goes.  The build records the fills while it plans; b200rwkv_engine::fill_weights runs them, once at creation and again
+// for every tensor a weight update lists, so an update writes exactly what creation wrote.
+enum FillKind {
+    FILL_SEG,       // a projection segment: rows [n0, n0 + N), columns [k0, k0 + K) of the [.][ld] matrix at element `off`,
+                    // repacked (qtype QT_NONE: `kb` f16 blocks per tile into rows of dst_kb blocks) or quantised
+    FILL_VEC,       // `count` elements from `off` as f32 * scale + bias
+    FILL_DECAY,     // `count` elements from `off` as the v5 decay table exp(-exp(x))
+    FILL_FOLD,      // the k-major copy of time_decay_w2 rows n0 .. n0 + 64 N - 1 ([C][K] as stored, N heads, K = Dd)
+    FILL_RAW,       // the `count` halves as stored
+    FILL_INIT,      // State::init rows of layer `layer` from a time_state tensor (F16, BF16 or F32; read on the host)
+};
+struct Fill {
+    int kind = FILL_RAW;
+    size_t off = 0, count = 0;
+    int ld = 0, n0 = 0, N = 0, k0 = 0, K = 0, tiles = 0, kb = 0, dst_kb = 0, qtype = QT_NONE, layer = 0;
+    float scale = 1.f, bias = 0.f;
+    void* dst = nullptr;
+    float* scales = nullptr;        // FP8: the segment's row scales
 };
 
 struct GemmLaunch {
@@ -724,15 +750,21 @@ struct b200rwkv_engine {
     void enqueue_shrink(const AdapterParams& p, const StepShape& sh, cudaStream_t s, Profiler* prof);
     void check_loras(const StFile& model) const;
     void blend_loras(const StTensor& t);
+    bool had_loras = false;                  // LoRA files were blended at creation (a weight update cannot redo the blend)
 
-    // temp upload buffer during build
+    // Every weight fill of the build, by the tensor it reads (FillKind), and the f16 staging buffer they read from: held
+    // during the build and during a weight update only, sized to the largest tensor of the call
+    std::map<std::string, std::vector<Fill>> fills;
     Buf<__half> d_tmp;
-    const StTensor* d_tmp_holds = nullptr;
+    // one tensor of a fill_weights call: host bytes (an image), or dense device bytes in a B200RWKV_DTYPE_*
+    struct WeightIn { std::string name; const StTensor* host; const void* dev; int dtype; int64_t numel; };
+    void fill_weights(const std::vector<WeightIn>& in);
+    void run_fill(const Fill& f, const __half* src, cudaStream_t s);
+    void put_adapter_tails(const SegDesc& d, int ke, uint8_t* dst, int dst_kb);
 
     ~b200rwkv_engine();
     void* dalloc(size_t bytes, bool zero = true);
     void build(const StFile& st);
-    const __half* upload_tmp(const StTensor& t);
     float* vec_f32(const StFile& st, const std::string& name, size_t off, size_t count, float scale = 1.f, float bias = 0.f);
     A16Buf a16_alloc(int K, int nmat = 1);
     GemmLaunch make_launch(std::vector<SegDesc>& segs, int force_grid = 0, int qtype = QT_NONE);
@@ -805,16 +837,6 @@ void* b200rwkv_engine::dalloc(size_t bytes, bool zero) {
     return allocs.back();
 }
 
-const __half* b200rwkv_engine::upload_tmp(const StTensor& t) {
-    if (d_tmp_holds != &t) {
-        REQUIRE(t.nbytes <= d_tmp.bytes, B200RWKV_ERR_INVALID, "internal: temp buffer too small");
-        CK(cudaMemcpy(d_tmp, t.data, t.nbytes, cudaMemcpyHostToDevice));
-        d_tmp_holds = &t;
-        blend_loras(t);
-    }
-    return d_tmp;
-}
-
 static bool ends_with(const std::string& s, const std::string& suf) {
     return s.size() >= suf.size() && s.compare(s.size() - suf.size(), suf.size(), suf) == 0;
 }
@@ -852,8 +874,8 @@ static const StTensor* st_find(const std::map<std::string, StTensor>& m, const s
 }
 
 // Every `<base>.lora.0/.lora.1` pair of a LoRA file must address a projection matrix this engine blends (the matrices that
-// go through upload_tmp); anything else is refused loudly rather than ignored.  `model`: the model's tensors (names and shapes
-// are what is read).
+// blend_loras changes as fill_weights reads them); anything else is refused loudly rather than ignored.  `model`: the model's
+// tensors (names and shapes are what is read).
 static void check_lora_files(const std::map<std::string, StTensor>& model, const std::vector<b200rwkv_engine::LoraSrc>& files) {
     for (const b200rwkv_engine::LoraSrc& lo : files) {
         int pairs = 0;
@@ -909,21 +931,22 @@ static void launch_lora_blend(int num_sms, __half* W, const __half* B, const __h
     lora_blend_kernel<<<num_sms * 8, 256>>>(W, B, At, out, in, r, alpha);
     CK(cudaGetLastError());
 }
-static void launch_f16_to_f32(const __half* src, float* dst, size_t count, float scale, float bias) {
-    f16_to_f32_kernel<<<cdiv((int)count, 256), 256>>>(src, dst, count, scale, bias);
+static void launch_f16_to_f32(const __half* src, float* dst, size_t count, float scale, float bias, cudaStream_t s = 0) {
+    f16_to_f32_kernel<<<cdiv((int)count, 256), 256, 0, s>>>(src, dst, count, scale, bias);
     CK(cudaGetLastError());
 }
-static void launch_decay_table(const __half* src, float* dst, int n) {
-    decay_table_kernel<<<cdiv(n, 256), 256>>>(src, dst, n);
+static void launch_decay_table(const __half* src, float* dst, int n, cudaStream_t s = 0) {
+    decay_table_kernel<<<cdiv(n, 256), 256, 0, s>>>(src, dst, n);
     CK(cudaGetLastError());
 }
-// rows [n0, n0 + N) and columns [k0, k0 + K) of src [.][ld] into ceil(N / 128) x ceil(K / 128) stage blocks at dst
+// rows [n0, n0 + N) and columns [k0, k0 + K) of src [.][ld] into ceil(N / 128) x ceil(K / 128) stage blocks at dst, dst_kb
+// blocks per tile row (0: ceil(K / 128))
 static void launch_repack(int num_sms, const __half* src, int ld, int n0, int k0, int N, int K, uint4* dst,
-                          cudaStream_t s = 0) {
+                          cudaStream_t s = 0, int dst_kb = 0) {
     const int tiles = cdiv(N, GEMM_BN), KB = cdiv(K, GEMM_BK);
     const size_t nchunk = (size_t)tiles * KB * (GEMM_WBYTES / 16);
     const int grid = (int)std::min<size_t>((nchunk + 255) / 256, (size_t)num_sms * 16);
-    repack_weight_kernel<<<grid, 256, 0, s>>>(src, ld, n0, k0, N, K, tiles, KB, dst);
+    repack_weight_kernel<<<grid, 256, 0, s>>>(src, ld, n0, k0, N, K, tiles, KB, dst_kb > 0 ? dst_kb : KB, dst);
     CK(cudaGetLastError());
 }
 
@@ -948,15 +971,15 @@ void b200rwkv_engine::blend_loras(const StTensor& t) {
     }
 }
 
+// an f32 vector, filled by fill_weights
 float* b200rwkv_engine::vec_f32(const StFile& st, const std::string& name, size_t off, size_t count, float scale, float bias) {
     const StTensor& t = st.get(name);
     REQUIRE((size_t)t.numel() >= off + count, B200RWKV_ERR_INVALID, "tensor too small: " + name);
-    float* d = (float*)dalloc(count * 4, false);
-    Buf<__half> tmp(count * 2);
-    CK(cudaMemcpy(tmp, t.data + off * 2, count * 2, cudaMemcpyHostToDevice));
-    launch_f16_to_f32(tmp, d, count, scale, bias);
-    CK(cudaDeviceSynchronize());
-    return d;
+    Fill f;
+    f.kind = FILL_VEC; f.off = off; f.count = count; f.scale = scale; f.bias = bias;
+    f.dst = dalloc(count * 4, false);
+    fills[name].push_back(f);
+    return (float*)f.dst;
 }
 
 A16Buf b200rwkv_engine::a16_alloc(int K, int nmat) {
@@ -966,6 +989,27 @@ A16Buf b200rwkv_engine::a16_alloc(int K, int nmat) {
     return b;
 }
 
+// The adapter tail blocks of a W' segment: E [N][ke] holds f16(alpha * lora.1) of every adapter file with a pair on the
+// segment's matrix in columns 128 a .. (zeros past the rank, and for an adapter without a pair here: adapter places are
+// created empty), re-tiled into rows of dst_kb blocks at dst.  The weight fills leave these blocks alone.
+void b200rwkv_engine::put_adapter_tails(const SegDesc& d, int ke, uint8_t* dst, int dst_kb) {
+    const std::string base = d.t->name.substr(0, d.t->name.size() - 7);
+    Buf<__half> E((size_t)d.N * ke * 2);
+    CK(cudaMemset(E, 0, E.bytes));
+    for (int a = 0; a < (int)adapters.size(); ++a) {
+        const StTensor* b = adapters[a].st->find(base + ".lora.1");
+        if (!b) continue;
+        const int r = (int)b->shape[1];
+        std::vector<__half> h((size_t)d.N * r);
+        memcpy(h.data(), b->data + (size_t)d.n0 * r * 2, h.size() * 2);
+        for (__half& v : h) v = __float2half_rn(adapters[a].alpha * __half2float(v));
+        CK(cudaMemcpy2D(E + (size_t)a * GEMM_BK, (size_t)ke * 2, h.data(), (size_t)r * 2, (size_t)r * 2, d.N, cudaMemcpyHostToDevice));
+    }
+    launch_repack(num_sms, E, ke, 0, 0, d.N, ke, reinterpret_cast<uint4*>(dst), 0, dst_kb);
+    CK(cudaDeviceSynchronize());
+}
+
+// The plan of one projection launch over `segs`; its weight blocks are written by the FILL_SEG fills it records.
 GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_grid, int qtype) {
     REQUIRE(!segs.empty() && (int)segs.size() <= GEMM_MAX_SEG, B200RWKV_ERR_INVALID, "internal: bad segment count");
     GemmLaunch g;
@@ -1018,81 +1062,34 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
     g.p.W = W;
     if (qtype == QT_FP8) g.p.scales = reinterpret_cast<const float*>(W + (size_t)wblk * blk_bytes);
     if (qtype != QT_NONE && tblk) g.p.tails = (const uint8_t*)dalloc((size_t)tblk * GEMM_WBYTES, false);
-    // W' = [W | a_1 B_1 | ... | a_n B_n]: columns col0 + 128 a of E [N][ld] hold f16(alpha * lora.1) of every adapter file
-    // with a pair on `t` (E starts zeroed: zeros past the rank, and for an adapter without a pair here)
-    auto put_tails = [&](__half* E, int ld, int col0, const StTensor& t, const SegDesc& d) {
-        const std::string base = t.name.substr(0, t.name.size() - 7);
-        for (int a = 0; a < (int)adapters.size(); ++a) {      // adapter places are created empty
-            const StTensor* b = adapters[a].st->find(base + ".lora.1");
-            if (!b) continue;
-            const int r = (int)b->shape[1];
-            std::vector<__half> h((size_t)d.N * r);
-            memcpy(h.data(), b->data + (size_t)d.n0 * r * 2, h.size() * 2);
-            for (__half& v : h) v = __float2half_rn(adapters[a].alpha * __half2float(v));
-            CK(cudaMemcpy2D(E + col0 + (size_t)a * GEMM_BK, (size_t)ld * 2, h.data(), (size_t)r * 2, (size_t)r * 2, d.N,
-                            cudaMemcpyHostToDevice));
-        }
-    };
     for (size_t i = 0; i < segs.size(); ++i) {
-        SegDesc& d = segs[i];
+        const SegDesc& d = segs[i];
         const GemmSeg& sg = g.p.seg[i];
         const StTensor& t = *d.t;
-        const __half* src = upload_tmp(t);
-        const int kbq = g.p.kbq[i];
-        uint8_t* const wq = W + (size_t)g.p.qblk[i] * blk_bytes;     // the segment's code blocks
-        if (qtype != QT_NONE && d.ad_tail) {
-            // the tail blocks alone, [tile][ad_tail], re-tiled as the f16 plan's
-            const int ke = d.ad_tail * GEMM_BK;
-            Buf<__half> E((size_t)d.N * ke * 2);
-            CK(cudaMemset(E, 0, E.bytes));
-            put_tails(E, ke, 0, t, d);
-            launch_repack(num_sms, E, ke, 0, 0, d.N, ke, reinterpret_cast<uint4*>(const_cast<uint8_t*>(g.p.tails) + (size_t)g.p.tblk[i] * GEMM_WBYTES));
-            CK(cudaDeviceSynchronize());
-        }
-        int ld;
+        Fill f;
+        f.kind = FILL_SEG; f.n0 = d.n0; f.N = d.N; f.k0 = d.k0; f.K = d.K; f.tiles = sg.tiles; f.kb = g.p.kbq[i]; f.qtype = qtype;
         if (d.slice >= 0) {
             REQUIRE(t.shape.size() == 3, B200RWKV_ERR_INVALID, "internal: slice of non-3D tensor");
-            ld = (int)t.shape[2];
-            src += (size_t)d.slice * t.shape[1] * t.shape[2];
+            f.ld = (int)t.shape[2];
+            f.off = (size_t)d.slice * t.shape[1] * t.shape[2];
             REQUIRE(d.slice < t.shape[0] && d.n0 + d.N <= t.shape[1] && d.k0 + d.K <= t.shape[2], B200RWKV_ERR_INVALID, "weight shape mismatch");
         } else {
             REQUIRE(t.shape.size() == 2, B200RWKV_ERR_INVALID, "internal: expected 2-D weight");
-            ld = (int)t.shape[1];
+            f.ld = (int)t.shape[1];
             REQUIRE(d.n0 + d.N <= t.shape[0] && d.k0 + d.K <= t.shape[1], B200RWKV_ERR_INVALID, "weight shape mismatch");
         }
-        if (qtype == QT_FP8) {
-            // one warp per row; the scale is the absmax of the whole source row, whichever k slice this segment holds
-            const int grid = std::min(cdiv(sg.tiles * GEMM_BN, 8), num_sms * 32);
-            float* scales = const_cast<float*>(g.p.scales) + (size_t)sg.tile_begin * GEMM_BN;
-            quantize_fp8_kernel<<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, kbq, wq, scales);
-            CK(cudaGetLastError());
-            CK(cudaDeviceSynchronize());
-            continue;
-        }
-        if (qtype != QT_NONE) {
-            const size_t nwarp = (size_t)sg.tiles * kbq * GEMM_BN;
-            const int grid = (int)std::min<size_t>((nwarp + 7) / 8, (size_t)num_sms * 32);
-            if (qtype == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, kbq, wq);
-            else if (qtype == QT_INT4) quantize_int4_kernel<<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, kbq, wq);
-            else quantize_weight_kernel<QT_NF4><<<grid, 256>>>(src, ld, d.n0, d.k0, d.N, sg.tiles, kbq, wq);
-            CK(cudaGetLastError());
-            CK(cudaDeviceSynchronize());
-            continue;
-        }
-        uint4* dst = reinterpret_cast<uint4*>(W + (size_t)sg.blk_begin * GEMM_WBYTES);
-        if (d.ad_tail) {
-            // W's columns padded to whole k blocks, then the tail blocks, re-tiled like any matrix
-            const int kbw = cdiv(d.K, GEMM_BK), ke = (kbw + d.ad_tail) * GEMM_BK;
-            Buf<__half> E((size_t)d.N * ke * 2);
-            CK(cudaMemset(E, 0, E.bytes));
-            CK(cudaMemcpy2D(E, (size_t)ke * 2, src + (size_t)d.n0 * ld + d.k0, (size_t)ld * 2, (size_t)d.K * 2, d.N,
-                            cudaMemcpyDeviceToDevice));
-            put_tails(E, ke, kbw * GEMM_BK, t, d);
-            launch_repack(num_sms, E, ke, 0, 0, d.N, ke, dst);
+        if (qtype == QT_NONE) {
+            // an f16 W' plan's rows are the segment's own k blocks, then its adapter tail blocks
+            f.dst = W + (size_t)sg.blk_begin * GEMM_WBYTES;
+            f.dst_kb = sg.KB;
+            if (d.ad_tail) put_adapter_tails(d, d.ad_tail * GEMM_BK, W + (size_t)(sg.blk_begin + f.kb) * GEMM_WBYTES, sg.KB);
         } else {
-            launch_repack(num_sms, src, ld, d.n0, d.k0, d.N, d.K, dst);
+            f.dst = W + (size_t)g.p.qblk[i] * blk_bytes;
+            if (qtype == QT_FP8) f.scales = const_cast<float*>(g.p.scales) + (size_t)sg.tile_begin * GEMM_BN;
+            // the tail blocks alone, [tile][ad_tail], re-tiled as the f16 plan's
+            if (d.ad_tail) put_adapter_tails(d, d.ad_tail * GEMM_BK, const_cast<uint8_t*>(g.p.tails) + (size_t)g.p.tblk[i] * GEMM_WBYTES, d.ad_tail);
         }
-        CK(cudaDeviceSynchronize());   // d_tmp is reused by the next upload
+        fills[t.name].push_back(f);
     }
     g.grid = std::max(1, std::min(num_sms, std::max(tile, cdiv(blk, 4))));
     g.grid = std::min(g.grid, blk);
@@ -1321,6 +1318,94 @@ static std::vector<__half> wd2_k_major(const __half* w2, int c0, int Hl, int Dd)
     return t;
 }
 
+// One fill from its tensor's f16 values at `src` (device), on the engine's stream with the build's launch shapes.
+void b200rwkv_engine::run_fill(const Fill& f, const __half* src, cudaStream_t s) {
+    switch (f.kind) {
+        case FILL_SEG: {
+            const __half* m = src + f.off;
+            uint8_t* dst = static_cast<uint8_t*>(f.dst);
+            if (f.qtype == QT_NONE) {
+                launch_repack(num_sms, m, f.ld, f.n0, f.k0, f.N, f.K, reinterpret_cast<uint4*>(dst), s, f.dst_kb);
+                return;
+            }
+            if (f.qtype == QT_FP8) {
+                // one warp per row; the scale is the absmax of the whole source row, whichever k slice this segment holds
+                const int grid = std::min(cdiv(f.tiles * GEMM_BN, 8), num_sms * 32);
+                quantize_fp8_kernel<<<grid, 256, 0, s>>>(m, f.ld, f.n0, f.k0, f.N, f.tiles, f.kb, dst, f.scales);
+            } else {
+                const size_t nwarp = (size_t)f.tiles * f.kb * GEMM_BN;
+                const int grid = (int)std::min<size_t>((nwarp + 7) / 8, (size_t)num_sms * 32);
+                if (f.qtype == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256, 0, s>>>(m, f.ld, f.n0, f.k0, f.N, f.tiles, f.kb, dst);
+                else if (f.qtype == QT_INT4) quantize_int4_kernel<<<grid, 256, 0, s>>>(m, f.ld, f.n0, f.k0, f.N, f.tiles, f.kb, dst);
+                else quantize_weight_kernel<QT_NF4><<<grid, 256, 0, s>>>(m, f.ld, f.n0, f.k0, f.N, f.tiles, f.kb, dst);
+            }
+            CK(cudaGetLastError());
+            return;
+        }
+        case FILL_VEC: launch_f16_to_f32(src + f.off, static_cast<float*>(f.dst), f.count, f.scale, f.bias, s); return;
+        case FILL_DECAY: launch_decay_table(src + f.off, static_cast<float*>(f.dst), (int)f.count, s); return;
+        case FILL_RAW: CK(cudaMemcpyAsync(f.dst, src, f.count * 2, cudaMemcpyDeviceToDevice, s)); return;
+        case FILL_FOLD: {
+            std::vector<__half> rows((size_t)C * f.K);
+            CK(cudaMemcpyAsync(rows.data(), src, rows.size() * 2, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            const std::vector<__half> t = wd2_k_major(rows.data(), f.n0, f.N, f.K);
+            CK(cudaMemcpyAsync(f.dst, t.data(), t.size() * 2, cudaMemcpyHostToDevice, s));
+            CK(cudaStreamSynchronize(s));        // `t` goes out of scope
+            return;
+        }
+        default: throw Error(B200RWKV_ERR_INVALID, "internal: fill kind");
+    }
+}
+
+// Every fill of each tensor of `in`, reading its values as F16 from d_tmp (grown to the largest tensor; the caller releases
+// it): an image's bytes are copied up (and LoRA files blended in at creation), device tensors converted with round-to-nearest
+// -even.  time_state is read on the host as F16, BF16 or F32, as creation reads it.  All on the engine's stream, complete on
+// return.  The caller has checked every name, dtype and shape.
+void b200rwkv_engine::fill_weights(const std::vector<WeightIn>& in) {
+    size_t need = 16;
+    for (const WeightIn& w : in) need = std::max(need, (size_t)w.numel * 2);
+    d_tmp.grow(need, need);
+    cudaStream_t s = stream;
+    for (const WeightIn& w : in) {
+        auto it = fills.find(w.name);
+        if (it == fills.end()) continue;           // a tensor of the model the engine does not read
+        if (it->second.front().kind == FILL_INIT) {
+            StTensor t;
+            std::vector<uint8_t> bytes;
+            if (w.host) t = *w.host;
+            else {
+                const size_t esz = w.dtype == B200RWKV_DTYPE_F32 ? 4 : 2;
+                bytes.resize((size_t)w.numel * esz);
+                CK(cudaMemcpyAsync(bytes.data(), w.dev, bytes.size(), cudaMemcpyDeviceToHost, s));
+                CK(cudaStreamSynchronize(s));
+                t.dtype = w.dtype == B200RWKV_DTYPE_F32 ? "F32" : w.dtype == B200RWKV_DTYPE_BF16 ? "BF16" : "F16";
+                t.data = bytes.data();
+                t.nbytes = bytes.size();
+            }
+            if (init_state.empty()) init_state.assign((size_t)L * (N + 2) * C, 0.f);
+            for (const Fill& f : it->second) time_state_rows(t, f.layer, H, N, C, init_state);
+            continue;
+        }
+        if (w.host) {
+            CK(cudaMemcpyAsync(d_tmp, w.host->data, w.host->nbytes, cudaMemcpyHostToDevice, s));
+            if (!loras.empty()) {
+                CK(cudaStreamSynchronize(s));
+                blend_loras(*w.host);              // synchronises the device
+            }
+        } else if (w.dtype == B200RWKV_DTYPE_F16) {
+            CK(cudaMemcpyAsync(d_tmp, w.dev, (size_t)w.numel * 2, cudaMemcpyDeviceToDevice, s));
+        } else {
+            const int grid = (int)std::min<size_t>(((size_t)w.numel + 255) / 256, (size_t)num_sms * 16);
+            if (w.dtype == B200RWKV_DTYPE_F32) to_f16_kernel<float><<<grid, 256, 0, s>>>(static_cast<const float*>(w.dev), d_tmp, w.numel);
+            else to_f16_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(static_cast<const __nv_bfloat16*>(w.dev), d_tmp, w.numel);
+            CK(cudaGetLastError());
+        }
+        for (const Fill& f : it->second) run_fill(f, d_tmp, s);     // the next tensor's copy into d_tmp waits on the stream
+    }
+    CK(cudaStreamSynchronize(s));
+}
+
 // -----------------------------------------------------------------------------------------
 // model build
 // -----------------------------------------------------------------------------------------
@@ -1357,17 +1442,21 @@ void b200rwkv_engine::build(const StFile& st) {
     for (auto& ev : meta_ev) ev = new_event(cudaEventDisableTiming);
     MetaView mv{d_meta, maxT, S};
 
-    // ---- temp upload buffer: largest tensor ----
-    size_t tmp_bytes = 0;
-    for (auto& kv : st.tensors) tmp_bytes = std::max(tmp_bytes, kv.second.nbytes);
-    d_tmp = Buf<__half>(tmp_bytes);
-
     // ---- state ----
     att_shift = (float*)dalloc((size_t)L * S * C * 4);
     ffn_shift = (float*)dalloc((size_t)L * S * C * 4);
     wkv_state = (float*)dalloc((size_t)L * S * Hl * N * N * 4);
     d_api = (float*)dalloc((size_t)L * (N + 2) * C * 4);
-    state_from_st(st, L, H, N, C, init_state);      // State::init() with a state-tuned model; empty otherwise
+    // State::init() with a state-tuned model (FILL_INIT rows); empty otherwise
+    {
+        std::vector<float> probe;
+        if (state_from_st(st, L, H, N, C, probe))
+            for (int l = 0; l < L; ++l) {
+                Fill f;
+                f.kind = FILL_INIT; f.layer = l;
+                fills["blocks." + std::to_string(l) + ".att.time_state"].push_back(f);
+            }
+    }
 
     // ---- activations ----
     const size_t TC = (size_t)maxT * C, TCl = (size_t)maxT * Cl;
@@ -1424,7 +1513,9 @@ void b200rwkv_engine::build(const StFile& st) {
     {
         const StTensor& e = st.get("emb.weight");
         emb = (__half*)dalloc(e.nbytes, false);
-        CK(cudaMemcpy(emb, e.data, e.nbytes, cudaMemcpyHostToDevice));
+        Fill f;
+        f.kind = FILL_RAW; f.count = (size_t)e.numel(); f.dst = emb;
+        fills[e.name].push_back(f);
         embed.emb = emb; embed.C = C; embed.V = V; embed.meta = mv;
         embed.ln_w = vec_f32(st, "blocks.0.ln0.weight", 0, C);
         embed.ln_b = vec_f32(st, "blocks.0.ln0.bias", 0, C);
@@ -1541,9 +1632,10 @@ void b200rwkv_engine::build(const StFile& st) {
             }
             if (pre6_fits(Dm, C)) {
                 auto upload_raw = [&](const StTensor& t) {
-                    __half* d = (__half*)dalloc(t.nbytes, false);
-                    CK(cudaMemcpy(d, t.data, t.nbytes, cudaMemcpyHostToDevice));
-                    return d;
+                    Fill f;
+                    f.kind = FILL_RAW; f.count = (size_t)t.numel(); f.dst = dalloc(t.nbytes, false);
+                    fills[t.name].push_back(f);
+                    return (__half*)f.dst;
                 };
                 Pre6Params& q = ly.pre6;
                 q.W1 = upload_raw(st.get(a + "time_mix_w1"));     // row-major copies of the ddlerp LoRA weights
@@ -1578,11 +1670,11 @@ void b200rwkv_engine::build(const StFile& st) {
             if (Dd <= 128 && Dd % 8 == 0) {
                 // k-major copy of this rank's time_decay_w2 rows, one contiguous [Dd][64] slice per head: the WKV
                 // kernels evaluate the decay LoRA stage 2 themselves (one launch / phase less per layer)
-                const StTensor& t = st.get(a + "time_decay_w2");
-                const std::vector<__half> tmp = wd2_k_major(reinterpret_cast<const __half*>(t.data), c0, Hl, Dd);
-                __half* dw = (__half*)dalloc(tmp.size() * 2, false);
-                CK(cudaMemcpy(dw, tmp.data(), tmp.size() * 2, cudaMemcpyHostToDevice));
-                wk.wd2t = dw;
+                Fill fd;
+                fd.kind = FILL_FOLD; fd.n0 = c0; fd.N = Hl; fd.K = Dd;
+                fd.dst = dalloc((size_t)Hl * Dd * 64 * 2, false);
+                fills[a + "time_decay_w2"].push_back(fd);
+                wk.wd2t = (__half*)fd.dst;
                 wk.decay_bias = time_decay;
                 wk.d1 = a_lora[1].p;
                 wk.Dd = Dd;
@@ -1610,12 +1702,10 @@ void b200rwkv_engine::build(const StFile& st) {
             {
                 const StTensor& td = st.get(a + "time_decay");
                 REQUIRE(td.numel() == C, B200RWKV_ERR_UNSUPPORTED, "v5 time_decay must be [H, N]");
-                float* d = (float*)dalloc((size_t)Cl * 4, false);
-                Buf<__half> tmp((size_t)Cl * 2);
-                CK(cudaMemcpy(tmp, td.data + (size_t)c0 * 2, (size_t)Cl * 2, cudaMemcpyHostToDevice));
-                launch_decay_table(tmp, d, Cl);
-                CK(cudaDeviceSynchronize());
-                wk.w_static = d;
+                Fill f;
+                f.kind = FILL_DECAY; f.off = (size_t)c0; f.count = (size_t)Cl; f.dst = dalloc((size_t)Cl * 4, false);
+                fills[td.name].push_back(f);
+                wk.w_static = (float*)f.dst;
             }
             wk.u = vec_f32(st, a + "time_first", c0, Cl);
         } else {
@@ -1754,7 +1844,7 @@ void b200rwkv_engine::build(const StFile& st) {
         if (ad_targets)
             REQUIRE(ad_mats.size() == ad_place_matrices(st.tensors, ad_targets, ad_quant_layers(), quant_type).size(),
                     B200RWKV_ERR_INVALID, "internal: a targeted matrix has no W' plan");
-        // load_adapter's staging, and the model's tensor shapes its file checks read
+        // load_adapter's staging
         size_t cols = 0, blocks = 0;
         for (const AdMatrix& m : ad_mats) {
             cols = std::max(cols, (size_t)m.N * GEMM_BK * 2);
@@ -1762,11 +1852,6 @@ void b200rwkv_engine::build(const StFile& st) {
         }
         ad_stage_cols = cols;
         ad_stage = (uint8_t*)dalloc(cols + blocks, false);
-        for (auto& kv : st.tensors) {
-            StTensor t = kv.second;
-            t.data = nullptr;
-            model_shapes.emplace(kv.first, std::move(t));
-        }
         place_full.assign(n_adapters, adapters.empty() ? 0 : 1);
     }
     gemm_ws = (float*)dalloc(gemm_ws_floats * 4, false);
@@ -1792,7 +1877,21 @@ void b200rwkv_engine::build(const StFile& st) {
         peer_base[0] = comm_base;
         finalize_tp();
     }
+    // the model's tensor names and shapes, for load_adapter's file checks and the weight updates' checks
+    for (auto& kv : st.tensors) {
+        StTensor t = kv.second;
+        t.data = nullptr;
+        model_shapes.emplace(kv.first, std::move(t));
+    }
+    had_loras = !loras.empty();
+    // every weight fill, after the zeroing and the adapter data above (the legacy stream) have landed
     CK(cudaDeviceSynchronize());
+    std::vector<WeightIn> in;
+    for (auto& kv : fills) {
+        const StTensor& t = st.tensors.at(kv.first);
+        in.push_back({kv.first, &t, nullptr, B200RWKV_DTYPE_F16, t.numel()});
+    }
+    fill_weights(in);
     d_tmp = Buf<__half>();
 }
 
@@ -3991,7 +4090,6 @@ static int32_t op_gemm_run(int32_t device, int32_t T, int32_t precision, int32_t
     auto mat_cols = [](const b200rwkv_gemm_seg& s) { return s.grp > 0 ? s.grp : s.ldo; };
     std::vector<StTensor> wt(nseg);
     std::vector<SegDesc> sv(nseg);
-    size_t wmax = 0;
     for (int i = 0; i < nseg; ++i) {
         const b200rwkv_gemm_seg& s = seg[i];
         wt[i].name = "op_gemm." + std::to_string(i) + ".weight";
@@ -3999,7 +4097,6 @@ static int32_t op_gemm_run(int32_t device, int32_t T, int32_t precision, int32_t
         wt[i].shape = {s.N, s.K};
         wt[i].data = reinterpret_cast<const uint8_t*>(s.w);
         wt[i].nbytes = (size_t)s.N * s.K * 2;
-        wmax = std::max(wmax, wt[i].nbytes);
         SegDesc& d = sv[i];
         d.t = &wt[i]; d.N = s.N; d.K = s.K;
         d.proto.out_mode = s.out_mode; d.proto.act = s.act; d.proto.grp = s.out_mode == OUT_F32 ? 0 : s.grp;
@@ -4024,8 +4121,13 @@ static int32_t op_gemm_run(int32_t device, int32_t T, int32_t precision, int32_t
         e->adapters.push_back({&tail_files[a], 1.f});
     }
     sv[0].ad_tail = ntail;
-    e->d_tmp = Buf<__half>(wmax);                  // make_launch uploads each matrix through the engine's staging buffer
     GemmLaunch g = e->make_launch(sv, grid, quant_type);
+    {
+        std::vector<b200rwkv_engine::WeightIn> in;      // the weight fills the plan recorded, as the build runs them
+        for (const StTensor& t : wt) in.push_back({t.name, &t, nullptr, B200RWKV_DTYPE_F16, t.numel()});
+        CK(cudaDeviceSynchronize());
+        e->fill_weights(in);
+    }
     e->gemm_ws = (float*)e->dalloc(e->gemm_ws_floats * 4, false);
     g.p.ws = e->gemm_ws;
 
@@ -4798,6 +4900,75 @@ int32_t b200rwkv_load_adapter(b200rwkv_engine* e, int32_t id, const uint8_t* ada
                 "adapter on " + base + ": this engine holds no W' plan for it (its kind was not targeted at creation)");
     }
     e->load_place(id, f, alpha);
+    API_END
+}
+
+// The refusals both weight updates share, on the host: the engine's kind, then each name against the model (known, listed
+// once, the model's shape when the caller gives one) and its dtype against what creation accepts for that tensor
+// (time_state: F16, BF16 or F32; any other tensor the build reads: F16; a tensor it does not read: anything).
+static void check_update(const b200rwkv_engine* e, const std::vector<b200rwkv_engine::WeightIn>& in) {
+    REQUIRE(e->world == 1 && !e->group, B200RWKV_ERR_UNSUPPORTED, "update_weights: tensor-parallel engines are not updated in place");
+    REQUIRE(!e->had_loras, B200RWKV_ERR_UNSUPPORTED,
+            "update_weights: this engine blended load-time LoRA files, which it no longer holds: create it again instead");
+    std::set<std::string> seen;
+    for (const b200rwkv_engine::WeightIn& w : in) {
+        const StTensor* m = st_find(e->model_shapes, w.name);
+        REQUIRE(m, B200RWKV_ERR_INVALID, "update_weights: the model has no tensor " + w.name);
+        REQUIRE(seen.insert(w.name).second, B200RWKV_ERR_INVALID, "update_weights: " + w.name + " is listed twice");
+        REQUIRE(!w.host || w.host->shape == m->shape, B200RWKV_ERR_INVALID, "update_weights: " + w.name + " differs in shape from the model's");
+        const std::string dt = w.host ? w.host->dtype
+                                      : w.dtype == B200RWKV_DTYPE_F16 ? "F16" : w.dtype == B200RWKV_DTYPE_BF16 ? "BF16" : "F32";
+        auto it = e->fills.find(w.name);
+        if (it == e->fills.end()) continue;
+        const bool init = it->second.front().kind == FILL_INIT;
+        if (w.host)
+            REQUIRE(dt == "F16" || (init && (dt == "BF16" || dt == "F32")), B200RWKV_ERR_UNSUPPORTED,
+                    "update_weights: tensor " + w.name + " is " + dt + (init ? ", expected F16 / F32 / BF16" : ", expected F16"));
+    }
+}
+
+// New weights in place (the infer task's call, like load_adapter); every refusal is decided on the host first
+int32_t b200rwkv_update_weights(b200rwkv_engine* e, const uint8_t* st, size_t len) {
+    API_BEGIN(e)
+    REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
+    REQUIRE(st, B200RWKV_ERR_INVALID, "null image");
+    StFile f(st, len);
+    REQUIRE(!f.duplicate, B200RWKV_ERR_INVALID, "update_weights: the image names a tensor twice");
+    REQUIRE(!f.tensors.empty(), B200RWKV_ERR_INVALID, "update_weights: the image holds no tensor");
+    std::vector<b200rwkv_engine::WeightIn> in;
+    for (auto& kv : f.tensors) in.push_back({kv.first, &kv.second, nullptr, B200RWKV_DTYPE_F16, kv.second.numel()});
+    std::lock_guard<std::mutex> lk(e->mu);
+    check_update(e, in);
+    CK(cudaSetDevice(e->dev));
+    struct Release { Buf<__half>& b; ~Release() { b = Buf<__half>(); } } release{e->d_tmp};
+    e->fill_weights(in);
+    API_END
+}
+
+int32_t b200rwkv_update_weights_device(b200rwkv_engine* e, int32_t n, const b200rwkv_weight_src* src) {
+    API_BEGIN(e)
+    REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
+    REQUIRE(src, B200RWKV_ERR_INVALID, "null tensor table");
+    REQUIRE(n >= 1, B200RWKV_ERR_INVALID, "update_weights_device: n must be >= 1");
+    std::vector<b200rwkv_engine::WeightIn> in;
+    for (int i = 0; i < n; ++i) {
+        REQUIRE(src[i].name && src[i].data, B200RWKV_ERR_INVALID, "update_weights_device: null name or data in entry " + std::to_string(i));
+        REQUIRE(src[i].dtype >= B200RWKV_DTYPE_F16 && src[i].dtype <= B200RWKV_DTYPE_F32, B200RWKV_ERR_INVALID,
+                "update_weights_device: dtype of " + std::string(src[i].name) + " must be B200RWKV_DTYPE_F16, _BF16 or _F32");
+        in.push_back({src[i].name, nullptr, src[i].data, src[i].dtype, 0});
+    }
+    std::lock_guard<std::mutex> lk(e->mu);
+    check_update(e, in);
+    for (b200rwkv_engine::WeightIn& w : in) w.numel = e->model_shapes.at(w.name).numel();
+    CK(cudaSetDevice(e->dev));
+    for (const b200rwkv_engine::WeightIn& w : in) {
+        cudaPointerAttributes pa;
+        CK(cudaPointerGetAttributes(&pa, w.dev));
+        REQUIRE(pa.type == cudaMemoryTypeDevice && pa.device == e->dev, B200RWKV_ERR_INVALID,
+                "update_weights_device: " + w.name + " is not memory of the engine's device");
+    }
+    struct Release { Buf<__half>& b; ~Release() { b = Buf<__half>(); } } release{e->d_tmp};
+    e->fill_weights(in);
     API_END
 }
 

@@ -565,10 +565,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, RING == 1 ? 2 : 1) gemm_kernel(c
 // One-time weight re-tiling:  W[N, K] row-major f16  ->  stage blocks in the canonical
 // K-major / no-swizzle layout:  block(tile, kb) = [k8 chunk 16][row group 16][row 8][8 halves], zero padded.
 // Supports a row-parallel / column-parallel shard: source sub-matrix rows [n0, n0+N), cols [k0, k0+K)
-// of a matrix with row stride ld.
+// of a matrix with row stride ld.  Block (tile, kb) goes to block tile * dst_kb + kb of dst (dst_kb >= KB: the first KB blocks
+// of every tile row of a wider plan, whose other blocks are left as they are).
 // ---------------------------------------------------------------------------------------
 __global__ void repack_weight_kernel(const __half* __restrict__ src, int ld, int n0, int k0, int N, int K,
-                                     int tiles, int KB, uint4* __restrict__ dst) {
+                                     int tiles, int KB, int dst_kb, uint4* __restrict__ dst) {
     // one thread per 16-byte chunk (8 halves)
     const size_t nchunk = (size_t)tiles * KB * (GEMM_WBYTES / 16);
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < nchunk; i += (size_t)gridDim.x * blockDim.x) {
@@ -591,7 +592,7 @@ __global__ void repack_weight_kernel(const __half* __restrict__ src, int ld, int
                 v = *reinterpret_cast<uint4*>(tmp);
             }
         }
-        dst[i] = v;
+        dst[((size_t)tile * dst_kb + kb) * (GEMM_WBYTES / 16) + i % (GEMM_WBYTES / 16)] = v;
     }
 }
 

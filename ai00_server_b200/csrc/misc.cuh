@@ -2,6 +2,10 @@
 #pragma once
 #include "common.cuh"
 
+#include <cuda_bf16.h>
+
+#include <type_traits>
+
 namespace b200 {
 
 // ---------------------------------------------------------------------------------------
@@ -148,6 +152,16 @@ __global__ void a16_from_f32_kernel(const float* __restrict__ src, int T, int K,
         const int t = (int)(i / K), k = (int)(i - (size_t)t * K);
         if (split) split_h(src[i], dst[a16_index(t, k, th)], dst[a16_index(t + 16, k, th)]);
         else dst[a16_index(t, k, th)] = f2h_sat(src[i]);
+    }
+}
+
+// BF16 or F32 weights handed over on the device (b200rwkv_update_weights_device) -> the F16 the build reads, rounded to nearest
+// even; BF16 widens to f32 exactly first
+template <typename T>
+__global__ void to_f16_kernel(const T* __restrict__ src, __half* __restrict__ dst, size_t n) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        if constexpr (std::is_same<T, float>::value) dst[i] = __float2half_rn(src[i]);
+        else dst[i] = __float2half_rn(__bfloat162float(src[i]));
     }
 }
 

@@ -615,6 +615,31 @@ class Model:
         """Empties adapter place `id`; no slot may be bound to it (b200rwkv_unload_adapter)."""
         capi.check(capi.lib().b200rwkv_unload_adapter(self._h, int(id)), self._h)
 
+    def update_weights(self, st) -> None:
+        """Replaces the tensors the safetensors image `st` holds (any subset of the model's) in place
+        (b200rwkv_update_weights).  Afterwards the engine computes what one created from the updated image would; slot
+        states, snapshots and kept rows still hold what the old weights computed."""
+        img = np.ascontiguousarray(st, dtype=np.uint8)
+        capi.check(capi.lib().b200rwkv_update_weights(self._h, capi.ptr(img), img.size), self._h)
+
+    def update_weights_from_tensors(self, tensors: dict) -> None:
+        """update_weights from torch tensors on the engine's device: {name: contiguous CUDA tensor} in float16, bfloat16 or
+        float32, each in the model's shape, rounded to F16 on the device (b200rwkv_update_weights_device)."""
+        import torch
+        kinds = {torch.float16: capi.DTYPE_F16, torch.bfloat16: capi.DTYPE_BF16, torch.float32: capi.DTYPE_F32}
+        if not tensors:
+            raise capi.B200Error(capi.ERR_INVALID, "update_weights_from_tensors: no tensors")
+        table = (capi.WeightSrc * len(tensors))()
+        names = []
+        for i, (name, t) in enumerate(tensors.items()):
+            if not isinstance(t, torch.Tensor) or not t.is_cuda or not t.is_contiguous() or t.dtype not in kinds:
+                raise capi.B200Error(capi.ERR_INVALID, f"update_weights_from_tensors: {name} must be a contiguous CUDA tensor "
+                                                       "in float16, bfloat16 or float32")
+            names.append(name.encode())
+            table[i].name, table[i].dtype, table[i].data = names[-1], kinds[t.dtype], t.data_ptr()
+        torch.cuda.synchronize(next(iter(tensors.values())).device)     # the producers' writes have landed
+        capi.check(capi.lib().b200rwkv_update_weights_device(self._h, len(tensors), table), self._h)
+
     def keep_hidden_pooled(self, layers, mode="last") -> None:
         """Reduce the residual stream after each listed layer to one row per entry of every following infer call
         (b200rwkv_keep_hidden_pooled): mode "last" keeps the row of the entry's last token, "mean" the f32 mean of its rows

@@ -213,6 +213,42 @@ int32_t b200rwkv_create_adapter_places(const uint8_t* st, size_t len, const b200
 int32_t b200rwkv_load_adapter(b200rwkv_engine*, int32_t id, const uint8_t* adapter_st, size_t adapter_len, float alpha);
 int32_t b200rwkv_unload_adapter(b200rwkv_engine*, int32_t id);
 
+/* New weights for a live engine, in place: a trainer's next iterate, or a same-shape fine-tune, without destroying the
+ * engine and creating it again.  Afterwards the engine computes, bit for bit, what an engine created now would compute with
+ * the same options and constructor, the same adapter files (for places: the same files loaded at the same ids), and the
+ * model image with the listed tensors replaced: logits rows, states, SCORE values and argmax ids, score_top lists, kept and
+ * pooled hidden rows, sample_topk / sample_probs results, and launch counts.
+ * b200rwkv_update_weights takes a safetensors image holding any subset of the model's tensors; the rest keep their values.
+ * b200rwkv_update_weights_device takes n tensors already on the engine's device, each dense in the model's shape: F16, BF16
+ * or F32, rounded to F16 (round to nearest even) by a conversion kernel, so the result is that of update_weights with an
+ * image of the rounded values.  time_state is read as f32 from any of the three, as creation reads it.
+ * Everything the build derives from a listed tensor is derived again by the build's own kernels: repacked f16 blocks,
+ * Int8 / NF4 / FP8 / Int4 codes and scales (an FP8 row scale over the whole row, split-K slices included), the base part of
+ * every W' plan, f32 vectors, the v5 decay table, the v6 k-major time_decay_w2 copy, the embedding, the head, and State::init
+ * (b200rwkv_state_init) from time_state.  Left alone: adapter tail blocks and A rows, adapter bindings, keep_hidden* and
+ * score_top settings, the captured step graphs (every weight buffer stays where it is), and slot states, snapshots and kept
+ * logits rows: those still hold what the OLD weights computed.  Dropping or recomputing them is the caller's decision; a
+ * rollout loop drops its cached states after every update (INTEGRATION.md §8).
+ * Refused, before any CUDA call and with nothing changed: a NULL engine, image or table, n < 1, a malformed image, a name
+ * the model does not have, a name listed twice, a shape that differs from the model's, or a device dtype other than the three
+ * are B200RWKV_ERR_INVALID; a dtype creation refuses for that tensor (an image's matrix in BF16, say), an engine created with
+ * load-time LoRA files (opt->lora_st: their images were only borrowed, so the blend cannot be redone) and a tensor-parallel
+ * engine are B200RWKV_ERR_UNSUPPORTED.  A device pointer that is not memory of the engine's device is B200RWKV_ERR_INVALID.
+ * Made by the infer task, like load_adapter.  The writes go on the engine's stream, so steps already enqueued finish with the
+ * old weights, and are complete when the call returns.  The call holds a staging buffer the size of its largest tensor (as
+ * creation does) and allocates no resident memory.  An image from b200rwkv_host_alloc (pinned) uploads faster than pageable
+ * memory (DESIGN.md §6). */
+int32_t b200rwkv_update_weights(b200rwkv_engine*, const uint8_t* st, size_t len);
+#define B200RWKV_DTYPE_F16  0
+#define B200RWKV_DTYPE_BF16 1
+#define B200RWKV_DTYPE_F32  2
+typedef struct {
+    const char* name;       /* the model's tensor name, e.g. "blocks.3.att.key.weight" */
+    int32_t dtype;          /* B200RWKV_DTYPE_* */
+    const void* data;       /* device pointer on the engine's device, dense, the model's shape */
+} b200rwkv_weight_src;
+int32_t b200rwkv_update_weights_device(b200rwkv_engine*, int32_t n, const b200rwkv_weight_src* src);
+
 /* Tensor-parallel construction, one process per GPU (head / column parallel, SURVEY.md §8e).
  * (The in-process alternative -- one handle, all ranks inside -- is b200rwkv_create_ex above.)
  * Every rank calls create_tp with the same model, then exchanges the opaque handle blobs
