@@ -223,6 +223,7 @@ SYMBOLS = [
     ("b200rwkv_unload_adapter", C.c_int32, [_P, C.c_int32]),
     ("b200rwkv_update_weights", C.c_int32, [_P, _P, C.c_size_t]),
     ("b200rwkv_update_weights_device", C.c_int32, [_P, C.c_int32, C.POINTER(WeightSrc)]),
+    ("b200rwkv_head_format", C.c_int32, [_P, C.c_int32]),
     ("b200rwkv_create_tp", C.c_int32, [_P, C.c_size_t, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(_P)]),
     ("b200rwkv_tp_export", C.c_int32, [_P, _P]),
     ("b200rwkv_tp_connect", C.c_int32, [_P, _P]),

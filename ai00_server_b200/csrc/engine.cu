@@ -588,6 +588,18 @@ struct b200rwkv_engine {
     std::vector<Layer> layers;
     LnOutParams lnout;
     GemmLaunch head;
+    // b200rwkv_head_format: the head's plan over quantised codes of head.weight (plan.qtype QT_NONE: none, the f16 head runs)
+    // and its copy for the snapshot rows (set once snap_setup has run).  The f16 head stays resident: NONE returns to it.
+    struct QHead {
+        GemmLaunch plan, snap;
+        Buf<uint8_t> codes;                       // code blocks, then (FP8) the row scales
+        Buf<unsigned> counters, snap_counters;
+    };
+    QHead qhead;
+    // the head launch of a step (ad: a slot of it is bound), and of its snapshot rows
+    const GemmLaunch& head_plan(bool ad) const { return qhead.plan.qtype != QT_NONE ? qhead.plan : ad ? ad_head : head; }
+    const GemmLaunch& snap_head_plan(bool ad) const { return qhead.plan.qtype != QT_NONE ? qhead.snap : ad ? snap_ad_head : snap_head; }
+    void set_head_format(int qtype);
 
     // state
     float *att_shift = nullptr, *ffn_shift = nullptr, *wkv_state = nullptr, *d_api = nullptr;
@@ -611,6 +623,7 @@ struct b200rwkv_engine {
         snap_bytes = snap_meta_bytes + 3 * (size_t)maxT * sizeof(void*);
     }
     void snap_setup();
+    GemmLaunch snap_rebase(const GemmLaunch& g, unsigned* counters) const;
     // one snapshot token of a step: its token row, its record, the snapshot's logits row (null: none)
     struct SnapTok { int t; float* rec; float* row; };
     int fill_snap(uint8_t* hs, const int* hm, int T, const std::vector<SnapTok>& tk) const;
@@ -1009,6 +1022,13 @@ void b200rwkv_engine::put_adapter_tails(const SegDesc& d, int ke, uint8_t* dst, 
     CK(cudaDeviceSynchronize());
 }
 
+// Algorithmic bytes of an [N][K] matrix in a quantised format: codes + block parameters (FP8: one f32 scale per row)
+static size_t quant_matrix_bytes(int qtype, size_t N, size_t K) {
+    if (qtype == QT_FP8) return N * K + N * 4;
+    if (qtype == QT_INT4) return N * K / 2 + N * (K / 128) * 4;
+    return qtype == QT_INT8 ? N * K + N * (K / 128) * 4 : N * K / 2 + N * (K / 64) * 2;
+}
+
 // The plan of one projection launch over `segs`; its weight blocks are written by the FILL_SEG fills it records.
 GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_grid, int qtype) {
     REQUIRE(!segs.empty() && (int)segs.size() <= GEMM_MAX_SEG, B200RWKV_ERR_INVALID, "internal: bad segment count");
@@ -1044,10 +1064,7 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
             // quantisation blocks are runs of 128 (Int8, Int4) / 64 (NF4) consecutive inputs of one output row of the FULL matrix
             REQUIRE(d.K % GEMM_BK == 0 && d.k0 % GEMM_BK == 0, B200RWKV_ERR_UNSUPPORTED,
                     "quantised projections need input dimensions that are multiples of 128");
-            if (qtype == QT_FP8) g.weight_bytes += (size_t)d.N * d.K + (size_t)d.N * 4;      // codes + one f32 scale per row
-            else if (qtype == QT_INT4) g.weight_bytes += (size_t)d.N * d.K / 2 + (size_t)d.N * (d.K / 128) * 4;
-            else g.weight_bytes += qtype == QT_INT8 ? (size_t)d.N * d.K + (size_t)d.N * (d.K / 128) * 4
-                                                    : (size_t)d.N * d.K / 2 + (size_t)d.N * (d.K / 64) * 2;
+            g.weight_bytes += quant_matrix_bytes(qtype, d.N, d.K);
         }
     }
     g.p.nseg = (int)segs.size();
@@ -2142,19 +2159,20 @@ void b200rwkv_engine::enqueue_step(cudaStream_t s, const StepShape& sh, Profiler
         }
         launch_ln_out(lo, sh, s, prof);
     }
+    // a quantised head (b200rwkv_head_format) has no W' plan, so its bound steps' shrink launches are empty
     if (sh.MTR > 0 && sh.ad) {
         enqueue_shrink(s_head, sh, s, prof);
-        gemm(ad_head, true);
+        gemm(head_plan(true), true);
     } else if (sh.MTR > 0) {
-        gemm(head, true);
+        gemm(head_plan(false), true);
     }
     if (sh.MTX > 0) {        // the snapshot tokens without an output row: a head launch of their own, the main one unchanged
         StepShape shx = sh;
         shx.MTR = sh.MTX;
         shx.th_rows = sh.split ? 32 : 16 * sh.MTX;
         if (sh.ad) enqueue_shrink(s_snap_head, shx, s, prof);
-        if (prof) prof->weight_bytes += head.weight_bytes;
-        launch_gemm(sh.ad ? snap_ad_head : snap_head, shx, s, prof, true);
+        if (prof) prof->weight_bytes += head_plan(false).weight_bytes;
+        launch_gemm(snap_head_plan(sh.ad), shx, s, prof, true);
     }
     if (world > 1) launch_k(tp_barrier_kernel, dim3(1), dim3(32), 0, tpbar, KC_OTHER, s, prof);
 }
@@ -2299,23 +2317,68 @@ void b200rwkv_engine::snap_setup() {
     a_snap_head = a16_alloc(K);
     snap_logits = Buf<float>((size_t)maxT * V * 4);
     const int* smeta = reinterpret_cast<const int*>(snap_dev.p);
-    auto rebase = [&](const GemmLaunch& g) {
-        GemmLaunch x = g;
-        for (int i = 0; i < x.p.nseg; ++i) {
-            x.p.seg[i].A = a_snap_head.p + (x.p.seg[i].A - a_head.p);
-            x.p.seg[i].out = snap_logits.p + ((float*)x.p.seg[i].out - d_logits);
-        }
-        x.p.nrows = smeta + 2;
-        x.p.counters = (unsigned*)dalloc((size_t)x.total_tiles * 4, true);
-        return x;
-    };
-    snap_head = rebase(head);
+    snap_head = snap_rebase(head, (unsigned*)dalloc((size_t)head.total_tiles * 4, true));
     if (n_adapters) {
-        snap_ad_head = rebase(ad_head);
+        snap_ad_head = snap_rebase(ad_head, (unsigned*)dalloc((size_t)ad_head.total_tiles * 4, true));
         s_snap_head = s_head;
         s_snap_head.meta = MetaView{smeta, maxT, S};
         for (int k = 0; k < s_snap_head.nproj; ++k) s_snap_head.p[k].op = a_snap_head.p + (s_head.p[k].op - a_head.p);
     }
+    if (qhead.plan.qtype != QT_NONE) qhead.snap = snap_rebase(qhead.plan, qhead.snap_counters);
+}
+
+// A head launch over the snapshot rows: a_snap_head into snap_logits, over the snapshot metadata's R rows, with `counters`
+// (zeroed, total_tiles of them) of its own
+GemmLaunch b200rwkv_engine::snap_rebase(const GemmLaunch& g, unsigned* counters) const {
+    GemmLaunch x = g;
+    for (int i = 0; i < x.p.nseg; ++i) {
+        x.p.seg[i].A = a_snap_head.p + (x.p.seg[i].A - a_head.p);
+        x.p.seg[i].out = snap_logits.p + ((float*)x.p.seg[i].out - d_logits);
+    }
+    x.p.nrows = reinterpret_cast<const int*>(snap_dev.p) + 2;
+    x.p.counters = counters;
+    return x;
+}
+
+// b200rwkv_head_format after its checks: the codes of head.weight in format `qt` (QT_NONE: none), quantised from the f16 head's
+// own blocks, unpacked into dense rows; the fill that derives them again on a weight update; the plans over them.  Everything
+// is allocated and written before the engine changes, so a failure leaves the previous head in place.  The captured step
+// graphs hold the old head launch and are dropped.
+void b200rwkv_engine::set_head_format(int qt) {
+    CK(cudaSetDevice(dev));
+    QHead q;
+    Fill f;
+    if (qt != QT_NONE) {
+        const int tiles = head.total_tiles, KB = head.p.seg[0].KB;       // one segment: [V][C], C a multiple of 128
+        const size_t code_bytes = (size_t)tiles * KB * q_block_bytes(qt);
+        q.codes = Buf<uint8_t>(code_bytes + (qt == QT_FP8 ? (size_t)tiles * FP8_SCALE_BYTES : 0));
+        q.counters = Buf<unsigned>((size_t)tiles * 4);
+        q.snap_counters = Buf<unsigned>((size_t)tiles * 4);
+        Buf<__half> rows((size_t)V * C * 2);
+        CK(cudaMemsetAsync(q.counters, 0, q.counters.bytes, stream));
+        CK(cudaMemsetAsync(q.snap_counters, 0, q.snap_counters.bytes, stream));
+        const size_t nchunk = (size_t)tiles * KB * (GEMM_WBYTES / 16);
+        const int grid = (int)std::min<size_t>((nchunk + 255) / 256, (size_t)num_sms * 16);
+        unpack_weight_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const uint4*>(head.p.W), V, C, tiles, KB, rows);
+        CK(cudaGetLastError());
+        f.kind = FILL_SEG; f.ld = C; f.N = V; f.K = C; f.tiles = tiles; f.kb = KB; f.qtype = qt; f.dst = q.codes.p;
+        if (qt == QT_FP8) f.scales = reinterpret_cast<float*>(q.codes.p + code_bytes);
+        run_fill(f, rows, stream);
+        CK(cudaStreamSynchronize(stream));
+        gemm_smem_limits(qt);
+        q.plan = head;
+        q.plan.qtype = qt;
+        q.plan.weight_bytes = quant_matrix_bytes(qt, V, C);
+        q.plan.p.W = q.codes;
+        q.plan.p.scales = f.scales;
+        q.plan.p.counters = q.counters;
+        if (snap_dev) q.snap = snap_rebase(q.plan, q.snap_counters);
+    }
+    std::vector<Fill>& hf = fills.at("head.weight");
+    if (qhead.plan.qtype != QT_NONE) hf.pop_back();       // the previous format's fill, pushed last
+    if (qt != QT_NONE) hf.push_back(f);
+    graphs.clear();
+    qhead = std::move(q);        // q now holds the previous codes, released on return (cudaFree waits for the device)
 }
 
 // allocate a snapshot record (+ a logits row when this rank keeps them)
@@ -4409,6 +4472,28 @@ int32_t b200rwkv_score_top(b200rwkv_engine* e, int32_t top_n) {
     API_END
 }
 
+// The head's weight format from the next infer call on (the infer task's call, like update_weights); every refusal is
+// decided on the host first
+int32_t b200rwkv_head_format(b200rwkv_engine* e, int32_t quant_type) {
+    API_BEGIN(e)
+    REQUIRE(e, B200RWKV_ERR_INVALID, "null engine");
+    REQUIRE(quant_type >= QT_NONE && quant_type <= QT_INT4, B200RWKV_ERR_INVALID,
+            "head_format: unknown quant_type " + std::to_string(quant_type));
+    REQUIRE(quant_type != 3 && quant_type != 5, B200RWKV_ERR_UNSUPPORTED,
+            "head_format: quant_type must be NONE, Int8, NF4, FP8 or Int4 (SF4 is not implemented)");
+    std::lock_guard<std::mutex> lk(e->mu);
+    if (quant_type == e->qhead.plan.qtype) return B200RWKV_OK;
+    if (quant_type != QT_NONE) {
+        REQUIRE(e->world == 1 && !e->group, B200RWKV_ERR_UNSUPPORTED, "head_format: a quantised head runs on one GPU (no tensor parallelism)");
+        REQUIRE(e->precision == 0, B200RWKV_ERR_UNSUPPORTED, "head_format: a quantised head runs with precision 0 (f16 operands)");
+        REQUIRE(e->C % GEMM_BK == 0, B200RWKV_ERR_UNSUPPORTED, "head_format: a quantised head needs num_emb to be a multiple of 128");
+        REQUIRE(e->n_adapters == 0 || e->s_head.nproj == 0, B200RWKV_ERR_UNSUPPORTED,
+                "head_format: this engine's adapters plan the head (a head pair or a B200RWKV_TARGET_HEAD place)");
+    }
+    e->set_head_format(quant_type);
+    API_END
+}
+
 // returns the number of scored tokens of the most recent infer call (negative status on error)
 int32_t b200rwkv_last_score_top(b200rwkv_engine* e, uint32_t* ids_out, float* logprobs_out, size_t cap) {
     return api_count([&]() -> int32_t {
@@ -4582,7 +4667,7 @@ int32_t b200rwkv_debug_gemm_time(b200rwkv_engine* e, int32_t which, int32_t reps
     auto pick = [&](int l) -> const GemmLaunch& {
         const Layer& ly = e->layers[l % e->L];
         const int nl = (int)ly.lora.size(), np = (int)ly.pre.size(), nf = (int)ly.ffn.size();
-        if (which == 30) return e->head;
+        if (which == 30) return e->head_plan(false);
         if (which == 10) return ly.o;
         if (which >= 20 && which < 20 + nf) return ly.ffn[which - 20];
         REQUIRE(which >= 0 && which < nl + np, B200RWKV_ERR_INVALID, "no such launch");

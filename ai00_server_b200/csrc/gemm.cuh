@@ -596,4 +596,20 @@ __global__ void repack_weight_kernel(const __half* __restrict__ src, int ld, int
     }
 }
 
+// The inverse of repack_weight_kernel for a whole matrix (n0 = k0 = 0, dst_kb = KB, K a multiple of 8): the stage blocks
+// back into dense [N][K] f16 rows, padding dropped.  The quantised head (b200rwkv_head_format) is quantised from these rows.
+__global__ void unpack_weight_kernel(const uint4* __restrict__ src, int N, int K, int tiles, int KB, __half* __restrict__ dst) {
+    const size_t nchunk = (size_t)tiles * KB * (GEMM_WBYTES / 16);
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < nchunk; i += (size_t)gridDim.x * blockDim.x) {
+        size_t r = i;
+        const int row = r % 8; r /= 8;
+        const int mi = r % 16; r /= 16;
+        const int kj = r % GEMM_K8; r /= GEMM_K8;
+        const int kb = r % KB; r /= KB;
+        const int n = (int)r * GEMM_BN + mi * 8 + row;
+        const int k = kb * GEMM_BK + kj * 8;
+        if (n < N && k < K) *reinterpret_cast<uint4*>(dst + (size_t)n * K + k) = src[i];
+    }
+}
+
 }  // namespace b200

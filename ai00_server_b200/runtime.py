@@ -70,6 +70,18 @@ def read_state(info: dict, st: np.ndarray) -> np.ndarray:
     return out
 
 
+def quant_kind(kind, what: str = "quant_type") -> int:
+    """A weight format's B200RWKV_QUANT_* value from its name (any case: None, Int8, NF4, SF4, FP8, Int4); an int is passed
+    through for the engine to check."""
+    if not isinstance(kind, str):
+        return int(kind)
+    kinds = {"none": capi.QUANT_NONE, "int8": capi.QUANT_INT8, "nf4": capi.QUANT_NF4, "sf4": 3, "fp8": capi.QUANT_FP8,
+             "int4": capi.QUANT_INT4}
+    if kind.lower() not in kinds:
+        raise capi.B200Error(capi.ERR_INVALID, f"{what} must be None, Int8, NF4, SF4, FP8 or Int4")
+    return kinds[kind.lower()]
+
+
 class TensorGpu:
     """Device-side state snapshot handle (`TensorGpu<f32, ReadWrite>` at run.rs:1104-1108)."""
 
@@ -228,7 +240,7 @@ class Model:
     def __init__(self, st: np.ndarray, max_batch: int = 8, token_chunk_size: int = 128, device: int = 0,
                  precision: int = 0, rank: int = 0, world: int = 1, exact: bool = False, devices=None, lora=None,
                  quant: int = 0, quant_type: int | str = 0, adapters=None, adapter_places: int = 0,
-                 adapter_targets=(), batch_invariant: bool = False, quant_adapters: bool = False):
+                 adapter_targets=(), batch_invariant: bool = False, quant_adapters: bool = False, quant_head=None):
         """devices: list of CUDA ordinals -> ONE engine object owning all tensor-parallel ranks (b200rwkv_create_ex);
         lora: list of (st_bytes, alpha) blended at load (reference lib.rs:466-485);
         quant / quant_type: the reload request's fields (lib.rs:211-215): the first `quant` layers in "Int8" or "NF4",
@@ -243,13 +255,11 @@ class Model:
         batch_invariant: every token's results are the bits a decode step gives it, whatever else shares its calls
         (b200rwkv_options.batch_invariant);
         quant_adapters: adapters and adapter places may pair matrices of the quantised layers
-        (b200rwkv_options.quant_adapters)."""
-        if isinstance(quant_type, str):
-            kinds = {"none": capi.QUANT_NONE, "int8": capi.QUANT_INT8, "nf4": capi.QUANT_NF4, "sf4": 3, "fp8": capi.QUANT_FP8,
-                     "int4": capi.QUANT_INT4}
-            if quant_type.lower() not in kinds:
-                raise capi.B200Error(capi.ERR_INVALID, "quant_type must be None, Int8, NF4, SF4, FP8 or Int4")
-            quant_type = kinds[quant_type.lower()]
+        (b200rwkv_options.quant_adapters);
+        quant_head: the vocabulary head's weight format, a quant_type value, set right after creation with head_format()
+        (None: the f16 head)."""
+        quant_type = quant_kind(quant_type)
+        head_kind = None if quant_head is None else quant_kind(quant_head, "quant_head")
         quantised = quant > 0 and quant_type != capi.QUANT_NONE
         if exact:
             precision = 1          # `Bundle::<f32>`: f32-exact activations (split hi + lo f16 operands)
@@ -309,6 +319,12 @@ class Model:
         self.info = info.as_dict()
         self.runtime = Runtime(self)
         self.state = State(self)
+        if head_kind is not None:
+            try:
+                self.head_format(head_kind)
+            except Exception:
+                self.close()
+                raise
 
     def close(self):
         if self._h:
@@ -621,6 +637,12 @@ class Model:
         states, snapshots and kept rows still hold what the old weights computed."""
         img = np.ascontiguousarray(st, dtype=np.uint8)
         capi.check(capi.lib().b200rwkv_update_weights(self._h, capi.ptr(img), img.size), self._h)
+
+    def head_format(self, kind) -> None:
+        """The vocabulary head's weight format from the next infer call on (b200rwkv_head_format): "None" (f16, the default),
+        "Int8", "NF4", "FP8" or "Int4", or a capi.QUANT_* value -- head.weight through the quantiser of quantised layers.
+        "None" returns to the f16 head bit for bit; slot states, snapshots and kept rows keep what the old head computed."""
+        capi.check(capi.lib().b200rwkv_head_format(self._h, quant_kind(kind, "head_format")), self._h)
 
     def update_weights_from_tensors(self, tensors: dict) -> None:
         """update_weights from torch tensors on the engine's device: {name: contiguous CUDA tensor} in float16, bfloat16 or

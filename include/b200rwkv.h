@@ -249,6 +249,31 @@ typedef struct {
 } b200rwkv_weight_src;
 int32_t b200rwkv_update_weights_device(b200rwkv_engine*, int32_t n, const b200rwkv_weight_src* src);
 
+/* The vocabulary head's weight format from the next infer call on.  quant_type: B200RWKV_QUANT_NONE (f16, the default), INT8,
+ * NF4, FP8 or INT4 -- the quantiser and block layout of quantised layers, applied to head.weight.  The head is the one matrix
+ * every decode step streams whole; once the layers are quantised it is a large share of the step's bytes (DESIGN.md §4a).
+ *   - Meaning: every head launch computes logits = x Wq^T, Wq the format's dequantised head.weight (Int8 / Int4: blocks of
+ *     128 inputs, NF4: blocks of 64, FP8: one f32 scale per vocabulary row, which multiplies x Wq^T as in the layer kernels),
+ *     x the unchanged f16 operand.  That is the step's head launch, the snapshot rows' head launch, the head launch of steps
+ *     with bound adapter slots, bench_decode, profile_step, profile_insitu and debug_gemm_time(which = 30).  SCORE,
+ *     score_top, sample_topk, sample_probs, kept rows and hidden rows read the rows the head wrote, unchanged.
+ *   - The codes are those b200rwkv_op_quantize gives for head.weight as creation saw it (LoRA files blended in), quantised on
+ *     the device from the resident f16 head.  b200rwkv_update_weights / _device with head.weight derive them again, so the
+ *     result is bit-identical to a new engine from the new image with the same head format.
+ *   - NONE returns to the f16 head bit for bit: rows, states and launch counts equal those of an engine that never called
+ *     this.  Setting the current format again does nothing.  Slot states, snapshots and kept rows are left as they are and
+ *     hold what the old head computed.  A quantised head launches exactly as many kernels as the f16 head.
+ *   - Memory: the f16 head stays resident.  The call allocates the codes (7B head, V = 65536, C = 4096: FP8 0.27 GB, Int8
+ *     0.28 GB, Int4 and NF4 0.14 GB) and releases those of the previous format; while it runs it also holds a staging
+ *     buffer the size of the f16 head.  If an allocation fails the call fails with the previous head in place.
+ *   - Made by the infer task, like update_weights.  The writes go on the engine's stream, so steps already enqueued finish
+ *     with the old head; the captured step graphs are dropped and captured again on their next use.
+ *   - Refused before any CUDA call, with nothing changed: a NULL engine or a value outside 0..6 is B200RWKV_ERR_INVALID;
+ *     3 (SF4) and 5, a tensor-parallel engine (either front end), precision 1, num_emb not a multiple of 128, and an engine
+ *     whose adapters plan the head (a b200rwkv_create_adapters file with a head pair, or places with B200RWKV_TARGET_HEAD)
+ *     are B200RWKV_ERR_UNSUPPORTED.  Batch-invariant engines keep their guarantee with a quantised head. */
+int32_t b200rwkv_head_format(b200rwkv_engine*, int32_t quant_type);
+
 /* Tensor-parallel construction, one process per GPU (head / column parallel, SURVEY.md §8e).
  * (The in-process alternative -- one handle, all ranks inside -- is b200rwkv_create_ex above.)
  * Every rank calls create_tp with the same model, then exchanges the opaque handle blobs
