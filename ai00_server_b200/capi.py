@@ -64,6 +64,21 @@ class WeightSrc(C.Structure):
     _fields_ = [("name", C.c_char_p), ("dtype", C.c_int32), ("data", C.c_void_p)]
 
 
+# b200rwkv_fill_info.kind and .plan: the weight fills b200rwkv_debug_fill reads back
+FILL_SEG, FILL_VEC, FILL_DECAY, FILL_FOLD, FILL_RAW, FILL_INIT = range(6)
+PLAN_BASE, PLAN_ADAPTER, PLAN_HEAD = range(3)
+
+
+class FillInfo(C.Structure):
+    """b200rwkv_fill_info (include/b200rwkv.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("kind", "qtype", "plan", "n0", "N", "k0", "K", "ld")] + [("off", C.c_int64)] + [
+                (n, C.c_int32) for n in ("tiles", "kb", "ad_tail")] + [
+                ("count", C.c_int64), ("scale", C.c_float), ("bias", C.c_float), ("bytes", C.c_uint64)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 class GemmSeg(C.Structure):
     """b200rwkv_gemm_seg (include/b200rwkv.h)."""
     _fields_ = [("N", C.c_int32), ("K", C.c_int32), ("w", C.c_void_p), ("x", C.c_void_p), ("bias", C.c_void_p),
@@ -270,6 +285,8 @@ SYMBOLS = [
     ("b200rwkv_score_top", C.c_int32, [_P, C.c_int32]),
     ("b200rwkv_last_score_top", C.c_int32, [_P, _P, _P, C.c_size_t]),
     ("b200rwkv_debug_read", C.c_int32, [_P, C.c_char_p, _P, C.c_size_t]),
+    ("b200rwkv_debug_fills", C.c_int32, [_P, C.c_char_p]),
+    ("b200rwkv_debug_fill", C.c_int32, [_P, C.c_char_p, C.c_int32, C.POINTER(FillInfo), _P, C.c_size_t]),
     ("b200rwkv_debug_trace", C.c_int32, [_P, _P, C.c_size_t, _P, _P]),
     ("b200rwkv_debug_gemm_time", C.c_int32, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_int64), _P]),
     ("b200rwkv_last_error", C.c_char_p, [_P]),

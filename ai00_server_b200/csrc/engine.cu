@@ -434,6 +434,9 @@ enum FillKind {
     FILL_RAW,       // the `count` halves as stored
     FILL_INIT,      // State::init rows of layer `layer` from a time_state tensor (F16, BF16 or F32; read on the host)
 };
+static_assert(FILL_SEG == B200RWKV_FILL_SEG && FILL_VEC == B200RWKV_FILL_VEC && FILL_DECAY == B200RWKV_FILL_DECAY &&
+                  FILL_FOLD == B200RWKV_FILL_FOLD && FILL_RAW == B200RWKV_FILL_RAW && FILL_INIT == B200RWKV_FILL_INIT,
+              "b200rwkv_fill_info.kind is the FillKind");
 struct Fill {
     int kind = FILL_RAW;
     size_t off = 0, count = 0;
@@ -441,6 +444,10 @@ struct Fill {
     float scale = 1.f, bias = 0.f;
     void* dst = nullptr;
     float* scales = nullptr;        // FP8: the segment's row scales
+    // what b200rwkv_debug_fill reads back beside `dst`: the plan (B200RWKV_PLAN_*) and a W' segment's adapter tail blocks,
+    // `ad_tail` per tile row at `tails`, rows tails_kb blocks apart (the fills leave them alone)
+    int plan = B200RWKV_PLAN_BASE, ad_tail = 0, tails_kb = 0;
+    const uint8_t* tails = nullptr;
 };
 
 struct GemmLaunch {
@@ -780,7 +787,7 @@ struct b200rwkv_engine {
     void build(const StFile& st);
     float* vec_f32(const StFile& st, const std::string& name, size_t off, size_t count, float scale = 1.f, float bias = 0.f);
     A16Buf a16_alloc(int K, int nmat = 1);
-    GemmLaunch make_launch(std::vector<SegDesc>& segs, int force_grid = 0, int qtype = QT_NONE);
+    GemmLaunch make_launch(std::vector<SegDesc>& segs, int force_grid = 0, int qtype = QT_NONE, int plan = B200RWKV_PLAN_BASE);
     int quant_layers = 0, quant_type = QT_NONE;     // the first `quant_layers` layers hold Int8 / NF4 / FP8 / Int4 projection matrices
     // b200rwkv_options.quant_adapters: adapters may pair matrices of the quantised layers (quantised W' plans: the base plan's
     // code blocks and f16 tail blocks, GemmParams::tails)
@@ -1030,7 +1037,7 @@ static size_t quant_matrix_bytes(int qtype, size_t N, size_t K) {
 }
 
 // The plan of one projection launch over `segs`; its weight blocks are written by the FILL_SEG fills it records.
-GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_grid, int qtype) {
+GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_grid, int qtype, int plan) {
     REQUIRE(!segs.empty() && (int)segs.size() <= GEMM_MAX_SEG, B200RWKV_ERR_INVALID, "internal: bad segment count");
     GemmLaunch g;
     memset(&g.p, 0, sizeof(g.p));
@@ -1085,6 +1092,7 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
         const StTensor& t = *d.t;
         Fill f;
         f.kind = FILL_SEG; f.n0 = d.n0; f.N = d.N; f.k0 = d.k0; f.K = d.K; f.tiles = sg.tiles; f.kb = g.p.kbq[i]; f.qtype = qtype;
+        f.plan = plan; f.ad_tail = d.ad_tail;
         if (d.slice >= 0) {
             REQUIRE(t.shape.size() == 3, B200RWKV_ERR_INVALID, "internal: slice of non-3D tensor");
             f.ld = (int)t.shape[2];
@@ -1099,11 +1107,15 @@ GemmLaunch b200rwkv_engine::make_launch(std::vector<SegDesc>& segs, int force_gr
             // an f16 W' plan's rows are the segment's own k blocks, then its adapter tail blocks
             f.dst = W + (size_t)sg.blk_begin * GEMM_WBYTES;
             f.dst_kb = sg.KB;
+            f.tails = W + (size_t)(sg.blk_begin + f.kb) * GEMM_WBYTES;
+            f.tails_kb = sg.KB;
             if (d.ad_tail) put_adapter_tails(d, d.ad_tail * GEMM_BK, W + (size_t)(sg.blk_begin + f.kb) * GEMM_WBYTES, sg.KB);
         } else {
             f.dst = W + (size_t)g.p.qblk[i] * blk_bytes;
             if (qtype == QT_FP8) f.scales = const_cast<float*>(g.p.scales) + (size_t)sg.tile_begin * GEMM_BN;
             // the tail blocks alone, [tile][ad_tail], re-tiled as the f16 plan's
+            f.tails = g.p.tails + (size_t)g.p.tblk[i] * GEMM_WBYTES;
+            f.tails_kb = d.ad_tail;
             if (d.ad_tail) put_adapter_tails(d, d.ad_tail * GEMM_BK, const_cast<uint8_t*>(g.p.tails) + (size_t)g.p.tblk[i] * GEMM_WBYTES, d.ad_tail);
         }
         fills[t.name].push_back(f);
@@ -1998,7 +2010,7 @@ GemmLaunch b200rwkv_engine::ad_launch(const GemmLaunch& base, AdapterParams& sp)
     }
     if (mats.empty()) return base;
     // quantised: the codes are quantised from the same rows as the base plan's, so they are its codes
-    GemmLaunch g = make_launch(segs, base.force_grid, base.qtype);
+    GemmLaunch g = make_launch(segs, base.force_grid, base.qtype, B200RWKV_PLAN_ADAPTER);
     for (size_t j = 0; j < mats.size(); ++j) {
         const GemmSeg& sg = g.p.seg[mat_seg[j]];
         mats[j].tiles = sg.tiles;
@@ -2362,6 +2374,7 @@ void b200rwkv_engine::set_head_format(int qt) {
         unpack_weight_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const uint4*>(head.p.W), V, C, tiles, KB, rows);
         CK(cudaGetLastError());
         f.kind = FILL_SEG; f.ld = C; f.N = V; f.K = C; f.tiles = tiles; f.kb = KB; f.qtype = qt; f.dst = q.codes.p;
+        f.plan = B200RWKV_PLAN_HEAD;
         if (qt == QT_FP8) f.scales = reinterpret_cast<float*>(q.codes.p + code_bytes);
         run_fill(f, rows, stream);
         CK(cudaStreamSynchronize(stream));
@@ -3645,9 +3658,66 @@ static int32_t rank_profile_insitu(b200rwkv_engine* e, int32_t nslot, const int3
     API_END
 }
 
+// The quantisers' code blocks on the host, untiled: blocks [tiles][KB] (q_block_bytes(qt) each) into one code per byte,
+// codes [rows][KB * 128] for rows < `rows` (<= tiles * 128: padding rows included up to there), and the block parameters:
+// Int8 / Int4 p0 = min, p1 = scale [rows][KB]; NF4 p0 = absmax [rows][2 KB].  FP8 blocks hold codes only (its row scales
+// are apart).  b200rwkv_op_quantize and b200rwkv_debug_fill both read blocks through this, so the layout oracle/quant_numpy.py,
+// tests/fp8_oracle.py and tests/int4_oracle.py are compared with is one.
+static void untile_codes(int qt, const uint8_t* h, int tiles, int KB, int rows, uint8_t* codes, uint16_t* p0, uint16_t* p1) {
+    const size_t blk = (size_t)q_block_bytes(qt), K = (size_t)KB * GEMM_BK;
+    for (int n = 0; n < rows; ++n) {
+        const int tile = n / GEMM_BN, r = n % GEMM_BN;
+        for (int kb = 0; kb < KB; ++kb) {
+            const uint8_t* b = h + ((size_t)tile * KB + kb) * blk;
+            uint8_t* c = codes + n * K + (size_t)kb * GEMM_BK;
+            if (qt == QT_FP8) {
+                for (int k = 0; k < GEMM_BK; ++k) c[k] = b[fp8_code_offset(r, k)];
+            } else if (qt == QT_INT8) {
+                for (int k = 0; k < GEMM_BK; ++k) c[k] = b[(size_t)((k >> 4) * GEMM_BN + r) * 16 + (k & 15)];
+                uint16_t pr[2];
+                memcpy(pr, b + GEMM_BN * GEMM_BK + r * 4, 4);
+                p1[(size_t)n * KB + kb] = pr[0];      // scale
+                p0[(size_t)n * KB + kb] = pr[1];      // min
+            } else if (qt == QT_INT4) {
+                for (int k = 0; k < GEMM_BK; ++k) {
+                    const int nib = int4_nibble(r, k);
+                    c[k] = (b[nib >> 1] >> (4 * (nib & 1))) & 15;
+                }
+                uint16_t pr[2];
+                memcpy(pr, b + int4_param_offset(r), 4);
+                p1[(size_t)n * KB + kb] = pr[0];      // scale
+                p0[(size_t)n * KB + kb] = pr[1];      // min
+            } else {
+                for (int k = 0; k < GEMM_BK; ++k) {
+                    const uint8_t by = b[(size_t)((k >> 5) * GEMM_BN + r) * 16 + ((k & 31) >> 1)];
+                    c[k] = (k & 1) ? (by >> 4) : (by & 15);
+                }
+                uint16_t pr[2];
+                memcpy(pr, b + GEMM_BN * GEMM_BK / 2 + r * 4, 4);
+                p0[(size_t)n * (2 * KB) + 2 * kb] = pr[0];
+                p0[(size_t)n * (2 * KB) + 2 * kb + 1] = pr[1];
+            }
+        }
+    }
+}
+
+// f16 weight blocks on the host, untiled: blocks kb0 .. kb0 + nkb - 1 of every tile row of [tiles][stride_kb] blocks
+// (repack_weight_kernel's layout: row r, column k of a block at half ((k / 8) * 128 + r) * 8 + k % 8) into
+// [tiles * 128][nkb * 128] rows
+static void untile_f16(const uint16_t* h, int tiles, int stride_kb, int kb0, int nkb, uint16_t* out) {
+    const size_t ld = (size_t)nkb * GEMM_BK, bh = GEMM_WBYTES / 2;
+    for (int tile = 0; tile < tiles; ++tile)
+        for (int kb = 0; kb < nkb; ++kb) {
+            const uint16_t* b = h + ((size_t)tile * stride_kb + kb0 + kb) * bh;
+            for (int r = 0; r < GEMM_BN; ++r)
+                for (int k = 0; k < GEMM_BK; ++k)
+                    out[((size_t)tile * GEMM_BN + r) * ld + (size_t)kb * GEMM_BK + k] = b[((k >> 3) * GEMM_BN + r) * 8 + (k & 7)];
+        }
+}
+
 // Operator-level entry for the parity tests: the load-time quantiser (qgemm.cuh, fp8gemm.cuh, int4gemm.cuh) on one matrix,
-// un-tiled on the host into plain row-major codes and per-block (per-row for FP8) parameters so that oracle/quant_numpy.py,
-// tests/fp8_oracle.py and tests/int4_oracle.py can be compared bit for bit.
+// un-tiled on the host (untile_codes) into plain row-major codes and per-block (per-row for FP8) parameters so that
+// oracle/quant_numpy.py, tests/fp8_oracle.py and tests/int4_oracle.py can be compared bit for bit.
 int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int32_t K, const uint16_t* w_f16, uint8_t* codes,
                              uint16_t* p0, uint16_t* p1) {
     API_BEGIN((b200rwkv_engine*)nullptr)
@@ -3665,57 +3735,19 @@ int32_t b200rwkv_op_quantize(int32_t device, int32_t quant_type, int32_t N, int3
     int nsm = 0;
     CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
     const int grid = (int)std::min<size_t>((nwarp + 7) / 8, (size_t)nsm * 32);
+    Buf<float> scales;
     if (quant_type == QT_FP8) {
-        Buf<float> scales((size_t)tiles * FP8_SCALE_BYTES);
+        scales = Buf<float>((size_t)tiles * FP8_SCALE_BYTES);
         quantize_fp8_kernel<<<std::min(cdiv(tiles * GEMM_BN, 8), nsm * 32), 256>>>(src, K, 0, 0, N, tiles, KB, dst, scales);
-        CK(cudaGetLastError());
-        CK(cudaDeviceSynchronize());
-        std::vector<uint8_t> h(total);
-        CK(cudaMemcpy(h.data(), dst, total, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(p0, scales, (size_t)N * 4, cudaMemcpyDeviceToHost));
-        for (int n = 0; n < N; ++n)
-            for (int k = 0; k < K; ++k)
-                codes[(size_t)n * K + k] = h[((size_t)(n / GEMM_BN) * KB + k / GEMM_BK) * blk + fp8_code_offset(n % GEMM_BN, k % GEMM_BK)];
-        return B200RWKV_OK;
-    }
-    if (quant_type == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256>>>(src, K, 0, 0, N, tiles, KB, dst);
+    } else if (quant_type == QT_INT8) quantize_weight_kernel<QT_INT8><<<grid, 256>>>(src, K, 0, 0, N, tiles, KB, dst);
     else if (quant_type == QT_INT4) quantize_int4_kernel<<<grid, 256>>>(src, K, 0, 0, N, tiles, KB, dst);
     else quantize_weight_kernel<QT_NF4><<<grid, 256>>>(src, K, 0, 0, N, tiles, KB, dst);
     CK(cudaGetLastError());
     CK(cudaDeviceSynchronize());
     std::vector<uint8_t> h(total);
     CK(cudaMemcpy(h.data(), dst, total, cudaMemcpyDeviceToHost));
-    for (int n = 0; n < N; ++n) {
-        const int tile = n / GEMM_BN, r = n % GEMM_BN;
-        for (int kb = 0; kb < KB; ++kb) {
-            const uint8_t* b = h.data() + ((size_t)tile * KB + kb) * blk;
-            if (quant_type == QT_INT8) {
-                for (int k = 0; k < GEMM_BK; ++k) codes[(size_t)n * K + kb * GEMM_BK + k] = b[(size_t)((k >> 4) * GEMM_BN + r) * 16 + (k & 15)];
-                uint16_t pr[2];
-                memcpy(pr, b + GEMM_BN * GEMM_BK + r * 4, 4);
-                p1[(size_t)n * KB + kb] = pr[0];      // scale
-                p0[(size_t)n * KB + kb] = pr[1];      // min
-            } else if (quant_type == QT_INT4) {
-                for (int k = 0; k < GEMM_BK; ++k) {
-                    const int nib = int4_nibble(r, k);
-                    codes[(size_t)n * K + kb * GEMM_BK + k] = (b[nib >> 1] >> (4 * (nib & 1))) & 15;
-                }
-                uint16_t pr[2];
-                memcpy(pr, b + int4_param_offset(r), 4);
-                p1[(size_t)n * KB + kb] = pr[0];      // scale
-                p0[(size_t)n * KB + kb] = pr[1];      // min
-            } else {
-                for (int k = 0; k < GEMM_BK; ++k) {
-                    const uint8_t by = b[(size_t)((k >> 5) * GEMM_BN + r) * 16 + ((k & 31) >> 1)];
-                    codes[(size_t)n * K + kb * GEMM_BK + k] = (k & 1) ? (by >> 4) : (by & 15);
-                }
-                uint16_t pr[2];
-                memcpy(pr, b + GEMM_BN * GEMM_BK / 2 + r * 4, 4);
-                p0[(size_t)n * (2 * KB) + 2 * kb] = pr[0];
-                p0[(size_t)n * (2 * KB) + 2 * kb + 1] = pr[1];
-            }
-        }
-    }
+    if (quant_type == QT_FP8) CK(cudaMemcpy(p0, scales, (size_t)N * 4, cudaMemcpyDeviceToHost));
+    untile_codes(quant_type, h.data(), tiles, KB, N, codes, p0, p1);
     API_END
 }
 
@@ -4633,6 +4665,82 @@ int32_t b200rwkv_debug_read(b200rwkv_engine* e, const char* name, float* out, si
             }
         throw Error(B200RWKV_ERR_INVALID, "unknown debug buffer: " + n);
     });
+}
+
+// Test aid: the weight fills of one tensor (b200rwkv_debug_fills), and one of them read back (b200rwkv_debug_fill).  Not used
+// on the product path.
+int32_t b200rwkv_debug_fills(b200rwkv_engine* e, const char* name) {
+    return api_count([&]() -> int32_t {
+        REQUIRE(e && name, B200RWKV_ERR_INVALID, "null argument");
+        std::lock_guard<std::mutex> lk(e->mu);
+        const auto it = e->fills.find(name);
+        return it == e->fills.end() ? 0 : (int32_t)it->second.size();
+    });
+}
+
+int32_t b200rwkv_debug_fill(b200rwkv_engine* e, const char* name, int32_t i, b200rwkv_fill_info* info, void* out, size_t cap) {
+    API_BEGIN(e)
+    REQUIRE(e && name && info, B200RWKV_ERR_INVALID, "null argument");
+    std::lock_guard<std::mutex> lk(e->mu);
+    const auto it = e->fills.find(name);
+    REQUIRE(it != e->fills.end(), B200RWKV_ERR_INVALID, std::string("debug_fill: the engine fills nothing from ") + name);
+    REQUIRE(i >= 0 && i < (int32_t)it->second.size(), B200RWKV_ERR_INVALID,
+            "debug_fill: " + std::string(name) + " has " + std::to_string(it->second.size()) + " fills, no fill " + std::to_string(i));
+    const Fill& f = it->second[i];
+    const size_t R = (size_t)f.tiles * GEMM_BN, Kp = (size_t)f.kb * GEMM_BK;
+    size_t bytes = 0, param_bytes = 0;
+    switch (f.kind) {
+        case FILL_SEG:
+            param_bytes = f.qtype == QT_FP8 ? R * 4 : f.qtype == QT_INT8 || f.qtype == QT_INT4 || f.qtype == QT_NF4 ? R * f.kb * 4 : 0;
+            bytes = R * Kp * (f.qtype == QT_NONE ? 2 : 1) + param_bytes + R * f.ad_tail * GEMM_BK * 2;
+            break;
+        case FILL_VEC: case FILL_DECAY: bytes = f.count * 4; break;
+        case FILL_RAW: bytes = f.count * 2; break;
+        case FILL_FOLD: bytes = (size_t)f.N * f.K * 64 * 2; break;
+        default: bytes = (size_t)(e->N + 2) * e->C * 4; break;          // FILL_INIT
+    }
+    REQUIRE(!out || cap >= bytes, B200RWKV_ERR_INVALID, "debug_fill: the buffer holds " + std::to_string(cap) + " bytes, the fill " +
+            std::to_string(bytes));
+    b200rwkv_fill_info fi;
+    memset(&fi, 0, sizeof(fi));
+    fi.kind = f.kind; fi.qtype = f.qtype; fi.plan = f.plan;
+    fi.n0 = f.kind == FILL_INIT ? f.layer : f.n0; fi.N = f.N; fi.k0 = f.k0; fi.K = f.K; fi.ld = f.ld; fi.off = (int64_t)f.off;
+    fi.tiles = f.tiles; fi.kb = f.kb; fi.ad_tail = f.ad_tail; fi.count = (int64_t)f.count; fi.scale = f.scale; fi.bias = f.bias;
+    fi.bytes = bytes;
+    *info = fi;
+    if (!out) return B200RWKV_OK;
+    uint8_t* o = static_cast<uint8_t*>(out);
+    if (f.kind == FILL_INIT) {
+        REQUIRE(!e->init_state.empty(), B200RWKV_ERR_INVALID, "internal: a time_state fill without State::init rows");
+        memcpy(o, e->init_state.data() + (size_t)f.layer * (e->N + 2) * e->C, bytes);
+        return B200RWKV_OK;
+    }
+    CK(cudaSetDevice(e->dev));
+    CK(cudaStreamSynchronize(e->stream));
+    if (f.kind != FILL_SEG) {
+        CK(cudaMemcpy(o, f.dst, bytes, cudaMemcpyDeviceToHost));
+        return B200RWKV_OK;
+    }
+    if (f.qtype == QT_NONE) {
+        std::vector<uint16_t> h((size_t)f.tiles * f.dst_kb * GEMM_WBYTES / 2);
+        CK(cudaMemcpy(h.data(), f.dst, h.size() * 2, cudaMemcpyDeviceToHost));
+        untile_f16(h.data(), f.tiles, f.dst_kb, 0, f.kb, reinterpret_cast<uint16_t*>(o));
+        o += R * Kp * 2;
+    } else {
+        std::vector<uint8_t> h((size_t)f.tiles * f.kb * q_block_bytes(f.qtype));
+        CK(cudaMemcpy(h.data(), f.dst, h.size(), cudaMemcpyDeviceToHost));
+        uint16_t* p0 = reinterpret_cast<uint16_t*>(o + R * Kp);
+        if (f.qtype == QT_FP8) CK(cudaMemcpy(p0, f.scales, R * 4, cudaMemcpyDeviceToHost));
+        untile_codes(f.qtype, h.data(), f.tiles, f.kb, (int)R, o, p0, p0 + R * f.kb);
+        o += R * Kp + param_bytes;
+    }
+    if (f.ad_tail) {
+        std::vector<uint16_t> h((size_t)f.tiles * f.ad_tail * GEMM_WBYTES / 2);
+        CK(cudaMemcpy2D(h.data(), (size_t)f.ad_tail * GEMM_WBYTES, f.tails, (size_t)f.tails_kb * GEMM_WBYTES,
+                        (size_t)f.ad_tail * GEMM_WBYTES, f.tiles, cudaMemcpyDeviceToHost));
+        untile_f16(h.data(), f.tiles, f.ad_tail, 0, f.ad_tail, reinterpret_cast<uint16_t*>(o));
+    }
+    API_END
 }
 
 // Profiling aid: the raw stamp rows of the most recent traced replay (b200rwkv_profile_insitu): one row of 512 uint64 per

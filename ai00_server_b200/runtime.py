@@ -82,6 +82,43 @@ def quant_kind(kind, what: str = "quant_type") -> int:
     return kinds[kind.lower()]
 
 
+def _fill_parts(info: dict, raw: np.ndarray, head_size: int, num_emb: int) -> dict:
+    """The parts of one b200rwkv_debug_fill read-back (Model.debug_fills)."""
+    kind = info["kind"]
+    if kind == capi.FILL_VEC or kind == capi.FILL_DECAY:
+        return {"v": raw.view(np.float32)}
+    if kind == capi.FILL_RAW:
+        return {"v": raw.view(np.uint16)}
+    if kind == capi.FILL_FOLD:
+        return {"v": raw.view(np.uint16).reshape(info["N"], info["K"], 64)}
+    if kind == capi.FILL_INIT:
+        return {"v": raw.view(np.float32).reshape(head_size + 2, num_emb)}
+    R, kb, qt = info["tiles"] * 128, info["kb"], info["qtype"]
+    Kp, o, parts = kb * 128, 0, {}
+
+    def take(name, dtype, shape):
+        nonlocal o
+        n = int(np.prod(shape)) * np.dtype(dtype).itemsize
+        parts[name] = raw[o:o + n].view(dtype).reshape(shape)
+        o += n
+
+    if qt == capi.QUANT_NONE:
+        take("w", np.uint16, (R, Kp))
+    else:
+        take("codes", np.uint8, (R, Kp))
+        if qt == capi.QUANT_FP8:
+            take("scale", np.float32, (R,))
+        elif qt == capi.QUANT_NF4:
+            take("absmax", np.float16, (R, 2 * kb))
+        else:
+            take("min", np.float16, (R, kb))
+            take("scale", np.float16, (R, kb))
+    if info["ad_tail"]:
+        take("tail", np.uint16, (R, info["ad_tail"] * 128))
+    assert o == raw.size
+    return parts
+
+
 class TensorGpu:
     """Device-side state snapshot handle (`TensorGpu<f32, ReadWrite>` at run.rs:1104-1108)."""
 
@@ -700,6 +737,22 @@ class Model:
         cols = capi.lib().b200rwkv_debug_read(self._h, name.encode(), capi.ptr(buf), buf.size)
         capi.check(cols, self._h)
         return buf[: rows * cols].reshape(rows, cols)
+
+    def debug_fills(self, name: str) -> list[tuple[dict, dict]]:
+        """Test aid: every weight fill the engine runs for tensor `name` (b200rwkv_debug_fill), read back from the device, as
+        (info, parts).  info: the b200rwkv_fill_info fields.  parts, R = tiles * 128 rows and Kp = kb * 128 columns, padding
+        included: SEG "w" f16 bits [R, Kp] (qtype NONE) or "codes" u8 [R, Kp] with Int8 / Int4 "min" and "scale" f16 [R, kb],
+        NF4 "absmax" f16 [R, 2 kb], FP8 "scale" f32 [R]; a W' segment also "tail" f16 bits [R, ad_tail * 128].  VEC / DECAY
+        "v" f32 [count], RAW "v" f16 bits [count], FOLD "v" f16 bits [N, K, 64], INIT "v" f32 [head_size + 2, num_emb]."""
+        lib, out = capi.lib(), []
+        for i in range(capi.check(lib.b200rwkv_debug_fills(self._h, name.encode()), self._h)):
+            fi = capi.FillInfo()
+            capi.check(lib.b200rwkv_debug_fill(self._h, name.encode(), i, C.byref(fi), None, 0), self._h)
+            raw = np.empty(fi.bytes, np.uint8)
+            capi.check(lib.b200rwkv_debug_fill(self._h, name.encode(), i, C.byref(fi), capi.ptr(raw), raw.size), self._h)
+            info = fi.as_dict()
+            out.append((info, _fill_parts(info, raw, self.info["head_size"], self.info["num_emb"])))
+        return out
 
     def bench_decode(self, slots, tokens: np.ndarray, warmup: int, steps: int, flush_l2: bool = False):
         a_slot = np.asarray(slots, np.int32)

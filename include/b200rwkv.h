@@ -781,6 +781,42 @@ int32_t b200rwkv_last_score_top(b200rwkv_engine*, uint32_t* ids_out, float* logp
  * B200RWKV_ERR_STATE on an engine without adapters. */
 int32_t b200rwkv_debug_read(b200rwkv_engine*, const char* name, float* out, size_t cap);
 
+/* Test aid, not on the product path: the weight fills the engine runs for one model tensor (at creation, and again on a weight
+ * update or a head format change), read back from the device.  b200rwkv_debug_fills returns how many fills read tensor
+ * `name` (0: none).  b200rwkv_debug_fill describes fill i in *info and, unless out is NULL, copies its destination to out
+ * (info->bytes bytes), untiled on the host, padding included.  R = tiles * 128 rows, Kp = kb * 128 columns:
+ *   SEG, qtype NONE: f16 [R][Kp], the rows [n0, n0 + N) and columns [k0, k0 + K) of the matrix (slice `off` of a 3-D tensor,
+ *     row stride ld), zero elsewhere.
+ *   SEG, quantised: codes u8 [R][Kp] (one code per byte), then Int8 / Int4: min f16 [R][kb] and scale f16 [R][kb]; NF4: absmax
+ *     f16 [R][2 kb]; FP8: scale f32 [R] -- b200rwkv_op_quantize's layout over the padded extent.
+ *   SEG with ad_tail > 0 (a W' plan): then the adapter tail blocks, f16 [R][ad_tail * 128].
+ *   VEC: f32 [count] = f32(x) * scale + bias of elements [off, off + count).  DECAY: f32 [count] = exp(-exp(x)).  RAW: f16 [count].
+ *   FOLD: the k-major time_decay_w2 copy as stored, f16 [N heads][K][64] of rows n0 ...  INIT: f32 [head_size + 2][num_emb],
+ *     State::init rows of layer n0.
+ * plan: the projection plan a SEG fill writes (base, W' of an adapter plan, or the quantised head of b200rwkv_head_format).
+ * A NULL engine or name, an unknown name, i out of range or cap < info->bytes is B200RWKV_ERR_INVALID before any CUDA call,
+ * and nothing is written to out. */
+#define B200RWKV_FILL_SEG 0
+#define B200RWKV_FILL_VEC 1
+#define B200RWKV_FILL_DECAY 2
+#define B200RWKV_FILL_FOLD 3
+#define B200RWKV_FILL_RAW 4
+#define B200RWKV_FILL_INIT 5
+#define B200RWKV_PLAN_BASE 0
+#define B200RWKV_PLAN_ADAPTER 1
+#define B200RWKV_PLAN_HEAD 2
+typedef struct {
+    int32_t kind, qtype, plan;
+    int32_t n0, N, k0, K, ld;
+    int64_t off;
+    int32_t tiles, kb, ad_tail;
+    int64_t count;
+    float scale, bias;
+    uint64_t bytes;
+} b200rwkv_fill_info;
+int32_t b200rwkv_debug_fills(b200rwkv_engine*, const char* name);
+int32_t b200rwkv_debug_fill(b200rwkv_engine*, const char* name, int32_t i, b200rwkv_fill_info* info, void* out, size_t cap);
+
 /* Profiling aid: raw stamp rows of the most recent b200rwkv_profile_insitu replay, one row of 512 uint64 per launch
  * (out = [launches][512]): globaltimer stamps of CTA 0 in [0..7] (entry, past griddepcontrol.wait, phase marks, exit), then
  * {SM id, last MMA issued, exit} of every projection CTA (or {entry, released, phase 1 done} of every CTA of the fused RWKV-6

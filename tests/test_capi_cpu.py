@@ -664,3 +664,43 @@ int main(int argc, char** argv) {
     if not has_gpu:
         rc, msg = out[1].split(" ", 1)
         assert int(rc) < 0 and "CUDA" in msg
+
+
+def test_debug_fill_refuses_bad_arguments_without_a_gpu():
+    """b200rwkv_debug_fills / debug_fill refuse a NULL engine, name or info with ERR_INVALID before any CUDA call, and write
+    nothing (the engine-side refusals are in tests/test_gpu_resident_weights.py)."""
+    lib = capi.lib()
+    info = capi.FillInfo()
+    info.kind = 77
+    out = np.full(64, 0xAB, np.uint8)
+    assert lib.b200rwkv_debug_fills(None, b"head.weight") == capi.ERR_INVALID
+    assert lib.b200rwkv_debug_fills(None, None) == capi.ERR_INVALID
+    for args in ((None, b"head.weight", 0, C.byref(info), capi.ptr(out), out.size), (None, None, 0, C.byref(info), None, 0),
+                 (None, b"emb.weight", -1, None, capi.ptr(out), 0)):
+        assert lib.b200rwkv_debug_fill(*args) == capi.ERR_INVALID
+        assert "null argument" in lib.b200rwkv_last_error(None).decode()
+    assert info.kind == 77 and np.all(out == 0xAB)
+
+
+def test_fill_info_matches_the_header(tmp_path):
+    """capi.FillInfo has the layout a C compiler gives b200rwkv_fill_info."""
+    import shutil
+    import subprocess
+    gcc = shutil.which("gcc")
+    if gcc is None:
+        pytest.skip("no C compiler")
+    fields = [n for n, _ in capi.FillInfo._fields_]
+    src = tmp_path / "fi.c"
+    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "b200rwkv.h"\nint main(void) {\n'
+                   '  printf("%zu\\n", sizeof(b200rwkv_fill_info));\n' +
+                   "".join(f'  printf("%zu\\n", offsetof(b200rwkv_fill_info, {n}));\n' for n in fields) + '  return 0; }\n')
+    exe = tmp_path / "fi"
+    subprocess.run([gcc, "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
+    got = [int(x) for x in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
+    assert got == [C.sizeof(capi.FillInfo)] + [getattr(capi.FillInfo, n).offset for n in fields]
+    assert (capi.FILL_SEG, capi.FILL_VEC, capi.FILL_DECAY, capi.FILL_FOLD, capi.FILL_RAW, capi.FILL_INIT) == tuple(range(6))
+    hdr = open(os.path.join(ROOT, "include", "b200rwkv.h")).read()
+    for i, k in enumerate(("SEG", "VEC", "DECAY", "FOLD", "RAW", "INIT")):
+        assert f"#define B200RWKV_FILL_{k} {i}\n" in hdr
+    for i, k in enumerate(("BASE", "ADAPTER", "HEAD")):
+        assert f"#define B200RWKV_PLAN_{k} {i}\n" in hdr
